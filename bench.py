@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py - headline benchmark of parakeet_b200 (contract in the task statement).
+"""bench.py - headline benchmark of parakeet_b200.
 
 Workload (BASELINE.json configs[1]): Parallel WaveGAN generator inference, batch 32, 80-mel x 400 frames -> 3.84 M
 samples of 24 kHz audio per step, CSMSC generator (30 residual layers, 64/128 channels, upsample [4,5,3,5]), random
 weights of that architecture, synthetic N(0,1) mel + noise.  One step = one pass of the generator over one batch.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 N > 1 is launched by torchrun (one rank per GPU); utterances are independent, so every rank runs its own batch of 32
 with no data-path collective (weak scaling) and `value` is the whole-job aggregate.  The same line also carries, at every N,
@@ -13,8 +13,11 @@ with no data-path collective (weak scaling) and `value` is the whole-job aggrega
 on rank 0 and copied to the host: strong scaling) and `cfg5_train` (BASELINE cfg 5: FastSpeech2 training step on a global
 batch of 64 with the NCCL all-reduce of the flat gradient; all-reduce time and bus bandwidth reported separately).
 `--impl reference` times the reference algorithm's CPU path (the torch-CPU oracle restatement; PaddlePaddle itself is not
-installable here, see DESIGN.md) with all host threads on a bounded sample of the same workload; the `cpu_baseline` of the
-N=1 line uses the same procedure and sample (cpu_leg).
+a dependency of this project, see DESIGN.md) with all host threads on a bounded sample of the same workload; the `cpu_baseline`
+of the N=1 line uses the same procedure and sample (cpu_leg).
+`--dump-outputs DIR` writes, after the timed steps, the waveform batch the last timed step returned (rank 0) as
+DIR/pwg_wav.npy (float32, 32 x 1 x 120 000 = 15.4 MB); the inputs and weights are seeded, so two builds can be compared
+output for output.
 """
 import argparse
 import json
@@ -33,7 +36,8 @@ FLOP_PER_SAMPLE = 30 * FLOP_PER_SAMPLE_LAYER + 2 * 64 * 64 + 2 * 64 + 2 * 64  # 
 
 
 def peaks():
-    p = dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3), for a card allowed 700 W; a card with a lower power limit clocks lower
+    p = dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             m = json.load(f)
@@ -313,6 +317,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-extra", action="store_true", help="skip the FastSpeech2 / end-to-end extras and the CPU baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output of the last timed step as DIR/pwg_wav.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -384,6 +390,10 @@ def main():
     gen._layer_events = None
     ms_per_step = ms_total / args.steps
     value = world * samples_per_step * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "pwg_wav.npy"), y.detach().float().cpu().numpy())
 
     # ---------------- end to end through the public API with host buffers ----------------
     wav_h = torch.empty(BATCH, 1, FRAMES * HOP, dtype=torch.float32).pin_memory()
@@ -422,23 +432,11 @@ def main():
     flops_per_launch = FLOP_PER_SAMPLE_LAYER * samples_per_step               # algorithmic (one pass), 330 GFLOP
     achieved_tf = flops_per_launch / (layer_launch_ms * 1e-3) / 1e12
     fcond = PWGGenerator._frame_cond()
-    kernel = "pk::fc::pwg_layer_fc_kernel" if fcond else "pk::pwg_layer_pair_kernel"
-    # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of that kernel at this exact configuration, from the committed
-    # `ncu --set full` capture (profiles/roofline_traffic.json, written by scripts/ncu_traffic.py from the .ncu-rep); null when
-    # no capture of the current kernel is on file
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            ent = json.load(f).get(kernel)
-        if ent:
-            traffic, traffic_src = ent["dram_bytes_per_launch"], ent.get("source")
-    except Exception:
-        pass
+    kernel = "pk::fc::pwg_layer_fc_kernel" if fcond else "pk::pwg_layer_kernel"
     bytes_per_sample = (256 + 256 + 512) if fcond else (256 + 256 + 512 + 320)   # x rd, x wr, skip rmw (+ conditioning planes)
     roofline = {"bound": "tensor", "kernel": kernel, "achieved": achieved_tf, "peak": pk["bf16_tflops_sustained"],
                 "unit": "TFLOP/s", "frac": achieved_tf / pk["bf16_tflops_sustained"],
-                "traffic": traffic, "traffic_unit": "bytes/launch", "traffic_source": traffic_src,
-                "peak_source": pk["source"] + ", sustained bf16 (kernel timed inside a long step)",
+                "peak_source": pk["source"] + ", dense bf16 (kernel timed inside a long step)",
                 "launch_ms": layer_launch_ms, "launches_per_step": 30,
                 "note": "algorithmic FLOPs of the reference's block (86 016 per sample per layer); split-bf16 operands execute 3 "
                         "tensor-core passes per product (+ the residual pass)",
@@ -549,7 +547,7 @@ def main():
                                                  "ms_per_step": pt_ms, "generator_loss": float(lt["generator_loss"]),
                                                  "discriminator_loss": float(lt["discriminator_loss"]),
                                                  "note": "PWGUpdater.update_core: G step (MR-STFT + adversarial) + D step, batch 6 x 25 500 samples, "
-                                                         "unfused training formulation (separate tcgen05 GEMMs + element-wise kernels)"}
+                                                         "unfused training formulation (separate wgmma GEMMs + element-wise kernels)"}
         except Exception as ex:  # extras must never break the headline line
             out.setdefault("extra", {})["error"] = repr(ex)
     if not args.no_extra and world == 1:

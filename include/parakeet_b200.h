@@ -1,4 +1,4 @@
-/* parakeet_b200 C-ABI: B200 (sm_100a) kernels for the Parakeet TTS hot path.
+/* parakeet_b200 C-ABI: H100 (sm_90a) kernels for the Parakeet TTS hot path.
  *
  * The reference (PaddlePaddle/Parakeet) has no FFI of its own: its hot path is Python calling paddle.nn ops.
  * This header is the boundary a Parakeet maintainer would bind instead of those ops (ctypes stub in
@@ -45,7 +45,7 @@ int64_t pk_launch_count(void);
 int pk_split_f32(const float* x, void* hi, void* lo, int64_t n, pk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Generic channels-last Conv1D / Linear / batched-matmul on tcgen05 tensor cores.
+ * Generic channels-last Conv1D / Linear / batched-matmul on wgmma tensor cores.
  *
  *   y[z, t, n] = act( scale * sum_{tap, k} A[za, t + (tap - pad) * dil, a_col + k] * B[zb, n, b_col + tap*Kp + k]
  *                     + bias[n] ) + residual[z, t, n]          ; rows t >= lens[b] are written as 0
@@ -184,8 +184,6 @@ typedef struct pk_pwg_layer_args {
   const float* bias2;      /* HOST pointer [128]: conv1x1_skip bias (ignored, see pk_pwg_tail) | conv1x1_out bias */
   float* skip;             /* fp32 (batch, t, 64) running sum of skips */
   int32_t skip_init;       /* 1: overwrite (first layer), 0: accumulate */
-  void* prof;              /* debug: NULL, or device uint64[64] phase-cycle counters accumulated by the kernel
-                              ([0..1] producer, [8..14] MMA issuer, [16..22]/[24..30] epilogue halves, [32] tiles) */
 } pk_pwg_layer_args;
 int pk_pwg_residual_layer(const pk_pwg_layer_args* args, pk_stream_t stream);
 
@@ -224,7 +222,6 @@ typedef struct pk_pwg_layer_fc_args {
   const float* bias2;
   float* skip;
   int32_t skip_init;
-  void* prof;
 } pk_pwg_layer_fc_args;
 int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* args, pk_stream_t stream);
 
@@ -260,7 +257,7 @@ int pk_masked_softmax(const float* s, const int32_t* key_lens, int32_t batch, in
  * TIME in the reference's batched forward).  x, y fp32 contiguous; in place allowed. */
 int pk_l2_normalize(const float* x, int32_t outer, int32_t n, int32_t inner, float eps, float* y, pk_stream_t stream);
 /* Fused scaled-dot-product attention of an FFT block (attention.py:88-131: scores = q k^T / sqrt(d_k), masked_fill(min) ->
- * softmax -> masked_fill(0), p_attn . v, heads merged) in one kernel: scores and probabilities stay in tensor memory.
+ * softmax -> masked_fill(0), p_attn . v, heads merged) in one kernel: scores and probabilities stay in registers.
  *   qkv planes (batch, t, 3 * heads * dk): [q | k | v] of the fused QKV projection, head h in columns h * dk of each third;
  *   vt planes (batch * heads, dk, tp): v transposed per head (pk_transpose_heads), columns >= t zero; both pairs of planes
  *   from one allocation each (lo after hi).  key_lens / row_lens: device int32 [batch] or NULL (keys >= key_lens[b] masked;
@@ -338,7 +335,7 @@ int pk_waveflow_layer_update(const float* o, int64_t rows, int32_t c, float* sta
 int pk_waveflow_row_out(const float* skip, const float* w, const float* bias, const float* z_row, int64_t z_batch_stride,
                         int32_t batch, int32_t width, int32_t c, float* x_next, int64_t x_batch_stride, pk_stream_t stream);
 
-/* One whole ResidualBlock.add_input (:248-285) as ONE CTA-pair kernel (channels == 64; the default layer path of
+/* One whole ResidualBlock.add_input (:248-285) as ONE kernel (channels == 64; the default layer path of
  * ConditionalWaveFlow.inverse, PK_WF_FUSED=0 selects the pk_conv_gemm_ex pair above):
  *   a | g = conv2d(3-row ring, dilation (1, 2^l)) + condition_proj(condition row) + bias1;  z = tanh(a) sigmoid(g);
  *   skip | res = out_proj(z) + bias2;  skip accumulator (=|+=) skip;  ring slot `slot` of the NEXT layer <- row + res.
@@ -367,7 +364,6 @@ typedef struct pk_waveflow_layer_args {
   void* next_lo;
   float* skip;
   int32_t skip_init;
-  void* prof;              /* debug: NULL, or device uint64[8]: MMA-issuer cycles [0] issue, [1] wait data, [2] wait acc2, [3] wait z; [4] tiles */
 } pk_waveflow_layer_args;
 int pk_waveflow_layer(const pk_waveflow_layer_args* args, pk_stream_t stream);
 
@@ -407,7 +403,6 @@ typedef struct pk_waveflow_flow_args {
   float* skip;
   uint32_t* flags;
   int64_t flags_len;
-  void* prof;              /* debug: as in pk_waveflow_layer_args */
 } pk_waveflow_flow_args;
 int pk_waveflow_flow(const pk_waveflow_flow_args* args, pk_stream_t stream);
 

@@ -62,7 +62,7 @@ class PwgLayerArgs(C.Structure):
                 ("lens", C.c_void_p), ("x_hi", C.c_void_p), ("x_lo", C.c_void_p), ("y_hi", C.c_void_p),
                 ("y_lo", C.c_void_p), ("c_hi", C.c_void_p), ("c_lo", C.c_void_p), ("w1_hi", C.c_void_p),
                 ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p), ("bias1", C.c_void_p),
-                ("bias2", C.c_void_p), ("skip", C.c_void_p), ("skip_init", C.c_int32), ("prof", C.c_void_p)]
+                ("bias2", C.c_void_p), ("skip", C.c_void_p), ("skip_init", C.c_int32)]
 
 
 class PwgLayerFcArgs(C.Structure):
@@ -72,7 +72,7 @@ class PwgLayerFcArgs(C.Structure):
                 ("u_end_base", C.c_int32), ("p_rows", C.c_int32), ("p_ld", C.c_int32),
                 ("p_frames", C.c_int32), ("p_row0", C.c_int32), ("p_hi", C.c_void_p), ("p_lo", C.c_void_p),
                 ("w1_hi", C.c_void_p), ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p),
-                ("bias1", C.c_void_p), ("bias2", C.c_void_p), ("skip", C.c_void_p), ("skip_init", C.c_int32), ("prof", C.c_void_p)]
+                ("bias1", C.c_void_p), ("bias2", C.c_void_p), ("skip", C.c_void_p), ("skip_init", C.c_int32)]
 
 
 class WaveflowLayerArgs(C.Structure):
@@ -81,7 +81,7 @@ class WaveflowLayerArgs(C.Structure):
                 ("cond_hi", C.c_void_p), ("cond_lo", C.c_void_p), ("cond_batch_stride", C.c_int64),
                 ("w1_hi", C.c_void_p), ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p),
                 ("bias1", C.c_void_p), ("bias2", C.c_void_p), ("next_hi", C.c_void_p), ("next_lo", C.c_void_p),
-                ("skip", C.c_void_p), ("skip_init", C.c_int32), ("prof", C.c_void_p)]
+                ("skip", C.c_void_p), ("skip_init", C.c_int32)]
 
 
 class WaveflowFlowArgs(C.Structure):
@@ -91,7 +91,7 @@ class WaveflowFlowArgs(C.Structure):
                 ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p), ("bias1", C.c_void_p),
                 ("bias2", C.c_void_p), ("in_w", C.c_void_p), ("in_b", C.c_void_p), ("out_w", C.c_void_p),
                 ("out_b", C.c_void_p), ("z", C.c_void_p), ("x", C.c_void_p), ("skip", C.c_void_p), ("flags", C.c_void_p),
-                ("flags_len", C.c_int64), ("prof", C.c_void_p)]
+                ("flags_len", C.c_int64)]
 
 
 def _declare(L):

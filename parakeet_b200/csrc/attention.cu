@@ -2,18 +2,19 @@
 // fastspeech2_transformer/attention.py:88-131) as ONE kernel per layer - scores, key-padding mask, softmax and P.V never
 // leave the SM (round 1 ran four launches per layer around an fp32 (B*H, T, T) score tensor in HBM).
 //
-//   S   = Q K^T                       tcgen05, split-bf16 operands (3 passes), fp32 in tensor memory     [128 q x 128 keys]
+//   S   = Q K^T                       wgmma, split-bf16 operands (3 passes), fp32 in registers           [128 q x 128 keys]
 //   P   = exp2((S - m) * scale*log2e) running row max m / row sum l (online softmax), keys >= key_len -> 0 (masked_fill)
-//   O   = O * alpha + P V             P is written (packed bf16x2, hi | lo) into tensor memory and is the A operand of the
-//                                     second GEMM straight from there; V^T tiles (K-major) come from pk_transpose_heads
+//   O   = O * alpha + P V             P (packed bf16x2, hi | lo) stays in registers and is the A operand of the second
+//                                     GEMM straight from there; V^T tiles (K-major) come from pk_transpose_heads
 //   ctx = O / l                       split planes (B, T, A), heads merged (attention.py:126-129)
 //
 // One CTA per (utterance, head, 128-query tile); K and V^T tiles of 128 keys stream through one 96 KB buffer, Q (96 KB for
-// d_k = 192) stays resident.  Roles: warp 0 TMA producer, warp 1 MMA issuer, warps 4-7 softmax / correction / epilogue
-// (one query row per thread).  The attention FLOPs of FastSpeech2 are tiny (T <= ~1 400, 2 heads); the point of the kernel
-// is to remove the HBM round trips and the launches, so the K / V phases of a tile are serialised rather than double-buffered.
+// d_k = 192) stays resident.  Roles: warps 0-7 two consumer warpgroups of 64 query rows each (S = Q K^T with wgmma into
+// registers, online softmax in registers, P as the register A operand of P.V, O in registers), warps 8-11 the producer
+// warpgroup (one TMA lane).  The attention FLOPs of FastSpeech2 are tiny (T <= ~1 400, 2 heads); the point of the kernel is
+// to remove the HBM round trips and the launches, so the K / V phases of a tile are serialised rather than double-buffered.
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 namespace attn {
@@ -23,8 +24,9 @@ constexpr int kChunkBytes = 2 * kTile;                // hi | lo
 constexpr int kMaxDkc = 3;                            // d_k <= 192
 constexpr int kBufBytes = kMaxDkc * kChunkBytes;      // 96 KB: Q, and the K / V^T stream buffer
 constexpr int kSmem = 2 * kBufBytes + 1024 + 128;
-constexpr int kThreads = 256;
-constexpr uint32_t kColS = 0, kColO = 128, kColP = 320;   // tensor-memory columns: S fp32 [128], O fp32 [<= 192], P bf16x2 [64 | 64]
+static_assert(kSmem <= 227 * 1024, "shared memory budget");
+constexpr int kConsumerThreads = 256;
+constexpr int kThreads = kConsumerThreads + 128;
 
 struct Args {
   int batch, t, heads, dkc, a_dim;      // dkc = d_k / 64, a_dim = heads * d_k
@@ -35,22 +37,6 @@ struct Args {
   __nv_bfloat16* ctx_lo;
 };
 
-__device__ __forceinline__ void tma_load_4d_a(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -64,53 +50,52 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
+
+template <int DK>
+__device__ __forceinline__ void wgmma_rs_o(float (&d)[DK / 2], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
+  if constexpr (DK == 64) wgmma_rs_n64(d, a, b, acc);
+  else if constexpr (DK == 128) wgmma_rs_n128(d, a, b, acc);
+  else wgmma_rs_n192(d, a, b, acc);
 }
 
+template <int DKC>
 __global__ void __launch_bounds__(kThreads, 1)
 fused_attention_kernel(const __grid_constant__ CUtensorMap tm_qkv,     // (3A, T, B, 2 planes): box 64 x 128 rows x both planes
                        const __grid_constant__ CUtensorMap tm_vt,      // (Tp, d_k, B*H, 2 planes): box 64 keys x d_k rows x both planes
                        const Args p) {
+  constexpr int dk = DKC * 64;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t qbuf = smem, kvbuf = smem + kBufBytes;
   const uint32_t bars = kvbuf + kBufBytes;
-  const uint32_t q_full = bars, kv_full = bars + 8, kv_empty = bars + 16, s_full = bars + 24, p_full = bars + 32, o_done = bars + 40;
-  const uint32_t tmem_slot = bars + 48;
+  const uint32_t q_full = bars, kv_full = bars + 8, kv_empty = bars + 16;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * 128;
-  const int dk = p.dkc * 64;
   const int rows_live = p.row_lens ? min(__ldg(p.row_lens + b), p.t) : p.t;
   const int klen = p.key_lens ? min(__ldg(p.key_lens + b), p.t) : p.t;
   const int nkv = (q0 < rows_live) ? (klen + 127) >> 7 : 0;            // no valid query row / no valid key: the tile is zeros
+  constexpr uint32_t chunk_bytes = kChunkBytes;
+  constexpr uint32_t vchunk = static_cast<uint32_t>(dk) * kSwizzleBytes;   // one plane of a V^T key chunk: d_k rows x 128 B
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_qkv); tma_prefetch_desc(&tm_vt);
-    mbar_init_a(q_full, 1); mbar_init_a(kv_full, 1); mbar_init_a(kv_empty, 1);
-    mbar_init_a(s_full, 1); mbar_init_a(p_full, 128); mbar_init_a(o_done, 1);
+    mbar_init_a(q_full, 1); mbar_init_a(kv_full, 1); mbar_init_a(kv_empty, kConsumerThreads / 32);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_a<512>(tmem_slot);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = lds_u32(tmem_slot);
-  const uint32_t chunk_bytes = kChunkBytes;
-  const uint32_t vchunk = static_cast<uint32_t>(dk) * kSwizzleBytes;   // one plane of a V^T key chunk: d_k rows x 128 B
 
-  if (warp == 0) {
-    if (lane == 0 && nkv > 0) {
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0 && nkv > 0) {
       // ------------------------------ TMA producer ------------------------------
-      mbar_arrive_expect_tx_a(q_full, p.dkc * chunk_bytes);
-      for (int c = 0; c < p.dkc; ++c) tma_load_4d_a(qbuf + c * chunk_bytes, &tm_qkv, q_full, h * dk + c * 64, q0, b, 0);
+      mbar_arrive_expect_tx_a(q_full, DKC * chunk_bytes);
+      for (int c = 0; c < DKC; ++c) tma_load_4d_a(qbuf + c * chunk_bytes, &tm_qkv, q_full, h * dk + c * 64, q0, b, 0);
       uint32_t n = 0;                                            // uses of the stream buffer
       for (int j = 0; j < nkv; ++j) {
         mbar_wait_a(kv_empty, (n & 1) ^ 1);
-        mbar_arrive_expect_tx_a(kv_full, p.dkc * chunk_bytes);   // K tile: keys [128 j, +128) x d_k
-        for (int c = 0; c < p.dkc; ++c) tma_load_4d_a(kvbuf + c * chunk_bytes, &tm_qkv, kv_full, p.a_dim + h * dk + c * 64, j * 128, b, 0);
+        mbar_arrive_expect_tx_a(kv_full, DKC * chunk_bytes);     // K tile: keys [128 j, +128) x d_k
+        for (int c = 0; c < DKC; ++c) tma_load_4d_a(kvbuf + c * chunk_bytes, &tm_qkv, kv_full, p.a_dim + h * dk + c * 64, j * 128, b, 0);
         ++n;
         mbar_wait_a(kv_empty, (n & 1) ^ 1);
         mbar_arrive_expect_tx_a(kv_full, 2 * 2 * vchunk);        // V^T tile: d_k rows x keys [128 j, +128) as two 64-key chunks
@@ -118,143 +103,123 @@ fused_attention_kernel(const __grid_constant__ CUtensorMap tm_qkv,     // (3A, T
         ++n;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && nkv > 0) {
-      // ------------------------------ MMA issuer ------------------------------
-      const uint32_t idesc_s = make_idesc_bf16_f32(128, 128);
-      const uint32_t idesc_o = make_idesc_bf16_f32(128, dk);
-      mbar_wait_a(q_full, 0);
-      uint32_t n = 0;
-      for (int j = 0; j < nkv; ++j) {
-        mbar_wait_a(kv_full, n & 1); ++n;
-        tcgen05_fence_after();
-        for (int c = 0; c < p.dkc; ++c) {
-          const uint64_t a_hi = make_smem_desc_sw128(qbuf + c * chunk_bytes), a_lo = make_smem_desc_sw128(qbuf + c * chunk_bytes + kTile);
-          const uint64_t b_hi = make_smem_desc_sw128(kvbuf + c * chunk_bytes), b_lo = make_smem_desc_sw128(kvbuf + c * chunk_bytes + kTile);
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16(tmem_base + kColS, a_hi + koff, b_hi + koff, idesc_s, !(c == 0 && k == 0));
-            umma_bf16(tmem_base + kColS, a_lo + koff, b_hi + koff, idesc_s, 1);
-            umma_bf16(tmem_base + kColS, a_hi + koff, b_lo + koff, idesc_s, 1);
-          }
-        }
-        umma_commit_a(kv_empty);                                 // the K tile may be overwritten by V^T
-        umma_commit_a(s_full);
-        mbar_wait_a(p_full, j & 1);                              // P (and the rescaled O) are in tensor memory
-        mbar_wait_a(kv_full, n & 1); ++n;
-        tcgen05_fence_after();
-        for (int kc = 0; kc < 2; ++kc) {
-          const uint64_t b_hi = make_smem_desc_sw128(kvbuf + kc * 2 * vchunk), b_lo = make_smem_desc_sw128(kvbuf + kc * 2 * vchunk + vchunk);
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            const uint32_t a_hi = tmem_base + kColP + 8 * (kc * 4 + k), a_lo = a_hi + 64;
-            umma_bf16_ts(tmem_base + kColO, a_hi, b_hi + koff, idesc_o, !(j == 0 && kc == 0 && k == 0));
-            umma_bf16_ts(tmem_base + kColO, a_lo, b_hi + koff, idesc_o, 1);
-            umma_bf16_ts(tmem_base + kColO, a_hi, b_lo + koff, idesc_o, 1);
-          }
-        }
-        umma_commit_a(kv_empty);
-        umma_commit_a(o_done);
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ softmax / correction / epilogue: one query row per thread ------------------------------
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t ts = tmem_base + lane_base + kColS, to = tmem_base + lane_base + kColO, tp = tmem_base + lane_base + kColP;
-    float m = -INFINITY, l = 0.f;
+  } else {
+    // ------------------ consumers: 64 query rows per warpgroup; this thread holds rows r0 and r0 + 8 ------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + 16 * (warp & 3) + (lane >> 2);   // row inside the tile
+    const int cq = 2 * (lane & 3);                            // first of this thread's two columns in each 8-column group
+    float o[dk / 2];
+#pragma unroll
+    for (int i = 0; i < dk / 2; ++i) o[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    if (nkv > 0) mbar_wait_a(q_full, 0);
+    uint32_t n = 0;
     for (int j = 0; j < nkv; ++j) {
       const int kv0 = j * 128;
-      mbar_wait_a(s_full, j & 1);
-      tcgen05_fence_after();
-      float tile_max = -INFINITY;
+      float s[64];
+      mbar_wait_a(kv_full, n & 1); ++n;
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        __syncwarp();
-        tmem_ld_32x32(ts + c * 32, v);
-        tmem_ld_wait();
+      for (int c = 0; c < DKC; ++c) {
+        const uint64_t a_hi = make_smem_desc_sw128(qbuf + c * chunk_bytes + wg * 64 * kSwizzleBytes);
+        const uint64_t a_lo = make_smem_desc_sw128(qbuf + c * chunk_bytes + kTile + wg * 64 * kSwizzleBytes);
+        const uint64_t b_hi = make_smem_desc_sw128(kvbuf + c * chunk_bytes), b_lo = make_smem_desc_sw128(kvbuf + c * chunk_bytes + kTile);
 #pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (kv0 + c * 32 + i < klen) tile_max = fmaxf(tile_max, v[i]);
-      }
-      const float m_new = fmaxf(m, tile_max);                       // finite: every streamed tile holds at least one valid key
-      const float alpha = ex2_approx((m - m_new) * p.scale_log2e);   // 0 on the first tile (m = -inf)
-      if (j > 0) {
-        mbar_wait_a(o_done, (j - 1) & 1);                           // P.V of the previous tile has landed in O
-        tcgen05_fence_after();
-        for (int c = 0; c < 2 * p.dkc; ++c) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(to + c * 32, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] *= alpha;
-          tmem_st_32x32(to + c * 32, reinterpret_cast<const uint32_t*>(v));
+        for (int k = 0; k < 4; ++k) {
+          wgmma_ss_n128(s, a_hi + desc_kstep(k), b_hi + desc_kstep(k), !(c == 0 && k == 0));
+          wgmma_ss_n128(s, a_lo + desc_kstep(k), b_hi + desc_kstep(k), 1);
+          wgmma_ss_n128(s, a_hi + desc_kstep(k), b_lo + desc_kstep(k), 1);
         }
       }
-      float lsum = 0.f;
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+      __syncwarp();
+      if (lane == 0) mbar_arrive_a(kv_empty);                    // the K tile may be overwritten by V^T
+      // online softmax over this tile's keys (row max / sum across the 4 lanes of a quad)
+      float tmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        float v[32];
-        uint32_t hi[16], lo[16];
-        __syncwarp();
-        tmem_ld_32x32(ts + c * 32, v);
-        tmem_ld_wait();
+      for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = (kv0 + c * 32 + i < klen) ? ex2_approx((v[i] - m_new) * p.scale_log2e) : 0.f;
-          const float p1 = (kv0 + c * 32 + i + 1 < klen) ? ex2_approx((v[i + 1] - m_new) * p.scale_log2e) : 0.f;
-          lsum += p0 + p1;
-          split2(p0, p1, hi[i >> 1], lo[i >> 1]);
-        }
-        // 16 packed columns per plane for these 32 keys: hi at P + 16 c, lo at P + 64 + 16 c
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                     ::"r"(tp + 16 * c), "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]), "r"(hi[4]), "r"(hi[5]), "r"(hi[6]), "r"(hi[7]),
-                       "r"(hi[8]), "r"(hi[9]), "r"(hi[10]), "r"(hi[11]), "r"(hi[12]), "r"(hi[13]), "r"(hi[14]), "r"(hi[15]) : "memory");
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                     ::"r"(tp + 64 + 16 * c), "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]), "r"(lo[4]), "r"(lo[5]), "r"(lo[6]), "r"(lo[7]),
-                       "r"(lo[8]), "r"(lo[9]), "r"(lo[10]), "r"(lo[11]), "r"(lo[12]), "r"(lo[13]), "r"(lo[14]), "r"(lo[15]) : "memory");
+        for (int e = 0; e < 4; ++e)
+          if (kv0 + 8 * jj + cq + (e & 1) < klen) tmax[e >> 1] = fmaxf(tmax[e >> 1], s[4 * jj + e]);
       }
-      l = l * alpha + lsum;
-      m = m_new;
-      tmem_st_wait();
-      tcgen05_fence_before();
-      mbar_arrive_a(p_full);
+      float alpha[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        tmax[hh] = fmaxf(tmax[hh], __shfl_xor_sync(0xffffffffu, tmax[hh], 1));
+        tmax[hh] = fmaxf(tmax[hh], __shfl_xor_sync(0xffffffffu, tmax[hh], 2));
+        const float m_new = fmaxf(m[hh], tmax[hh]);             // finite: every streamed tile holds at least one valid key
+        alpha[hh] = ex2_approx((m[hh] - m_new) * p.scale_log2e);   // 0 on the first tile (m = -inf)
+        m[hh] = m_new;
+      }
+#pragma unroll
+      for (int i = 0; i < dk / 8; ++i) {
+        o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0]; o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
+      }
+      float lsum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float v = (kv0 + 8 * jj + cq + (e & 1) < klen) ? ex2_approx((s[4 * jj + e] - m[e >> 1]) * p.scale_log2e) : 0.f;
+          s[4 * jj + e] = v;
+          lsum[e >> 1] += v;
+        }
+      }
+      l[0] = l[0] * alpha[0] + lsum[0];
+      l[1] = l[1] * alpha[1] + lsum[1];
+      // O += P V^T-tile: two 64-key chunks, 4 K-steps each; P hi / lo packed from the S fragments
+      mbar_wait_a(kv_full, n & 1); ++n;
+#pragma unroll
+      for (int kc = 0; kc < 2; ++kc) {
+        uint32_t ph[4][4], pl[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int kk = 4 * kc + k;                 // keys [16 kk, 16 kk + 16) = S column groups 2 kk, 2 kk + 1
+          split2(s[8 * kk + 0], s[8 * kk + 1], ph[k][0], pl[k][0]);
+          split2(s[8 * kk + 2], s[8 * kk + 3], ph[k][1], pl[k][1]);
+          split2(s[8 * kk + 4], s[8 * kk + 5], ph[k][2], pl[k][2]);
+          split2(s[8 * kk + 6], s[8 * kk + 7], ph[k][3], pl[k][3]);
+        }
+        const uint64_t b_hi = make_smem_desc_sw128(kvbuf + kc * 2 * vchunk), b_lo = make_smem_desc_sw128(kvbuf + kc * 2 * vchunk + vchunk);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_rs_o<dk>(o, ph[k], b_hi + desc_kstep(k), 1);
+          wgmma_rs_o<dk>(o, pl[k], b_hi + desc_kstep(k), 1);
+          wgmma_rs_o<dk>(o, ph[k], b_lo + desc_kstep(k), 1);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(o);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive_a(kv_empty);
     }
     // epilogue: ctx[b, q0 + r, h d_k + :] = O / l (zeros for rows / tiles without valid queries or keys)
-    const int row = q0 + r;
-    if (nkv > 0) {
-      mbar_wait_a(o_done, (nkv - 1) & 1);
-      tcgen05_fence_after();
-    }
-    const bool live = nkv > 0 && row < rows_live;
-    const float inv = live ? 1.f / l : 0.f;
-    const long long off = (static_cast<long long>(b) * p.t + row) * p.a_dim + h * dk;
-    for (int c = 0; c < 2 * p.dkc; ++c) {
-      float v[32];
-      uint32_t oh[16], ol[16];
-      if (nkv > 0) {
-        __syncwarp();
-        tmem_ld_32x32(to + c * 32, v);
-        tmem_ld_wait();
-      }
 #pragma unroll
-      for (int i = 0; i < 32; i += 2) split2(live ? v[i] * inv : 0.f, live ? v[i + 1] * inv : 0.f, oh[i >> 1], ol[i >> 1]);
+    for (int hh = 0; hh < 2; ++hh) {
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = q0 + r0 + 8 * hh;
+      const bool live = nkv > 0 && row < rows_live;
+      const float inv = live ? 1.f / l[hh] : 0.f;
       if (row < p.t) {
-        st_global_v8(p.ctx_hi + off + c * 32, oh);
-        st_global_v8(p.ctx_hi + off + c * 32 + 16, oh + 8);
-        st_global_v8(p.ctx_lo + off + c * 32, ol);
-        st_global_v8(p.ctx_lo + off + c * 32 + 16, ol + 8);
+        const long long off = (static_cast<long long>(b) * p.t + row) * p.a_dim + h * dk + cq;
+#pragma unroll
+        for (int i = 0; i < dk / 8; ++i) {
+          uint32_t wh, wl;
+          split2(live ? o[4 * i + 2 * hh] * inv : 0.f, live ? o[4 * i + 2 * hh + 1] * inv : 0.f, wh, wl);
+          *reinterpret_cast<uint32_t*>(p.ctx_hi + off + 8 * i) = wh;
+          *reinterpret_cast<uint32_t*>(p.ctx_lo + off + 8 * i) = wl;
+        }
       }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -278,7 +243,9 @@ extern "C" int pk_fused_attention(const void* qkv_hi, const void* qkv_lo, const 
   if ((rc = encode_tmap_bf16_planes(&tv, vt_hi, vt_lo, tp, dk, static_cast<uint64_t>(batch) * heads, tp, static_cast<uint64_t>(dk) * tp, dk))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     attr_set = true;
   }
   Args p;
@@ -287,7 +254,10 @@ extern "C" int pk_fused_attention(const void* qkv_hi, const void* qkv_lo, const 
   p.scale_log2e = scale * 1.4426950408889634f;
   p.ctx_hi = static_cast<__nv_bfloat16*>(ctx_hi); p.ctx_lo = static_cast<__nv_bfloat16*>(ctx_lo);
   dim3 grid((t + 127) / 128, heads, batch);
-  fused_attention_kernel<<<grid, kThreads, kSmem, static_cast<cudaStream_t>(stream)>>>(tq, tv, p);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (p.dkc == 1) fused_attention_kernel<1><<<grid, kThreads, kSmem, st>>>(tq, tv, p);
+  else if (p.dkc == 2) fused_attention_kernel<2><<<grid, kThreads, kSmem, st>>>(tq, tv, p);
+  else fused_attention_kernel<3><<<grid, kThreads, kSmem, st>>>(tq, tv, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

@@ -1,13 +1,13 @@
-// pk_conv_gemm: channels-last Conv1D / Linear / batched matmul as an im2col-free tiled GEMM on tcgen05.
+// pk_conv_gemm: channels-last Conv1D / Linear / batched matmul as an im2col-free tiled GEMM on wgmma.
 //
-//   - persistent CTAs (one per SM) walking 128(time) x BLOCK_N(channel) output tiles, two TMEM accumulators so that the
-//     epilogue of tile i overlaps the main loop of tile i+1; 192 threads:
-//       warp 0   : TMA producer  (one elected lane)
-//       warp 1   : TMEM allocator + tcgen05.mma issuer (one elected lane)
-//       warps 2-5: epilogue (TMEM -> registers -> bias/act/residual/mask -> global), one output row per thread
+//   - persistent CTAs (one per SM) walking 128(time) x BLOCK_N(channel) output tiles; 384 threads:
+//       warps 0-7: two consumer warpgroups, each accumulating 64 rows x BLOCK_N in registers (wgmma) and then running the
+//                  epilogue (registers -> shared-memory staging -> bias/act/residual/mask -> global), one output row per thread
+//       warps 8-11: producer warpgroup: one TMA lane running ahead of the consumers through a ring of shared-memory stages;
+//                  it drops to 40 registers so that the consumers can hold a 64 x 256 fp32 accumulator (232 registers)
 //   - K loop over (tap, 64-channel chunk): each conv tap is just the same A tensor read `(tap - pad) * dil` rows
 //     further along; TMA zero-fills rows outside the utterance, which is the conv's zero padding (no im2col).
-//   - split-bf16 operands, 3 MMAs per K-step (hi*hi + lo*hi + hi*lo), fp32 accumulation in TMEM.
+//   - split-bf16 operands, 3 wgmma per K-step (hi*hi + lo*hi + hi*lo), fp32 accumulation.
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -15,12 +15,13 @@
 #include <algorithm>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 
 constexpr int kBlockM = 128;
-constexpr int kGemmThreads = 192;
+constexpr int kConsumerThreads = 256;                            // two warpgroups of 64 rows each
+constexpr int kGemmThreads = kConsumerThreads + 128;             // + the producer warpgroup (one TMA lane; registers handed over)
 
 template <int BLOCK_N>
 struct GemmCfg {
@@ -28,8 +29,9 @@ struct GemmCfg {
   static constexpr int kBBytes = BLOCK_N * kSwizzleBytes;       // one plane of one B chunk
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;  // hi + lo
   static constexpr int kStages = (BLOCK_N >= 256) ? 2 : (BLOCK_N >= 128 ? 3 : 4);
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr uint32_t kTmemCols = BLOCK_N < 32 ? 32 : BLOCK_N;
+  static constexpr int kStagingBytes = 2 * 2 * kStageSlotBytes;  // two epilogue slots per warpgroup
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
 struct GemmKernelArgs {
@@ -221,7 +223,7 @@ __device__ __forceinline__ void gemm_epilogue_pair(const GemmKernelArgs& p, floa
 struct GemmTile {     // persistent tile schedule: (batch, head) fastest, then m-tile, then n-tile, so that the CTAs running
   int m0, n0, bz, hz; // at the same time share one n-tile of B (the weights stay hot in L2) AND the dead tiles of a ragged
 };                    // batch (all utterances' m-tile k for large k) are consecutive indices, i.e. spread evenly over the
-                      // grid-strided CTAs (with m fastest and 148 % tiles_m == 0 some CTAs would own only dead tiles)
+                      // grid-strided CTAs (with m fastest and 132 % tiles_m == 0 some CTAs would own only dead tiles)
 __device__ __forceinline__ GemmTile gemm_tile(int tile, int tiles_m, int zdim, int heads, int block_n) {
   GemmTile t;
   const int z = tile % zdim;
@@ -243,48 +245,46 @@ __device__ __forceinline__ bool gemm_tile_live(const GemmKernelArgs& p, int m0, 
 }
 
 template <int BLOCK_N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[BLOCK_N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (BLOCK_N == 64) wgmma_ss_n64(d, a, b, acc);
+  else if constexpr (BLOCK_N == 128) wgmma_ss_n128(d, a, b, acc);
+  else wgmma_ss_n256(d, a, b, acc);
+}
+
+template <int BLOCK_N>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                  const GemmKernelArgs p) {
   using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int kChunks = BLOCK_N / 32;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-B alignment for SWIZZLE_128B tiles
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* acc_full = empty_bar + Cfg::kStages;     // [2] MMA issuer -> epilogue: accumulator of tile i is complete
-  uint64_t* acc_empty = acc_full + 2;                // [2] epilogue -> MMA issuer: accumulator buffer drained
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;     // 1024-B alignment for SWIZZLE_128B tiles
+  const uint32_t staging = smem + Cfg::kStages * Cfg::kStageBytes;
+  const uint32_t full_bar = staging + Cfg::kStagingBytes;         // [stages] TMA bytes landed
+  const uint32_t empty_bar = full_bar + 8 * Cfg::kStages;         // [stages] both warpgroups have read the stage
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_chunks = p.taps * p.k_chunks;
   const int zdim = p.batch * p.heads;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_a_hi);
     tma_prefetch_desc(&tm_a_lo);
     tma_prefetch_desc(&tm_b_hi);
     tma_prefetch_desc(&tm_b_lo);
     for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 128);
+      mbar_init_a(full_bar + 8 * s, 1);
+      mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32);       // one elected lane per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<2 * Cfg::kTmemCols>(tmem_base_slot);   // two accumulators: epilogue(i) overlaps mainloop(i+1)
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
       // ------------------------------ TMA producer ------------------------------
       const uint32_t tx_bytes = (p.passes == 3) ? Cfg::kStageBytes : (Cfg::kABytes + Cfg::kBBytes);
       uint32_t it = 0;                                 // running stage counter across tiles
@@ -300,72 +300,40 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
           const uint32_t ph = (it / Cfg::kStages) & 1;
           const int tap = i / p.k_chunks;
           const int kc = i % p.k_chunks;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* st = smem + s * Cfg::kStageBytes;
-          mbar_arrive_expect_tx(&full_bar[s], tx_bytes);
+          mbar_wait_a(empty_bar + 8 * s, ph ^ 1);
+          const uint32_t st = smem + s * Cfg::kStageBytes;
+          const uint32_t fb = full_bar + 8 * s;
+          mbar_arrive_expect_tx_a(fb, tx_bytes);
           const int a_row = t.m0 + (tap - p.pad) * p.dil;
-          tma_load_3d(st, &tm_a_hi, &full_bar[s], a_col + kc * kChunkK, a_row, a_batch);
-          tma_load_3d(st + 2 * Cfg::kABytes, &tm_b_hi, &full_bar[s], b_col + tap * p.b_tap_stride + kc * kChunkK, t.n0, b_batch);
+          const int bc = b_col + tap * p.b_tap_stride + kc * kChunkK;
+          tma_load_3d_a(st, &tm_a_hi, fb, a_col + kc * kChunkK, a_row, a_batch);
+          tma_load_3d_a(st + 2 * Cfg::kABytes, &tm_b_hi, fb, bc, t.n0, b_batch);
           if (p.passes == 3) {
-            tma_load_3d(st + Cfg::kABytes, &tm_a_lo, &full_bar[s], a_col + kc * kChunkK, a_row, a_batch);
-            tma_load_3d(st + 2 * Cfg::kABytes + Cfg::kBBytes, &tm_b_lo, &full_bar[s],
-                        b_col + tap * p.b_tap_stride + kc * kChunkK, t.n0, b_batch);
+            tma_load_3d_a(st + Cfg::kABytes, &tm_a_lo, fb, a_col + kc * kChunkK, a_row, a_batch);
+            tma_load_3d_a(st + 2 * Cfg::kABytes + Cfg::kBBytes, &tm_b_lo, fb, bc, t.n0, b_batch);
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------ MMA issuer ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(kBlockM, BLOCK_N);
-      uint32_t it = 0;
-      int lt = 0;                                      // tiles processed by this CTA
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const GemmTile t = gemm_tile(tile, p.tiles_m, zdim, p.heads, BLOCK_N);
-        if (!gemm_tile_live(p, t.m0, t.bz)) continue;
-        const int buf = lt & 1;
-        mbar_wait(&acc_empty[buf], ((lt >> 1) & 1) ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * Cfg::kTmemCols;
-        for (int i = 0; i < num_chunks; ++i, ++it) {
-          const int s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tcgen05_fence_after();
-          const uint32_t st = smem_u32(smem + s * Cfg::kStageBytes);
-          const uint64_t a_hi = make_smem_desc_sw128(st);
-          const uint64_t a_lo = make_smem_desc_sw128(st + Cfg::kABytes);
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * Cfg::kABytes);
-          const uint64_t b_lo = make_smem_desc_sw128(st + 2 * Cfg::kABytes + Cfg::kBBytes);
-#pragma unroll
-          for (int k = 0; k < kChunkK / kUmmaK; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);  // 32 B per K-step inside the 128B row
-            umma_bf16(d_tmem, a_hi + koff, b_hi + koff, idesc, (i | k) != 0);
-            if (p.passes == 3) {
-              umma_bf16(d_tmem, a_lo + koff, b_hi + koff, idesc, 1);
-              umma_bf16(d_tmem, a_hi + koff, b_lo + koff, idesc, 1);
-            }
-          }
-          umma_commit(&empty_bar[s]);  // frees this smem stage when the MMAs above have read it
-        }
-        umma_commit(&acc_full[buf]);   // accumulator complete
-        ++lt;
       }
     }
   } else {
-    // ------------------------------ epilogue ------------------------------
-    const int quarter = warp & 3;               // TMEM lane quarter this warp may access
-    int lt = 0;
+    // ------------------------------ consumers: wgmma main loop + epilogue ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;                        // rows [64 wg, 64 wg + 64) of the tile
+    const int wt = threadIdx.x & 127;                // thread inside the warpgroup
+    const int er = wt & 63;                          // epilogue: the row this thread owns ...
+    const int eh = wt >> 6;                          // ... and which of the two staged chunks
+    const uint32_t slots = staging + wg * 2 * kStageSlotBytes;
+    uint32_t it = 0;
+    float acc[BLOCK_N / 2];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const GemmTile t = gemm_tile(tile, p.tiles_m, zdim, p.heads, BLOCK_N);
-      const int buf = lt & 1;
-      const int row = t.m0 + quarter * 32 + lane;   // output time step
+      const int row = t.m0 + wg * 64 + er;           // output time step
       const bool row_ok = row < p.m;
       const bool row_live = row_ok && (p.lens == nullptr || row < __ldg(p.lens + t.bz));
       const long long y_off = t.bz * p.y_batch_stride + t.hz * p.y_head_stride + static_cast<long long>(row) * p.y_ld;
       if (!gemm_tile_live(p, t.m0, t.bz)) {        // dead tile: zero rows, nothing to wait for
 #pragma unroll 1
-        for (int c = 0; c < BLOCK_N / 32; ++c) {
+        for (int c = eh; c < kChunks; c += 2) {
           float v[32];
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] = 0.f;
@@ -373,237 +341,64 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
         }
         continue;
       }
-      ++lt;
-      mbar_wait(&acc_full[buf], ((lt - 1) >> 1) & 1);
-      tcgen05_fence_after();
-      const uint32_t t_acc = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + buf * Cfg::kTmemCols;
-      if (p.epi == PK_EPI_NONE) {
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N / 32; ++c) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(t_acc + c * 32, v);
-          tmem_ld_wait();
-          if (c == BLOCK_N / 32 - 1) {            // last read of this accumulator: hand it back to the MMA issuer
-            tcgen05_fence_before();
-            mbar_arrive(&acc_empty[buf]);
+      for (int i = 0; i < num_chunks; ++i, ++it) {
+        const int s = it % Cfg::kStages;
+        mbar_wait_a(full_bar + 8 * s, (it / Cfg::kStages) & 1);
+        const uint32_t st = smem + s * Cfg::kStageBytes;
+        const uint64_t a_hi = make_smem_desc_sw128(st + wg * 64 * kSwizzleBytes);
+        const uint64_t a_lo = make_smem_desc_sw128(st + Cfg::kABytes + wg * 64 * kSwizzleBytes);
+        const uint64_t b_hi = make_smem_desc_sw128(st + 2 * Cfg::kABytes);
+        const uint64_t b_lo = make_smem_desc_sw128(st + 2 * Cfg::kABytes + Cfg::kBBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kChunkK / kWgmmaK; ++k) {
+          wgmma_ss<BLOCK_N>(acc, a_hi + desc_kstep(k), b_hi + desc_kstep(k), (i | k) != 0);
+          if (p.passes == 3) {
+            wgmma_ss<BLOCK_N>(acc, a_lo + desc_kstep(k), b_hi + desc_kstep(k), 1);
+            wgmma_ss<BLOCK_N>(acc, a_hi + desc_kstep(k), b_lo + desc_kstep(k), 1);
           }
-          gemm_epilogue_chunk(p, v, t.n0 + c * 32, row_ok, row_live, y_off);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_a(empty_bar + 8 * s);   // this warp is done reading the stage
+      }
+      if (p.epi == PK_EPI_NONE) {
+#pragma unroll
+        for (int c = 0; c < kChunks; c += 2) {
+          stage_store(slots, acc, c, wt);
+          if (c + 1 < kChunks) stage_store(slots + kStageSlotBytes, acc, c + 1, wt);
+          named_bar_sync(1 + wg, 128);
+          if (c + eh < kChunks) {
+            float v[32];
+            stage_load_row(slots + eh * kStageSlotBytes, er, v);
+            gemm_epilogue_chunk(p, v, t.n0 + (c + eh) * 32, row_ok, row_live, y_off);
+          }
+          named_bar_sync(1 + wg, 128);
         }
       } else {
         // fused pair epilogues: the tile holds columns [0, 2C); chunk c of the first half with chunk c of the second half
         const int hc = p.epi_c / 32;
-#pragma unroll 1
-        for (int c = 0; c < hc; ++c) {
-          float va[32], vg[32];
-          __syncwarp();
-          tmem_ld_32x32(t_acc + c * 32, va);
-          tmem_ld_32x32(t_acc + p.epi_c + c * 32, vg);
-          tmem_ld_wait();
-          if (c == hc - 1) {
-            tcgen05_fence_before();
-            mbar_arrive(&acc_empty[buf]);
-          }
-          gemm_epilogue_pair(p, va, vg, c * 32, t.bz, row, row_ok);
-        }
-      }
-    }
-    tcgen05_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<2 * Cfg::kTmemCols>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2, clusters of 2) for wide outputs: one M = 256 x BLOCK_N tile per pair.
-// Each CTA loads its own 128 rows of A and HALF of the B tile (BLOCK_N / 2 rows), so the L2 -> SM operand stream per CTA
-// drops from 96 KB to 64 KB per K-chunk at BLOCK_N = 256 (the single-CTA kernel needs 62 B/clk/SM there against a
-// 42 B/clk/SM share of the L2 throughput cap) and three 64 KB stages fit instead of two 96 KB ones.
-// Leader CTA (cluster rank 0): issues every MMA / commit, owns full[s] (TMA bytes of both CTAs) and acc_empty[2]
-// (warp-elected relaxed remote arrivals); both CTAs: producer, epilogue, local empty[s] / acc_full[2] (multicast commits).
-// ---------------------------------------------------------------------------------------------------------------
-template <int BLOCK_N>
-struct GemmPairCfg {
-  static constexpr int kABytes = kBlockM * kSwizzleBytes;             // one plane of this CTA's A chunk (16 KB)
-  static constexpr int kBBytes = (BLOCK_N / 2) * kSwizzleBytes;       // one plane of this CTA's half of the B chunk
-  static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-  static constexpr int kStages = 3;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-  static constexpr uint32_t kTmemCols = BLOCK_N <= 128 ? 128 : 256;   // accumulator stride (2 buffers: power-of-two allocation)
-};
-
-template <int BLOCK_N>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-conv_gemm_pair_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-                      const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
-                      const GemmKernelArgs p) {
-  using Cfg = GemmPairCfg<BLOCK_N>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem + Cfg::kStages * Cfg::kStageBytes;
-  const uint32_t full_bar = bars;                              // [stages] (the leader's copy is live)
-  const uint32_t empty_bar = full_bar + 8 * Cfg::kStages;      // [stages]
-  const uint32_t acc_full = empty_bar + 8 * Cfg::kStages;      // [2]
-  const uint32_t acc_empty = acc_full + 16;                    // [2] leader
-  const uint32_t tmem_slot = acc_empty + 16;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int num_chunks = p.taps * p.k_chunks;
-  const int zdim = p.batch * p.heads;
-  const int pair_id = blockIdx.x >> 1, pair_step = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a_hi);
-    tma_prefetch_desc(&tm_a_lo);
-    tma_prefetch_desc(&tm_b_hi);
-    tma_prefetch_desc(&tm_b_lo);
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init_a(full_bar + 8 * s, 1);
-      mbar_init_a(empty_bar + 8 * s, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc_full + 8 * i, 1);
-      mbar_init_a(acc_empty + 8 * i, 2 * 4);                   // 4 epilogue warps in each CTA, one elected arrival each
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm_a<2 * Cfg::kTmemCols>(tmem_slot);
-  tcgen05_fence_before();
-  cluster_sync();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = lds_u32(tmem_slot);
-
-  // tile schedule of the pair: (batch, head) fastest, then m-pair-tile (256 rows), then n-tile; p.tiles_m counts pair tiles
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------ TMA producer (both CTAs) ------------------------------
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      const uint32_t tx_bytes = 2 * ((p.passes == 3) ? Cfg::kStageBytes : (Cfg::kABytes + Cfg::kBBytes));   // both CTAs
-      uint32_t it = 0;
-      for (int tile = pair_id; tile < p.total_tiles; tile += pair_step) {
-        const int z = tile % zdim;
-        const int r = tile / zdim;
-        const int mt = r % p.tiles_m;
-        const int m0 = mt * 2 * kBlockM + static_cast<int>(rank) * kBlockM;
-        const int n0 = (r / p.tiles_m) * BLOCK_N + static_cast<int>(rank) * (BLOCK_N / 2);
-        const int bz = z / p.heads, hz = z % p.heads;
-        if (!gemm_tile_live(p, mt * 2 * kBlockM, bz)) continue;      // the PAIR tile (256 rows) is the unit that is skipped
-        const int a_batch = bz * p.a_bmul + hz * p.a_hmul;
-        const int b_batch = bz * p.b_bmul + hz * p.b_hmul;
-        const int a_col = p.a_col0 + hz * p.a_colh;
-        const int b_col = p.b_col0 + hz * p.b_colh;
-        for (int i = 0; i < num_chunks; ++i, ++it) {
-          const int s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1;
-          const int tap = i / p.k_chunks;
-          const int kc = i % p.k_chunks;
-          mbar_wait_a(empty_bar + 8 * s, ph ^ 1);
-          const uint32_t st = smem + s * Cfg::kStageBytes;
-          const uint32_t fb = full_leader + 8 * s;
-          if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, tx_bytes);
-          const int a_row = m0 + (tap - p.pad) * p.dil;
-          const int bc = b_col + tap * p.b_tap_stride + kc * kChunkK;
-          tma_load_3d_2sm_a(st, &tm_a_hi, fb, a_col + kc * kChunkK, a_row, a_batch);
-          tma_load_3d_2sm_a(st + 2 * Cfg::kABytes, &tm_b_hi, fb, bc, n0, b_batch);
-          if (p.passes == 3) {
-            tma_load_3d_2sm_a(st + Cfg::kABytes, &tm_a_lo, fb, a_col + kc * kChunkK, a_row, a_batch);
-            tma_load_3d_2sm_a(st + 2 * Cfg::kABytes + Cfg::kBBytes, &tm_b_lo, fb, bc, n0, b_batch);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer (leader CTA) ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(2 * kBlockM, BLOCK_N);
-      uint32_t it = 0;
-      int lt = 0;
-      for (int tile = pair_id; tile < p.total_tiles; tile += pair_step) {
-        if (!gemm_tile_live(p, ((tile / zdim) % p.tiles_m) * 2 * kBlockM, (tile % zdim) / p.heads)) continue;
-        const int buf = lt & 1;
-        mbar_wait_a(acc_empty + 8 * buf, ((lt >> 1) & 1) ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * Cfg::kTmemCols;
-        for (int i = 0; i < num_chunks; ++i, ++it) {
-          const int s = it % Cfg::kStages;
-          const uint32_t ph = (it / Cfg::kStages) & 1;
-          mbar_wait_a(full_bar + 8 * s, ph);
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * Cfg::kStageBytes;
-          const uint64_t a_hi = make_smem_desc_sw128(st);
-          const uint64_t a_lo = make_smem_desc_sw128(st + Cfg::kABytes);
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * Cfg::kABytes);
-          const uint64_t b_lo = make_smem_desc_sw128(st + 2 * Cfg::kABytes + Cfg::kBBytes);
 #pragma unroll
-          for (int k = 0; k < kChunkK / kUmmaK; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16_2sm(d_tmem, a_hi + koff, b_hi + koff, idesc, (i | k) != 0);
-            if (p.passes == 3) {
-              umma_bf16_2sm(d_tmem, a_lo + koff, b_hi + koff, idesc, 1);
-              umma_bf16_2sm(d_tmem, a_hi + koff, b_lo + koff, idesc, 1);
+        for (int c = 0; c < kChunks / 2; ++c) {
+          if (c < hc) {
+            stage_store(slots, acc, c, wt);
+#pragma unroll
+            for (int g = 1; g < kChunks; ++g)
+              if (g == c + hc) stage_store(slots + kStageSlotBytes, acc, g, wt);
+            named_bar_sync(1 + wg, 128);
+            if (eh == 0) {
+              float va[32], vg[32];
+              stage_load_row(slots, er, va);
+              stage_load_row(slots + kStageSlotBytes, er, vg);
+              gemm_epilogue_pair(p, va, vg, c * 32, t.bz, row, row_ok);
             }
+            named_bar_sync(1 + wg, 128);
           }
-          umma_commit_2sm_a(empty_bar + 8 * s);
         }
-        umma_commit_2sm_a(acc_full + 8 * buf);
-        ++lt;
       }
     }
-  } else {
-    // ------------------------------ epilogue (both CTAs, own 128 rows, all BLOCK_N columns) ------------------------------
-    const int quarter = warp & 3;
-    const uint32_t acc_empty_l = mapa_shared(acc_empty, 0);
-    int lt = 0;
-    for (int tile = pair_id; tile < p.total_tiles; tile += pair_step) {
-      const int z = tile % zdim;
-      const int r = tile / zdim;
-      const int mt = r % p.tiles_m;
-      const int tn0 = (r / p.tiles_m) * BLOCK_N;
-      const int bz = z / p.heads, hz = z % p.heads;
-      const int buf = lt & 1;
-      const int row = mt * 2 * kBlockM + static_cast<int>(rank) * kBlockM + quarter * 32 + lane;
-      const bool row_ok = row < p.m;
-      const bool row_live = row_ok && (p.lens == nullptr || row < __ldg(p.lens + bz));
-      const long long y_off = bz * p.y_batch_stride + hz * p.y_head_stride + static_cast<long long>(row) * p.y_ld;
-      if (!gemm_tile_live(p, mt * 2 * kBlockM, bz)) {
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N / 32; ++c) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0.f;
-          gemm_epilogue_chunk(p, v, tn0 + c * 32, row_ok, false, y_off);
-        }
-        continue;
-      }
-      ++lt;
-      mbar_wait_a(acc_full + 8 * buf, ((lt - 1) >> 1) & 1);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BLOCK_N / 32; ++c) {
-        float v[32];
-        __syncwarp();
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + buf * Cfg::kTmemCols + c * 32, v);
-        tmem_ld_wait();
-        if (c == BLOCK_N / 32 - 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster_relaxed_a(acc_empty_l + 8 * buf);
-        }
-        gemm_epilogue_chunk(p, v, tn0 + c * 32, row_ok, row_live, y_off);
-      }
-    }
-    tcgen05_fence_before();
-  }
-  cluster_sync();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<2 * Cfg::kTmemCols>(tmem_base);
   }
 }
 
@@ -755,45 +550,6 @@ static int launch(const pk_conv_gemm_args* a, cudaStream_t stream, const pk_gemm
   return PK_OK;
 }
 
-static bool use_pair() {
-  static const bool v = []() {
-    const char* e = getenv("PK_GEMM_PAIR");
-    return !(e && e[0] == '0') && sm_count() >= 2;
-  }();
-  return v;
-}
-
-template <int BLOCK_N>
-static int launch_pair(const pk_conv_gemm_args* a, cudaStream_t stream) {
-  using Cfg = GemmPairCfg<BLOCK_N>;
-  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-  int rc;
-  if ((rc = encode_tmap_bf16_3d(&ta_hi, a->a.hi, a->a.cols, a->a.rows, a->a.batches, a->a.ld, a->a.batch_stride, kBlockM))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tb_hi, a->b.hi, a->b.cols, a->b.rows, a->b.batches, a->b.ld, a->b.batch_stride, BLOCK_N / 2))) return rc;
-  if (a->passes == 3) {
-    if ((rc = encode_tmap_bf16_3d(&ta_lo, a->a.lo, a->a.cols, a->a.rows, a->a.batches, a->a.ld, a->a.batch_stride, kBlockM))) return rc;
-    if ((rc = encode_tmap_bf16_3d(&tb_lo, a->b.lo, a->b.cols, a->b.rows, a->b.batches, a->b.ld, a->b.batch_stride, BLOCK_N / 2))) return rc;
-  } else {
-    ta_lo = ta_hi;
-    tb_lo = tb_hi;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_pair_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  GemmKernelArgs p = to_kernel_args(a);
-  p.tiles_m = (a->m + 2 * kBlockM - 1) / (2 * kBlockM);        // pair tiles of 256 rows
-  const long long total = static_cast<long long>(p.tiles_m) * ((a->n + BLOCK_N - 1) / BLOCK_N) * a->batch * a->heads;
-  PK_CHECK_ARG(total < (1LL << 31), "too many output tiles");
-  p.total_tiles = static_cast<int>(total);
-  const int grid = 2 * static_cast<int>(std::min<long long>(total, sm_count() / 2));
-  conv_gemm_pair_kernel<BLOCK_N><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
-
 }  // namespace pk
 
 extern "C" int pk_conv_gemm(const pk_conv_gemm_args* args, pk_stream_t stream) {
@@ -804,14 +560,7 @@ extern "C" int pk_conv_gemm(const pk_conv_gemm_args* args, pk_stream_t stream) {
   const int n = args->n;
   auto waste = [n](int bn) { return (n + bn - 1) / bn * bn - n; };
   if (n <= 64) return pk::launch<64>(args, s);
-  if (waste(256) <= waste(128) && n > 128) {
-    // wide outputs: CTA pairs (half of the B tile per CTA) unless PK_GEMM_PAIR=0 or the rows fit one 128-row tile
-    if (pk::use_pair() && args->m > 128) return pk::launch_pair<256>(args, s);
-    return pk::launch<256>(args, s);
-  }
-  // N = 384 / 1152 / ... : 192-wide pair tiles have no padded columns and a pair instruction of 96 clk of work
-  if (pk::use_pair() && args->m > 128 && n >= 384 && waste(192) < waste(256) && waste(192) <= waste(128))
-    return pk::launch_pair<192>(args, s);
+  if (waste(256) <= waste(128) && n > 128) return pk::launch<256>(args, s);
   return pk::launch<128>(args, s);
 }
 
@@ -830,7 +579,7 @@ extern "C" int pk_conv_gemm_simt(const pk_conv_gemm_args* args, pk_stream_t stre
   const pk::GemmKernelArgs p = pk::to_kernel_args(args);
   const long long total = static_cast<long long>(args->batch) * args->heads * args->m * args->n;
   const int threads = 256;
-  const int blocks = static_cast<int>(std::min<long long>((total + threads - 1) / threads, 148LL * 16));
+  const int blocks = static_cast<int>(std::min<long long>((total + threads - 1) / threads, 132LL * 16));
   pk::conv_gemm_simt_kernel<<<blocks, threads, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(args->a.hi), static_cast<const __nv_bfloat16*>(args->a.lo),
       static_cast<const __nv_bfloat16*>(args->b.hi), static_cast<const __nv_bfloat16*>(args->b.lo), args->a, args->b, p,

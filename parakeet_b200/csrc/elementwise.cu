@@ -1,6 +1,6 @@
 // HBM-bound helper kernels: fp32 -> split-bf16, length regulator (integer prefix-sum + row gather).
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 

@@ -1,7 +1,7 @@
 // Element-wise / reduction kernels of the Parallel WaveGAN training step (reference: PWGUpdater.update_core,
 // parakeet/models/parallel_wavegan/parallel_wavegan_updater.py:76-153; SURVEY.md 8f.1).  The GEMM-shaped work of that step
 // (every Conv1D forward, data gradient and weight gradient of generator and discriminator, the DFT of the STFT losses and its
-// adjoint) runs through pk_conv_gemm on tcgen05; this file holds what sits between the GEMMs:
+// adjoint) runs through pk_conv_gemm on wgmma; this file holds what sits between the GEMMs:
 //   gate (ResidualBlock :307-310) forward / backward, LeakyReLU forward / backward (PWGDiscriminator :579-582),
 //   weight norm w = g v / ||v|| forward / backward (nn.utils.weight_norm, dim 0), MSE against a constant (criterion_mse),
 //   the generator's residual / skip update, the upsampling stages (Stretch2D + FIR Conv2D, :48-63,119-138) one stage at a time
@@ -10,7 +10,7 @@
 #include <math.h>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 namespace gan {

@@ -1,0 +1,234 @@
+// Device primitives for sm_90a (Hopper): mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with operands in
+// shared memory or, for A, in registers) and its shared-memory descriptors.  Inline PTX only - no CUTLASS dependency.
+//
+// Conventions used by every kernel in this library:
+//   * GEMM operands are "split-bf16": a 32-bit value v is stored as two bf16 planes hi = bf16(v), lo = bf16(v - hi)
+//     (16-bit effective mantissa).  A product A*B is evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo with fp32
+//     accumulation in registers (3 wgmma per K-step) - relative error ~2^-16, which keeps the fp32 1e-3 parity
+//     contract through 30 residual layers where a single TF32 pass does not (measured in DESIGN.md).
+//   * Operand tiles are K-major, 64 bf16 (=128 B) per row, 128B-swizzled, written by TMA and read by wgmma.
+//   * Accumulator fragments (wgmma m64nN, f32): warp w of the warpgroup owns rows 16 w + g and 16 w + g + 8 (g = lane / 4);
+//     d[4 j + {0, 1}] are row 16 w + g, columns 8 j + 2 (lane % 4) + {0, 1}; d[4 j + {2, 3}] the same columns of row + 8.
+#pragma once
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace pk {
+
+constexpr int kSwizzleBytes = 128;     // one K-chunk row: 64 bf16
+constexpr int kChunkK = 64;            // bf16 elements per K-chunk
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+// ----------------------------------------------------------------------------------------------------------------
+// mbarrier
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void fence_barrier_init() {
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+
+// ----------------------------------------------------------------------------------------------------------------
+// proxies / fences
+// ----------------------------------------------------------------------------------------------------------------
+// all generic-proxy writes of this thread -> visible to later async-proxy (TMA / wgmma) reads
+__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
+
+// ----------------------------------------------------------------------------------------------------------------
+// TMA
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------------------------
+// wgmma
+// ----------------------------------------------------------------------------------------------------------------
+constexpr int kWgmmaK = 16;            // K per wgmma.mma_async (bf16)
+
+// Shared-memory matrix descriptor: K-major tile, rows of 128 B, SWIZZLE_128B, 8-row groups 1024 B apart; the tile must be
+// 1024-B aligned (base offset 0).  Advancing the start address by 32 B selects the next K-step of 16 inside the 128 B row.
+// (bit layout: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | base offset [49,52) | layout 1 = SWIZZLE_128B [62,64))
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;             // LBO (unused for swizzled K-major; canonical value 1)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO: 8 rows * 128 B
+  d |= static_cast<uint64_t>(1) << 62;             // SWIZZLE_128B
+  return d;
+}
+__device__ __forceinline__ uint64_t desc_kstep(int k) { return static_cast<uint64_t>((k * kWgmmaK * 2) >> 4); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// register budget of the executing warpgroup (all of its warps execute it): producers give registers back, consumers take them
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+// named barrier over `threads` threads (a warpgroup: 128)
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// wgmma.mma_async m64nNk16, bf16 x bf16 -> f32, K-major operands; d (N / 2 floats per thread) is accumulated in place.
+// ss: A and B from shared memory (descriptors); rs: A from registers (the m64k16 A fragment, 4 x bf16x2 per thread).
+#define PK_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define PK_F32(i) PK_F8(i), PK_F8(i + 8), PK_F8(i + 16), PK_F8(i + 24)
+#define PK_D32 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+#define PK_D64 PK_D32 ",%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+#define PK_D96 PK_D64 ",%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95"
+#define PK_D128 PK_D96 ",%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {" PK_D32 "}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+               : PK_F32(0) : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {" PK_D64 "}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+               : PK_F32(0), PK_F32(32) : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_ss_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {" PK_D128 "}, %128, %129, p, 1, 1, 0, 0;\n}\n"
+               : PK_F32(0), PK_F32(32), PK_F32(64), PK_F32(96) : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {" PK_D32 "}, {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n}\n"
+               : PK_F32(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {" PK_D64 "}, {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n}\n"
+               : PK_F32(0), PK_F32(32) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_rs_n192(float (&d)[96], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %101, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 {" PK_D96 "}, {%96,%97,%98,%99}, %100, p, 1, 1, 0;\n}\n"
+               : PK_F32(0), PK_F32(32), PK_F32(64) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+#undef PK_F32
+#undef PK_F8
+
+// ----------------------------------------------------------------------------------------------------------------
+// split-bf16 helpers
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+  hi = __float2bfloat16_rn(v);
+  lo = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
+  return static_cast<uint32_t>(__bfloat16_as_ushort(a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(b)) << 16);
+}
+// split 8 floats -> two uint4 of packed bf16 (hi plane, lo plane)
+__device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
+  __nv_bfloat16 h[8], l[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) split_bf16(v[i], h[i], l[i]);
+  hi = make_uint4(pack_bf16x2(h[0], h[1]), pack_bf16x2(h[2], h[3]), pack_bf16x2(h[4], h[5]), pack_bf16x2(h[6], h[7]));
+  lo = make_uint4(pack_bf16x2(l[0], l[1]), pack_bf16x2(l[2], l[3]), pack_bf16x2(l[4], l[5]), pack_bf16x2(l[6], l[7]));
+}
+
+
+// ----------------------------------------------------------------------------------------------------------------
+// Shared-memory access by 32-bit shared-space address.  Kernels round their dynamic smem base up to 1024 B with
+// integer arithmetic, after which the compiler can no longer prove a pointer is in shared space and would emit
+// generic LD/ST (long-scoreboard latency); these helpers keep the accesses on the LDS/STS path.
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float4 lds_f4(uint32_t addr) {   // ordered w.r.t. the other volatile smem helpers
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+
+// mbarrier / TMA helpers taking shared-space addresses
+__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx_a(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_a(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// Bounded spin: a protocol bug must trap (-> launch error reported through the C-ABI), never hang the GPU.
+__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
+  uint32_t ok = 0;
+  for (uint32_t spin = 0; spin < (1u << 26); ++spin) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    if (ok) return;
+  }
+  __trap();
+}
+__device__ __forceinline__ void tma_load_3d_a(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_a(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+
+
+// ----------------------------------------------------------------------------------------------------------------
+// Accumulator staging: a warpgroup's m64 x 32-column slice of a wgmma accumulator goes through a [64][32] fp32 slot of
+// shared memory (8 KB, 16-byte chunks XOR-swizzled by row) so that a thread can then read one whole row of it - the
+// row-per-thread layout the epilogues are written in.
+// ----------------------------------------------------------------------------------------------------------------
+constexpr int kStageSlotBytes = 64 * 32 * 4;
+__device__ __forceinline__ uint32_t stage_addr(uint32_t slot, int row, int col) {   // col: multiple of 2
+  return slot + row * 128 + ((((col >> 2) ^ (row & 7)) << 4) | ((col & 3) << 2));
+}
+// columns [32 C, 32 C + 32) of the accumulator d; wg_thread = thread index inside the warpgroup.  Call it from fully
+// unrolled loops only: C must fold to a constant, or the accumulator would be indexed dynamically (local memory).
+template <int R>
+__device__ __forceinline__ void stage_store(uint32_t slot, const float (&d)[R], int C, int wg_thread) {
+  const int w = wg_thread >> 5, lane = wg_thread & 31;
+  const int r0 = 16 * w + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * C + jj;
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_addr(slot, r0, 8 * jj + c0)), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_addr(slot, r0 + 8, 8 * jj + c0)), "f"(d[4 * j + 2]), "f"(d[4 * j + 3])
+                 : "memory");
+  }
+}
+__device__ __forceinline__ void stage_load_row(uint32_t slot, int row, float (&v)[32]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float4 x = lds_f4(slot + row * 128 + ((k ^ (row & 7)) << 4));
+    v[4 * k] = x.x; v[4 * k + 1] = x.y; v[4 * k + 2] = x.z; v[4 * k + 3] = x.w;
+  }
+}
+
+}  // namespace pk

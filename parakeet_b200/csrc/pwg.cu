@@ -1,14 +1,12 @@
 // Parallel WaveGAN generator kernels (reference: parakeet/models/parallel_wavegan/parallel_wavegan.py).
 //
-//   pk_pwg_residual_layer : one fused ResidualBlock (:284-315) over the whole batch, channels-last, tcgen05:
+//   pk_pwg_residual_layer : one fused ResidualBlock (:284-315) over the whole batch, channels-last, wgmma:
 //        GEMM1  h[128 t x 128]  = sum_{tap} x[t + (tap-1) d, 0:64] W_conv[tap] + c[t, 0:80] W_aux      (K = 272)
-//        gate   z[128 x 64]     = tanh(h[:, :64] + b) * sigmoid(h[:, 64:] + b)       (TMEM -> regs -> smem, never HBM)
-//        GEMM2  [skip | out]    = z W_so                                              (K = 64)
-//        epi    skip_acc += skip (its bias is summed into the tail);  x_out = (out + b_out + x) * sqrt(0.5), where +x is a
-//               tensor-core pass x [0 | I] into the GEMM2 accumulator
-//     persistent CTAs, 16 warps: TMA producer, MMA issuer, 4 gate warps, 8 store warps; double-buffered TMEM accumulators so
-//     GEMM1 of tile i+1 overlaps the gate / stores of tile i.  Two variants: pwg_layer_pair_kernel (CTA pairs, cta_group::2,
-//     weights resident in shared memory; default) and pwg_layer_kernel (one CTA per SM, weights streamed per tile).
+//        gate   z[128 x 64]     = tanh(h[:, :64] + b) * sigmoid(h[:, 64:] + b)       (in registers, never memory)
+//        GEMM2  [skip | out]    = [0 | x] + z W_so                                    (K = 64, z as register A operand)
+//        epi    skip_acc += skip (its bias is summed into the tail);  x_out = (out + b_out + x) * sqrt(0.5)
+//     persistent CTAs over 128-sample tiles: a producer warpgroup (one TMA lane) streams A and W1 chunks through a 2-deep
+//     ring, W2 stays resident, two consumer warpgroups (64 samples each) run both GEMMs, the gate and the stores.
 //   pk_pwg_upsample       : ConvInUpsampleNet (:201-216) conv_in + [nearest stretch + FIR] x scales, fused per frame.
 //   pk_pwg_first_conv     : first_conv 1 -> R channels (:464).
 //   pk_pwg_tail           : skips * sqrt(1/L) -> ReLU -> 1x1 -> ReLU -> 1x1 (:469-471).
@@ -18,33 +16,24 @@
 #include <algorithm>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 
 // ---------------------------------------------------------------------------------------------------------------
 // fused residual layer
 // ---------------------------------------------------------------------------------------------------------------
-// Warp roles (16 warps, 1 CTA per SM, persistent over 128-sample tiles):
-//   warp 0      TMA producer   : per tile 5 K-chunks for GEMM1 (3 dilated taps of x, 2 chunks of c; A and B = 64 KB
-//                                per stage) + 1 chunk for GEMM2 (W2 only; the A half of that stage receives z)
-//   warp 1      MMA issuer     : G1(0); then per tile { G1(i+1); G2(i) } so GEMM1 of the next tile overlaps the gate
-//   warps 4-7   gate  warps    : acc1 (TMEM) -> tanh * sigmoid -> split-bf16 z tile written (128B-swizzled) into the
-//                                A half of the pipeline stage reserved for GEMM2
-//   warps 8-15  store warps    : acc2 (TMEM) -> skip half: red.global.add.v4 into the fp32 skip sum; out half: + bias,
-//                                * sqrt(1/2), split planes with 256-bit stores (row per thread)
-// TMEM: acc1[2] at columns 0/128, acc2[2] at 256/384 (fp32 128x128 each).
 constexpr int kPwgR = 64;        // residual channels
 constexpr int kPwgG = 128;       // gate channels
 constexpr int kPwgS = 64;        // skip channels
-constexpr int kPwgStages = 3;
+constexpr int kPwgStages = 2;
 constexpr int kPwgTile = 128 * kSwizzleBytes;                 // 16 KB: one plane of a 128-row K-chunk
 constexpr int kPwgStageBytes = 4 * kPwgTile;                  // A hi, A lo, B hi, B lo
-constexpr int kPwgSmem = kPwgStages * kPwgStageBytes + kPwgTile + 1024 + 256;  // + [0 | I] tile + align + barriers
-constexpr int kPwgGateWarps = 4;
-constexpr int kPwgStoreWarps = 8;
-constexpr int kPwgFirstGateWarp = 4;                          // warps 2-3 idle: keeps each role on whole warpgroups
-constexpr int kPwgThreads = (kPwgFirstGateWarp + kPwgGateWarps + kPwgStoreWarps) * 32;   // 512 -> 128 registers per thread
+constexpr int kPwgW2Bytes = 2 * kPwgTile;                     // resident W2: 128 outputs (skip | out) x 64, both planes
+constexpr int kPwgSmem = kPwgStages * kPwgStageBytes + kPwgW2Bytes + 1024 + 256;
+static_assert(kPwgSmem <= 227 * 1024, "shared memory budget");
+constexpr int kPwgConsumerThreads = 256;
+constexpr int kPwgThreads = kPwgConsumerThreads + 128;
 constexpr int kPwgG1Chunks = 5;                               // 3 taps + 2 aux chunks (64 + 16 channels)
 
 struct PwgLayerArgs {
@@ -53,27 +42,12 @@ struct PwgLayerArgs {
   const int32_t* lens;          // valid samples per utterance or NULL
   float gate_c[128];            // constant bank: [0,64) -2*log2e*bias_a, [64,128) -log2e*bias_g (conv bias, pre-scaled)
   float out_b[64];              // constant bank: conv1x1_out bias (the skip biases are summed into the tail)
-  float k_a, k_g;               // -2*log2e, -log2e as run-time values: keeps the FFMA's immediate slot free for c[0][bias]
+  float k_a, k_g;               // -2*log2e, -log2e
   float* skip;                  // fp32 (B, T, 64) accumulator
   int skip_init;                // 1: write, 0: accumulate
-  const __nv_bfloat16* x_hi;    // layer input planes (B, T, 64) (re-read for the residual add)
-  const __nv_bfloat16* x_lo;
   __nv_bfloat16* y_hi;          // layer output planes
   __nv_bfloat16* y_lo;
-  unsigned long long* prof;     // optional phase-timing counters (debug), see pk_pwg_layer_args.prof
 };
-
-// phase timing (only when p.prof != NULL): accumulate clock64() deltas per section
-#define PK_TICK(k)                                      \
-  if (kProf) {                                          \
-    const long long n_ = clock64();                     \
-    tacc[k] += n_ - tlast;                              \
-    tlast = n_;                                         \
-  }
-#define PK_TICK_FLUSH(base, n)                                                              \
-  if (kProf) {                                                                              \
-    for (int k_ = 0; k_ < (n); ++k_) atomicAdd(p.prof + (base) + k_, static_cast<unsigned long long>(tacc[k_])); \
-  }
 
 struct PwgTileIter {
   int idx, step, tiles_per_b, total, t;
@@ -114,13 +88,6 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// 256-bit global store (STG.E.256): 8 packed words = 16 bf16 of one row
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
-
-template <bool kProf>
 __global__ void __launch_bounds__(kPwgThreads, 1)
 pwg_layer_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
                  const __grid_constant__ CUtensorMap tm_c_hi, const __grid_constant__ CUtensorMap tm_c_lo,
@@ -128,73 +95,43 @@ pwg_layer_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_const
                  const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
                  const PwgLayerArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  // all shared-memory accesses go through 32-bit shared-space addresses (see pk_sm100.cuh)
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;      // 1024-B aligned for SWIZZLE_128B
-  const uint32_t ident = smem + kPwgStages * kPwgStageBytes;   // B operand [0 | I]: rows n < 64 zero, row 64 + k = e_k (K-major, SW128)
-  const uint32_t bars = ident + kPwgTile;
+  const uint32_t w2 = smem + kPwgStages * kPwgStageBytes;
+  const uint32_t bars = w2 + kPwgW2Bytes;
   const uint32_t full_bar = bars;                       // [stages]
   const uint32_t empty_bar = full_bar + 8 * kPwgStages; // [stages]
-  const uint32_t acc1_full = empty_bar + 8 * kPwgStages;  // [2]
-  const uint32_t acc1_empty = acc1_full + 16;           // [2]
-  const uint32_t acc2_full = acc1_empty + 16;           // [2]
-  const uint32_t acc2_empty = acc2_full + 16;           // [2]
-  const uint32_t z_full = acc2_empty + 16;              // [2] gate warps -> MMA issuer: z of tile i is in its stage
-  const uint32_t g2_free = z_full + 16;                 // [2] producer -> gate warps: the GEMM2 stage of tile i may be written
-  const uint32_t tmem_slot = g2_free + 16;
+  const uint32_t w_bar = empty_bar + 8 * kPwgStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr float kLog2e = 1.4426950408889634f;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kPwgConsumerThreads) {
     tma_prefetch_desc(&tm_x_hi); tma_prefetch_desc(&tm_x_lo); tma_prefetch_desc(&tm_c_hi); tma_prefetch_desc(&tm_c_lo);
     tma_prefetch_desc(&tm_w1_hi); tma_prefetch_desc(&tm_w1_lo); tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kPwgStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc1_full + 8 * i, 1); mbar_init_a(acc1_empty + 8 * i, kPwgGateWarps * 32);
-      mbar_init_a(acc2_full + 8 * i, 1); mbar_init_a(acc2_empty + 8 * i, kPwgStoreWarps * 32);
-    }
-    for (int i = 0; i < 2; ++i) { mbar_init_a(z_full + 8 * i, kPwgGateWarps * 32); mbar_init_a(g2_free + 8 * i, 1); }
+    for (int s = 0; s < kPwgStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kPwgConsumerThreads / 32); }
+    mbar_init_a(w_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 256) {
-    // residual add as a tensor-core pass: x [0 | I] initialises acc2 = [0 | x] while the centre tap of x is in smem
-    const int n = threadIdx.x - 128;              // row of the B tile (output column of GEMM2)
-    const int k = n - 64;                         // the one non-zero K index of this row (n >= 64)
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {                 // 8 x 16-byte chunks of 8 bf16 each
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (k >= 0 && (k >> 3) == c) {
-        const uint32_t one = (k & 1) ? 0x3f800000u : 0x00003f80u;   // bf16 1.0 in the odd / even half of a word
-        const int w = (k & 7) >> 1;
-        v.x = w == 0 ? one : 0; v.y = w == 1 ? one : 0; v.z = w == 2 ? one : 0; v.w = w == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_smem();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = lds_u32(tmem_slot);
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= kPwgConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kPwgConsumerThreads / 32 && lane == 0) {
       // ------------------------------ TMA producer ------------------------------
-      uint32_t it = 0;  // running stage counter
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      auto load_g1 = [&](int b, int m0) {
+      mbar_arrive_expect_tx_a(w_bar, kPwgW2Bytes);
+      tma_load_3d_a(w2, &tm_w2_hi, w_bar, 0, 0, 0);
+      tma_load_3d_a(w2 + kPwgTile, &tm_w2_lo, w_bar, 0, 0, 0);
+      uint32_t it = 0;
+      PwgTileIter ti(p);
+      int b, m0;
+      while (ti.next(b, m0)) {
         for (int j = 0; j < kPwgG1Chunks; ++j, ++it) {
           const int s = it % kPwgStages;
-          PK_TICK(1)
           mbar_wait_a(empty_bar + 8 * s, ((it / kPwgStages) & 1) ^ 1);
-          PK_TICK(0)
           const uint32_t st = smem + s * kPwgStageBytes;
           const uint32_t fb = full_bar + 8 * s;
           mbar_arrive_expect_tx_a(fb, kPwgStageBytes);
-          // chunk order: tap -d, tap +d, aux[0:64], aux[64:], centre tap (last: it also feeds the residual pass)
+          // chunk order: tap -d, tap +d, aux[0:64], aux[64:], centre tap (last: it also supplies the residual x)
           const int wj = j == 0 ? 0 : j == 1 ? 2 : j == 2 ? 3 : j == 3 ? 4 : 1;   // K-chunk of the packed weight
           if (wj < 3) {
             const int row = m0 + (wj - 1) * p.dil;
@@ -207,714 +144,115 @@ pwg_layer_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_const
           tma_load_3d_a(st + 2 * kPwgTile, &tm_w1_hi, fb, wj * kChunkK, 0, 0);
           tma_load_3d_a(st + 3 * kPwgTile, &tm_w1_lo, fb, wj * kChunkK, 0, 0);
         }
-      };
-      int n_g2 = 0;   // tiles whose GEMM2 stage has been claimed
-      auto load_g2 = [&]() {
-        const int s = it % kPwgStages;
-        PK_TICK(1)
-        mbar_wait_a(empty_bar + 8 * s, ((it / kPwgStages) & 1) ^ 1);
-        PK_TICK(0)
-        const uint32_t st = smem + s * kPwgStageBytes;
-        mbar_arrive_a(g2_free + 8 * (n_g2 & 1));   // the gate warps may now write z of this tile into the stage's A half
-        ++n_g2;
-        mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kPwgTile);
-        tma_load_3d_a(st + 2 * kPwgTile, &tm_w2_hi, full_bar + 8 * s, 0, 0, 0);
-        tma_load_3d_a(st + 3 * kPwgTile, &tm_w2_lo, full_bar + 8 * s, 0, 0, 0);
-        ++it;
-      };
-      PwgTileIter ti(p);
-      int b, m0, nb, nm0;
-      bool have = ti.next(b, m0);
-      if (have) load_g1(b, m0);
-      while (have) {
-        const bool have_next = ti.next(nb, nm0);
-        if (have_next) load_g1(nb, nm0);
-        load_g2();
-        have = have_next; b = nb; m0 = nm0;
       }
-      PK_TICK(1)
-      PK_TICK_FLUSH(0, 2)
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------ MMA issuer ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(128, 128);
-      const int aux_tail_ksteps = ((p.aux_ch - kChunkK) + kUmmaK - 1) / kUmmaK;  // k-steps in the 2nd aux chunk
-      uint32_t it = 0;
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      auto mma_chunk = [&](uint32_t d_tmem, uint32_t st, int ksteps, bool first) {
-        const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kPwgTile);
-        const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kPwgTile), b_lo = make_smem_desc_sw128(st + 3 * kPwgTile);
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          umma_bf16(d_tmem, a_hi + koff, b_hi + koff, idesc, !(first && k == 0));
-          umma_bf16(d_tmem, a_lo + koff, b_hi + koff, idesc, 1);
-          umma_bf16(d_tmem, a_hi + koff, b_lo + koff, idesc, 1);
-        }
-      };
-      auto g1 = [&](int i) {
-        const int buf = i & 1;
-        PK_TICK(6)
-        mbar_wait_a(acc1_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
-        const uint32_t d = tmem_base + buf * 128;
-        for (int j = 0; j < kPwgG1Chunks; ++j, ++it) {
-          const int s = it % kPwgStages;
-          PK_TICK(2)
-          mbar_wait_a(full_bar + 8 * s, (it / kPwgStages) & 1);
-          PK_TICK(1)
-          tcgen05_fence_after();
-          mma_chunk(d, smem + s * kPwgStageBytes, j == 3 ? aux_tail_ksteps : 4, j == 0);
-          if (j == kPwgG1Chunks - 1) {
-            // residual pass: acc2(i) = [0 | x_hi + x_lo] from the centre-tap tile; GEMM2 of this tile accumulates on top
-            PK_TICK(2)
-            mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-            PK_TICK(4)
-            tcgen05_fence_after();
-            const uint32_t st = smem + s * kPwgStageBytes;
-            const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kPwgTile);
-            const uint64_t b_id = make_smem_desc_sw128(ident);
-            const uint32_t d2 = tmem_base + 256 + buf * 128;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-              umma_bf16(d2, a_hi + koff, b_id + koff, idesc, k != 0);
-              umma_bf16(d2, a_lo + koff, b_id + koff, idesc, 1);
-            }
-          }
-          umma_commit_a(empty_bar + 8 * s);
-        }
-        umma_commit_a(acc1_full + 8 * buf);
-      };
-      auto g2 = [&](int i) {
-        const int buf = i & 1;
-        const int s = it % kPwgStages;
-        PK_TICK(2)
-        mbar_wait_a(z_full + 8 * (i & 1), (i >> 1) & 1);   // gate warps wrote z into the A half of stage s
-        PK_TICK(3)
-        mbar_wait_a(full_bar + 8 * s, (it / kPwgStages) & 1);
-        PK_TICK(5)
-        tcgen05_fence_after();
-        mma_chunk(tmem_base + 256 + buf * 128, smem + s * kPwgStageBytes, 4, false);   // on top of the residual pass
-        umma_commit_a(empty_bar + 8 * s);
-        umma_commit_a(acc2_full + 8 * buf);
-        ++it;
-      };
-      PwgTileIter ti(p);
-      int b, m0;
-      int n_issued = 0, n_done = 0;
-      bool have = ti.next(b, m0);
-      if (have) g1(n_issued++);
-      while (have) {
-        const bool have_next = ti.next(b, m0);
-        if (have_next) g1(n_issued++);
-        g2(n_done++);
-        have = have_next;
-      }
-      PK_TICK(6)
-      PK_TICK_FLUSH(8, 7)
-      if (kProf) atomicAdd(p.prof + 32, static_cast<unsigned long long>(n_done));
-    }
-  } else if (warp < kPwgFirstGateWarp) {
-    // idle warps
-  } else if (warp < kPwgFirstGateWarp + kPwgGateWarps) {
-    // ------------------------------ gate warps ------------------------------
-    const int quarter = warp & 3;                 // TMEM lane quarter accessible to this warp
-    const int r = quarter * 32 + lane;            // row inside the tile
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
-    float k_a, k_g;   // in vector registers (opaque to the compiler), so that the FFMA can take the bias as c[0][..]
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    uint32_t it = kPwgG1Chunks;                   // mirrors the producer's stage counter: G1(0) used stages 0..4
-    PwgTileIter ti(p);
-    int b, m0, nb, nm0;
-    bool have = ti.next(b, m0);
-    for (int i = 0; have; ++i) {
-      const bool have_next = ti.next(nb, nm0);
-      if (have_next) it += kPwgG1Chunks;          // G1(i+1) is loaded before the GEMM2 chunk of tile i
-      const uint32_t st2 = smem + (it % kPwgStages) * kPwgStageBytes;
-      ++it;
-      const int buf = i & 1;
-      PK_TICK(6)
-      mbar_wait_a(acc1_full + 8 * buf, (i >> 1) & 1);
-      PK_TICK(0)
-      tcgen05_fence_after();
-      uint32_t zh[32], zl[32];                    // 64 z columns of this thread's row, packed bf16x2 hi / lo
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float va[32], vb[32];
-        __syncwarp();
-        tmem_ld_32x32(tmem_base + lane_base + buf * 128 + half * 32, va);
-        tmem_ld_32x32(tmem_base + lane_base + buf * 128 + 64 + half * 32, vb);
-        tmem_ld_wait();
-        if (half == 1) {
-          tcgen05_fence_before();
-          mbar_arrive_a(acc1_empty + 8 * buf);
-        }
-        // z = tanh(a + ba) * sigmoid(g + bg) = (1 - e1) / ((1 + e1)(1 + e2)), e1 = exp(-2(a+ba)), e2 = exp(-(g+bg))
-        // (one reciprocal; the exp2 argument of e1 is clamped at 60 so that the product cannot overflow where z != 0)
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          // the biases sit in the kernel-parameter constant bank: every index below is a compile-time constant after
-          // unrolling, so they are immediate c[0][..] operands of the FFMAs (no shared-memory traffic in this loop)
-          float z[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, p.gate_c[half * 32 + j + e]), 60.f));
-            const float e2 = ex2_approx(fmaf(vb[j + e], k_g, p.gate_c[64 + half * 32 + j + e]));
-            const float t1 = 1.f + e1;
-            z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
-          }
-          split2(z[0], z[1], zh[half * 16 + j / 2], zl[half * 16 + j / 2]);
-          split2(z[2], z[3], zh[half * 16 + j / 2 + 1], zl[half * 16 + j / 2 + 1]);
-        }
-      }
-      PK_TICK(1)
-      // The GEMM2 stage of this tile is ours once the producer has claimed it (it waited for the MMA to release it).
-      // g2_free completes exactly once per tile and cannot run more than one tile ahead of this wait (the next claim
-      // needs GEMM2 of this tile, which needs our z), so the parity wait cannot alias.
-      mbar_wait_a(g2_free + 8 * (i & 1), (i >> 1) & 1);
-      PK_TICK(2)
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int chunk = q ^ (r & 7);               // 128B swizzle: 16-byte chunk index XOR (row mod 8)
-        sts_u4(st2 + r * kSwizzleBytes + chunk * 16, make_uint4(zh[4 * q], zh[4 * q + 1], zh[4 * q + 2], zh[4 * q + 3]));
-        sts_u4(st2 + kPwgTile + r * kSwizzleBytes + chunk * 16, make_uint4(zl[4 * q], zl[4 * q + 1], zl[4 * q + 2], zl[4 * q + 3]));
-      }
-      fence_proxy_async_smem();
-      mbar_arrive_a(z_full + 8 * (i & 1));
-      PK_TICK(3)
-      have = have_next; b = nb; m0 = nm0;
-    }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0) { PK_TICK_FLUSH(16, 7) }
   } else {
-    // ------------------------------ store warps ------------------------------
-    const int sw = warp - kPwgFirstGateWarp - kPwgGateWarps;   // 0..7
-    const int quarter = warp & 3;
-    const int half = sw >> 2;                     // 0: skip columns (acc2 cols 0..63), 1: out columns (64..127)
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
-    PwgTileIter ti(p);
-    int b, m0;
-    bool have = ti.next(b, m0);
-    if (half == 0) {
-      // skip half: acc2[:, 0:64] -> red.global.add into the fp32 skip accumulator (row per thread, 2 x 128 B)
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int tt = m0 + quarter * 32 + lane;
-        float* dst = p.skip + (static_cast<long long>(b) * p.t + tt) * 64;
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
-#pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            mbar_arrive_a(acc2_empty + 8 * buf);
-          }
-          if (tt < p.t) {
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              float* d4 = dst + pass * 32 + 4 * c;
-              if (p.skip_init) {
-                *reinterpret_cast<float4*>(d4) = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-              } else {
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d4), "f"(v[4 * c]), "f"(v[4 * c + 1]),
-                             "f"(v[4 * c + 2]), "f"(v[4 * c + 3]) : "memory");
-              }
-            }
-          }
-          PK_TICK(5)
-        }
-        PK_TICK(1)
-        have = ti.next(b, m0);
-      }
-    } else {
-      // out half: x' = (acc2[:, 64:128] + b_out) * sqrt(1/2) -> split planes (acc2 already holds conv1x1_out(z) + x: the
-      // residual input was accumulated by the tensor core).  Row per thread, 256-bit stores (one 32-byte sector each).
-      const float kSqrtHalf = 0.70710678118654752440f;
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
-        const int trow = m0 + quarter * 32 + lane;
-        const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-        const bool live = trow < len;
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
-#pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + 64 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            mbar_arrive_a(acc2_empty + 8 * buf);
-          }
-          uint32_t oh[16], ol[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float y0 = live ? (v[2 * e] + p.out_b[pass * 32 + 2 * e]) * kSqrtHalf : 0.f;
-            const float y1 = live ? (v[2 * e + 1] + p.out_b[pass * 32 + 2 * e + 1]) * kSqrtHalf : 0.f;
-            split2(y0, y1, oh[e], ol[e]);
-          }
-          if (trow < p.t) {
-            st_global_v8(p.y_hi + row_off + pass * 32, oh);
-            st_global_v8(p.y_hi + row_off + pass * 32 + 16, oh + 8);
-            st_global_v8(p.y_lo + row_off + pass * 32, ol);
-            st_global_v8(p.y_lo + row_off + pass * 32 + 16, ol + 8);
-          }
-          PK_TICK(5)
-        }
-        PK_TICK(1)
-        have = ti.next(b, m0);
-      }
-    }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0) { PK_TICK_FLUSH(40 + half * 8, 7) }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// fused residual layer, CTA-pair version (tcgen05 cta_group::2, clusters of 2 CTAs on one TPC)
-// ---------------------------------------------------------------------------------------------------------------
-// The single-CTA kernel above re-loads the layer's weights (192 KB split-bf16) for every 128-sample tile; at ~9 k cycles
-// per tile that is 148 x 352 KB of L2->SM traffic per tile time = the L2 throughput cap.  Here two CTAs share one
-// M = 256 MMA: each keeps ITS HALF of the weights (64 of the 128 output channels of W1 and W2, 96 KB) resident in shared
-// memory for the whole launch and streams only its own 128 rows of activations (A operand, 32 KB per K-chunk).
-// L2->SM traffic per tile drops from 328 KB to 136 KB, UMMA operand reads per CTA from 8 KB to 6 KB per instruction.
-//   leader (cluster rank 0): issues every tcgen05.mma / commit (multicast to both CTAs' barriers) and owns the barriers
-//     its MMA thread waits on: full[s] (TMA bytes of BOTH CTAs), acc1_empty, z_full, acc2_empty (warp-elected remote arrivals)
-//   both CTAs: TMA producer (own rows), gate warps (own TMEM lanes), store warps; local barriers empty[s], acc1_full,
-//     acc2_full (multicast commits), g2_free (producer -> gate warps)
-//   Only z_full is waited on with cluster-scope acquire (it publishes generic-proxy smem writes of the peer CTA); every
-//   other barrier orders tensor-core / TMA / TMEM traffic only, and a cluster-scope acquire would cost an L1 invalidate
-//   (CCTL.IVALL) per wait on the MMA issuer's critical path.
-constexpr int kP2Stages = 3;
-constexpr int kP2StageBytes = 2 * kPwgTile;                  // A hi, A lo
-constexpr int kP2WTile = 64 * kSwizzleBytes;                 // 8 KB: 64 output channels x one K-chunk of one plane
-constexpr int kP2W1Bytes = kPwgG1Chunks * 2 * kP2WTile;      // 80 KB
-constexpr int kP2W2Bytes = 2 * kP2WTile;                     // 16 KB
-constexpr int kP2Smem = kP2Stages * kP2StageBytes + kP2W1Bytes + kP2W2Bytes + kP2WTile + 1024 + 256;
-
-struct PwgPairTileIter {   // 256-sample tiles of the pair; this CTA owns rows [m0 + 128 * rank, +128)
-  int idx, step, tiles_per_b, total, t;
-  const int32_t* lens;
-  __device__ PwgPairTileIter(const PwgLayerArgs& p)
-      : idx(static_cast<int>(blockIdx.x >> 1) - static_cast<int>(gridDim.x >> 1)), step(gridDim.x >> 1),
-        tiles_per_b((p.t + 255) >> 8), total(((p.t + 255) >> 8) * p.batch), t(p.t), lens(p.lens) {}
-  __device__ bool next(int& b, int& m0) {
-    for (;;) {
-      idx += step;
-      if (idx >= total) return false;
-      b = idx / tiles_per_b;
-      m0 = (idx % tiles_per_b) * 256;
-      const int len = lens ? min(__ldg(lens + b), t) : t;
-      if (m0 < len) return true;
-    }
-  }
-};
-
-template <bool kProf>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kPwgThreads, 1)
-pwg_layer_pair_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
-                      const __grid_constant__ CUtensorMap tm_c_hi, const __grid_constant__ CUtensorMap tm_c_lo,
-                      const __grid_constant__ CUtensorMap tm_w1_hi, const __grid_constant__ CUtensorMap tm_w1_lo,
-                      const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
-                      const PwgLayerArgs p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w1 = smem + kP2Stages * kP2StageBytes;        // [chunk][hi | lo] 64-row tiles, resident
-  const uint32_t w2 = w1 + kP2W1Bytes;                         // [hi | lo]
-  const uint32_t ident = w2 + kP2W2Bytes;                      // this CTA's 64 rows of [0 | I]
-  const uint32_t bars = ident + kP2WTile;
-  const uint32_t full_bar = bars;                              // [stages]   (leader's copy is the live one)
-  const uint32_t empty_bar = full_bar + 8 * kP2Stages;         // [stages]
-  const uint32_t acc1_full = empty_bar + 8 * kP2Stages;        // [2]
-  const uint32_t acc1_empty = acc1_full + 16;                  // [2] leader
-  const uint32_t acc2_full = acc1_empty + 16;                  // [2]
-  const uint32_t acc2_empty = acc2_full + 16;                  // [2] leader
-  const uint32_t z_full = acc2_empty + 16;                     // [2] leader
-  const uint32_t g2_free = z_full + 16;                        // [2]
-  const uint32_t w_bar = g2_free + 16;
-  const uint32_t tmem_slot = w_bar + 8;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  constexpr float kLog2e = 1.4426950408889634f;
-  (void)kLog2e;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_x_hi); tma_prefetch_desc(&tm_x_lo); tma_prefetch_desc(&tm_c_hi); tma_prefetch_desc(&tm_c_lo);
-    tma_prefetch_desc(&tm_w1_hi); tma_prefetch_desc(&tm_w1_lo); tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kP2Stages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc1_full + 8 * i, 1); mbar_init_a(acc1_empty + 8 * i, 2 * kPwgGateWarps);
-      mbar_init_a(acc2_full + 8 * i, 1); mbar_init_a(acc2_empty + 8 * i, 2 * kPwgStoreWarps);
-      mbar_init_a(z_full + 8 * i, 2 * kPwgGateWarps); mbar_init_a(g2_free + 8 * i, 1);
-    }
-    mbar_init_a(w_bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 192) {
-    // this CTA's half of the B operand [0 | I] of the residual pass: rank 0 holds output columns 0..63 (all zero: the
-    // skip half starts from 0), rank 1 holds columns 64..127 (row n = e_n: out column n receives x[:, n])
-    const int n = threadIdx.x - 128;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (rank == 1 && (n >> 3) == c) {
-        const uint32_t one = (n & 1) ? 0x3f800000u : 0x00003f80u;
-        const int w = (n & 7) >> 1;
-        v.x = w == 0 ? one : 0; v.y = w == 1 ? one : 0; v.z = w == 2 ? one : 0; v.w = w == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_all();
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // barriers of both CTAs are initialised before any remote arrive / TMA credit
-  tcgen05_fence_after();
-  if (warp == 0 && lane == 0) {
-    // resident weights: this CTA's 64 output channels of every K-chunk (W1: 5 chunks, W2: 1), both planes
-    mbar_arrive_expect_tx_a(w_bar, kP2W1Bytes + kP2W2Bytes);
-    for (int j = 0; j < kPwgG1Chunks; ++j) {
-      tma_load_3d_a(w1 + j * 2 * kP2WTile, &tm_w1_hi, w_bar, j * kChunkK, 64 * rank, 0);
-      tma_load_3d_a(w1 + j * 2 * kP2WTile + kP2WTile, &tm_w1_lo, w_bar, j * kChunkK, 64 * rank, 0);
-    }
-    tma_load_3d_a(w2, &tm_w2_hi, w_bar, 0, 64 * rank, 0);
-    tma_load_3d_a(w2 + kP2WTile, &tm_w2_lo, w_bar, 0, 64 * rank, 0);
+    // ------------------------------ consumers: 64 samples per warpgroup ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rl = 16 * (warp & 3) + (lane >> 2);              // this thread's rows: rl and rl + 8 of the warpgroup's 64
+    const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, + 1
+    const int aux_tail_ksteps = ((p.aux_ch - kChunkK) + kWgmmaK - 1) / kWgmmaK;  // k-steps in the 2nd aux chunk
+    const float kSqrtHalf = 0.70710678118654752440f;
     mbar_wait_a(w_bar, 0);
-  }
-  cluster_sync();                      // both halves of the weights are in place before the leader's first MMA
-  const uint32_t tmem_base = lds_u32(tmem_slot);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------ TMA producer (both CTAs, own rows) ------------------------------
-      uint32_t it = 0;
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      auto load_g1 = [&](int b, int m0) {
-        for (int j = 0; j < kPwgG1Chunks; ++j, ++it) {
-          const int s = it % kP2Stages;
-          PK_TICK(1)
-          mbar_wait_a(empty_bar + 8 * s, ((it / kP2Stages) & 1) ^ 1);
-          PK_TICK(0)
-          const uint32_t st = smem + s * kP2StageBytes;
-          const uint32_t fb = full_leader + 8 * s;
-          if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kP2StageBytes);   // the A chunks of both CTAs
-          const int wj = j == 0 ? 0 : j == 1 ? 2 : j == 2 ? 3 : j == 3 ? 4 : 1;
-          if (wj < 3) {
-            const int row = m0 + (wj - 1) * p.dil;
-            tma_load_3d_2sm_a(st, &tm_x_hi, fb, 0, row, b);
-            tma_load_3d_2sm_a(st + kPwgTile, &tm_x_lo, fb, 0, row, b);
-          } else {
-            tma_load_3d_2sm_a(st, &tm_c_hi, fb, (wj - 3) * kChunkK, m0, b);
-            tma_load_3d_2sm_a(st + kPwgTile, &tm_c_lo, fb, (wj - 3) * kChunkK, m0, b);
-          }
-        }
-      };
-      int n_g2 = 0;
-      auto load_g2 = [&]() {
-        const int s = it % kP2Stages;
-        PK_TICK(1)
-        mbar_wait_a(empty_bar + 8 * s, ((it / kP2Stages) & 1) ^ 1);
-        PK_TICK(0)
-        mbar_arrive_a(g2_free + 8 * (n_g2 & 1));   // own gate warps may write z of this tile into the stage
-        ++n_g2;
-        if (leader) mbar_arrive_a(full_bar + 8 * s);   // no TMA in this slot; keeps the stage ring's phases uniform
-        ++it;
-      };
-      PwgPairTileIter ti(p);
-      int b, m0, nb, nm0;
-      bool have = ti.next(b, m0);
-      if (have) load_g1(b, m0 + 128 * rank);
-      while (have) {
-        const bool have_next = ti.next(nb, nm0);
-        if (have_next) load_g1(nb, nm0 + 128 * rank);
-        load_g2();
-        have = have_next; b = nb; m0 = nm0;
-      }
-      PK_TICK(1)
-      if (leader) { PK_TICK_FLUSH(0, 2) }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(256, 128);
-      const int aux_tail_ksteps = ((p.aux_ch - kChunkK) + kUmmaK - 1) / kUmmaK;
-      uint32_t it = 0;
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      auto mma_chunk = [&](uint32_t d_tmem, uint32_t a_addr, uint32_t b_addr, int ksteps, bool first) {
-        const uint64_t a_hi = make_smem_desc_sw128(a_addr), a_lo = make_smem_desc_sw128(a_addr + kPwgTile);
-        const uint64_t b_hi = make_smem_desc_sw128(b_addr), b_lo = make_smem_desc_sw128(b_addr + kP2WTile);
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          umma_bf16_2sm(d_tmem, a_hi + koff, b_hi + koff, idesc, !(first && k == 0));
-          umma_bf16_2sm(d_tmem, a_lo + koff, b_hi + koff, idesc, 1);
-          umma_bf16_2sm(d_tmem, a_hi + koff, b_lo + koff, idesc, 1);
-        }
-      };
-      auto g1 = [&](int i) {
-        const int buf = i & 1;
-        PK_TICK(6)
-        mbar_wait_a(acc1_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
-        const uint32_t d = tmem_base + buf * 128;
-        for (int j = 0; j < kPwgG1Chunks; ++j, ++it) {
-          const int s = it % kP2Stages;
-          PK_TICK(2)
-          mbar_wait_a(full_bar + 8 * s, (it / kP2Stages) & 1);
-          PK_TICK(1)
-          tcgen05_fence_after();
-          const int wj = j == 0 ? 0 : j == 1 ? 2 : j == 2 ? 3 : j == 3 ? 4 : 1;
-          const uint32_t st = smem + s * kP2StageBytes;
-          mma_chunk(d, st, w1 + wj * 2 * kP2WTile, j == 3 ? aux_tail_ksteps : 4, j == 0);
-          if (j == kPwgG1Chunks - 1) {
-            // residual pass: acc2(i) = [0 | x_hi + x_lo] from the centre-tap tiles of both CTAs
-            PK_TICK(2)
-            mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-            PK_TICK(4)
-            tcgen05_fence_after();
-            const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kPwgTile);
-            const uint64_t b_id = make_smem_desc_sw128(ident);
-            const uint32_t d2 = tmem_base + 256 + buf * 128;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-              umma_bf16_2sm(d2, a_hi + koff, b_id + koff, idesc, k != 0);
-              umma_bf16_2sm(d2, a_lo + koff, b_id + koff, idesc, 1);
-            }
-          }
-          umma_commit_2sm_a(empty_bar + 8 * s);
-        }
-        umma_commit_2sm_a(acc1_full + 8 * buf);
-      };
-      auto g2 = [&](int i) {
-        const int buf = i & 1;
-        const int s = it % kP2Stages;
-        PK_TICK(2)
-        mbar_wait_cluster_a(z_full + 8 * (i & 1), (i >> 1) & 1);   // the gate warps of both CTAs wrote z into stage s
-        PK_TICK(3)
-        mbar_wait_a(full_bar + 8 * s, (it / kP2Stages) & 1);
-        PK_TICK(5)
-        tcgen05_fence_after();
-        mma_chunk(tmem_base + 256 + buf * 128, smem + s * kP2StageBytes, w2, 4, false);
-        umma_commit_2sm_a(empty_bar + 8 * s);
-        umma_commit_2sm_a(acc2_full + 8 * buf);
-        ++it;
-      };
-      PwgPairTileIter ti(p);
-      int b, m0;
-      int n_issued = 0, n_done = 0;
-      bool have = ti.next(b, m0);
-      if (have) g1(n_issued++);
-      while (have) {
-        const bool have_next = ti.next(b, m0);
-        if (have_next) g1(n_issued++);
-        g2(n_done++);
-        have = have_next;
-      }
-      PK_TICK(6)
-      PK_TICK_FLUSH(8, 7)
-      if (kProf) atomicAdd(p.prof + 32, static_cast<unsigned long long>(n_done));
-    }
-  } else if (warp < kPwgFirstGateWarp) {
-    // idle warps
-  } else if (warp < kPwgFirstGateWarp + kPwgGateWarps) {
-    // ------------------------------ gate warps (both CTAs, own TMEM lanes) ------------------------------
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc1_empty_l = mapa_shared(acc1_empty, 0), z_full_l = mapa_shared(z_full, 0);
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
-    float k_a, k_g;
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    uint32_t it = kPwgG1Chunks;
-    PwgPairTileIter ti(p);
-    int b, m0, nb, nm0;
-    bool have = ti.next(b, m0);
-    for (int i = 0; have; ++i) {
-      const bool have_next = ti.next(nb, nm0);
-      if (have_next) it += kPwgG1Chunks;
-      const uint32_t st2 = smem + (it % kP2Stages) * kP2StageBytes;
-      ++it;
-      const int buf = i & 1;
-      PK_TICK(6)
-      mbar_wait_a(acc1_full + 8 * buf, (i >> 1) & 1);
-      PK_TICK(0)
-      tcgen05_fence_after();
-      uint32_t zh[32], zl[32];
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float va[32], vb[32];
-        __syncwarp();
-        tmem_ld_32x32(tmem_base + lane_base + buf * 128 + half * 32, va);
-        tmem_ld_32x32(tmem_base + lane_base + buf * 128 + 64 + half * 32, vb);
-        tmem_ld_wait();
-        if (half == 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster_relaxed_a(acc1_empty_l + 8 * buf);
-        }
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float z[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, p.gate_c[half * 32 + j + e]), 60.f));
-            const float e2 = ex2_approx(fmaf(vb[j + e], k_g, p.gate_c[64 + half * 32 + j + e]));
-            const float t1 = 1.f + e1;
-            z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
-          }
-          split2(z[0], z[1], zh[half * 16 + j / 2], zl[half * 16 + j / 2]);
-          split2(z[2], z[3], zh[half * 16 + j / 2 + 1], zl[half * 16 + j / 2 + 1]);
-        }
-      }
-      PK_TICK(1)
-      mbar_wait_a(g2_free + 8 * (i & 1), (i >> 1) & 1);
-      PK_TICK(2)
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int chunk = q ^ (r & 7);
-        sts_u4(st2 + r * kSwizzleBytes + chunk * 16, make_uint4(zh[4 * q], zh[4 * q + 1], zh[4 * q + 2], zh[4 * q + 3]));
-        sts_u4(st2 + kPwgTile + r * kSwizzleBytes + chunk * 16, make_uint4(zl[4 * q], zl[4 * q + 1], zl[4 * q + 2], zl[4 * q + 3]));
-      }
-      fence_proxy_async_smem();          // z lives in this CTA's smem and is read by this CTA's tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_a(z_full_l + 8 * (i & 1));
-      PK_TICK(3)
-      have = have_next; b = nb; m0 = nm0;
-    }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0 && leader) { PK_TICK_FLUSH(16, 7) }
-  } else {
-    // ------------------------------ store warps (both CTAs) ------------------------------
-    const int sw = warp - kPwgFirstGateWarp - kPwgGateWarps;
-    const int quarter = warp & 3;
-    const int half = sw >> 2;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc2_empty_l = mapa_shared(acc2_empty, 0);
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
-    PwgPairTileIter ti(p);
+    uint32_t it = 0;
+    PwgTileIter ti(p);
     int b, m0;
-    bool have = ti.next(b, m0);
-    if (half == 0) {
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int tt = m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-        float* dst = p.skip + (static_cast<long long>(b) * p.t + tt) * 64;
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
+    while (ti.next(b, m0)) {
+      float acc1[64], acc2[64];
+      for (int j = 0; j < kPwgG1Chunks; ++j, ++it) {
+        const int s = it % kPwgStages;
+        mbar_wait_a(full_bar + 8 * s, (it / kPwgStages) & 1);
+        const uint32_t st = smem + s * kPwgStageBytes;
+        const uint32_t sa = st + wg * 64 * kSwizzleBytes;
+        const uint64_t a_hi = make_smem_desc_sw128(sa), a_lo = make_smem_desc_sw128(sa + kPwgTile);
+        const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kPwgTile), b_lo = make_smem_desc_sw128(st + 3 * kPwgTile);
+        const int ksteps = j == 3 ? aux_tail_ksteps : 4;
+        wgmma_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          wgmma_ss_n128(acc1, a_hi + desc_kstep(k), b_hi + desc_kstep(k), !(j == 0 && k == 0));
+          wgmma_ss_n128(acc1, a_lo + desc_kstep(k), b_hi + desc_kstep(k), 1);
+          wgmma_ss_n128(acc1, a_hi + desc_kstep(k), b_lo + desc_kstep(k), 1);
+        }
+        wgmma_commit();
+        if (j == kPwgG1Chunks - 1) {
+          // GEMM2's accumulator starts as [0 | x]: x = hi + lo of this tile's own rows, from the centre-tap chunk
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
-          }
-          if (tt < p.t) {
+          for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              float* d4 = dst + pass * 32 + 4 * c;
-              if (p.skip_init) {
-                *reinterpret_cast<float4*>(d4) = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-              } else {
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d4), "f"(v[4 * c]), "f"(v[4 * c + 1]),
-                             "f"(v[4 * c + 2]), "f"(v[4 * c + 3]) : "memory");
-              }
+            for (int hh = 0; hh < 2; ++hh) {
+              const int r = rl + 8 * hh;
+              const uint32_t off = r * kSwizzleBytes + ((((8 * jj + cq) >> 3) ^ (r & 7)) << 4) + (cq & 7) * 2;
+              const uint32_t xh = lds_u32(sa + off), xl = lds_u32(sa + kPwgTile + off);
+              acc2[4 * jj + 2 * hh] = 0.f;
+              acc2[4 * jj + 2 * hh + 1] = 0.f;
+              acc2[32 + 4 * jj + 2 * hh] = __uint_as_float(xh << 16) + __uint_as_float(xl << 16);
+              acc2[32 + 4 * jj + 2 * hh + 1] = __uint_as_float(xh & 0xffff0000u) + __uint_as_float(xl & 0xffff0000u);
             }
           }
-          PK_TICK(5)
         }
-        PK_TICK(1)
-        have = ti.next(b, m0);
+        wgmma_wait<0>();
+        reg_fence(acc1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_a(empty_bar + 8 * s);
       }
-    } else {
-      const float kSqrtHalf = 0.70710678118654752440f;
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
-        const int trow = m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-        const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-        const bool live = trow < len;
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
+      // gate: z = tanh(a + ba) * sigmoid(g + bg) = (1 - e1) / ((1 + e1)(1 + e2)), e1 = exp(-2(a+ba)), e2 = exp(-(g+bg))
+      // (one reciprocal; the exp2 argument of e1 is clamped at 60 so that the product cannot overflow where z != 0).
+      // a column c and its g column 64 + c sit in the same thread (fragments j and j + 8).
+      uint32_t zh[16], zl[16];
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + 64 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
-          }
-          uint32_t oh[16], ol[16];
+      for (int jj = 0; jj < 8; ++jj) {
+        float z[4];
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float y0 = live ? (v[2 * e] + p.out_b[pass * 32 + 2 * e]) * kSqrtHalf : 0.f;
-            const float y1 = live ? (v[2 * e + 1] + p.out_b[pass * 32 + 2 * e + 1]) * kSqrtHalf : 0.f;
-            split2(y0, y1, oh[e], ol[e]);
-          }
-          if (trow < p.t) {
-            st_global_v8(p.y_hi + row_off + pass * 32, oh);
-            st_global_v8(p.y_hi + row_off + pass * 32 + 16, oh + 8);
-            st_global_v8(p.y_lo + row_off + pass * 32, ol);
-            st_global_v8(p.y_lo + row_off + pass * 32 + 16, ol + 8);
-          }
-          PK_TICK(5)
+        for (int e = 0; e < 4; ++e) {
+          const int c = 8 * jj + cq + (e & 1);
+          const float e1 = ex2_approx(fminf(fmaf(acc1[4 * jj + e], p.k_a, p.gate_c[c]), 60.f));
+          const float e2 = ex2_approx(fmaf(acc1[32 + 4 * jj + e], p.k_g, p.gate_c[64 + c]));
+          const float t1 = 1.f + e1;
+          z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
         }
-        PK_TICK(1)
-        have = ti.next(b, m0);
+        split2(z[0], z[1], zh[2 * jj], zl[2 * jj]);            // row rl
+        split2(z[2], z[3], zh[2 * jj + 1], zl[2 * jj + 1]);    // row rl + 8
+      }
+      // GEMM2: [skip | out] += z W2, K = 64 = 4 K-steps; A fragment of K-step k = z column groups 2k, 2k + 1
+      const uint64_t b2_hi = make_smem_desc_sw128(w2), b2_lo = make_smem_desc_sw128(w2 + kPwgTile);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t ah[4] = {zh[4 * k], zh[4 * k + 1], zh[4 * k + 2], zh[4 * k + 3]};
+        const uint32_t al[4] = {zl[4 * k], zl[4 * k + 1], zl[4 * k + 2], zl[4 * k + 3]};
+        wgmma_rs_n128(acc2, ah, b2_hi + desc_kstep(k), 1);
+        wgmma_rs_n128(acc2, al, b2_hi + desc_kstep(k), 1);
+        wgmma_rs_n128(acc2, ah, b2_lo + desc_kstep(k), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc2);
+      // stores: skip half -> fp32 skip sum (write or red.add), out half -> (out + b_out) * sqrt(1/2) as split planes
+      const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int trow = m0 + wg * 64 + rl + 8 * hh;
+        if (trow < p.t) {
+          const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
+          const bool live = trow < len;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int c = 8 * jj + cq;
+            float* d2 = p.skip + row_off + c;
+            const float s0 = acc2[4 * jj + 2 * hh], s1 = acc2[4 * jj + 2 * hh + 1];
+            if (p.skip_init) *reinterpret_cast<float2*>(d2) = make_float2(s0, s1);
+            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d2), "f"(s0), "f"(s1) : "memory");
+            const float y0 = live ? (acc2[32 + 4 * jj + 2 * hh] + p.out_b[c]) * kSqrtHalf : 0.f;
+            const float y1 = live ? (acc2[32 + 4 * jj + 2 * hh + 1] + p.out_b[c + 1]) * kSqrtHalf : 0.f;
+            uint32_t oh, ol;
+            split2(y0, y1, oh, ol);
+            *reinterpret_cast<uint32_t*>(p.y_hi + row_off + c) = oh;
+            *reinterpret_cast<uint32_t*>(p.y_lo + row_off + c) = ol;
+          }
+        }
       }
     }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0 && leader) { PK_TICK_FLUSH(40 + half * 8, 7) }
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // neither CTA may free its TMEM / exit while the pair's MMAs can still touch it
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
   }
 }
 
@@ -1200,12 +538,7 @@ extern "C" int pk_pwg_residual_layer(const pk_pwg_layer_args* a, pk_stream_t str
   CUtensorMap tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo;
   int rc;
   const uint64_t T = a->t, B = a->batch;
-  // CTA-pair kernel (weights resident, half per CTA) unless PK_PWG_PAIR=0
-  static const bool use_pair = []() {
-    const char* e = getenv("PK_PWG_PAIR");
-    return !(e && e[0] == '0') && sm_count() >= 2;
-  }();
-  const uint32_t w_box_rows = use_pair ? 64 : 128;
+  const uint32_t w_box_rows = 128;
   if ((rc = encode_tmap_bf16_3d(&tx_hi, a->x_hi, kPwgR, T, B, kPwgR, T * kPwgR, 128))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tx_lo, a->x_lo, kPwgR, T, B, kPwgR, T * kPwgR, 128))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tc_hi, a->c_hi, a->aux_channels, T, B, a->aux_channels, T * a->aux_channels, 128))) return rc;
@@ -1218,10 +551,7 @@ extern "C" int pk_pwg_residual_layer(const pk_pwg_layer_args* a, pk_stream_t str
   if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, w_box_rows))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwgSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwgSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2Smem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kP2Smem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwgSmem));
     attr_set = true;
   }
   PwgLayerArgs p;
@@ -1236,24 +566,10 @@ extern "C" int pk_pwg_residual_layer(const pk_pwg_layer_args* a, pk_stream_t str
     p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
     p.out_b[i] = a->bias2[64 + i];
   }
-  p.x_hi = static_cast<const __nv_bfloat16*>(a->x_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->x_lo);
   p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
-  p.prof = static_cast<unsigned long long*>(a->prof);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (use_pair) {
-    const int pair_tiles = ((a->t + 255) / 256) * a->batch;
-    const int grid = 2 * std::min(pair_tiles, sm_count() / 2);
-    if (p.prof != nullptr)
-      pwg_layer_pair_kernel<true><<<grid, kPwgThreads, kP2Smem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
-    else
-      pwg_layer_pair_kernel<false><<<grid, kPwgThreads, kP2Smem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
-  } else {
-    const int grid = std::min(p.total_tiles, sm_count());
-    if (p.prof != nullptr)
-      pwg_layer_kernel<true><<<grid, kPwgThreads, kPwgSmem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
-    else
-      pwg_layer_kernel<false><<<grid, kPwgThreads, kPwgSmem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
-  }
+  const int grid = std::min(p.total_tiles, sm_count());
+  pwg_layer_kernel<<<grid, kPwgThreads, kPwgSmem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

@@ -1,48 +1,42 @@
-// pk_pwg_residual_layer_fc: the CTA-pair residual-layer kernel of pwg.cu with FRAME-RATE CONDITIONING (the default
+// pk_pwg_residual_layer_fc: the fused Parallel WaveGAN residual layer (pwg.cu) with FRAME-RATE CONDITIONING (the default
 // residual-stack path of the Python model - DESIGN.md 5).
 //
 // The upsampling network is linear and per channel, so conv1x1_aux(upsample(m'))[t, n] = sum_j U[t, j] (W_aux m')[j, n].
 // GEMM1's two conditioning K-chunks (80 channels of the 1.23 GB sample-rate conditioning tensor, 5 K-steps, 32 KB of
 // resident W_aux) become ONE K-step: A = the tile-relative band table of U (constants of the model,
 // models/_pwg_frame_cond.py), B = the 16-frame window of P = W_aux m' that the tile touches (frame rate, L2 resident).
-// Pipeline (round 2, after the phase profile of the round-1 pair kernel showed the tensor pipe waiting ~50 % of the time on
-// its feeders - profiles/r02_pwg_phase_profile.txt):
-//   * 4 smem stages of 32 KB and exactly 4 K-chunks per tile (tap -d, tap +d, conditioning, centre tap): chunk j of every
-//     tile lives in stage j, a stage is refilled one whole tile ahead;
-//   * z never touches shared memory: the gate warps write it (packed bf16x2, hi | lo) with tcgen05.st OVER the GEMM1
-//     accumulator columns they have just read, and GEMM2 takes its A operand from tensor memory.  This removes the z
-//     staging slot from the ring, the generic->async proxy fence and the cluster-scope release on the critical path
-//     (2.4 k cycles per tile), 12 x 4 KB of UMMA smem operand reads per tile, and the acc1_empty barrier: GEMM1 of tile i+2
-//     is issued after GEMM2 of tile i by the same thread, and tcgen05.mma execute in issue order.
+//
+// Hopper structure: persistent CTAs over 128-sample tiles (the two halves of the 256-sample window that one band-table /
+// P-window pair describes), 384 threads:
+//   * warps 8-11 (producer warpgroup, one TMA lane): per tile 4 A chunks (tap -d, tap +d, conditioning, centre tap) through a
+//     2-deep ring of 32 KB stages, plus the P window of the tile; W1 (three tap chunks) and W2 stay resident (128 KB);
+//   * warps 0-7 (two consumer warpgroups, 64 samples each): GEMM1 (wgmma, accumulator in registers), the gate in registers,
+//     z as the register A operand of GEMM2 - z never touches shared memory - and the stores straight from the fragments.
+//     The residual add `+ x` is folded in by starting GEMM2's accumulator at [0 | x], read from the centre-tap chunk
+//     while it is in shared memory.
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 namespace fc {
 
 constexpr int kPwgR = 64;
 constexpr int kPwgG = 128;
-constexpr int kPwgTile = 128 * kSwizzleBytes;
-constexpr int kPwgGateWarps = 4;
-constexpr int kPwgStoreWarps = 8;
-constexpr int kPwgFirstGateWarp = 4;
-constexpr int kPwgThreads = (kPwgFirstGateWarp + kPwgGateWarps + kPwgStoreWarps) * 32;
+constexpr int kATile = 128 * kSwizzleBytes;                  // 16 KB: one plane of a 128-row K-chunk
+constexpr int kConsumerThreads = 256;
+constexpr int kThreads = kConsumerThreads + 128;
 constexpr int kFcG1Chunks = 4;                               // tap -d, tap +d, conditioning, centre tap
-constexpr int kFcStages = 4;                                 // == kFcG1Chunks: chunk j of every tile uses stage j
-constexpr int kFcStageBytes = 2 * kPwgTile;                  // A hi, A lo
-constexpr int kFcWTile = 64 * kSwizzleBytes;                 // 8 KB: 64 output channels x one K-chunk of one plane
-constexpr int kFcW1Bytes = 3 * 2 * kFcWTile;                 // 48 KB: three tap chunks
-constexpr int kFcW2Bytes = 2 * kFcWTile;                     // 16 KB
-constexpr int kFcPBytes = 2 * kFcWTile;                      // 16 KB: hi | lo of one P window
-// one P buffer is enough: the window of tile i+1 is loaded into it when stage 2 is handed back, i.e. after the commit that
-// follows the conditioning MMAs of tile i
-constexpr int kFcSmem = kFcStages * kFcStageBytes + kFcW1Bytes + kFcW2Bytes + kFcWTile + kFcPBytes + 1024 + 256;
-static_assert(kFcStages == kFcG1Chunks, "the P buffer / stage reuse argument needs one ring revolution per tile");
+constexpr int kFcStages = 2;
+constexpr int kFcStageBytes = 2 * kATile;                    // A hi, A lo
+constexpr int kFcW1Bytes = 3 * 2 * kATile;                   // 96 KB: three tap chunks x 128 output channels
+constexpr int kFcW2Bytes = 2 * kATile;                       // 32 KB: 128 outputs (skip | out) x 64
+constexpr int kFcPBytes = 2 * kATile;                        // 32 KB: hi | lo of the P window of 128 output channels
+constexpr int kFcSmem = kFcStages * kFcStageBytes + kFcW1Bytes + kFcW2Bytes + kFcPBytes + 1024 + 256;
 static_assert(kFcSmem <= 227 * 1024, "shared memory budget");
 
 struct FcLayerArgs {
@@ -55,23 +49,9 @@ struct FcLayerArgs {
   float k_a, k_g;
   float* skip;
   int skip_init;
-  const __nv_bfloat16* x_hi;    // layer input planes (re-read for the residual add when kResidMma == false)
-  const __nv_bfloat16* x_lo;
   __nv_bfloat16* y_hi;
   __nv_bfloat16* y_lo;
-  unsigned long long* prof;
 };
-
-#define PK_TICK(k)                                      \
-  if (kProf) {                                          \
-    const long long n_ = clock64();                     \
-    tacc[k] += n_ - tlast;                              \
-    tlast = n_;                                         \
-  }
-#define PK_TICK_FLUSH(base, n)                                                              \
-  if (kProf) {                                                                              \
-    for (int k_ = 0; k_ < (n); ++k_) atomicAdd(p.prof + (base) + k_, static_cast<unsigned long long>(tacc[k_])); \
-  }
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -91,470 +71,221 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-}
 
-struct FcTileIter {   // 256-sample tiles of the pair; this CTA owns rows [m0 + 128 * rank, +128)
+struct FcTileIter {   // 128-sample tiles = halves of the 256-sample windows; live windows only
   int idx, step, tiles_per_b, total, t;
   const int32_t* lens;
   __device__ FcTileIter(const FcLayerArgs& p)
-      : idx(static_cast<int>(blockIdx.x >> 1) - static_cast<int>(gridDim.x >> 1)), step(gridDim.x >> 1),
-        tiles_per_b((p.t + 255) >> 8), total(((p.t + 255) >> 8) * p.batch), t(p.t), lens(p.lens) {}
-  __device__ bool next(int& b, int& m0) {
+      : idx(static_cast<int>(blockIdx.x) - static_cast<int>(gridDim.x)), step(gridDim.x),
+        tiles_per_b((p.t + 255) >> 8), total(((p.t + 255) >> 8) * p.batch * 2), t(p.t), lens(p.lens) {}
+  // b, m0 (first row of the 256-sample window), half (which 128 rows of it)
+  __device__ bool next(int& b, int& m0, int& half) {
     for (;;) {
       idx += step;
       if (idx >= total) return false;
-      b = idx / tiles_per_b;
-      m0 = (idx % tiles_per_b) * 256;
+      const int w = idx >> 1;
+      half = idx & 1;
+      b = w / tiles_per_b;
+      m0 = (w % tiles_per_b) * 256;
       const int len = lens ? min(__ldg(lens + b), t) : t;
       if (m0 < len) return true;
     }
   }
 };
 
-// kResid selects where the residual add `+ x` happens.  2 (PK_PWG_RESID=gate): the gate warps preload the GEMM2 accumulator
-// with [0 | x_hi + x_lo] (x re-read from global memory - L2 hot, TMA has just streamed it - and written with tcgen05.st while
-// GEMM1 of the tile is still running), GEMM2 accumulates on top: no extra MMAs and nothing added to the store warps.
-// 1 (kResidMma): the residual add `+ x` as a tensor-core pass (x [0 | I] into the GEMM2 accumulator, 8 MMAs per tile, no global
-// loads) or, when false, in the out-store warps from global memory (the rows were just streamed by TMA, so they hit L2):
-// 8 fewer shared-memory-fed MMAs against 16 LDG.128 per thread and tile.  PK_PWG_RESID=ldg selects the latter (experiment).
-template <bool kProf, int kResid>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kPwgThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_u,
                     const __grid_constant__ CUtensorMap tm_p,          // 4-D maps: both planes of a tile in one TMA box
-                      const __grid_constant__ CUtensorMap tm_w1_hi, const __grid_constant__ CUtensorMap tm_w1_lo,
-                      const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
-                      const FcLayerArgs p) {
-  constexpr bool kResidMma = kResid == 1;
-  constexpr bool kResidGate = kResid == 2;
+                    const __grid_constant__ CUtensorMap tm_w1_hi, const __grid_constant__ CUtensorMap tm_w1_lo,
+                    const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
+                    const FcLayerArgs p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w1 = smem + kFcStages * kFcStageBytes;        // [chunk][hi | lo] 64-row tiles, resident
+  const uint32_t w1 = smem + kFcStages * kFcStageBytes;        // [tap chunk][hi | lo] 128-row tiles, resident
   const uint32_t w2 = w1 + kFcW1Bytes;                         // [hi | lo]
-  const uint32_t ident = w2 + kFcW2Bytes;                      // this CTA's 64 rows of [0 | I]
-  const uint32_t pbuf = ident + kFcWTile;                      // [hi | lo] this CTA's 64 rows of the P window of a tile
+  const uint32_t pbuf = w2 + kFcW2Bytes;                       // [hi | lo] P window of the current tile
   const uint32_t bars = pbuf + kFcPBytes;
-  const uint32_t full_bar = bars;                              // [stages]   (leader's copy is the live one)
+  const uint32_t full_bar = bars;                              // [stages]
   const uint32_t empty_bar = full_bar + 8 * kFcStages;         // [stages]
-  const uint32_t acc1_full = empty_bar + 8 * kFcStages;        // [2]
-  const uint32_t acc2_full = acc1_full + 16;                   // [2]
-  const uint32_t acc2_empty = acc2_full + 16;                  // [2] leader
-  const uint32_t z_full = acc2_empty + 16;                     // [2] leader: z of tile i is in tensor memory (both CTAs)
-  const uint32_t w_bar = z_full + 16;
-  const uint32_t tmem_slot = w_bar + 8;
+  const uint32_t w_bar = empty_bar + 8 * kFcStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  constexpr float kLog2e = 1.4426950408889634f;
-  (void)kLog2e;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_u); tma_prefetch_desc(&tm_p);
     tma_prefetch_desc(&tm_w1_hi); tma_prefetch_desc(&tm_w1_lo); tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kFcStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc1_full + 8 * i, 1);
-      // kResidGate: each CTA's gate warps wait for their own CTA's store warps (local barrier); else the issuer waits for both CTAs'
-      mbar_init_a(acc2_full + 8 * i, 1); mbar_init_a(acc2_empty + 8 * i, kResidGate ? kPwgStoreWarps : 2 * kPwgStoreWarps);
-      mbar_init_a(z_full + 8 * i, 2 * kPwgGateWarps);
-    }
+    for (int s = 0; s < kFcStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
     mbar_init_a(w_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2sm_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 192) {
-    // this CTA's half of the B operand [0 | I] of the residual pass: rank 0 holds output columns 0..63 (all zero: the
-    // skip half starts from 0), rank 1 holds columns 64..127 (row n = e_n: out column n receives x[:, n])
-    const int n = threadIdx.x - 128;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (rank == 1 && (n >> 3) == c) {
-        const uint32_t one = (n & 1) ? 0x3f800000u : 0x00003f80u;
-        const int w = (n & 7) >> 1;
-        v.x = w == 0 ? one : 0; v.y = w == 1 ? one : 0; v.z = w == 2 ? one : 0; v.w = w == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_all();
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // barriers of both CTAs are initialised before any remote arrive / TMA credit
-  tcgen05_fence_after();
-  if (warp == 0 && lane == 0) {
-    // resident weights: this CTA's 64 output channels of the three tap chunks of W1 and of W2, both planes
-    mbar_arrive_expect_tx_a(w_bar, kFcW1Bytes + kFcW2Bytes);
-    for (int j = 0; j < 3; ++j) {
-      tma_load_3d_a(w1 + j * 2 * kFcWTile, &tm_w1_hi, w_bar, j * kChunkK, 64 * rank, 0);
-      tma_load_3d_a(w1 + j * 2 * kFcWTile + kFcWTile, &tm_w1_lo, w_bar, j * kChunkK, 64 * rank, 0);
-    }
-    tma_load_3d_a(w2, &tm_w2_hi, w_bar, 0, 64 * rank, 0);
-    tma_load_3d_a(w2 + kFcWTile, &tm_w2_lo, w_bar, 0, 64 * rank, 0);
-    mbar_wait_a(w_bar, 0);
-  }
-  cluster_sync();                      // both halves of the weights are in place before the leader's first MMA
-  const uint32_t tmem_base = lds_u32(tmem_slot);
+  __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------ TMA producer (both CTAs, own rows) ------------------------------
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
+      // ------------------------------ TMA producer ------------------------------
+      // resident weights: all 128 output channels of the three tap chunks of W1 and of W2, both planes
+      mbar_arrive_expect_tx_a(w_bar, kFcW1Bytes + kFcW2Bytes);
+      for (int j = 0; j < 3; ++j) {
+        tma_load_3d_a(w1 + j * 2 * kATile, &tm_w1_hi, w_bar, j * kChunkK, 0, 0);
+        tma_load_3d_a(w1 + j * 2 * kATile + kATile, &tm_w1_lo, w_bar, j * kChunkK, 0, 0);
+      }
+      tma_load_3d_a(w2, &tm_w2_hi, w_bar, 0, 0, 0);
+      tma_load_3d_a(w2 + kATile, &tm_w2_lo, w_bar, 0, 0, 0);
       uint32_t it = 0;
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      auto load_g1 = [&](int b, int m0) {
+      FcTileIter ti(p);
+      int b, m0, half;
+      while (ti.next(b, m0, half)) {
+        const int mh = m0 + 128 * half;
         for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
-          const int s = j;                                     // kFcStages == kFcG1Chunks
-          PK_TICK(1)
+          const int s = it % kFcStages;
           mbar_wait_a(empty_bar + 8 * s, ((it / kFcStages) & 1) ^ 1);
-          PK_TICK(0)
           const uint32_t st = smem + s * kFcStageBytes;
-          const uint32_t fb = full_leader + 8 * s;
-          // chunk order: tap -d, tap +d, conditioning, centre tap (last: it also feeds the residual pass)
+          const uint32_t fb = full_bar + 8 * s;
+          // chunk order: tap -d, tap +d, conditioning, centre tap (last: it also supplies the residual x)
           if (j == 2) {
-            // conditioning as U (W_aux m'): A = tile-relative band table rows [m0, m0 + 128) (K window = 16 frames inside a
-            // 64-wide box), B = the same 16 frames of P for this CTA's 64 output channels; frames outside the utterance are
-            // out of bounds of the tensor map and read as zero
-            if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * (kFcStageBytes + kFcPBytes));
+            // conditioning as U (W_aux m'): A = tile-relative band table rows (K window = 16 frames inside a 64-wide box),
+            // B = the same 16 frames of P for the 128 output channels; frames outside the utterance are out of bounds of
+            // the tensor map and read as zero.  The P buffer's previous reader (this chunk of the previous tile) finished
+            // before the stage now being refilled was handed back.
+            mbar_arrive_expect_tx_a(fb, kFcStageBytes + kFcPBytes);
             // band rows of this half tile: first 128 rows of an utterance, the half tiles touching its last 128 rows
             // (per-utterance block; 2 * 128 clamps halves lying wholly past the end onto the zero block), else interior
             const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
             const int m1 = ((len - 128) >> 7) << 7;
-            const int urow = m0 == 0 ? p.u_start_row
-                             : (m0 + 128 > len - 128) ? p.u_end_base + 384 * b + min(m0 - m1, 256)
-                                                      : m0 % p.u_period;
-            tma_load_4d_2sm_a(st, &tm_u, fb, 0, urow, 0, 0);
-            // one K window per PAIR tile (the two CTAs supply the two halves of the same B operand): it starts at the frame of
-            // the pair's first row, aligned down to 8 frames (16 B) - TMA faults on an unaligned innermost coordinate
-            const int j0 = ((m0 - 128 * static_cast<int>(rank)) / p.hop - 2) & ~7;
-            tma_load_4d_2sm_a(pbuf, &tm_p, fb, j0, p.p_row0 + 64 * static_cast<int>(rank), b, 0);
+            const int urow = mh == 0 ? p.u_start_row
+                             : (mh + 128 > len - 128) ? p.u_end_base + 384 * b + min(mh - m1, 256)
+                                                      : mh % p.u_period;
+            tma_load_4d_a(st, &tm_u, fb, 0, urow, 0, 0);
+            // one K window per 256-sample window: it starts at the frame of the window's first row, aligned down to
+            // 8 frames (16 B) - TMA faults on an unaligned innermost coordinate
+            const int j0 = (m0 / p.hop - 2) & ~7;
+            tma_load_4d_a(pbuf, &tm_p, fb, j0, p.p_row0, b, 0);
           } else {
-            if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kFcStageBytes);   // the A chunks of both CTAs
+            mbar_arrive_expect_tx_a(fb, kFcStageBytes);
             const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
-            const int row = m0 + (wj - 1) * p.dil;
-            tma_load_4d_2sm_a(st, &tm_x, fb, 0, row, b, 0);
+            tma_load_4d_a(st, &tm_x, fb, 0, mh + (wj - 1) * p.dil, b, 0);
           }
         }
-      };
-      FcTileIter ti(p);
-      int b, m0;
-      while (ti.next(b, m0)) load_g1(b, m0 + 128 * rank);
-      PK_TICK(1)
-      if (leader) { PK_TICK_FLUSH(0, 2) }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(256, 128);
-      uint32_t it = 0;
-      long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      long long tlast = clock64();
-      auto mma_chunk = [&](uint32_t d_tmem, uint32_t a_addr, uint32_t b_addr, int ksteps, bool first) {
-        const uint64_t a_hi = make_smem_desc_sw128(a_addr), a_lo = make_smem_desc_sw128(a_addr + kPwgTile);
-        const uint64_t b_hi = make_smem_desc_sw128(b_addr), b_lo = make_smem_desc_sw128(b_addr + kFcWTile);
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          umma_bf16_2sm(d_tmem, a_hi + koff, b_hi + koff, idesc, !(first && k == 0));
-          umma_bf16_2sm(d_tmem, a_lo + koff, b_hi + koff, idesc, 1);
-          umma_bf16_2sm(d_tmem, a_hi + koff, b_lo + koff, idesc, 1);
-        }
-      };
-      auto g1 = [&](int i) {
-        // acc1(i & 1) needs no "empty" barrier: its previous user is tile i-2, whose GEMM2 (the last reader: z lives in the
-        // accumulator's own columns) was issued by this thread before this point, and tcgen05.mma execute in issue order
-        const int buf = i & 1;
-        const uint32_t d = tmem_base + buf * 128;
-        for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
-          const int s = j;
-          PK_TICK(2)
-          mbar_wait_a(full_bar + 8 * s, (it / kFcStages) & 1);
-          if (kProf) {                       // wait-for-data time per chunk: buckets 0 (tap -d), 1 (tap +d), 6 (conditioning), 7 (centre)
-            const long long n_ = clock64();
-            tacc[j == 0 ? 0 : j == 1 ? 1 : j == 2 ? 6 : 7] += n_ - tlast;
-            tlast = n_;
-          }
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * kFcStageBytes;
-          if (j == 2) {
-            mma_chunk(d, st, pbuf, 1, false);                            // one K-step: 16 frames of band table x P window
-          } else {
-            const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
-            mma_chunk(d, st, w1 + wj * 2 * kFcWTile, 4, j == 0);
-          }
-          if (kResidMma && j == kFcG1Chunks - 1) {
-            // residual pass: acc2(i) = [0 | x_hi + x_lo] from the centre-tap tiles of both CTAs
-            PK_TICK(2)
-            mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-            PK_TICK(4)
-            tcgen05_fence_after();
-            const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kPwgTile);
-            const uint64_t b_id = make_smem_desc_sw128(ident);
-            const uint32_t d2 = tmem_base + 256 + buf * 128;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-              umma_bf16_2sm(d2, a_hi + koff, b_id + koff, idesc, k != 0);
-              umma_bf16_2sm(d2, a_lo + koff, b_id + koff, idesc, 1);
-            }
-          }
-          umma_commit_2sm_a(empty_bar + 8 * s);
-        }
-        umma_commit_2sm_a(acc1_full + 8 * buf);
-      };
-      auto g2 = [&](int i) {
-        const int buf = i & 1;
-        PK_TICK(2)
-        mbar_wait_a(z_full + 8 * buf, (i >> 1) & 1);   // the gate warps of both CTAs wrote z over acc1(buf), tcgen05.wait::st done
-        PK_TICK(3)
-        if (kResid == 0) {
-          mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-          PK_TICK(4)
-        }
-        tcgen05_fence_after();
-        // A from tensor memory: z_hi / z_lo of channels [32 h, 32 h + 32) sit in columns 32 h + [0, 16) / 32 h + [16, 32) of
-        // acc1(buf), one 32-bit column per channel pair, so K-step k (channels 16 k ..) starts at column 32 (k / 2) + 8 (k % 2)
-        const uint32_t za = tmem_base + buf * 128;
-        const uint32_t d2 = tmem_base + 256 + buf * 128;
-        const uint64_t b_hi = make_smem_desc_sw128(w2), b_lo = make_smem_desc_sw128(w2 + kFcWTile);
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          const uint32_t a_hi = za + 32 * (k >> 1) + 8 * (k & 1), a_lo = a_hi + 16;
-          umma_bf16_2sm_ts(d2, a_hi, b_hi + koff, idesc, kResid != 0 || k != 0);   // on top of the residual pass / preload (if any)
-          umma_bf16_2sm_ts(d2, a_lo, b_hi + koff, idesc, 1);
-          umma_bf16_2sm_ts(d2, a_hi, b_lo + koff, idesc, 1);
-        }
-        PK_TICK(5)
-        umma_commit_2sm_a(acc2_full + 8 * buf);
-      };
-      FcTileIter ti(p);
-      int b, m0;
-      int n_issued = 0, n_done = 0;
-      bool have = ti.next(b, m0);
-      if (have) g1(n_issued++);
-      while (have) {
-        const bool have_next = ti.next(b, m0);
-        if (have_next) g1(n_issued++);
-        g2(n_done++);
-        have = have_next;
       }
-      PK_TICK(6)
-      PK_TICK_FLUSH(8, 7)
-      if (kProf) atomicAdd(p.prof + 32, static_cast<unsigned long long>(n_done));
     }
-  } else if (warp < kPwgFirstGateWarp) {
-    // idle warps
-  } else if (warp < kPwgFirstGateWarp + kPwgGateWarps) {
-    // ------------------------------ gate warps (both CTAs, own TMEM lanes) ------------------------------
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t z_full_l = mapa_shared(z_full, 0);
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
-    float k_a, k_g;
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    FcTileIter ti(p);
-    int b, m0;
-    (void)r;
-    for (int i = 0; ti.next(b, m0); ++i) {
-      const int buf = i & 1;
-      PK_TICK(6)
-      if (kResidGate) {
-        // GEMM2's accumulator starts as [0 | x]: this thread's row, 64 channels, while GEMM1 of the tile is still in flight
-        const int trow = m0 + 128 * static_cast<int>(rank) + r;
-        const bool in = trow < p.t;
-        const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-        uint4 xh[8], xl[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          xh[q] = in ? __ldg(reinterpret_cast<const uint4*>(p.x_hi + row_off) + q) : make_uint4(0, 0, 0, 0);
-          xl[q] = in ? __ldg(reinterpret_cast<const uint4*>(p.x_lo + row_off) + q) : make_uint4(0, 0, 0, 0);
-        }
-        mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);     // this CTA's store warps have read tile i-2
-        tcgen05_fence_after();
-        const uint32_t acc2 = tmem_base + lane_base + 256 + buf * 128;
-        uint32_t f[32];
-#pragma unroll
-        for (int e = 0; e < 32; ++e) f[e] = 0u;
-        __syncwarp();
-        tmem_st_32x32(acc2, f);
-        tmem_st_32x32(acc2 + 32, f);
-        const uint32_t* wh = reinterpret_cast<const uint32_t*>(xh);
-        const uint32_t* wl = reinterpret_cast<const uint32_t*>(xl);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            f[2 * e] = __float_as_uint(__uint_as_float(wh[16 * h + e] << 16) + __uint_as_float(wl[16 * h + e] << 16));
-            f[2 * e + 1] = __float_as_uint(__uint_as_float(wh[16 * h + e] & 0xffff0000u) + __uint_as_float(wl[16 * h + e] & 0xffff0000u));
-          }
-          tmem_st_32x32(acc2 + 64 + 32 * h, f);
-        }
-        // (tcgen05.wait::st before the z_full arrive below covers these stores)
-      }
-      mbar_wait_a(acc1_full + 8 * buf, (i >> 1) & 1);
-      PK_TICK(0)
-      tcgen05_fence_after();
-      const uint32_t acc = tmem_base + lane_base + buf * 128;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float va[32], vb[32];
-        uint32_t zw[32];                          // [0, 16): z_hi of channels 32 half + (0 .. 31), [16, 32): z_lo
-        __syncwarp();
-        tmem_ld_32x32(acc + half * 32, va);
-        tmem_ld_32x32(acc + 64 + half * 32, vb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float z[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, p.gate_c[half * 32 + j + e]), 60.f));
-            const float e2 = ex2_approx(fmaf(vb[j + e], k_g, p.gate_c[64 + half * 32 + j + e]));
-            const float t1 = 1.f + e1;
-            z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
-          }
-          split2(z[0], z[1], zw[j / 2], zw[16 + j / 2]);
-          split2(z[2], z[3], zw[j / 2 + 1], zw[16 + j / 2 + 1]);
-        }
-        // over the a-columns this half has just been read from (the g-columns [64, 128) stay untouched until GEMM1 of tile i+2)
-        tmem_st_32x32(acc + half * 32, zw);
-      }
-      PK_TICK(1)
-      tmem_st_wait();                    // z is in tensor memory
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_relaxed_a(z_full_l + 8 * buf);
-      PK_TICK(3)
-    }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0 && leader) { PK_TICK_FLUSH(16, 7) }
   } else {
-    // ------------------------------ store warps (both CTAs) ------------------------------
-    const int sw = warp - kPwgFirstGateWarp - kPwgGateWarps;
-    const int quarter = warp & 3;
-    const int half = sw >> 2;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc2_empty_l = mapa_shared(acc2_empty, kResidGate ? rank : 0);
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tlast = clock64();
+    // ------------------------------ consumers: 64 samples per warpgroup ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rl = 16 * (warp & 3) + (lane >> 2);              // this thread's rows: rl and rl + 8 of the warpgroup's 64
+    const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, + 1
+    const float kSqrtHalf = 0.70710678118654752440f;
+    mbar_wait_a(w_bar, 0);
+    uint32_t it = 0;
     FcTileIter ti(p);
-    int b, m0;
-    bool have = ti.next(b, m0);
-    if (half == 0) {
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int tt = m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-        float* dst = p.skip + (static_cast<long long>(b) * p.t + tt) * 64;
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
+    int b, m0, half;
+    while (ti.next(b, m0, half)) {
+      const int mh = m0 + 128 * half;
+      float acc1[64], acc2[64];
+      for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
+        const int s = it % kFcStages;
+        mbar_wait_a(full_bar + 8 * s, (it / kFcStages) & 1);
+        const uint32_t st = smem + s * kFcStageBytes + wg * 64 * kSwizzleBytes;
+        const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kATile);
+        wgmma_fence();
+        if (j == 2) {                                          // one K-step: 16 frames of band table x P window
+          const uint64_t b_hi = make_smem_desc_sw128(pbuf), b_lo = make_smem_desc_sw128(pbuf + kATile);
+          wgmma_ss_n128(acc1, a_hi, b_hi, 1);
+          wgmma_ss_n128(acc1, a_lo, b_hi, 1);
+          wgmma_ss_n128(acc1, a_hi, b_lo, 1);
+        } else {
+          const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
+          const uint64_t b_hi = make_smem_desc_sw128(w1 + wj * 2 * kATile), b_lo = make_smem_desc_sw128(w1 + wj * 2 * kATile + kATile);
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
+          for (int k = 0; k < 4; ++k) {
+            wgmma_ss_n128(acc1, a_hi + desc_kstep(k), b_hi + desc_kstep(k), !(j == 0 && k == 0));
+            wgmma_ss_n128(acc1, a_lo + desc_kstep(k), b_hi + desc_kstep(k), 1);
+            wgmma_ss_n128(acc1, a_hi + desc_kstep(k), b_lo + desc_kstep(k), 1);
           }
-          if (tt < p.t) {
+        }
+        wgmma_commit();
+        if (j == kFcG1Chunks - 1) {
+          // GEMM2's accumulator starts as [0 | x]: x = hi + lo of this tile's own rows, from the centre-tap chunk
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              float* d4 = dst + pass * 32 + 4 * c;
-              if (p.skip_init) {
-                *reinterpret_cast<float4*>(d4) = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-              } else {
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d4), "f"(v[4 * c]), "f"(v[4 * c + 1]),
-                             "f"(v[4 * c + 2]), "f"(v[4 * c + 3]) : "memory");
-              }
+          for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int r = rl + 8 * hh;
+              const uint32_t off = r * kSwizzleBytes + ((((8 * jj + cq) >> 3) ^ (r & 7)) << 4) + (cq & 7) * 2;
+              const uint32_t xh = lds_u32(st + off), xl = lds_u32(st + kATile + off);
+              acc2[4 * jj + 2 * hh] = 0.f;
+              acc2[4 * jj + 2 * hh + 1] = 0.f;
+              acc2[32 + 4 * jj + 2 * hh] = __uint_as_float(xh << 16) + __uint_as_float(xl << 16);
+              acc2[32 + 4 * jj + 2 * hh + 1] = __uint_as_float(xh & 0xffff0000u) + __uint_as_float(xl & 0xffff0000u);
             }
           }
-          PK_TICK(5)
         }
-        PK_TICK(1)
-        have = ti.next(b, m0);
+        wgmma_wait<0>();
+        reg_fence(acc1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive_a(empty_bar + 8 * s);
       }
-    } else {
-      const float kSqrtHalf = 0.70710678118654752440f;
-      for (int i = 0; have; ++i) {
-        const int buf = i & 1;
-        const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
-        const int trow = m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-        const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-        const bool live = trow < len;
-        uint4 xh[4], xl[4];                       // kResidMma == false: 32 channels of this row's input, both planes
-        auto load_x = [&](int pass) {
+      // gate: z = tanh(a + ba) * sigmoid(g + bg) = (1 - e1) / ((1 + e1)(1 + e2)), e1 = exp(-2(a+ba)), e2 = exp(-(g+bg))
+      // (one reciprocal; the exp2 argument of e1 is clamped at 60 so that the product cannot overflow where z != 0).
+      // a column c and its g column 64 + c sit in the same thread (fragments j and j + 8).
+      uint32_t zh[16], zl[16];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            xh[q] = live ? __ldg(reinterpret_cast<const uint4*>(p.x_hi + row_off + pass * 32) + q) : make_uint4(0, 0, 0, 0);
-            xl[q] = live ? __ldg(reinterpret_cast<const uint4*>(p.x_lo + row_off + pass * 32) + q) : make_uint4(0, 0, 0, 0);
-          }
-        };
-        if (kResid == 0) load_x(0);               // issued before the wait: the latency hides behind GEMM2 of this tile
-        PK_TICK(6)
-        mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(0)
-        tcgen05_fence_after();
+      for (int jj = 0; jj < 8; ++jj) {
+        float z[4];
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          float v[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + 64 + pass * 32, v);
-          tmem_ld_wait();
-          PK_TICK(2)
-          if (pass == 1) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
-          }
-          if (kResid == 0) {
-            const uint32_t* wh = reinterpret_cast<const uint32_t*>(xh);
-            const uint32_t* wl = reinterpret_cast<const uint32_t*>(xl);
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              v[2 * e] += __uint_as_float(wh[e] << 16) + __uint_as_float(wl[e] << 16);
-              v[2 * e + 1] += __uint_as_float(wh[e] & 0xffff0000u) + __uint_as_float(wl[e] & 0xffff0000u);
-            }
-            if (pass == 0) load_x(1);
-          }
-          uint32_t oh[16], ol[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float y0 = live ? (v[2 * e] + p.out_b[pass * 32 + 2 * e]) * kSqrtHalf : 0.f;
-            const float y1 = live ? (v[2 * e + 1] + p.out_b[pass * 32 + 2 * e + 1]) * kSqrtHalf : 0.f;
-            split2(y0, y1, oh[e], ol[e]);
-          }
-          if (trow < p.t) {
-            st_global_v8(p.y_hi + row_off + pass * 32, oh);
-            st_global_v8(p.y_hi + row_off + pass * 32 + 16, oh + 8);
-            st_global_v8(p.y_lo + row_off + pass * 32, ol);
-            st_global_v8(p.y_lo + row_off + pass * 32 + 16, ol + 8);
-          }
-          PK_TICK(5)
+        for (int e = 0; e < 4; ++e) {
+          const int c = 8 * jj + cq + (e & 1);
+          const float e1 = ex2_approx(fminf(fmaf(acc1[4 * jj + e], p.k_a, p.gate_c[c]), 60.f));
+          const float e2 = ex2_approx(fmaf(acc1[32 + 4 * jj + e], p.k_g, p.gate_c[64 + c]));
+          const float t1 = 1.f + e1;
+          z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
         }
-        PK_TICK(1)
-        have = ti.next(b, m0);
+        split2(z[0], z[1], zh[2 * jj], zl[2 * jj]);            // row rl
+        split2(z[2], z[3], zh[2 * jj + 1], zl[2 * jj + 1]);    // row rl + 8
+      }
+      // GEMM2: [skip | out] += z W2, K = 64 = 4 K-steps; A fragment of K-step k = z column groups 2k, 2k + 1
+      const uint64_t b2_hi = make_smem_desc_sw128(w2), b2_lo = make_smem_desc_sw128(w2 + kATile);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t ah[4] = {zh[4 * k], zh[4 * k + 1], zh[4 * k + 2], zh[4 * k + 3]};
+        const uint32_t al[4] = {zl[4 * k], zl[4 * k + 1], zl[4 * k + 2], zl[4 * k + 3]};
+        wgmma_rs_n128(acc2, ah, b2_hi + desc_kstep(k), 1);
+        wgmma_rs_n128(acc2, al, b2_hi + desc_kstep(k), 1);
+        wgmma_rs_n128(acc2, ah, b2_lo + desc_kstep(k), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc2);
+      // stores: skip half -> fp32 skip sum (write or red.add), out half -> (out + b_out) * sqrt(1/2) as split planes
+      const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int trow = mh + wg * 64 + rl + 8 * hh;
+        if (trow < p.t) {
+          const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
+          const bool live = trow < len;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int c = 8 * jj + cq;
+            float* d2 = p.skip + row_off + c;
+            const float s0 = acc2[4 * jj + 2 * hh], s1 = acc2[4 * jj + 2 * hh + 1];
+            if (p.skip_init) *reinterpret_cast<float2*>(d2) = make_float2(s0, s1);
+            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d2), "f"(s0), "f"(s1) : "memory");
+            const float y0 = live ? (acc2[32 + 4 * jj + 2 * hh] + p.out_b[c]) * kSqrtHalf : 0.f;
+            const float y1 = live ? (acc2[32 + 4 * jj + 2 * hh + 1] + p.out_b[c + 1]) * kSqrtHalf : 0.f;
+            uint32_t oh, ol;
+            split2(y0, y1, oh, ol);
+            *reinterpret_cast<uint32_t*>(p.y_hi + row_off + c) = oh;
+            *reinterpret_cast<uint32_t*>(p.y_lo + row_off + c) = ol;
+          }
+        }
       }
     }
-    PK_TICK(6)
-    if (lane == 0 && quarter == 0 && leader) { PK_TICK_FLUSH(40 + half * 8, 7) }
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // neither CTA may free its TMEM / exit while the pair's MMAs can still touch it
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
   }
 }
-
 
 }  // namespace fc
 }  // namespace pk
@@ -571,7 +302,6 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
                a->u_rows >= a->u_end_base + 384 * a->batch, "bad compact band table layout");
   PK_CHECK_ARG(a->p_rows > 0 && a->p_row0 >= 0 && a->p_row0 + 128 <= a->p_rows && (a->p_ld % 8) == 0 && a->p_ld >= 64 && a->p_frames > 0 &&
                a->p_frames <= a->p_ld, "bad P plane geometry");
-  PK_CHECK_ARG(sm_count() >= 2, "needs at least one SM pair");
   CUtensorMap tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo;
   int rc;
   const uint64_t T = a->t, B = a->batch;
@@ -581,20 +311,15 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
   // P planes (batch, p_rows, p_ld): frames are the K axis; columns >= p_frames (and < 0) read as zero
   const uint64_t prow = a->p_rows, pld = a->p_ld;
   // (the extent is the padded row length p_ld >= 64: columns [p_frames, p_ld) hold zeros in memory, frames < 0 are out of bounds)
-  if ((rc = encode_tmap_bf16_planes(&tp, a->p_hi, a->p_lo, pld, prow, B, pld, prow * pld, 64))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&tp, a->p_hi, a->p_lo, pld, prow, B, pld, prow * pld, 128))) return rc;
   const uint64_t k1 = 5 * kChunkK;     // row pitch of the packed W1 (pk_pwg_residual_layer layout); only the 3 tap chunks are read
-  if ((rc = encode_tmap_bf16_3d(&tw1_hi, a->w1_hi, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 64))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw1_lo, a->w1_lo, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 64))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, 128, 1, 64, 0, 64))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, 64))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw1_hi, a->w1_hi, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 128))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw1_lo, a->w1_lo, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 128))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, 128, 1, 64, 0, 128))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, 128))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
     attr_set = true;
   }
   FcLayerArgs p;
@@ -609,23 +334,11 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
     p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
     p.out_b[i] = a->bias2[64 + i];
   }
-  p.x_hi = static_cast<const __nv_bfloat16*>(a->x_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->x_lo);
   p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
-  p.prof = static_cast<unsigned long long*>(a->prof);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int pair_tiles = ((a->t + 255) / 256) * a->batch;
-  const int grid = 2 * std::min(pair_tiles, sm_count() / 2);
-  static const int resid = [] {
-    const char* e = getenv("PK_PWG_RESID");
-    return e && strcmp(e, "ldg") == 0 ? 0 : e && strcmp(e, "gate") == 0 ? 2 : 1;
-  }();
-#define PK_FC_LAUNCH(PROF, RES) pwg_layer_fc_kernel<PROF, RES><<<grid, kPwgThreads, kFcSmem, st>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p)
-  if (p.prof != nullptr) {
-    if (resid == 0) PK_FC_LAUNCH(true, 0); else if (resid == 1) PK_FC_LAUNCH(true, 1); else PK_FC_LAUNCH(true, 2);
-  } else {
-    if (resid == 0) PK_FC_LAUNCH(false, 0); else if (resid == 1) PK_FC_LAUNCH(false, 1); else PK_FC_LAUNCH(false, 2);
-  }
-#undef PK_FC_LAUNCH
+  const int tiles = ((a->t + 255) / 256) * 2 * a->batch;
+  const int grid = std::min(tiles, sm_count());
+  pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

@@ -5,7 +5,7 @@
 #include <algorithm>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 

@@ -1,22 +1,21 @@
 // pk_waveflow_layer: one ResidualBlock.add_input of the WaveFlow inverse (reference parakeet/models/waveflow.py:248-285) as
-// ONE CTA-pair kernel - the row-by-row autoregressive path spends its time here (8 flows x 15 rows x 8 layers launches).
+// ONE kernel - the row-by-row autoregressive path spends its time here (8 flows x 15 rows x 8 layers launches).
 //
 //   a | g   = conv2d(ring of the last 3 rows, dilation 2^l along the width) + condition_proj(condition row) + biases
 //   z       = tanh(a) * sigmoid(g)
 //   res|skip= out_proj(z);   new row = row + res  -> next layer's ring slot (split planes);   skip (=|+=) skip
 //
 // It replaces, per layer, two pk_conv_gemm_ex launches (gate epilogue, wf_update epilogue), one fp32 read of the hoisted
-// condition projections (2C floats per position) and the fp32 state read-modify-write.  Structure = pwg_fc.cu:
-//   * M = 256 positions per pair tile (128 per CTA), cta_group::2 MMAs, N = 128 = a | g channels;
-//   * GEMM1 has 11 K-chunks: 3 width taps x 3 ring slots of 64 channels + the 80 condition channels (64 + 16).  K = 656 per
-//     output channel does not fit shared memory as a resident operand (168 KB per CTA with both planes), so every stage of
-//     the 4-deep ring carries the A chunk (32 KB: hi | lo) AND this CTA's 64 output channels of the weight chunk
-//     (16 KB: hi | lo, L2 resident: 360 KB per layer variant);
-//   * z goes back into tensor memory over the accumulator columns it was computed from and is GEMM2's A operand;
-//   * the residual add is a tensor-core pass of the centre-tap / newest-slot chunk with [0 | I] (no fp32 state tensor: the
-//     running row lives in the ring slot as hi + lo, 16 mantissa bits, re-split after every layer);
-//   * GEMM2's B operand is out_proj with its rows reordered to [skip | res] so that the accumulator halves line up with the
-//     two groups of store warps.
+// condition projections (2C floats per position) and the fp32 state read-modify-write.  Structure (shared with
+// pk_waveflow_flow below and with pwg.cu):
+//   * persistent CTAs over 128-position tiles, 384 threads: a producer warpgroup (one TMA lane) and two consumer warpgroups
+//     of 64 positions each;
+//   * GEMM1 has 11 K-chunks: 3 width taps x 3 ring slots of 64 channels + the 80 condition channels (64 + 16); every stage
+//     of a 2-deep ring carries the A chunk (32 KB: hi | lo) and the weight chunk for all 128 gate channels (32 KB), and
+//     out_proj follows as one more weight-only chunk;
+//   * the accumulators live in registers (wgmma), the gate runs on them in place and z is GEMM2's register A operand;
+//   * the residual add reads the newest row (hi + lo, 16 mantissa bits, re-split after every layer) from its ring slot;
+//   * out_proj's rows are ordered [skip | res] so that the accumulator halves line up with the two kinds of stores.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -25,47 +24,31 @@
 #include <mutex>
 
 #include "pk_host.h"
-#include "pk_sm100.cuh"
+#include "pk_sm90.cuh"
 
 namespace pk {
 namespace wf {
 
-constexpr int kC = 64;                                       // residual channels
+constexpr int kC = 64;                                       // residual channels of pk_waveflow_layer
 constexpr int kG = 128;                                      // gate channels (a | g) == out_proj outputs (skip | res)
 constexpr int kATile = 128 * kSwizzleBytes;                  // 16 KB: 128 positions x one 64-channel chunk of one plane
-constexpr int kWTile = 64 * kSwizzleBytes;                   // 8 KB: 64 output channels x one chunk of one plane
-constexpr int kStages = 4;
-constexpr int kStageBytes = 2 * kATile + 2 * kWTile;         // A hi | A lo | W hi | W lo
 constexpr int kChunks = 11;                                  // 9 conv chunks + 2 condition chunks
 constexpr int kW1Cols = kChunks * kChunkK;                   // 704: row length of the packed GEMM1 weight
-constexpr int kGateWarps = 4;
-constexpr int kStoreWarps = 8;
-constexpr int kFirstGateWarp = 4;
-constexpr int kThreads = (kFirstGateWarp + kGateWarps + kStoreWarps) * 32;
-constexpr int kSmem = kStages * kStageBytes + 2 * kWTile + kWTile + 1024 + 256;
-static_assert(kSmem <= 227 * 1024, "shared memory budget");
+constexpr int kConsumerThreads = 256;
+constexpr int kThreads = kConsumerThreads + 128;
+constexpr int kStages = 2;
 
-struct LayerArgs {
-  int batch, w, dil;
-  int resid_chunk;              // 3 + slot: the centre-tap chunk of the newest row's ring slot
-  int cond_ksteps_last;         // K-steps of the second condition chunk ((n_mels - 64 + 15) / 16)
-  float gate_c[128];            // pre-scaled biases of the gate (see the host code)
-  float out_b[128];             // out_proj bias in accumulator order: skip | res
-  float k_a, k_g;
-  float* skip;
-  int skip_init;
-  __nv_bfloat16* y_hi;          // next layer's ring planes (batch, w, y_ld), written at column y_col0; NULL on the last layer
-  __nv_bfloat16* y_lo;
-  int y_ld, y_col0;
-  unsigned long long* prof;
+// ring geometry for C residual channels: N = 2C gate channels (a | g per 64-channel block)
+template <int C>
+struct Geo {
+  static constexpr int kN = 2 * C;
+  static constexpr int kWBytes = 2 * kN * kSwizzleBytes;     // hi | lo of one weight chunk, all kN rows
+  static constexpr int kStageBytes = 2 * kATile + kWBytes;
+  static constexpr int kG1Chunks = 9 * (C / 64) + 2;
+  static constexpr int kG2Chunks = C / 64;
+  static constexpr int kSmem = kStages * kStageBytes + 1024 + 256;
+  static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
-
-#define PK_TICK(k)                                      \
-  if (kProf) {                                          \
-    const long long n_ = clock64();                     \
-    tacc[k] += n_ - tlast;                              \
-    tlast = n_;                                         \
-  }
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -85,350 +68,263 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t* w) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
+__device__ __forceinline__ uint32_t ld_cg_u32(const void* ptr) {
+  uint32_t v;
+  asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 ld_cg_f2(const float* ptr) {
+  float2 v;
+  asm volatile("ld.global.cg.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(ptr) : "memory");
+  return v;
+}
+// hi + lo of two consecutive bf16 split-plane elements
+__device__ __forceinline__ float2 ld_split2(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long long off) {
+  const uint32_t h = ld_cg_u32(hi + off), l = ld_cg_u32(lo + off);
+  return make_float2(__uint_as_float(h << 16) + __uint_as_float(l << 16),
+                     __uint_as_float(h & 0xffff0000u) + __uint_as_float(l & 0xffff0000u));
 }
 
-struct TileIter {   // 256-position tiles of the pair, per batch element; this CTA owns positions [m0 + 128 * rank, +128)
-  int idx, step, tiles_per_b, total;
-  __device__ TileIter(const LayerArgs& p)
-      : idx(static_cast<int>(blockIdx.x >> 1) - static_cast<int>(gridDim.x >> 1)), step(gridDim.x >> 1),
-        tiles_per_b((p.w + 255) >> 8), total(((p.w + 255) >> 8) * p.batch) {}
-  __device__ bool next(int& b, int& m0) {
-    idx += step;
-    if (idx >= total) return false;
-    b = idx / tiles_per_b;
-    m0 = (idx % tiles_per_b) * 256;
-    return true;
+template <int N>
+__device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (N == 128) wgmma_ss_n128(d, a, b, acc);
+  else wgmma_ss_n256(d, a, b, acc);
+}
+
+// Consumer side of one 128-position tile: GEMM1 over the G1 chunks of the ring, the gate in registers, then GEMM2 with z as
+// the register A operand, one 128-column output block [skip_blk | res_blk] at a time (64 accumulator registers), each block
+// handed to epi(blk, acc) without biases / residual.  The C / 64 out_proj K-chunks stay in their stages until the last block.
+// gc: pre-scaled gate biases in accumulator order; `it` is the running ring counter of this consumer.
+template <int C, class Epi>
+__device__ __forceinline__ void consume_tile(uint32_t smem, uint32_t full_bar, uint32_t empty_bar, uint32_t& it, int wg, int lane,
+                                             const float* gc, float k_a, float k_g, int cond_ksteps_last, Epi&& epi) {
+  using G = Geo<C>;
+  constexpr int N = G::kN;
+  const int cq = 2 * (lane & 3);
+  uint32_t zh[C / 64][16], zl[C / 64][16];
+  {
+    float acc1[C];
+    for (int j = 0; j < G::kG1Chunks; ++j, ++it) {
+      const int s = it % kStages;
+      mbar_wait_a(full_bar + 8 * s, (it / kStages) & 1);
+      const uint32_t st = smem + s * G::kStageBytes;
+      const uint64_t a_hi = make_smem_desc_sw128(st + wg * 64 * kSwizzleBytes), a_lo = make_smem_desc_sw128(st + kATile + wg * 64 * kSwizzleBytes);
+      const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kATile), b_lo = make_smem_desc_sw128(st + 2 * kATile + N * kSwizzleBytes);
+      const int ksteps = j == G::kG1Chunks - 1 ? cond_ksteps_last : 4;
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k) {
+        mma_ss<N>(acc1, a_hi + desc_kstep(k), b_hi + desc_kstep(k), !(j == 0 && k == 0));
+        mma_ss<N>(acc1, a_lo + desc_kstep(k), b_hi + desc_kstep(k), 1);
+        mma_ss<N>(acc1, a_hi + desc_kstep(k), b_lo + desc_kstep(k), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive_a(empty_bar + 8 * s);
+    }
+    // tanh(a) sigmoid(g) = (1 - e1) / ((1 + e1) (1 + e2)), e1 = exp(-2a) (clamped: e1 * e2 must stay finite), e2 = exp(-g);
+    // channel c of block blk: a in fragment 16 blk + c / 8, g in 16 blk + 8 + c / 8 (same thread)
+#pragma unroll
+    for (int blk = 0; blk < C / 64; ++blk) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        float z[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int c = 128 * blk + 8 * jj + cq + (e & 1);
+          const float e1 = ex2_approx(fminf(fmaf(acc1[4 * (16 * blk + jj) + e], k_a, gc[c]), 60.f));
+          const float e2 = ex2_approx(fminf(fmaf(acc1[4 * (16 * blk + 8 + jj) + e], k_g, gc[c + 64]), 60.f));
+          const float t1 = 1.f + e1;
+          z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
+        }
+        split2(z[0], z[1], zh[blk][2 * jj], zl[blk][2 * jj]);
+        split2(z[2], z[3], zh[blk][2 * jj + 1], zl[blk][2 * jj + 1]);
+      }
+    }
   }
+  const uint32_t s0 = it % kStages;                            // out_proj K-chunk kc (= z of channel block kc) is in stage
+  for (int kc = 0; kc < G::kG2Chunks; ++kc)                    // (it + kc) % kStages
+    mbar_wait_a(full_bar + 8 * ((s0 + kc) % kStages), ((it + kc) / kStages) & 1);
+#pragma unroll
+  for (int blk = 0; blk < C / 64; ++blk) {
+    float acc2[64];
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < G::kG2Chunks; ++kc) {
+      const uint32_t st = smem + ((s0 + kc) % kStages) * G::kStageBytes + 2 * kATile + blk * 128 * kSwizzleBytes;
+      const uint64_t b_hi = make_smem_desc_sw128(st), b_lo = make_smem_desc_sw128(st + N * kSwizzleBytes);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t ah[4] = {zh[kc][4 * k], zh[kc][4 * k + 1], zh[kc][4 * k + 2], zh[kc][4 * k + 3]};
+        const uint32_t al[4] = {zl[kc][4 * k], zl[kc][4 * k + 1], zl[kc][4 * k + 2], zl[kc][4 * k + 3]};
+        wgmma_rs_n128(acc2, ah, b_hi + desc_kstep(k), !(kc == 0 && k == 0));
+        wgmma_rs_n128(acc2, al, b_hi + desc_kstep(k), 1);
+        wgmma_rs_n128(acc2, ah, b_lo + desc_kstep(k), 1);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc2);
+    if (blk == C / 64 - 1) {
+      __syncwarp();
+      if (lane == 0)
+        for (int kc = 0; kc < G::kG2Chunks; ++kc) mbar_arrive_a(empty_bar + 8 * ((s0 + kc) % kStages));
+    }
+    epi(blk, acc2);
+  }
+  it += G::kG2Chunks;
+}
+
+struct LayerArgs {
+  int batch, w, dil, slot;
+  int cond_ksteps_last;         // K-steps of the second condition chunk ((n_mels - 64 + 15) / 16)
+  int tiles_per_b, total_tiles;
+  float gate_c[128];            // pre-scaled biases of the gate (see the host code)
+  float out_b[128];             // out_proj bias in accumulator order: skip | res
+  float k_a, k_g;
+  float* skip;
+  int skip_init;
+  const __nv_bfloat16* x_hi;    // this layer's ring planes (batch, w, 3C): the residual reads the newest slot
+  const __nv_bfloat16* x_lo;
+  __nv_bfloat16* y_hi;          // next layer's ring planes (batch, w, y_ld), written at column y_col0; NULL on the last layer
+  __nv_bfloat16* y_lo;
+  int y_ld, y_col0;
 };
 
-template <bool kProf>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 waveflow_layer_kernel(const __grid_constant__ CUtensorMap tm_x,    // ring planes (batch, w, 3C): 4-D, both planes in one box
                       const __grid_constant__ CUtensorMap tm_c,    // condition row planes (batch, w, n_mels)
-                      const __grid_constant__ CUtensorMap tm_w1,   // packed GEMM1 weight planes (128, 704), box = 64 rows
+                      const __grid_constant__ CUtensorMap tm_w1,   // packed GEMM1 weight planes (128, 704), box = 128 rows
                       const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
                       const LayerArgs p) {
+  using G = Geo<kC>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w2 = smem + kStages * kStageBytes;            // [hi | lo] this CTA's 64 rows of out_proj
-  const uint32_t ident = w2 + 2 * kWTile;                      // this CTA's 64 rows of [0 | I]
-  const uint32_t bars = ident + kWTile;
-  const uint32_t full_bar = bars;                              // [stages]   (leader's copy is the live one)
+  const uint32_t full_bar = smem + kStages * G::kStageBytes;   // [stages]
   const uint32_t empty_bar = full_bar + 8 * kStages;           // [stages]
-  const uint32_t acc1_full = empty_bar + 8 * kStages;          // [2]
-  const uint32_t acc2_full = acc1_full + 16;                   // [2]
-  const uint32_t acc2_empty = acc2_full + 16;                  // [2] leader
-  const uint32_t z_full = acc2_empty + 16;                     // [2] leader
-  const uint32_t w_bar = z_full + 16;
-  const uint32_t tmem_slot = w_bar + 8;
-
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_c); tma_prefetch_desc(&tm_w1);
     tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc1_full + 8 * i, 1);
-      mbar_init_a(acc2_full + 8 * i, 1); mbar_init_a(acc2_empty + 8 * i, 2 * kStoreWarps);
-      mbar_init_a(z_full + 8 * i, 2 * kGateWarps);
-    }
-    mbar_init_a(w_bar, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2sm_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 192) {
-    // this CTA's half of [0 | I]: rank 0 supplies accumulator columns 0..63 (skip half: nothing added), rank 1 columns
-    // 64..127 (row n = e_n: column 64 + n receives channel n of the newest row)
-    const int n = threadIdx.x - 128;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (rank == 1 && (n >> 3) == c) {
-        const uint32_t one = (n & 1) ? 0x3f800000u : 0x00003f80u;
-        const int wd = (n & 7) >> 1;
-        v.x = wd == 0 ? one : 0; v.y = wd == 1 ? one : 0; v.z = wd == 2 ? one : 0; v.w = wd == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_all();
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // barriers of both CTAs are initialised before any remote arrive / TMA credit
-  tcgen05_fence_after();
-  if (warp == 0 && lane == 0) {
-    mbar_arrive_expect_tx_a(w_bar, 2 * kWTile);
-    tma_load_3d_a(w2, &tm_w2_hi, w_bar, 0, 64 * rank, 0);
-    tma_load_3d_a(w2 + kWTile, &tm_w2_lo, w_bar, 0, 64 * rank, 0);
-    mbar_wait_a(w_bar, 0);
-  }
-  cluster_sync();                      // both halves of out_proj are in place before the leader's first GEMM2
-  const uint32_t tmem_base = lds_u32(tmem_slot);
+  __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------ TMA producer (both CTAs: own positions, own weight rows) ------------------------------
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
+      // ------------------------------ TMA producer ------------------------------
       uint32_t it = 0;
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      TileIter ti(p);
-      int b, m0;
-      while (ti.next(b, m0)) {
-        const int row0 = m0 + 128 * static_cast<int>(rank);
-        for (int j = 0; j < kChunks; ++j, ++it) {
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int b = tile / p.tiles_per_b, row0 = (tile % p.tiles_per_b) * 128;
+        for (int j = 0; j < G::kG1Chunks + G::kG2Chunks; ++j, ++it) {
           const int s = it % kStages;
           mbar_wait_a(empty_bar + 8 * s, ((it / kStages) & 1) ^ 1);
-          const uint32_t st = smem + s * kStageBytes;
-          const uint32_t fb = full_leader + 8 * s;
-          if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kStageBytes);       // the chunks of both CTAs
-          if (j < 9) {
-            const int tap = j / 3, slot = j - 3 * tap;
-            tma_load_4d_2sm_a(st, &tm_x, fb, slot * kC, row0 + (tap - 1) * p.dil, b, 0);   // rows outside [0, w) read as zero
-          } else {
-            tma_load_4d_2sm_a(st, &tm_c, fb, (j - 9) * kChunkK, row0, b, 0);               // columns >= n_mels read as zero
-          }
-          tma_load_4d_2sm_a(st + 2 * kATile, &tm_w1, fb, j * kChunkK, 64 * static_cast<int>(rank), 0, 0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(256, 128);
-      uint32_t it = 0;
-      long long tacc[4] = {0, 0, 0, 0};
-      long long tlast = clock64();
-      auto g1 = [&](int i) {
-        // acc1(i & 1): its previous user is tile i-2, whose GEMM2 (the last reader - z lives in the accumulator's own columns)
-        // was issued by this thread before this point; tcgen05.mma execute in issue order
-        const int buf = i & 1;
-        const uint32_t d = tmem_base + buf * 128;
-        for (int j = 0; j < kChunks; ++j, ++it) {
-          const int s = it % kStages;
-          PK_TICK(0)
-          mbar_wait_a(full_bar + 8 * s, (it / kStages) & 1);
-          PK_TICK(1)
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * kStageBytes;
-          const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kATile);
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kATile), b_lo = make_smem_desc_sw128(st + 2 * kATile + kWTile);
-          const int ksteps = j == kChunks - 1 ? p.cond_ksteps_last : 4;
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16_2sm(d, a_hi + koff, b_hi + koff, idesc, !(j == 0 && k == 0));
-            umma_bf16_2sm(d, a_lo + koff, b_hi + koff, idesc, 1);
-            umma_bf16_2sm(d, a_hi + koff, b_lo + koff, idesc, 1);
-          }
-          if (j == p.resid_chunk) {
-            // residual pass: acc2(i) = [0 | row_hi + row_lo] from the newest row's centre-tap tiles of both CTAs
-            mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-            PK_TICK(2)
-            tcgen05_fence_after();
-            const uint64_t b_id = make_smem_desc_sw128(ident);
-            const uint32_t d2 = tmem_base + 256 + buf * 128;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-              umma_bf16_2sm(d2, a_hi + koff, b_id + koff, idesc, k != 0);
-              umma_bf16_2sm(d2, a_lo + koff, b_id + koff, idesc, 1);
+          const uint32_t st = smem + s * G::kStageBytes;
+          const uint32_t fb = full_bar + 8 * s;
+          if (j < kChunks) {
+            mbar_arrive_expect_tx_a(fb, G::kStageBytes);
+            if (j < 9) {
+              const int tap = j / 3, slot = j - 3 * tap;
+              tma_load_4d_a(st, &tm_x, fb, slot * kC, row0 + (tap - 1) * p.dil, b, 0);   // rows outside [0, w) read as zero
+            } else {
+              tma_load_4d_a(st, &tm_c, fb, (j - 9) * kChunkK, row0, b, 0);               // columns >= n_mels read as zero
             }
+            tma_load_4d_a(st + 2 * kATile, &tm_w1, fb, j * kChunkK, 0, 0, 0);
+          } else {
+            mbar_arrive_expect_tx_a(fb, G::kWBytes);                                       // out_proj: weights only
+            tma_load_3d_a(st + 2 * kATile, &tm_w2_hi, fb, 0, 0, 0);
+            tma_load_3d_a(st + 2 * kATile + kG * kSwizzleBytes, &tm_w2_lo, fb, 0, 0, 0);
           }
-          umma_commit_2sm_a(empty_bar + 8 * s);
         }
-        umma_commit_2sm_a(acc1_full + 8 * buf);
-      };
-      auto g2 = [&](int i) {
-        const int buf = i & 1;
-        PK_TICK(0)
-        mbar_wait_a(z_full + 8 * buf, (i >> 1) & 1);   // the gate warps of both CTAs wrote z over acc1(buf)
-        PK_TICK(3)
-        tcgen05_fence_after();
-        // A from tensor memory: z_hi / z_lo of channels [32 h, 32 h + 32) sit in columns 32 h + [0, 16) / 32 h + [16, 32) of
-        // acc1(buf), one 32-bit column per channel pair: K-step k (channels 16 k ..) starts at column 32 (k / 2) + 8 (k % 2)
-        const uint32_t za = tmem_base + buf * 128;
-        const uint32_t d2 = tmem_base + 256 + buf * 128;
-        const uint64_t b_hi = make_smem_desc_sw128(w2), b_lo = make_smem_desc_sw128(w2 + kWTile);
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          const uint32_t a_hi = za + 32 * (k >> 1) + 8 * (k & 1), a_lo = a_hi + 16;
-          umma_bf16_2sm_ts(d2, a_hi, b_hi + koff, idesc, 1);   // on top of the residual pass
-          umma_bf16_2sm_ts(d2, a_lo, b_hi + koff, idesc, 1);
-          umma_bf16_2sm_ts(d2, a_hi, b_lo + koff, idesc, 1);
-        }
-        umma_commit_2sm_a(acc2_full + 8 * buf);
-      };
-      TileIter ti(p);
-      int b, m0;
-      int n_issued = 0, n_done = 0;
-      bool have = ti.next(b, m0);
-      if (have) g1(n_issued++);
-      while (have) {
-        const bool have_next = ti.next(b, m0);
-        if (have_next) g1(n_issued++);
-        g2(n_done++);
-        have = have_next;
       }
-      PK_TICK(0)
-      if (kProf) {
-        for (int k = 0; k < 4; ++k) atomicAdd(p.prof + k, static_cast<unsigned long long>(tacc[k]));
-        atomicAdd(p.prof + 4, static_cast<unsigned long long>(n_done));
-      }
-    }
-  } else if (warp < kFirstGateWarp) {
-    // idle warps
-  } else if (warp < kFirstGateWarp + kGateWarps) {
-    // ------------------------------ gate warps (both CTAs, own TMEM lanes) ------------------------------
-    const int quarter = warp & 3;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t z_full_l = mapa_shared(z_full, 0);
-    float k_a, k_g;
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    TileIter ti(p);
-    int b, m0;
-    for (int i = 0; ti.next(b, m0); ++i) {
-      const int buf = i & 1;
-      mbar_wait_a(acc1_full + 8 * buf, (i >> 1) & 1);
-      tcgen05_fence_after();
-      const uint32_t acc = tmem_base + lane_base + buf * 128;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float va[32], vb[32];
-        uint32_t zw[32];                          // [0, 16): z_hi of channels 32 half + (0 .. 31), [16, 32): z_lo
-        __syncwarp();
-        tmem_ld_32x32(acc + half * 32, va);
-        tmem_ld_32x32(acc + 64 + half * 32, vb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float z[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            // tanh(a) sigmoid(g) = (1 - e1) / ((1 + e1) (1 + e2)), e1 = exp(-2a) (clamped: e1 * e2 must stay finite), e2 = exp(-g)
-            const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, p.gate_c[half * 32 + j + e]), 60.f));
-            const float e2 = ex2_approx(fminf(fmaf(vb[j + e], k_g, p.gate_c[64 + half * 32 + j + e]), 60.f));
-            const float t1 = 1.f + e1;
-            z[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
-          }
-          split2(z[0], z[1], zw[j / 2], zw[16 + j / 2]);
-          split2(z[2], z[3], zw[j / 2 + 1], zw[16 + j / 2 + 1]);
-        }
-        // over the a-columns this half has just been read from (the g-columns [64, 128) stay untouched until GEMM1 of tile i+2)
-        tmem_st_32x32(acc + half * 32, zw);
-      }
-      tmem_st_wait();                    // z is in tensor memory
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_relaxed_a(z_full_l + 8 * buf);
     }
   } else {
-    // ------------------------------ store warps (both CTAs) ------------------------------
-    const int sw = warp - kFirstGateWarp - kGateWarps;
-    const int quarter = warp & 3;
-    const int half = sw >> 2;                 // 0: skip columns [0, 64), 1: new row columns [64, 128)
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc2_empty_l = mapa_shared(acc2_empty, 0);
-    TileIter ti(p);
-    int b, m0;
-    for (int i = 0; ti.next(b, m0); ++i) {
-      const int buf = i & 1;
-      const int row = m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-      const long long pos = static_cast<long long>(b) * p.w + row;
-      mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-      tcgen05_fence_after();
+    // ------------------------------ consumers ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rl = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int b = tile / p.tiles_per_b, row0 = (tile % p.tiles_per_b) * 128;
+      consume_tile<kC>(smem, full_bar, empty_bar, it, wg, lane, p.gate_c, p.k_a, p.k_g, p.cond_ksteps_last,
+                       [&](int, const float (&acc2)[64]) {
 #pragma unroll
-      for (int pass = 0; pass < 2; ++pass) {
-        float v[32];
-        __syncwarp();
-        tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + half * 64 + pass * 32, v);
-        tmem_ld_wait();
-        if (pass == 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
-        }
-        const float* ob = p.out_b + half * 64 + pass * 32;
-        if (row >= p.w) {
-          // positions past the end of the row: nothing to store
-        } else if (half == 0) {
-          float* dst = p.skip + pos * kC + pass * 32;
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = row0 + rl + 8 * hh;
+          if (row >= p.w) continue;                            // positions past the end of the row: nothing to store
+          const long long pos = static_cast<long long>(b) * p.w + row;
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float4 o = make_float4(v[4 * c] + ob[4 * c], v[4 * c + 1] + ob[4 * c + 1], v[4 * c + 2] + ob[4 * c + 2],
-                                         v[4 * c + 3] + ob[4 * c + 3]);
-            if (p.skip_init) {
-              *reinterpret_cast<float4*>(dst + 4 * c) = o;
-            } else {
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * c), "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w)
-                           : "memory");
+          for (int jj = 0; jj < 8; ++jj) {
+            const int c = 8 * jj + cq;
+            float* dst = p.skip + pos * kC + c;
+            const float o0 = acc2[4 * jj + 2 * hh] + p.out_b[c], o1 = acc2[4 * jj + 2 * hh + 1] + p.out_b[c + 1];
+            if (p.skip_init) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(o0), "f"(o1) : "memory");
+            if (p.y_hi != nullptr) {
+              const float2 x = ld_split2(p.x_hi, p.x_lo, pos * (3 * kC) + p.slot * kC + c);
+              uint32_t oh, ol;
+              split2(acc2[4 * (8 + jj) + 2 * hh] + p.out_b[64 + c] + x.x, acc2[4 * (8 + jj) + 2 * hh + 1] + p.out_b[64 + c + 1] + x.y, oh, ol);
+              const long long off = pos * p.y_ld + p.y_col0 + c;
+              *reinterpret_cast<uint32_t*>(p.y_hi + off) = oh;
+              *reinterpret_cast<uint32_t*>(p.y_lo + off) = ol;
             }
           }
-        } else if (p.y_hi != nullptr) {
-          uint32_t oh[16], ol[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) split2(v[2 * e] + ob[2 * e], v[2 * e + 1] + ob[2 * e + 1], oh[e], ol[e]);
-          const long long off = pos * p.y_ld + p.y_col0 + pass * 32;
-          st_global_v8(p.y_hi + off, oh);
-          st_global_v8(p.y_hi + off + 16, oh + 8);
-          st_global_v8(p.y_lo + off, ol);
-          st_global_v8(p.y_lo + off + 16, ol + 8);
         }
-      }
+      });
     }
-  }
-  tcgen05_fence_before();
-  cluster_sync();                      // neither CTA may free its TMEM / exit while the pair's MMAs can still touch it
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
   }
 }
 
 
 // ------------------------------------------------------------------------------------------------------------------------
-// pk_waveflow_flow: ALL row steps x layers of one Flow.inverse (:515-556) in ONE persistent launch.
+// pk_waveflow_flow: ALL row steps x layers of one Flow.inverse (:515-556) in ONE persistent launch, for 64 or 128 residual
+// channels (the reference's shipped config, examples/waveflow/config.py, has 128: gate channels a0 | g0 | a1 | g1, out_proj
+// rows skip0 | res0 | skip1 | res1, 64 each, so that every 64-channel block runs the 64-channel code).
 //
 // Layer-step s = (row step, layer) touches, for a 256-position tile, only the tiles m-1, m, m+1 of step s-1 (width dilation
 // <= 128, the row boundary - output_proj, inverse transform, input_proj - is pointwise), so the (G-1) x L steps run as a
-// DATAFLOW over tiles instead of (G-1) x (L+2) grid-wide launches: tile T = s * tiles_per_step + (b, m) is processed by pair
-// T mod n_pairs; its TMA producers first acquire the completion counters of the (up to) three tiles they read from; the store
-// warps publish a tile with a gpu-scope release once its rows are written.  All pairs are co-resident (the grid is sized by
-// cudaOccupancyMaxActiveClusters) and every pair walks its tiles in increasing T, so the lowest unfinished tile can always
-// run.  Gone with the launches: their prologues, the drain of each launch's last wave (400 pair tiles over 74 pairs = 5.4
-// waves, 10 % idle) and the separate row_out / input_proj passes - the last layer's skip warps finish the row in registers.
+// DATAFLOW over tiles instead of (G-1) x (L+2) grid-wide launches: tile T = s * tiles_per_step + (b, m) is processed by CTA
+// T mod grid (as two 128-position halves); its TMA producer first acquires the completion counters of the (up to) three
+// tiles it reads from; each consumer warp publishes its rows of a half with a gpu-scope release.  All CTAs are co-resident
+// (the grid is sized by the occupancy query) and every CTA walks its tiles in increasing T, so the lowest unfinished tile
+// can always run; a tile may wait for the CTA's own previous tile, which needs nothing more from the producer.  The last
+// layer's skip stores finish the row in registers (output_proj, inverse transform, next row's input_proj).
 // ------------------------------------------------------------------------------------------------------------------------
 constexpr int kMaxLayers = 8;
 constexpr int kMaxGroup = 16;
-constexpr unsigned kTileDone = 2 * kStoreWarps;              // arrivals on a tile's counter: the store warps of both CTAs
+constexpr unsigned kTileDone = 2 * kConsumerThreads / 32;    // arrivals on a tile's counter: every consumer warp, per half
 
+template <int C>
 struct FlowArgs {
-  CUtensorMap tm_x[kMaxLayers];          // ring planes of each layer (batch, w, 192)
-  CUtensorMap tm_w1[kMaxLayers][3];      // GEMM1 weight planes per layer and row-step variant
-  CUtensorMap tm_w2[kMaxLayers];         // out_proj planes (128, 64): skip | res
+  CUtensorMap tm_x[kMaxLayers];          // ring planes of each layer (batch, w, 3C)
+  CUtensorMap tm_w1[kMaxLayers][3];      // GEMM1 weight planes per layer and row-step variant, box = all 2C rows
+  CUtensorMap tm_w2[kMaxLayers];         // out_proj planes (2C, C): [skip | res] per block
   CUtensorMap tm_c;                      // condition planes as (batch * n_group, w, n_mels): one row of one utterance per index
   int batch, w, n_layers, n_rows, n_group, tiles_per_b, tiles_per_step, total_tiles, cond_ksteps_last;
-  int serial;                            // 1: GEMM2(i) is issued before GEMM1(i+1) (tiny problems, see the host code)
   int cmap[kMaxGroup];                   // condition row (after the flows' permutations) of row step i
-  float gate_c[kMaxLayers][128];
-  float out_b[kMaxLayers][128];
-  float in_w[kC], in_b[kC];              // input_proj (1 -> 64)
-  float po_w[2 * kC], po_b[2];           // output_proj (64 -> logs, b)
+  float gate_c[kMaxLayers][2 * C];       // accumulator order, pre-scaled
+  float out_b[kMaxLayers][2 * C];
+  float in_w[C], in_b[C];                // input_proj (1 -> C)
+  float po_w[2 * C], po_b[2];            // output_proj (C -> logs, b)
   float k_a, k_g;
-  float* skip;
+  float* skip;                           // (batch, w, C)
   const float* z;                        // (batch, n_group, w) rows of this flow's input
   float* x;                              // (batch, n_group, w) rows of its output; row 0 is filled by the caller
   __nv_bfloat16* ring_hi[kMaxLayers];
   __nv_bfloat16* ring_lo[kMaxLayers];
   unsigned* flags;                       // [total_tiles] completion counters, zeroed by the caller
-  unsigned long long* prof;
 };
 
 struct FlowTile {
   int s, l, r, b, m0, mt;
-  __device__ void decode(const FlowArgs& p, int t) {
+  template <class A>
+  __device__ void decode(const A& p, int t) {
     s = t / p.tiles_per_step;
     const int rem = t - s * p.tiles_per_step;
     r = s / p.n_layers;
@@ -439,10 +335,6 @@ struct FlowTile {
   }
 };
 
-// GEMM1 chunk order: the centre tap comes last among the taps - its newest-slot chunk also feeds the residual pass, which
-// needs GEMM2's accumulator of tile i-2 back from the store warps (the later, the more slack)
-__device__ __forceinline__ int chunk_tap(int j) { return j < 3 ? 0 : j < 6 ? 2 : 1; }
-
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* ptr) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
@@ -450,11 +342,6 @@ __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* ptr) {
 }
 __device__ __forceinline__ void red_release_gpu_inc(unsigned* ptr) {
   asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ptr) : "memory");
-}
-__device__ __forceinline__ float4 ld_cg_f4(const float* ptr) {
-  float4 v;
-  asm volatile("ld.global.cg.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr) : "memory");
-  return v;
 }
 __device__ __forceinline__ void wait_tile_done(const unsigned* flag) {
   const long long t0 = clock64();
@@ -467,755 +354,157 @@ __device__ __forceinline__ void wait_tile_done(const unsigned* flag) {
   }
 }
 
-template <bool kProf>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-waveflow_flow_kernel(const __grid_constant__ FlowArgs p) {
+template <int C>
+__global__ void __launch_bounds__(kThreads, 1)
+waveflow_flow_kernel(const __grid_constant__ FlowArgs<C> p) {
+  using G = Geo<C>;
+  constexpr int kPer = C / 64;                                 // 64-channel blocks
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w2 = smem + kStages * kStageBytes;            // [hi | lo] this CTA's 64 rows of the current out_proj
-  const uint32_t ident = w2 + 2 * kWTile;
-  const uint32_t bars = ident + kWTile;
-  const uint32_t full_bar = bars;                              // [stages]   (leader's copy is the live one)
+  const uint32_t full_bar = smem + kStages * G::kStageBytes;   // [stages]
   const uint32_t empty_bar = full_bar + 8 * kStages;           // [stages]
-  const uint32_t acc1_full = empty_bar + 8 * kStages;          // [2]
-  const uint32_t acc2_full = acc1_full + 16;                   // [2]
-  const uint32_t acc2_empty = acc2_full + 16;                  // [2] leader
-  const uint32_t z_full = acc2_empty + 16;                     // [2] leader
-  const uint32_t w2_full = z_full + 16;                        // leader: both halves of out_proj of the next step landed
-  const uint32_t w2_empty = w2_full + 8;                       // both: the GEMM2s reading the previous out_proj are complete
-  const uint32_t tmem_slot = w2_empty + 8;
-
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = static_cast<int>(blockIdx.x >> 1), n_pairs = static_cast<int>(gridDim.x >> 1);
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init_a(acc1_full + 8 * i, 1);
-      mbar_init_a(acc2_full + 8 * i, 1); mbar_init_a(acc2_empty + 8 * i, 2 * kStoreWarps);
-      mbar_init_a(z_full + 8 * i, 2 * kGateWarps);
-    }
-    mbar_init_a(w2_full, 1); mbar_init_a(w2_empty, 1);
+  if (threadIdx.x == kConsumerThreads) {
+    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2sm_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 192) {
-    const int n = threadIdx.x - 128;     // [0 | I], as in waveflow_layer_kernel
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (rank == 1 && (n >> 3) == c) {
-        const uint32_t one = (n & 1) ? 0x3f800000u : 0x00003f80u;
-        const int wd = (n & 7) >> 1;
-        v.x = wd == 0 ? one : 0; v.y = wd == 1 ? one : 0; v.z = wd == 2 ? one : 0; v.w = wd == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_all();
-  }
-  tcgen05_fence_before();
-  cluster_sync();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = lds_u32(tmem_slot);
+  __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ------------------------------ TMA producer (both CTAs: own positions, own weight rows) ------------------------------
-      uint32_t it = 0;
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      const uint32_t w2_full_leader = mapa_shared(w2_full, 0);
-      int n_w2 = 0;            // out_proj loads issued so far
-      int pend = -1;           // layer whose out_proj is loaded once the GEMM2s of the previous step are known to be complete
-      int prev_s = -1;
-      auto load_w2 = [&](int l) {
-        if (n_w2 > 0) mbar_wait_a(w2_empty, (n_w2 - 1) & 1);
-        if (leader) mbar_arrive_expect_tx_a(w2_full, 2 * 2 * kWTile);
-        tma_load_4d_2sm_a(w2, &p.tm_w2[l], w2_full_leader, 0, 64 * static_cast<int>(rank), 0, 0);
-        ++n_w2;
-      };
-      FlowTile t;
-      for (int T = pair; T < p.total_tiles; T += n_pairs) {
-        t.decode(p, T);
-        if (t.s > 0) {
-          // the rows this tile reads were written by tiles mt-1 .. mt+1 of the previous step (other pairs, generic-proxy stores)
-          const unsigned* f = p.flags + (T - p.tiles_per_step);
-          const bool lo = t.mt > 0, hi = t.mt + 1 < p.tiles_per_b;
-          const bool ready = (!lo || ld_acquire_gpu(f - 1) >= kTileDone) && ld_acquire_gpu(f) >= kTileDone &&
-                             (!hi || ld_acquire_gpu(f + 1) >= kTileDone);
-          if (!ready) {
-            // a tile this one waits for may be the pair's own previous tile, which cannot finish without its out_proj
-            if (pend >= 0) {
-              load_w2(pend);
-              pend = -1;
-            }
-            if (lo) wait_tile_done(f - 1);
-            wait_tile_done(f);
-            if (hi) wait_tile_done(f + 1);
-          }
-          fence_proxy_async_all();       // ... and are read here through the async proxy
-        }
-        const int row0 = t.m0 + 128 * static_cast<int>(rank);
-        const int variant = (t.r + 1) % 3;                     // row step i = r + 1
-        const int crow = t.b * p.n_group + p.cmap[t.r + 1];
-        if (prev_s < 0) load_w2(t.l);
-        for (int j = 0; j < kChunks; ++j, ++it) {
-          const int s = it % kStages;
-          mbar_wait_a(empty_bar + 8 * s, ((it / kStages) & 1) ^ 1);
-          if (j == 4 && pend >= 0) {     // GEMM1 of this tile has started, so GEMM2 of the tile before the previous one is complete
-            load_w2(pend);
-            pend = -1;
-          }
-          const uint32_t st = smem + s * kStageBytes;
-          const uint32_t fb = full_leader + 8 * s;
-          if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kStageBytes);
-          if (j < 9) {
-            const int tap = chunk_tap(j), sl = j % 3;
-            tma_load_4d_2sm_a(st, &p.tm_x[t.l], fb, sl * kC, row0 + (tap - 1) * (1 << t.l), t.b, 0);
-            tma_load_4d_2sm_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, (3 * tap + sl) * kChunkK, 64 * static_cast<int>(rank), 0, 0);
-          } else {
-            tma_load_4d_2sm_a(st, &p.tm_c, fb, (j - 9) * kChunkK, row0, crow, 0);
-            tma_load_4d_2sm_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, j * kChunkK, 64 * static_cast<int>(rank), 0, 0);
-          }
-        }
-        if (prev_s >= 0 && t.s != prev_s) pend = t.l;
-        prev_s = t.s;
-      }
-      if (pend >= 0) load_w2(pend);
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer (leader CTA only) ------------------------------
-      constexpr uint32_t idesc = make_idesc_bf16_f32(256, 128);
-      uint32_t it = 0;
-      long long tacc[4] = {0, 0, 0, 0};
-      long long tlast = clock64();
-      int n_w2 = 0;
-      auto g1 = [&](int i, const FlowTile& t) {
-        const int buf = i & 1;
-        const uint32_t d = tmem_base + buf * 128;
-        const int resid_chunk = 6 + t.r % 3;       // centre tap (chunks 6..8), ring slot of the newest row
-        for (int j = 0; j < kChunks; ++j, ++it) {
-          const int s = it % kStages;
-          PK_TICK(0)
-          mbar_wait_a(full_bar + 8 * s, (it / kStages) & 1);
-          PK_TICK(1)
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * kStageBytes;
-          const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kATile);
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kATile), b_lo = make_smem_desc_sw128(st + 2 * kATile + kWTile);
-          const int ksteps = j == kChunks - 1 ? p.cond_ksteps_last : 4;
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16_2sm(d, a_hi + koff, b_hi + koff, idesc, !(j == 0 && k == 0));
-            umma_bf16_2sm(d, a_lo + koff, b_hi + koff, idesc, 1);
-            umma_bf16_2sm(d, a_hi + koff, b_lo + koff, idesc, 1);
-          }
-          if (j == resid_chunk) {
-            mbar_wait_a(acc2_empty + 8 * buf, ((i >> 1) & 1) ^ 1);
-            PK_TICK(2)
-            tcgen05_fence_after();
-            const uint64_t b_id = make_smem_desc_sw128(ident);
-            const uint32_t d2 = tmem_base + 256 + buf * 128;
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-              umma_bf16_2sm(d2, a_hi + koff, b_id + koff, idesc, k != 0);
-              umma_bf16_2sm(d2, a_lo + koff, b_id + koff, idesc, 1);
-            }
-          }
-          umma_commit_2sm_a(empty_bar + 8 * s);
-        }
-        umma_commit_2sm_a(acc1_full + 8 * buf);
-      };
-      auto g2 = [&](int i, bool new_w2, bool release_w2) {
-        const int buf = i & 1;
-        PK_TICK(0)
-        if (new_w2) {
-          mbar_wait_a(w2_full, n_w2 & 1);
-          ++n_w2;
-        }
-        mbar_wait_a(z_full + 8 * buf, (i >> 1) & 1);
-        PK_TICK(3)
-        tcgen05_fence_after();
-        const uint32_t za = tmem_base + buf * 128;
-        const uint32_t d2 = tmem_base + 256 + buf * 128;
-        const uint64_t b_hi = make_smem_desc_sw128(w2), b_lo = make_smem_desc_sw128(w2 + kWTile);
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-          const uint32_t a_hi = za + 32 * (k >> 1) + 8 * (k & 1), a_lo = a_hi + 16;
-          umma_bf16_2sm_ts(d2, a_hi, b_hi + koff, idesc, 1);
-          umma_bf16_2sm_ts(d2, a_lo, b_hi + koff, idesc, 1);
-          umma_bf16_2sm_ts(d2, a_hi, b_lo + koff, idesc, 1);
-        }
-        if (release_w2) umma_commit_2sm_a(w2_empty);   // the next tile belongs to another step: its out_proj may replace this one
-        umma_commit_2sm_a(acc2_full + 8 * buf);
-      };
-      FlowTile cur, nxt;
-      int T = pair;
-      bool have = T < p.total_tiles;
-      int i = 0;
-      bool cur_new = true;
-      if (have) {
-        cur.decode(p, T);
-        g1(0, cur);
-      }
-      while (have) {
-        const int Tn = T + n_pairs;
-        const bool have_next = Tn < p.total_tiles;
-        bool next_new = false;
-        if (have_next) {
-          nxt.decode(p, Tn);
-          next_new = nxt.s != cur.s;
-          if (!p.serial) g1(i + 1, nxt);           // GEMM1 of the next tile covers the gate warps' latency on this one
-        }
-        g2(i, cur_new, have_next && next_new);
-        if (have_next && p.serial) g1(i + 1, nxt);
-        cur = nxt; cur_new = next_new; T = Tn; have = have_next; ++i;
-      }
-      PK_TICK(0)
-      if (kProf) {
-        for (int k = 0; k < 4; ++k) atomicAdd(p.prof + k, static_cast<unsigned long long>(tacc[k]));
-        atomicAdd(p.prof + 4, static_cast<unsigned long long>(i));
-      }
-    }
-  } else if (warp < kFirstGateWarp) {
-    // idle warps
-  } else if (warp < kFirstGateWarp + kGateWarps) {
-    // ------------------------------ gate warps (both CTAs, own TMEM lanes) ------------------------------
-    const int quarter = warp & 3;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t z_full_l = mapa_shared(z_full, 0);
-    float k_a, k_g;
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    FlowTile t;
-    int i = 0;
-    for (int T = pair; T < p.total_tiles; T += n_pairs, ++i) {
-      t.decode(p, T);
-      const float* gc = p.gate_c[t.l];
-      const int buf = i & 1;
-      mbar_wait_a(acc1_full + 8 * buf, (i >> 1) & 1);
-      tcgen05_fence_after();
-      const uint32_t acc = tmem_base + lane_base + buf * 128;
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float va[32], vb[32];
-        uint32_t zw[32];
-        __syncwarp();
-        tmem_ld_32x32(acc + half * 32, va);
-        tmem_ld_32x32(acc + 64 + half * 32, vb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float zz[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, gc[half * 32 + j + e]), 60.f));
-            const float e2 = ex2_approx(fminf(fmaf(vb[j + e], k_g, gc[64 + half * 32 + j + e]), 60.f));
-            const float t1 = 1.f + e1;
-            zz[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
-          }
-          split2(zz[0], zz[1], zw[j / 2], zw[16 + j / 2]);
-          split2(zz[2], zz[3], zw[j / 2 + 1], zw[16 + j / 2 + 1]);
-        }
-        tmem_st_32x32(acc + half * 32, zw);
-      }
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_relaxed_a(z_full_l + 8 * buf);
-    }
-  } else {
-    // ------------------------------ store warps (both CTAs) ------------------------------
-    const int sw = warp - kFirstGateWarp - kGateWarps;
-    const int quarter = warp & 3;
-    const int half = sw >> 2;                 // 0: skip columns [0, 64), 1: new row columns [64, 128)
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc2_empty_l = mapa_shared(acc2_empty, 0);
-    FlowTile t;
-    int i = 0;
-    for (int T = pair; T < p.total_tiles; T += n_pairs, ++i) {
-      t.decode(p, T);
-      const int buf = i & 1;
-      const int row = t.m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-      const long long pos = static_cast<long long>(t.b) * p.w + row;
-      const bool last_layer = t.l == p.n_layers - 1;
-      const bool live = row < p.w;
-      const float* ob = p.out_b[t.l] + half * 64;
-      mbar_wait_a(acc2_full + 8 * buf, (i >> 1) & 1);
-      tcgen05_fence_after();
-      const bool idle = half == 1 && last_layer;       // the residual half of the last layer feeds nothing
-      float v[64];
-      __syncwarp();
-      if (!idle) {
-        // both halves of this warp's 64 columns first, so that the accumulator goes back to the issuer before any store
-        tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + half * 64, v);
-        tmem_ld_32x32(tmem_base + lane_base + 256 + buf * 128 + half * 64 + 32, v + 32);
-        tmem_ld_wait();
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l + 8 * buf);
-      if (idle || !live) {
-        // nothing to store: the last layer's residual half, or positions past the end of the row
-      } else if (half == 0) {
-        float* dst = p.skip + pos * kC;
-        float s0 = 0.f, s1 = 0.f;                        // output_proj (last layer)
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          float4 o = make_float4(v[4 * c] + ob[4 * c], v[4 * c + 1] + ob[4 * c + 1], v[4 * c + 2] + ob[4 * c + 2],
-                                 v[4 * c + 3] + ob[4 * c + 3]);
-          if (last_layer) {
-            // the sum of the skips is complete here: output_proj in registers instead of a last read-modify-write
-            if (p.n_layers > 1) {
-              const float4 a = ld_cg_f4(dst + 4 * c);
-              o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-            }
-            const float* w0 = p.po_w + 4 * c;
-            s0 = fmaf(w0[0], o.x, fmaf(w0[1], o.y, fmaf(w0[2], o.z, fmaf(w0[3], o.w, s0))));
-            s1 = fmaf(w0[kC], o.x, fmaf(w0[kC + 1], o.y, fmaf(w0[kC + 2], o.z, fmaf(w0[kC + 3], o.w, s1))));
-          } else if (t.l == 0) {
-            *reinterpret_cast<float4*>(dst + 4 * c) = o;
-          } else {
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * c), "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w)
-                         : "memory");
-          }
-        }
-        if (last_layer) {
-          // Flow._inverse_transform_row (:505-510) and, for the next row step, Flow.input_proj (:437-442) into layer 0's ring
-          const int irow = t.r + 1;
-          const long long xi = (static_cast<long long>(t.b) * p.n_group + irow) * p.w + row;
-          const float logs = s0 + p.po_b[0], bb = s1 + p.po_b[1];
-          const float xn = (__ldg(p.z + xi) - bb) * expf(-logs);
-          p.x[xi] = xn;
-          if (irow + 1 < p.n_group) {
-            const long long off = pos * (3 * kC) + (irow % 3) * kC;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              uint32_t oh[8], ol[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const int c = 16 * q + 2 * e;
-                split2(fmaf(p.in_w[c], xn, p.in_b[c]), fmaf(p.in_w[c + 1], xn, p.in_b[c + 1]), oh[e], ol[e]);
-              }
-              st_global_v8(p.ring_hi[0] + off + 16 * q, oh);
-              st_global_v8(p.ring_lo[0] + off + 16 * q, ol);
-            }
-          }
-        }
-      } else {
-        const long long off = pos * (3 * kC) + (t.r % 3) * kC;
-        __nv_bfloat16* yh = p.ring_hi[t.l + 1];
-        __nv_bfloat16* yl = p.ring_lo[t.l + 1];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint32_t oh[8], ol[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int c = 16 * q + 2 * e;
-            split2(v[c] + ob[c], v[c + 1] + ob[c + 1], oh[e], ol[e]);
-          }
-          st_global_v8(yh + off + 16 * q, oh);
-          st_global_v8(yl + off + 16 * q, ol);
-        }
-      }
-      // publish the tile: this warp's rows are written (generic proxy) -> visible to the async-proxy reads of the consumers
-      __syncwarp();
-      if (lane == 0) {
-        fence_proxy_async_all();
-        __threadfence();
-        red_release_gpu_inc(p.flags + T);
-      }
-    }
-  }
-  tcgen05_fence_before();
-  cluster_sync();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------------
-// 128 residual channels (examples/waveflow/config.py): the same dataflow over tiles, with the channel dimension as TWO blocks
-// of 64.  Gate channels are ordered a0 | g0 | a1 | g1 (64 each) and out_proj rows skip0 | res0 | skip1 | res1, so one N = 256
-// MMA fills both blocks and the gate / store warps run the 64-channel code once per block.  Both accumulators take 256
-// columns each: they are single-buffered and a pair finishes tile i (GEMM1 -> gate -> GEMM2) before it starts tile i + 1 -
-// GEMM1 alone is 240 MMAs here, the exposed gate latency is ~10 % of a tile.  K = 9 x 128 + 80: 20 chunks of GEMM1, each
-// stage = A chunk (32 KB) + this CTA's 128 rows of the weight chunk (32 KB), 3 stages; out_proj (K = 128) follows as two
-// weight-only chunks through the same ring.
-// ------------------------------------------------------------------------------------------------------------------------
-namespace c128 {
-constexpr int kCh = 128;
-constexpr int kStages3 = 3;
-constexpr int kWBytes = 2 * kATile;                          // hi | lo of this CTA's 128 weight rows of one chunk
-constexpr int kStage = 2 * kATile + kWBytes;                 // 64 KB
-constexpr int kG1Chunks = 20;                                // 18 conv chunks + 2 condition chunks
-constexpr int kG2Chunks = 2;
-constexpr int kW1Cols128 = kG1Chunks * kChunkK;              // 1280
-constexpr int kSmem128 = kStages3 * kStage + kWTile + 1024 + 256;
-static_assert(kSmem128 <= 227 * 1024, "shared memory budget");
-
-struct Flow128Args {
-  CUtensorMap tm_x[kMaxLayers];          // ring planes (batch, w, 384)
-  CUtensorMap tm_w1[kMaxLayers][3];      // (256, 1280) planes, box 128 rows
-  CUtensorMap tm_w2[kMaxLayers];         // (256, 128) planes, box 128 rows
-  CUtensorMap tm_c;
-  int batch, w, n_layers, n_rows, n_group, tiles_per_b, tiles_per_step, total_tiles, cond_ksteps_last;
-  int cmap[kMaxGroup];
-  float gate_c[kMaxLayers][256];         // accumulator order a0 | g0 | a1 | g1, pre-scaled
-  float out_b[kMaxLayers][256];          // skip0 | res0 | skip1 | res1
-  float in_w[kCh], in_b[kCh];
-  float po_w[2 * kCh], po_b[2];
-  float k_a, k_g;
-  float* skip;                           // (batch, w, 128)
-  const float* z;
-  float* x;
-  __nv_bfloat16* ring_hi[kMaxLayers];
-  __nv_bfloat16* ring_lo[kMaxLayers];
-  unsigned* flags;
-};
-
-struct Tile128 {
-  int s, l, r, b, m0, mt;
-  __device__ void decode(const Flow128Args& p, int t) {
-    s = t / p.tiles_per_step;
-    const int rem = t - s * p.tiles_per_step;
-    r = s / p.n_layers;
-    l = s - r * p.n_layers;
-    b = rem / p.tiles_per_b;
-    mt = rem - b * p.tiles_per_b;
-    m0 = mt * 256;
-  }
-};
-
-// GEMM1 chunk j < 18 -> (tap, ring slot, channel half); the centre tap comes last (its newest-slot chunks feed the residual pass)
-__device__ __forceinline__ void chunk_of(int j, int& tap, int& slot, int& half) {
-  const int t3 = j / 6, rem = j - 6 * t3;
-  tap = t3 == 0 ? 0 : t3 == 1 ? 2 : 1;
-  slot = rem >> 1;
-  half = rem & 1;
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-waveflow_flow128_kernel(const __grid_constant__ Flow128Args p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t ident = smem + kStages3 * kStage;             // this CTA's 64 rows of [0 | I] (N = 128 residual pass)
-  const uint32_t bars = ident + kWTile;
-  const uint32_t full_bar = bars;                              // [3] leader
-  const uint32_t empty_bar = full_bar + 8 * kStages3;          // [3]
-  const uint32_t acc1_full = empty_bar + 8 * kStages3;
-  const uint32_t acc2_full = acc1_full + 8;
-  const uint32_t acc2_empty = acc2_full + 8;                   // leader
-  const uint32_t z_full = acc2_empty + 8;                      // [2] leader: z of channel block 0 / 1 is in tensor memory
-  const uint32_t tmem_slot = z_full + 16;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = static_cast<int>(blockIdx.x >> 1), n_pairs = static_cast<int>(gridDim.x >> 1);
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < kStages3; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 1); }
-    mbar_init_a(acc1_full, 1);
-    mbar_init_a(acc2_full, 1);
-    mbar_init_a(acc2_empty, 2 * kStoreWarps);
-    mbar_init_a(z_full, 2 * kGateWarps);
-    mbar_init_a(z_full + 8, 2 * kGateWarps);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm_a<512>(tmem_slot);
-  if (threadIdx.x >= 128 && threadIdx.x < 192) {
-    const int n = threadIdx.x - 128;     // [0 | I] over the pair: rank 1's rows put channel n into column 64 + n of the block
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (rank == 1 && (n >> 3) == c) {
-        const uint32_t one = (n & 1) ? 0x3f800000u : 0x00003f80u;
-        const int wd = (n & 7) >> 1;
-        v.x = wd == 0 ? one : 0; v.y = wd == 1 ? one : 0; v.z = wd == 2 ? one : 0; v.w = wd == 3 ? one : 0;
-      }
-      sts_u4(ident + n * kSwizzleBytes + ((c ^ (n & 7)) * 16), v);
-    }
-    fence_proxy_async_all();
-  }
-  tcgen05_fence_before();
-  cluster_sync();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = lds_u32(tmem_slot);
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
       // ------------------------------ TMA producer ------------------------------
       uint32_t it = 0;
-      const uint32_t full_leader = mapa_shared(full_bar, 0);
-      Tile128 t;
-      for (int T = pair; T < p.total_tiles; T += n_pairs) {
+      FlowTile t;
+      for (int T = blockIdx.x; T < p.total_tiles; T += gridDim.x) {
         t.decode(p, T);
         if (t.s > 0) {
+          // the rows this tile reads were written by tiles mt-1 .. mt+1 of the previous step (generic-proxy stores) ...
           const unsigned* f = p.flags + (T - p.tiles_per_step);
           if (t.mt > 0) wait_tile_done(f - 1);
           wait_tile_done(f);
           if (t.mt + 1 < p.tiles_per_b) wait_tile_done(f + 1);
-          fence_proxy_async_all();
+          fence_proxy_async_all();       // ... and are read here through the async proxy
         }
-        const int row0 = t.m0 + 128 * static_cast<int>(rank);
-        const int variant = (t.r + 1) % 3;
+        const int variant = (t.r + 1) % 3;                     // row step i = r + 1
         const int crow = t.b * p.n_group + p.cmap[t.r + 1];
-        for (int j = 0; j < kG1Chunks + kG2Chunks; ++j, ++it) {
-          const int s = it % kStages3;
-          mbar_wait_a(empty_bar + 8 * s, ((it / kStages3) & 1) ^ 1);
-          const uint32_t st = smem + s * kStage;
-          const uint32_t fb = full_leader + 8 * s;
-          if (j < kG1Chunks) {
-            if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kStage);
-            if (j < 18) {
-              int tap, slot, half;
-              chunk_of(j, tap, slot, half);
-              tma_load_4d_2sm_a(st, &p.tm_x[t.l], fb, slot * kCh + half * kC, row0 + (tap - 1) * (1 << t.l), t.b, 0);
-              tma_load_4d_2sm_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, ((3 * tap + slot) * 2 + half) * kChunkK,
-                                128 * static_cast<int>(rank), 0, 0);
-            } else {
-              tma_load_4d_2sm_a(st, &p.tm_c, fb, (j - 18) * kChunkK, row0, crow, 0);
-              tma_load_4d_2sm_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, j * kChunkK, 128 * static_cast<int>(rank), 0, 0);
-            }
-          } else {
-            // out_proj K-chunk (channels of z block j - 20): weights only
-            if (leader) mbar_arrive_expect_tx_a(full_bar + 8 * s, 2 * kWBytes);
-            tma_load_4d_2sm_a(st + 2 * kATile, &p.tm_w2[t.l], fb, (j - kG1Chunks) * kChunkK, 128 * static_cast<int>(rank), 0, 0);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ------------------------------ MMA issuer ------------------------------
-      constexpr uint32_t idesc256 = make_idesc_bf16_f32(256, 256);
-      constexpr uint32_t idesc128 = make_idesc_bf16_f32(256, 128);
-      uint32_t it = 0;
-      Tile128 t;
-      int i = 0;
-      for (int T = pair; T < p.total_tiles; T += n_pairs, ++i) {
-        t.decode(p, T);
-        const uint32_t d1 = tmem_base;               // acc1: a0 | g0 | a1 | g1
-        const uint32_t d2 = tmem_base + 256;         // acc2: skip0 | res0 | skip1 | res1
-        const int newest = t.r % 3;
-        for (int j = 0; j < kG1Chunks; ++j, ++it) {
-          const int s = it % kStages3;
-          mbar_wait_a(full_bar + 8 * s, (it / kStages3) & 1);
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * kStage;
-          const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kATile);
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kATile), b_lo = make_smem_desc_sw128(st + 3 * kATile);
-          const int ksteps = j == kG1Chunks - 1 ? p.cond_ksteps_last : 4;
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            umma_bf16_2sm(d1, a_hi + koff, b_hi + koff, idesc256, !(j == 0 && k == 0));
-            umma_bf16_2sm(d1, a_lo + koff, b_hi + koff, idesc256, 1);
-            umma_bf16_2sm(d1, a_hi + koff, b_lo + koff, idesc256, 1);
-          }
-          if (j >= 12 && j < 18) {
-            int tap, slot, half;
-            chunk_of(j, tap, slot, half);
-            if (slot == newest) {
-              // residual pass of channel block `half`: acc2 block = [0 | row_hi + row_lo] (this also clears the skip half)
-              if (half == 0) {
-                mbar_wait_a(acc2_empty, (i & 1) ^ 1);      // the store warps have read tile i-1
-                tcgen05_fence_after();
-              }
-              const uint64_t b_id = make_smem_desc_sw128(ident);
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-                umma_bf16_2sm(d2 + 128 * half, a_hi + koff, b_id + koff, idesc128, k != 0);
-                umma_bf16_2sm(d2 + 128 * half, a_lo + koff, b_id + koff, idesc128, 1);
-              }
-            }
-          }
-          umma_commit_2sm_a(empty_bar + 8 * s);
-        }
-        umma_commit_2sm_a(acc1_full);
-        for (int kc = 0; kc < kG2Chunks; ++kc, ++it) {
-          const int s = it % kStages3;
-          mbar_wait_a(z_full + 8 * kc, i & 1);       // z of block kc is in tensor memory (over the a-columns of acc1): K-chunk kc of GEMM2
-          mbar_wait_a(full_bar + 8 * s, (it / kStages3) & 1);
-          tcgen05_fence_after();
-          const uint32_t st = smem + s * kStage;
-          const uint64_t b_hi = make_smem_desc_sw128(st + 2 * kATile), b_lo = make_smem_desc_sw128(st + 3 * kATile);
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t koff = static_cast<uint64_t>((k * kUmmaK * 2) >> 4);
-            const uint32_t a_hi = d1 + 128 * kc + 32 * (k >> 1) + 8 * (k & 1), a_lo = a_hi + 16;
-            umma_bf16_2sm_ts(d2, a_hi, b_hi + koff, idesc256, 1);
-            umma_bf16_2sm_ts(d2, a_lo, b_hi + koff, idesc256, 1);
-            umma_bf16_2sm_ts(d2, a_hi, b_lo + koff, idesc256, 1);
-          }
-          umma_commit_2sm_a(empty_bar + 8 * s);
-        }
-        umma_commit_2sm_a(acc2_full);
-      }
-    }
-  } else if (warp < kFirstGateWarp) {
-    // idle warps
-  } else if (warp < kFirstGateWarp + kGateWarps) {
-    // ------------------------------ gate warps ------------------------------
-    const int quarter = warp & 3;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t z_full_l = mapa_shared(z_full, 0);
-    float k_a, k_g;
-    asm volatile("mov.f32 %0, %2;\n\tmov.f32 %1, %3;" : "=f"(k_a), "=f"(k_g) : "f"(p.k_a), "f"(p.k_g));
-    Tile128 t;
-    int i = 0;
-    for (int T = pair; T < p.total_tiles; T += n_pairs, ++i) {
-      t.decode(p, T);
-      mbar_wait_a(acc1_full, i & 1);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int blk = 0; blk < 2; ++blk) {
-        const float* gc = p.gate_c[t.l] + 128 * blk;
-        const uint32_t acc = tmem_base + lane_base + 128 * blk;
-#pragma unroll
         for (int half = 0; half < 2; ++half) {
-          float va[32], vb[32];
-          uint32_t zw[32];
-          __syncwarp();
-          tmem_ld_32x32(acc + half * 32, va);
-          tmem_ld_32x32(acc + 64 + half * 32, vb);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float zz[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float e1 = ex2_approx(fminf(fmaf(va[j + e], k_a, gc[half * 32 + j + e]), 60.f));
-              const float e2 = ex2_approx(fminf(fmaf(vb[j + e], k_g, gc[64 + half * 32 + j + e]), 60.f));
-              const float t1 = 1.f + e1;
-              zz[e] = (1.f - e1) * rcp_approx(fmaf(t1, e2, t1));
+          const int row0 = t.m0 + 128 * half;
+          for (int j = 0; j < G::kG1Chunks + G::kG2Chunks; ++j, ++it) {
+            const int s = it % kStages;
+            mbar_wait_a(empty_bar + 8 * s, ((it / kStages) & 1) ^ 1);
+            const uint32_t st = smem + s * G::kStageBytes;
+            const uint32_t fb = full_bar + 8 * s;
+            if (j < 9 * kPer) {
+              // (tap, ring slot, channel block); the centre tap comes last among the taps
+              const int t3 = j / (3 * kPer), rem = j - 3 * kPer * t3;
+              const int tap = t3 == 0 ? 0 : t3 == 1 ? 2 : 1, slot = rem / kPer, hb = rem % kPer;
+              mbar_arrive_expect_tx_a(fb, G::kStageBytes);
+              tma_load_4d_a(st, &p.tm_x[t.l], fb, slot * C + hb * 64, row0 + (tap - 1) * (1 << t.l), t.b, 0);
+              tma_load_4d_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, ((3 * tap + slot) * kPer + hb) * kChunkK, 0, 0, 0);
+            } else if (j < G::kG1Chunks) {
+              mbar_arrive_expect_tx_a(fb, G::kStageBytes);
+              tma_load_4d_a(st, &p.tm_c, fb, (j - 9 * kPer) * kChunkK, row0, crow, 0);
+              tma_load_4d_a(st + 2 * kATile, &p.tm_w1[t.l][variant], fb, j * kChunkK, 0, 0, 0);
+            } else {
+              mbar_arrive_expect_tx_a(fb, G::kWBytes);                                   // out_proj K-chunk: weights only
+              tma_load_4d_a(st + 2 * kATile, &p.tm_w2[t.l], fb, (j - G::kG1Chunks) * kChunkK, 0, 0, 0);
             }
-            split2(zz[0], zz[1], zw[j / 2], zw[16 + j / 2]);
-            split2(zz[2], zz[3], zw[j / 2 + 1], zw[16 + j / 2 + 1]);
           }
-          tmem_st_32x32(acc + half * 32, zw);
         }
-        tmem_st_wait();                  // block blk is complete: GEMM2 can start on it while the other block is gated
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster_relaxed_a(z_full_l + 8 * blk);
       }
     }
   } else {
-    // ------------------------------ store warps ------------------------------
-    const int sw = warp - kFirstGateWarp - kGateWarps;
-    const int quarter = warp & 3;
-    const int half = sw >> 2;                 // 0: skip columns, 1: new row columns of each block
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t acc2_empty_l = mapa_shared(acc2_empty, 0);
-    Tile128 t;
-    int i = 0;
-    for (int T = pair; T < p.total_tiles; T += n_pairs, ++i) {
+    // ------------------------------ consumers ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rl = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    uint32_t it = 0;
+    FlowTile t;
+    for (int T = blockIdx.x; T < p.total_tiles; T += gridDim.x) {
       t.decode(p, T);
-      const int row = t.m0 + 128 * static_cast<int>(rank) + quarter * 32 + lane;
-      const long long pos = static_cast<long long>(t.b) * p.w + row;
       const bool last_layer = t.l == p.n_layers - 1;
-      const bool live = row < p.w;
-      const bool idle = half == 1 && last_layer;
-      mbar_wait_a(acc2_full, i & 1);
-      tcgen05_fence_after();
-      float s0 = 0.f, s1 = 0.f;
-#pragma unroll 1
-      for (int blk = 0; blk < 2; ++blk) {
-        const float* ob = p.out_b[t.l] + 128 * blk + 64 * half;
-        float v[64];
-        __syncwarp();
-        if (!idle) {
-          tmem_ld_32x32(tmem_base + lane_base + 256 + 128 * blk + 64 * half, v);
-          tmem_ld_32x32(tmem_base + lane_base + 256 + 128 * blk + 64 * half + 32, v + 32);
-          tmem_ld_wait();
-        }
-        if (blk == 1) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster_relaxed_a(acc2_empty_l);
-        }
-        if (idle || !live) {
-          // nothing to store
-        } else if (half == 0) {
-          float* dst = p.skip + pos * kCh + 64 * blk;
+      const float* ob = p.out_b[t.l];
+      for (int half = 0; half < 2; ++half) {
+        float s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f};          // output_proj partial sums (last layer)
+        consume_tile<C>(smem, full_bar, empty_bar, it, wg, lane, p.gate_c[t.l], p.k_a, p.k_g, p.cond_ksteps_last,
+                        [&](int blk, const float (&acc2)[64]) {
 #pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            float4 o = make_float4(v[4 * c] + ob[4 * c], v[4 * c + 1] + ob[4 * c + 1], v[4 * c + 2] + ob[4 * c + 2],
-                                   v[4 * c + 3] + ob[4 * c + 3]);
-            if (last_layer) {
-              if (p.n_layers > 1) {
-                const float4 a = ld_cg_f4(dst + 4 * c);
-                o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
+          for (int hh = 0; hh < 2; ++hh) {
+            const int row = t.m0 + 128 * half + rl + 8 * hh;
+            if (row >= p.w) continue;                          // positions past the end of the row: nothing to store
+            const long long pos = static_cast<long long>(t.b) * p.w + row;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int c = 64 * blk + 8 * jj + cq;            // channel inside C
+              const int ca = 128 * blk + 8 * jj + cq;          // accumulator column of its skip value
+              float o0 = acc2[4 * jj + 2 * hh] + ob[ca], o1 = acc2[4 * jj + 2 * hh + 1] + ob[ca + 1];
+              float* dst = p.skip + pos * C + c;
+              if (last_layer) {
+                // the sum of the skips is complete here: output_proj in registers instead of a last read-modify-write
+                if (p.n_layers > 1) {
+                  const float2 a = ld_cg_f2(dst);
+                  o0 += a.x; o1 += a.y;
+                }
+                s0[hh] = fmaf(p.po_w[c], o0, fmaf(p.po_w[c + 1], o1, s0[hh]));
+                s1[hh] = fmaf(p.po_w[C + c], o0, fmaf(p.po_w[C + c + 1], o1, s1[hh]));
+              } else {
+                if (t.l == 0) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+                else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(o0), "f"(o1) : "memory");
+                // new row = newest row + res -> the next layer's ring, same slot
+                const long long off = pos * (3 * C) + (t.r % 3) * C + c;
+                const float2 x = ld_split2(p.ring_hi[t.l], p.ring_lo[t.l], off);
+                uint32_t oh, ol;
+                split2(acc2[4 * (8 + jj) + 2 * hh] + ob[ca + 64] + x.x, acc2[4 * (8 + jj) + 2 * hh + 1] + ob[ca + 65] + x.y, oh, ol);
+                *reinterpret_cast<uint32_t*>(p.ring_hi[t.l + 1] + off) = oh;
+                *reinterpret_cast<uint32_t*>(p.ring_lo[t.l + 1] + off) = ol;
               }
-              const float* w0 = p.po_w + 64 * blk + 4 * c;
-              s0 = fmaf(w0[0], o.x, fmaf(w0[1], o.y, fmaf(w0[2], o.z, fmaf(w0[3], o.w, s0))));
-              s1 = fmaf(w0[kCh], o.x, fmaf(w0[kCh + 1], o.y, fmaf(w0[kCh + 2], o.z, fmaf(w0[kCh + 3], o.w, s1))));
-            } else if (t.l == 0) {
-              *reinterpret_cast<float4*>(dst + 4 * c) = o;
-            } else {
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4 * c), "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w)
-                           : "memory");
             }
           }
-        } else {
-          const long long off = pos * (3 * kCh) + (t.r % 3) * kCh + 64 * blk;
-          __nv_bfloat16* yh = p.ring_hi[t.l + 1];
-          __nv_bfloat16* yl = p.ring_lo[t.l + 1];
+        });
+        if (last_layer) {
+          // Flow._inverse_transform_row (:505-510) and, for the next row step, Flow.input_proj (:437-442) into layer 0's ring
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t oh[8], ol[8];
+          for (int hh = 0; hh < 2; ++hh) {
+            s0[hh] += __shfl_xor_sync(0xffffffffu, s0[hh], 1);
+            s0[hh] += __shfl_xor_sync(0xffffffffu, s0[hh], 2);
+            s1[hh] += __shfl_xor_sync(0xffffffffu, s1[hh], 1);
+            s1[hh] += __shfl_xor_sync(0xffffffffu, s1[hh], 2);
+            const int row = t.m0 + 128 * half + rl + 8 * hh;
+            if (row >= p.w) continue;
+            const long long pos = static_cast<long long>(t.b) * p.w + row;
+            const int irow = t.r + 1;
+            const long long xi = (static_cast<long long>(t.b) * p.n_group + irow) * p.w + row;
+            const float logs = s0[hh] + p.po_b[0], bb = s1[hh] + p.po_b[1];
+            const float xn = (__ldg(p.z + xi) - bb) * expf(-logs);
+            if ((lane & 3) == 0) p.x[xi] = xn;
+            if (irow + 1 < p.n_group) {
+              const long long off = pos * (3 * C) + (irow % 3) * C;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const int c = 16 * q + 2 * e;
-              split2(v[c] + ob[c], v[c + 1] + ob[c + 1], oh[e], ol[e]);
+              for (int jj = 0; jj < C / 8; ++jj) {
+                const int c = 8 * jj + cq;
+                uint32_t oh, ol;
+                split2(fmaf(p.in_w[c], xn, p.in_b[c]), fmaf(p.in_w[c + 1], xn, p.in_b[c + 1]), oh, ol);
+                *reinterpret_cast<uint32_t*>(p.ring_hi[0] + off + c) = oh;
+                *reinterpret_cast<uint32_t*>(p.ring_lo[0] + off + c) = ol;
+              }
             }
-            st_global_v8(yh + off + 16 * q, oh);
-            st_global_v8(yl + off + 16 * q, ol);
           }
         }
-      }
-      if (half == 0 && last_layer && live) {
-        const int irow = t.r + 1;
-        const long long xi = (static_cast<long long>(t.b) * p.n_group + irow) * p.w + row;
-        const float logs = s0 + p.po_b[0], bb = s1 + p.po_b[1];
-        const float xn = (__ldg(p.z + xi) - bb) * expf(-logs);
-        p.x[xi] = xn;
-        if (irow + 1 < p.n_group) {
-          const long long off = pos * (3 * kCh) + (irow % 3) * kCh;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            uint32_t oh[8], ol[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const int c = 16 * q + 2 * e;
-              split2(fmaf(p.in_w[c], xn, p.in_b[c]), fmaf(p.in_w[c + 1], xn, p.in_b[c + 1]), oh[e], ol[e]);
-            }
-            st_global_v8(p.ring_hi[0] + off + 16 * q, oh);
-            st_global_v8(p.ring_lo[0] + off + 16 * q, ol);
-          }
+        // publish: this warp's rows of the half are written (generic proxy) -> visible to the async-proxy reads of the consumers
+        __syncwarp();
+        if (lane == 0) {
+          fence_proxy_async_all();
+          __threadfence();
+          red_release_gpu_inc(p.flags + T);
         }
-      }
-      __syncwarp();
-      if (lane == 0) {
-        fence_proxy_async_all();
-        __threadfence();
-        red_release_gpu_inc(p.flags + T);
       }
     }
   }
-  tcgen05_fence_before();
-  cluster_sync();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
-  }
 }
-}  // namespace c128
 
 }  // namespace wf
 }  // namespace pk
@@ -1234,25 +523,25 @@ extern "C" int pk_waveflow_layer(const pk_waveflow_layer_args* a, pk_stream_t st
   PK_CHECK_ARG(a->next_hi != a->buf_hi, "the next layer's ring must not alias this layer's");
   PK_CHECK_ARG(a->cond_batch_stride >= static_cast<int64_t>(a->width) * a->n_mels && (a->cond_batch_stride % 8) == 0,
                "bad condition batch stride");
-  PK_CHECK_ARG(sm_count() >= 2, "needs at least one SM pair");
+  using G = Geo<kC>;
   CUtensorMap tx, tc, tw1, tw2_hi, tw2_lo;
   int rc;
   const uint64_t W = a->width, B = a->batch;
   if ((rc = encode_tmap_bf16_planes(&tx, a->buf_hi, a->buf_lo, 3 * kC, W, B, 3 * kC, W * 3 * kC, 128))) return rc;
   if ((rc = encode_tmap_bf16_planes(&tc, a->cond_hi, a->cond_lo, a->n_mels, W, B, a->n_mels, a->cond_batch_stride, 128))) return rc;
-  if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, kW1Cols, kG, 1, kW1Cols, 0, 64))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, 128, 1, 64, 0, 64))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, 64))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, kW1Cols, kG, 1, kW1Cols, 0, kG))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, kG, 1, 64, 0, kG))) return rc;
+  if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, kG, 1, 64, 0, kG))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_layer_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_layer_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem));
     attr_set = true;
   }
   LayerArgs p;
-  p.batch = a->batch; p.w = a->width; p.dil = a->dilation;
-  p.resid_chunk = 3 + a->slot;
-  p.cond_ksteps_last = (a->n_mels - 64 + kUmmaK - 1) / kUmmaK;
+  p.batch = a->batch; p.w = a->width; p.dil = a->dilation; p.slot = a->slot;
+  p.cond_ksteps_last = (a->n_mels - 64 + kWgmmaK - 1) / kWgmmaK;
+  p.tiles_per_b = (a->width + 127) / 128;
+  p.total_tiles = p.tiles_per_b * a->batch;
   constexpr float kLog2e = 1.4426950408889634f;
   p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
   for (int i = 0; i < 64; ++i) {
@@ -1261,69 +550,55 @@ extern "C" int pk_waveflow_layer(const pk_waveflow_layer_args* a, pk_stream_t st
   }
   for (int i = 0; i < 128; ++i) p.out_b[i] = a->bias2[i];
   p.skip = a->skip; p.skip_init = a->skip_init;
+  p.x_hi = static_cast<const __nv_bfloat16*>(a->buf_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->buf_lo);
   p.y_hi = static_cast<__nv_bfloat16*>(a->next_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->next_lo);
   p.y_ld = 3 * kC; p.y_col0 = a->slot * kC;
-  p.prof = static_cast<unsigned long long*>(a->prof);
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int pair_tiles = ((a->width + 255) / 256) * a->batch;
-  const int grid = 2 * std::min(pair_tiles, sm_count() / 2);
-  if (p.prof != nullptr) {
-    waveflow_layer_kernel<true><<<grid, kThreads, kSmem, st>>>(tx, tc, tw1, tw2_hi, tw2_lo, p);
-  } else {
-    waveflow_layer_kernel<false><<<grid, kThreads, kSmem, st>>>(tx, tc, tw1, tw2_hi, tw2_lo, p);
-  }
+  const int grid = std::min(p.total_tiles, sm_count());
+  waveflow_layer_kernel<<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tx, tc, tw1, tw2_hi, tw2_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
 }
 
-
-static int flow128_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
+template <int C>
+static int flow_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
   using namespace pk;
   using namespace pk::wf;
-  using namespace pk::wf::c128;
-  PK_CHECK_ARG(a->prof == nullptr, "no phase counters in the 128-channel flow kernel");
+  using G = Geo<C>;
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
-  static int max_pairs = 0;
+  static int max_ctas = 0;
   static bool attr_set = false;
   if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_flow128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem128));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * (sm_count() / 2));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = kSmem128;
-    cudaLaunchAttribute at;
-    at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = 1;
+    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_flow_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem));
+    // every CTA must be resident at once (tiles wait for tiles of other CTAs): ask the driver how many fit
     int n = 0;
-    PK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, waveflow_flow128_kernel, &cfg));
-    PK_CHECK_ARG(n >= 1, "no resident CTA pair available for pk_waveflow_flow");
-    max_pairs = std::min(n, sm_count() / 2);
+    PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, waveflow_flow_kernel<C>, kThreads, G::kSmem));
+    PK_CHECK_ARG(n >= 1, "no resident CTA available for pk_waveflow_flow");
+    max_ctas = n * sm_count();
     attr_set = true;
   }
-  static Flow128Args p;   // built in place under `mu`; the launch copies it
+  static FlowArgs<C> p;    // up to 22 KB of kernel parameters, built in place under `mu`; the launch copies them
   const uint64_t W = a->width, B = a->batch;
   int rc;
   constexpr float kLog2e = 1.4426950408889634f;
   for (int l = 0; l < a->n_layers; ++l) {
     PK_CHECK_ARG(a->ring_hi[l] && a->ring_lo[l] && a->w2_hi[l] && a->w2_lo[l] && a->bias1[l] && a->bias2[l], "NULL entry for layer %d", l);
-    if ((rc = encode_tmap_bf16_planes(&p.tm_x[l], a->ring_hi[l], a->ring_lo[l], 3 * kCh, W, B, 3 * kCh, W * 3 * kCh, 128))) return rc;
+    if ((rc = encode_tmap_bf16_planes(&p.tm_x[l], a->ring_hi[l], a->ring_lo[l], 3 * C, W, B, 3 * C, W * 3 * C, 128))) return rc;
     for (int v = 0; v < 3; ++v) {
       PK_CHECK_ARG(a->w1_hi[3 * l + v] && a->w1_lo[3 * l + v], "NULL GEMM1 weight for layer %d variant %d", l, v);
-      if ((rc = encode_tmap_bf16_planes(&p.tm_w1[l][v], a->w1_hi[3 * l + v], a->w1_lo[3 * l + v], kW1Cols128, 256, 1, kW1Cols128, 0, 128)))
+      if ((rc = encode_tmap_bf16_planes(&p.tm_w1[l][v], a->w1_hi[3 * l + v], a->w1_lo[3 * l + v], G::kG1Chunks * kChunkK, 2 * C, 1,
+                                        G::kG1Chunks * kChunkK, 0, 2 * C)))
         return rc;
     }
-    if ((rc = encode_tmap_bf16_planes(&p.tm_w2[l], a->w2_hi[l], a->w2_lo[l], kCh, 256, 1, kCh, 0, 128))) return rc;
-    for (int blk = 0; blk < 2; ++blk) {
+    if ((rc = encode_tmap_bf16_planes(&p.tm_w2[l], a->w2_hi[l], a->w2_lo[l], C, 2 * C, 1, C, 0, 2 * C))) return rc;
+    for (int blk = 0; blk < C / 64; ++blk) {
       for (int i = 0; i < 64; ++i) {
         p.gate_c[l][128 * blk + i] = -2.f * kLog2e * a->bias1[l][128 * blk + i];
         p.gate_c[l][128 * blk + 64 + i] = -kLog2e * a->bias1[l][128 * blk + 64 + i];
       }
     }
-    for (int i = 0; i < 256; ++i) p.out_b[l][i] = a->bias2[l][i];
+    for (int i = 0; i < 2 * C; ++i) p.out_b[l][i] = a->bias2[l][i];
     p.ring_hi[l] = static_cast<__nv_bfloat16*>(a->ring_hi[l]);
     p.ring_lo[l] = static_cast<__nv_bfloat16*>(a->ring_lo[l]);
   }
@@ -1335,18 +610,17 @@ static int flow128_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
   const long long total = static_cast<long long>(p.tiles_per_step) * p.n_rows * p.n_layers;
   PK_CHECK_ARG(total < (1ll << 30) && a->flags_len >= total, "flags must hold one counter per tile (%lld)", total);
   p.total_tiles = static_cast<int>(total);
-  p.cond_ksteps_last = (a->n_mels - 64 + kUmmaK - 1) / kUmmaK;
+  p.cond_ksteps_last = (a->n_mels - 64 + kWgmmaK - 1) / kWgmmaK;
   for (int i = 0; i < a->n_group; ++i) {
     PK_CHECK_ARG(a->cond_rows[i] >= 0 && a->cond_rows[i] < a->n_group, "cond_rows[%d] out of range", i);
     p.cmap[i] = a->cond_rows[i];
   }
-  for (int i = 0; i < kCh; ++i) { p.in_w[i] = a->in_w[i]; p.in_b[i] = a->in_b[i]; p.po_w[i] = a->out_w[i]; p.po_w[kCh + i] = a->out_w[kCh + i]; }
+  for (int i = 0; i < C; ++i) { p.in_w[i] = a->in_w[i]; p.in_b[i] = a->in_b[i]; p.po_w[i] = a->out_w[i]; p.po_w[C + i] = a->out_w[C + i]; }
   p.po_b[0] = a->out_b[0]; p.po_b[1] = a->out_b[1];
   p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
   p.skip = a->skip; p.z = a->z; p.x = a->x; p.flags = a->flags;
-  // a pair finishes a tile before it starts the next one: a tile may wait for the pair's own previous tile, any grid size works
-  const int n_pairs = std::max(1, std::min(max_pairs, p.tiles_per_step));
-  waveflow_flow128_kernel<<<2 * n_pairs, kThreads, kSmem128, static_cast<cudaStream_t>(stream)>>>(p);
+  const int grid = std::max(1, std::min(max_ctas, p.total_tiles));
+  waveflow_flow_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -1357,7 +631,7 @@ extern "C" int pk_waveflow_flow(const pk_waveflow_flow_args* a, pk_stream_t stre
   using namespace pk::wf;
   PK_CHECK_ARG(a != nullptr, "args is NULL");
   PK_CHECK_ARG(a->batch > 0 && a->width > 0, "bad batch/width");
-  PK_CHECK_ARG(a->channels == kC || a->channels == c128::kCh, "the fused WaveFlow flow is built for 64 or 128 residual channels (got %d)",
+  PK_CHECK_ARG(a->channels == 64 || a->channels == 128, "the fused WaveFlow flow is built for 64 or 128 residual channels (got %d)",
                a->channels);
   PK_CHECK_ARG(a->n_mels > 64 && a->n_mels <= 128 && (a->n_mels % 8) == 0, "n_mels must be in (64, 128], a multiple of 8");
   PK_CHECK_ARG(a->n_layers >= 1 && a->n_layers <= kMaxLayers && a->n_group >= 2 && a->n_group <= kMaxGroup,
@@ -1365,85 +639,5 @@ extern "C" int pk_waveflow_flow(const pk_waveflow_flow_args* a, pk_stream_t stre
   PK_CHECK_ARG(a->cond_rows && a->ring_hi && a->ring_lo && a->cond_hi && a->cond_lo && a->w1_hi && a->w1_lo && a->w2_hi && a->w2_lo &&
                a->bias1 && a->bias2 && a->in_w && a->in_b && a->out_w && a->out_b && a->z && a->x && a->skip && a->flags,
                "NULL pointer in pk_waveflow_flow_args");
-  if (a->channels == c128::kCh) return flow128_launch(a, stream);
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
-  static int max_pairs = 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_flow_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_flow_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    // every pair must be resident at once (tiles wait for tiles of other pairs): ask the driver how many clusters of 2 fit
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * (sm_count() / 2));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = kSmem;
-    cudaLaunchAttribute at;
-    at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = 2; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = 1;
-    int n = 0;
-    PK_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, waveflow_flow_kernel<false>, &cfg));
-    PK_CHECK_ARG(n >= 1, "no resident CTA pair available for pk_waveflow_flow");
-    max_pairs = std::min(n, sm_count() / 2);
-    attr_set = true;
-  }
-  static FlowArgs p;       // 14 KB of kernel parameters, built in place under `mu`; the launch copies them
-  const uint64_t W = a->width, B = a->batch;
-  int rc;
-  for (int l = 0; l < a->n_layers; ++l) {
-    PK_CHECK_ARG(a->ring_hi[l] && a->ring_lo[l] && a->w2_hi[l] && a->w2_lo[l] && a->bias1[l] && a->bias2[l], "NULL entry for layer %d", l);
-    if ((rc = encode_tmap_bf16_planes(&p.tm_x[l], a->ring_hi[l], a->ring_lo[l], 3 * kC, W, B, 3 * kC, W * 3 * kC, 128))) return rc;
-    for (int v = 0; v < 3; ++v) {
-      PK_CHECK_ARG(a->w1_hi[3 * l + v] && a->w1_lo[3 * l + v], "NULL GEMM1 weight for layer %d variant %d", l, v);
-      if ((rc = encode_tmap_bf16_planes(&p.tm_w1[l][v], a->w1_hi[3 * l + v], a->w1_lo[3 * l + v], kW1Cols, kG, 1, kW1Cols, 0, 64))) return rc;
-    }
-    if ((rc = encode_tmap_bf16_planes(&p.tm_w2[l], a->w2_hi[l], a->w2_lo[l], 64, kG, 1, 64, 0, 64))) return rc;
-    constexpr float kLog2e = 1.4426950408889634f;
-    for (int i = 0; i < 64; ++i) {
-      p.gate_c[l][i] = -2.f * kLog2e * a->bias1[l][i];
-      p.gate_c[l][64 + i] = -kLog2e * a->bias1[l][64 + i];
-    }
-    for (int i = 0; i < 128; ++i) p.out_b[l][i] = a->bias2[l][i];
-    p.ring_hi[l] = static_cast<__nv_bfloat16*>(a->ring_hi[l]);
-    p.ring_lo[l] = static_cast<__nv_bfloat16*>(a->ring_lo[l]);
-  }
-  if ((rc = encode_tmap_bf16_planes(&p.tm_c, a->cond_hi, a->cond_lo, a->n_mels, W, B * a->n_group, a->n_mels, W * a->n_mels, 128)))
-    return rc;
-  p.batch = a->batch; p.w = a->width; p.n_layers = a->n_layers; p.n_group = a->n_group; p.n_rows = a->n_group - 1;
-  p.tiles_per_b = (a->width + 255) / 256;
-  p.tiles_per_step = p.tiles_per_b * a->batch;
-  const long long total = static_cast<long long>(p.tiles_per_step) * p.n_rows * p.n_layers;
-  PK_CHECK_ARG(total < (1ll << 30) && a->flags_len >= total, "flags must hold one counter per tile (%lld)", total);
-  p.total_tiles = static_cast<int>(total);
-  p.cond_ksteps_last = (a->n_mels - 64 + kUmmaK - 1) / kUmmaK;
-  for (int i = 0; i < a->n_group; ++i) {
-    PK_CHECK_ARG(a->cond_rows[i] >= 0 && a->cond_rows[i] < a->n_group, "cond_rows[%d] out of range", i);
-    p.cmap[i] = a->cond_rows[i];
-  }
-  for (int i = 0; i < kC; ++i) { p.in_w[i] = a->in_w[i]; p.in_b[i] = a->in_b[i]; p.po_w[i] = a->out_w[i]; p.po_w[kC + i] = a->out_w[kC + i]; }
-  p.po_b[0] = a->out_b[0]; p.po_b[1] = a->out_b[1];
-  constexpr float kLog2e = 1.4426950408889634f;
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
-  p.skip = a->skip; p.z = a->z; p.x = a->x; p.flags = a->flags;
-  p.prof = static_cast<unsigned long long*>(a->prof);
-  // GEMM2 of tile i is issued after GEMM1 of the pair's next tile i + n_pairs, which waits for tiles up to
-  // i + n_pairs - tiles_per_step + 1: that must stay below i, or the pair waits for itself.  Tiny problems run unpipelined.
-  const int reach = p.tiles_per_b > 1 ? 1 : 0;
-  int n_pairs = std::min(max_pairs, p.tiles_per_step - 1 - reach);
-  p.serial = 0;
-  if (n_pairs < 1) {
-    n_pairs = std::min(max_pairs, p.tiles_per_step);
-    p.serial = 1;
-  }
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (p.prof != nullptr) {
-    waveflow_flow_kernel<true><<<2 * n_pairs, kThreads, kSmem, st>>>(p);
-  } else {
-    waveflow_flow_kernel<false><<<2 * n_pairs, kThreads, kSmem, st>>>(p);
-  }
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
+  return a->channels == 128 ? flow_launch<128>(a, stream) : flow_launch<64>(a, stream);
 }

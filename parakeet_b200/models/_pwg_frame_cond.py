@@ -15,7 +15,7 @@ multiplies it with the matching window of P, frames outside [0, frames) reading 
 import torch
 import torch.nn.functional as F
 
-TILE = 256          # rows of a CTA-pair tile: both CTAs of the pair multiply with the SAME 16-frame window of P
+TILE = 256          # rows of a band-table window: both 128-row tiles of the window multiply with the SAME 16-frame window of P
 KWIN = 16
 EDGE = 128          # rows next to either end of an utterance that carry their own coefficients (edge effects reach < 128)
 
@@ -63,7 +63,7 @@ def tile_band_table(firs, scales, frames, width=8):
         rows[T - EDGE:] = ref[ref_frames * hop - EDGE:]
     t = torch.arange(T)
     # the kernel's K window starts at window_start(t0) = floor8(t0 // hop - 2): TMA needs the innermost coordinate of a box
-    # 16-byte aligned (8 bf16 frames) - an unaligned start raises an illegal-instruction fault on sm_100a
+    # 16-byte aligned (8 bf16 frames) - an unaligned start makes the copy fault
     shift = (t // hop - 2) - window_start(t // TILE * TILE, hop)        # 0 .. 8
     assert int(shift.min()) >= 0 and int(shift.max()) + width <= KWIN
     out = torch.zeros(T, KWIN, dtype=torch.float64)

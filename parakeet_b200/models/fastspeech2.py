@@ -1,4 +1,4 @@
-"""FastSpeech2 on B200 - host side.
+"""FastSpeech2 on H100 - host side.
 
 Mirrors parakeet/models/fastspeech2/fastspeech2.py of the reference: `FastSpeech2` (:37-659) with the same constructor
 keywords, `forward(text, text_lengths, speech, speech_lengths, durations, pitch, energy, ...)` -> the reference's 7-tuple,
@@ -6,7 +6,7 @@ keywords, `forward(text, text_lengths, speech, speech_lengths, durations, pitch,
 Conv1D [out, in, k], BatchNorm `_mean` / `_variance`), and `FastSpeech2Inference` (:662-671).
 
 Every FLOP runs in libparakeet_b200.so: GEMM-shaped work (QKV / output projections, QK^T, PV, Conv1D feed-forward,
-predictor convs, feat_out, postnet) through pk_conv_gemm on tcgen05; row-wise work (embedding + positional encoding,
+predictor convs, feat_out, postnet) through pk_conv_gemm on wgmma; row-wise work (embedding + positional encoding,
 LayerNorm, masked softmax, duration rounding, length regulator) through the pk_* kernels of fs2.cu / elementwise.cu.
 There is one device->host copy per call: the B output lengths (sum of durations), needed to size the decoder buffers
 (the reference syncs twice per utterance, nets_utils.py:80 `.tolist()` and length_regulator.py:53 `.numpy()`).

@@ -1,4 +1,4 @@
-"""Parallel WaveGAN generator on B200 - host side.
+"""Parallel WaveGAN generator on H100 - host side.
 
 Mirrors parakeet/models/parallel_wavegan/parallel_wavegan.py of the reference: `PWGGenerator` (:318-520) with the same
 constructor keywords, `forward(x, c)`, `inference(c)`, `apply_weight_norm` / `remove_weight_norm`, and the same
@@ -67,7 +67,7 @@ class PWGGenerator(Layer):
         if interpolate_mode != "nearest" or freq_axis_kernel_size != 1:
             raise NotImplementedError("only nearest interpolation / freq_axis_kernel_size=1 are supported")
         if (in_channels, out_channels, kernel_size, residual_channels, gate_channels, skip_channels) != (1, 1, 3, 64, 128, 64):
-            raise NotImplementedError("the sm_100a kernels are specialised for 1/1 io channels, kernel 3, 64/128/64 channels")
+            raise NotImplementedError("the sm_90a kernels are specialised for 1/1 io channels, kernel 3, 64/128/64 channels")
         if not (64 < aux_channels <= 128 and aux_channels % 8 == 0):
             raise NotImplementedError("aux_channels must be in (64, 128] and a multiple of 8")
         if dropout != 0.0:
@@ -226,7 +226,7 @@ class PWGGenerator(Layer):
             # host copy of the lengths: they select the band-table end blocks (lengths are host data in the reference's callers
             # too, synthesize.py:96-104)
             lens_key = tuple(int(v) for v in torch.div(lens, self.upsample_factor, rounding_mode="floor").cpu().tolist())
-        eager = (not self._frame_cond() or getattr(self, "_layer_events", None) is not None or getattr(self, "_prof", None) is not None)
+        eager = not self._frame_cond() or getattr(self, "_layer_events", None) is not None
         if eager:
             return self._forward_impl(x, c, lens, lens_key)
         fn = lambda x_, c_, *l_: self._forward_impl(x_, c_, l_[0] if l_ else None, lens_key)   # noqa: E731
@@ -268,7 +268,6 @@ class PWGGenerator(Layer):
         args.lens = lens.data_ptr() if lens is not None else None
         args.c_hi, args.c_lo = ws["c"].hi.data_ptr(), ws["c"].lo.data_ptr()
         args.skip = ws["skip"].data_ptr()
-        args.prof = self._prof.data_ptr() if getattr(self, "_prof", None) is not None else None
         ev = getattr(self, "_layer_events", None)
         if ev is not None:   # bench.py: CUDA events around the 30 residual-layer launches, on the launching stream
             ev_a, ev_b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -345,7 +344,6 @@ class PWGGenerator(Layer):
         args.u_period, args.u_start_row, args.u_end_base = lay["period"], lay["start_row"], lay["end_base"]
         args.p_hi, args.p_lo, args.p_rows, args.p_ld, args.p_frames = P.hi.data_ptr(), P.lo.data_ptr(), NL * 128, Fp, frames
         args.skip = ws["skip"].data_ptr()
-        args.prof = self._prof.data_ptr() if getattr(self, "_prof", None) is not None else None
         ev = getattr(self, "_layer_events", None)
         if ev is not None:   # bench.py: CUDA events around the 30 residual-layer launches, on the launching stream
             ev_a, ev_b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

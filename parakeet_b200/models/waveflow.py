@@ -1,4 +1,4 @@
-"""ConditionalWaveFlow inference on B200 - host side (reference parakeet/models/waveflow.py:714-909).
+"""ConditionalWaveFlow inference on H100 - host side (reference parakeet/models/waveflow.py:714-909).
 
 Same constructor as the reference (`upsample_factors, n_flows, n_layers, n_group, channels, n_mels, kernel_size`), same
 state-dict keys (`encoder.{i}.{weight_g,weight_v,bias}`, `decoder.{f}.input_proj.*`,
@@ -164,7 +164,7 @@ class ConditionalWaveFlow(Layer):
     def _flow_mode(self):
         return self._fusable() and os.environ.get("PK_WF_FUSED", "1") != "layer"
 
-    def _run_flow(self, fw, z, x, cond_s, cmap, bufs, skip, flags, prof, st):
+    def _run_flow(self, fw, z, x, cond_s, cmap, bufs, skip, flags, st):
         """Rows 1 .. G-1 of one flow in one launch (row 0 and the ring contents are prepared by the caller)."""
         L = _lib.lib()
         B, G, W = z.shape
@@ -184,8 +184,6 @@ class ConditionalWaveFlow(Layer):
         h = fw["host"]
         a.in_w, a.in_b, a.out_w, a.out_b = (h[k].ctypes.data for k in ("in_w", "in_b", "out_w", "out_b"))
         a.z, a.x, a.skip, a.flags, a.flags_len = _ptr(z), _ptr(x), _ptr(skip), _ptr(flags), flags.numel()
-        if prof is not None:
-            a.prof = _ptr(prof)
         _lib.check(L.pk_waveflow_flow(C_.byref(a), st), "pk_waveflow_flow")
 
     def encode(self, mel, trim_conv_artifact=True):
@@ -224,7 +222,6 @@ class ConditionalWaveFlow(Layer):
         fused = self._fusable()
         flow_mode = self._flow_mode()
         flags = torch.empty((G - 1) * NL * B * ((W + 255) // 256), dtype=torch.int32, device=dev) if flow_mode else None
-        prof = getattr(self, "_prof", None)                                               # debug: device uint64[8] phase counters
         for fi in reversed(range(self.n_flows)):
             perm = self.perms[fi]
             z = z.index_select(1, pk["perms"][fi])                                        # geo.shuffle_dim(z, 2, perm)
@@ -241,7 +238,7 @@ class ConditionalWaveFlow(Layer):
                                                     _ptr(state), _ptr(bufs[0].hi), _ptr(bufs[0].lo), 3 * C, 0, st),
                            "pk_waveflow_input_proj")
                 flags.zero_()
-                self._run_flow(fw, z, x, cond_s, cmap, bufs, skip, flags, prof, st)
+                self._run_flow(fw, z, x, cond_s, cmap, bufs, skip, flags, st)
                 z = x
                 continue
             for i in range(1, G):
@@ -263,8 +260,6 @@ class ConditionalWaveFlow(Layer):
                         if l + 1 < NL:
                             a.next_hi, a.next_lo = _ptr(bufs[l + 1].hi), _ptr(bufs[l + 1].lo)
                         a.skip, a.skip_init = _ptr(skip), 1 if l == 0 else 0
-                        if prof is not None:
-                            a.prof = _ptr(prof)
                         _lib.check(L.pk_waveflow_layer(C_.byref(a), st), "pk_waveflow_layer")
                     _lib.check(L.pk_waveflow_row_out(_ptr(skip), _ptr(fw["out_w"]), _ptr(fw["out_b"]), _ptr(z[:, i]), G * W, B, W, C,
                                                      _ptr(x[:, i]), G * W, st), "pk_waveflow_row_out")

@@ -1,4 +1,4 @@
-"""STFT / MelScale on B200 (reference parakeet/modules/audio.py:74-229) and the numpy feature extractors of
+"""STFT / MelScale on H100 (reference parakeet/modules/audio.py:74-229) and the numpy feature extractors of
 parakeet/data/get_feats.py (LogMelFBank :20-88, Energy :167-220) - all transforms run in pk_stft (radix-2 FFT kernel).
 
 Window tables (scipy get_window, centre-padded), FFT twiddles and the Slaney mel filterbank (what librosa.filters.mel

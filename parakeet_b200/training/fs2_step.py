@@ -1,4 +1,4 @@
-"""FastSpeech2 training step on B200 (reference: FastSpeech2Updater.update_core, parakeet/models/fastspeech2/
+"""FastSpeech2 training step on H100 (reference: FastSpeech2Updater.update_core, parakeet/models/fastspeech2/
 fastspeech2_updater.py:51-99; data-parallel set-up examples/fastspeech2/train.py:51-56,135-139).
 
     forward (train mode: BatchNorm uses batch statistics; Dropout at the reference's sites with Philox masks that the backward

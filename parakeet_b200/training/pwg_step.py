@@ -1,4 +1,4 @@
-"""Parallel WaveGAN training step on B200 (reference: PWGUpdater.update_core, parakeet/models/parallel_wavegan/
+"""Parallel WaveGAN training step on H100 (reference: PWGUpdater.update_core, parakeet/models/parallel_wavegan/
 parallel_wavegan_updater.py:76-153; set-up examples/GANVocoder/parallelwave_gan/baker/train.py; SURVEY.md 8f.1).
 
     generator step      wav_ = G(noise, mel);  loss = MR-STFT(wav_, wav) [+ lambda_adv * MSE(D(wav_), 1) once
@@ -7,7 +7,7 @@ parallel_wavegan_updater.py:76-153; set-up examples/GANVocoder/parallelwave_gan/
                         loss = MSE(D(wav), 1) + MSE(D(wav_), 0);  backward;  clip + Adam
 
 This is the training-mode formulation of the generator: every intermediate the backward pass needs (pre-gate activations,
-z, the layer inputs, the upsampling stages) is kept, so the residual stack runs as separate tcgen05 GEMMs (`pk_conv_gemm`:
+z, the layer inputs, the upsampling stages) is kept, so the residual stack runs as separate wgmma GEMMs (`pk_conv_gemm`:
 dilated conv + aux 1x1 accumulated through the residual operand, skip|out 1x1) around the element-wise kernels of csrc/gan.cu
 instead of the fused inference kernel (csrc/pwg_fc.cu), which keeps nothing.  Data gradients are convolutions with flipped taps,
 weight gradients NT matmuls over the flattened batch x time axis on transposed split planes - the scheme of training/fs2_step.py

@@ -1,4 +1,4 @@
-"""GPU diagnostic for pk_conv_gemm: tcgen05 path vs SIMT path vs torch fp64 (prints error tables)."""
+"""GPU diagnostic for pk_conv_gemm: wgmma path vs SIMT path vs torch fp64 (prints error tables)."""
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

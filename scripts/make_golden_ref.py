@@ -21,6 +21,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, HERE)
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from _golden import sample_index  # noqa: E402
 from refexec import loader, paddle_standin  # noqa: E402
 
 REF = "/root/reference/parakeet"
@@ -309,6 +311,23 @@ def wrappers_and_stft(out):
     with torch.no_grad():
         sc, mag = MultiResolutionSTFTLoss()(T(wavs), T(other))
     out["mrstft_loss"] = np.asarray([float(sc), float(mag)], dtype=np.float64)
+# Large arrays of the models file are stored as a fixed sample of their elements (tests/_golden.py reads them back), which keeps
+# the file under 1 MB: the compared-against outputs, the seeded speech targets (regenerated by the tests) and the gradients.
+SAMPLED = ("wf_cond", "fs2_fwd_out_before", "fs2_fwd_out_after", "fs2_inf_mel", "fs2_inf_mel_alpha", "fs2ms_a_inf_mel", "fs2ms_b_inf_mel",
+           "fs2ms_a_fwd_after", "fs2ms_b_fwd_after", "stft_a_re", "stft_a_im", "stft_a_mag", "stft_b_re", "stft_b_im", "stft_b_mag",
+           "fs2_fwd_speech", "fs2_train_speech", "fs2ms_a_fwd_speech", "fs2ms_b_fwd_speech")
+
+
+def sampled(models):
+    out = {}
+    for k, v in models.items():
+        if k in SAMPLED or k.startswith("fs2_train_grad/"):
+            flat = np.asarray(v).reshape(-1)
+            out[k + "@sample"] = flat[sample_index(flat.size, 1024 if k.startswith("fs2_train_grad/") else 2048)]
+            out[k + "@shape"] = np.asarray(np.shape(v), dtype=np.int64)
+        else:
+            out[k] = v
+    return out
 
 
 def main():
@@ -326,6 +345,7 @@ def main():
     finally:
         uninstall()
     np.savez(os.path.join(GOLD, "ref_executed.npz"), **small)
+    models = sampled(models)
     np.savez_compressed(os.path.join(GOLD, "ref_executed_models.npz"), **models)
     for name, d in (("ref_executed.npz", small), ("ref_executed_models.npz", models)):
         print(name, os.path.getsize(os.path.join(GOLD, name)) // 1024, "KB", len(d), "arrays")

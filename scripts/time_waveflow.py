@@ -1,5 +1,5 @@
 """ConditionalWaveFlow.infer at cfg4 shapes: CUDA-event time of a graph replay (third call of the same shape).
-PK_WF_FUSED=0 selects the two-GEMM layer path; --prof adds the MMA-issuer phase counters of pk_waveflow_layer (eager run)."""
+PK_WF_FUSED=0 selects the two-GEMM layer path."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -22,12 +22,3 @@ e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / 3
 print(f"waveflow {CH} ch b16 x 400 frames (PK_WF_FUSED={os.environ.get('PK_WF_FUSED', '1')}): {ms:.1f} ms/call, "
       f"{y.numel() / ms * 1e3 / 1e6:.2f} M samples/s, replays {wf._graphs.replays}, finite {bool(torch.isfinite(y).all())}", flush=True)
-if "--prof" in sys.argv and wf._fusable():
-    wf._prof = torch.zeros(8, dtype=torch.int64, device=dev)
-    wf.inverse(z, wf.encode(mel))
-    torch.cuda.synchronize()
-    c = wf._prof.cpu().tolist()
-    tot = sum(c[:4])
-    names = ["issue", "wait data", "wait acc2", "wait z"]
-    print("MMA issuer: " + ", ".join(f"{n} {100 * v / tot:.1f}%" for n, v in zip(names, c[:4])) +
-          f"; {tot / max(c[4], 1):.0f} clk per pair tile over {c[4]} tiles")

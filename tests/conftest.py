@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -23,6 +23,13 @@ def cuda():
 
 
 def rel_err(a, b):
+    import torch
+    from _golden import NOT_STORED
     a = a.detach().double().cpu()
-    b = b.detach().double().cpu()
+    b = b.detach().cpu()
+    if b.dtype == torch.float32:    # a golden reference stored as a sample of its elements: compare the stored ones
+        known = b.view(torch.int32) != NOT_STORED
+        if not known.all():
+            a, b = a.expand_as(b)[known], b[known]
+    b = b.double()
     return ((a - b).abs().max() / b.abs().max().clamp_min(1e-30)).item()

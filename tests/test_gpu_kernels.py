@@ -1,4 +1,4 @@
-"""GPU parity tests for the generic kernels, through the C-ABI (run with -m gpu on a B200)."""
+"""GPU parity tests for the generic kernels, through the C-ABI (run with -m gpu on an H100)."""
 import math
 import os
 
@@ -40,9 +40,9 @@ def _ref_conv(x, w, bias, taps, dil, act, residual, lens):
     (2, 1000, 64, 128, 3, 8, None, False, False),     # dilated
     (1, 3000, 64, 128, 3, 512, None, False, False),   # dilation larger than the tile
     (3, 37, 256, 1, 1, 1, None, False, True),         # predictor head, T < one tile
-    (5, 129, 128, 256, 3, 2, "relu", True, True),     # CTA-pair kernel: second CTA of the pair owns a single row
-    (40, 448, 384, 1536, 3, 1, "relu", False, True),  # CTA-pair kernel, more pair tiles (480) than CTA pairs (persistent walk)
-    (7, 700, 256, 300, 5, 1, "tanh", False, False),   # CTA-pair kernel: partial N tile (300 of 512), partial 256-row tile
+    (5, 129, 128, 256, 3, 2, "relu", True, True),     # wide N, the second 128-row tile holds a single row
+    (40, 448, 384, 1536, 3, 1, "relu", False, True),  # wide N, more tiles (480) than SMs (persistent walk)
+    (7, 700, 256, 300, 5, 1, "tanh", False, False),   # partial N tile (300 of 512), partial 128-row tile
     (33, 250, 192, 128, 1, 1, None, True, False),     # single-CTA persistent kernel, more tiles than SMs is not required: odd counts
 ])
 def test_conv_gemm_matches_fp64(cuda, B, T, Cin, N, taps, dil, act, res, lens):

@@ -75,6 +75,31 @@ def test_pwg_ragged_batch_equals_single_utterances(cuda, pwg):
         assert rel_err(y[i, :, :f * hop], refs[i]) < TOL
 
 
+def test_pwg_sample_rate_conditioning_path_vs_oracle(cuda, pwg, monkeypatch):
+    """PK_PWG_FRAME_COND=0 selects pk_pwg_residual_layer (sample-rate conditioning planes): whole batch and a ragged batch
+    against the oracle, like the default frame-rate path."""
+    from oracle import pwg as opwg
+    gen, folded = pwg
+    monkeypatch.setenv("PK_PWG_FRAME_COND", "0")
+    x, c = opwg.synth_inputs(6, batch=2, mel_frames=40)
+    with torch.no_grad():
+        y_ref = opwg.generator_forward(folded, x, c)
+    assert rel_err(gen(x.to(cuda), c.to(cuda)), y_ref) < TOL
+    frames, hop = [40, 25, 33], 300
+    xs = torch.zeros(3, 1, max(frames) * hop)
+    cs = torch.zeros(3, 80, max(frames) + 4)
+    refs = []
+    for i, f in enumerate(frames):
+        xi, ci = opwg.synth_inputs(20 + i, batch=1, mel_frames=f)
+        xs[i, :, :f * hop], cs[i, :, :f + 4] = xi[0], ci[0]
+        with torch.no_grad():
+            refs.append(opwg.generator_forward(folded, xi, ci)[0])
+    lens = torch.tensor([f * hop for f in frames], dtype=torch.int32, device=cuda)
+    y = gen(xs.to(cuda), cs.to(cuda), lens=lens)
+    for i, f in enumerate(frames):
+        assert rel_err(y[i, :, :f * hop], refs[i]) < TOL
+
+
 def test_pwg_ragged_batch_graph_replay_and_empty_utterance(cuda, pwg):
     """A ragged batch holding an EMPTY utterance, run three times (eager, CUDA-graph capture, replay): every call reproduces the
     single-utterance oracle results, the empty row stays zero, and a different set of lengths of the same padded shape (another

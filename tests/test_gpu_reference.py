@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from _golden import Golden
 from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -16,7 +17,7 @@ TOL = 1e-3   # north_star: "within 1e-3 rel fp32" (max-abs error / max-abs refer
 
 @pytest.fixture(scope="module")
 def g():
-    return np.load(os.path.join(GOLD, "ref_executed_models.npz"))
+    return Golden(np.load(os.path.join(GOLD, "ref_executed_models.npz")))
 
 
 def test_fastspeech2_cuda_vs_executed_reference(cuda, g):

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+from _golden import Golden
 from conftest import rel_err
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -20,7 +21,7 @@ TOL = 2e-6        # same arithmetic, same torch kernels underneath: the oracle r
 
 @pytest.fixture(scope="module")
 def g():
-    return np.load(os.path.join(GOLD, "ref_executed_models.npz"))
+    return Golden(np.load(os.path.join(GOLD, "ref_executed_models.npz")))
 
 
 def test_state_dict_keys_equal_the_reference_class_trees(g):

@@ -81,9 +81,11 @@ int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t cols, uint6
 }
 
 int encode_tmap_bf16_planes(CUtensorMap* out, const void* hi, const void* lo, uint64_t cols, uint64_t rows, uint64_t batches,
-                            uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows) {
+                            uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) return fail(PK_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
+  if (box_cols != 64 && box_cols != 16) return fail(PK_ERR_INVALID_ARG, "box_cols must be 64 or 16 (got %u)", box_cols);
+  const CUtensorMapSwizzle swz = box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B;
   const long long plane = static_cast<const char*>(lo) - static_cast<const char*>(hi);
   if (plane <= 0 || (plane & 15) || plane >= (1ll << 40))
     return fail(PK_ERR_INVALID_ARG, "split planes must come from one allocation, lo after hi at a 16-byte multiple (ops.Split.empty / zeros)");
@@ -91,11 +93,11 @@ int encode_tmap_bf16_planes(CUtensorMap* out, const void* hi, const void* lo, ui
   if (batch_stride_elems == 0) batch_stride_elems = row_stride_elems * rows;
   cuuint64_t dims[4] = {cols, rows, batches, 2};
   cuuint64_t strides[3] = {row_stride_elems * 2, batch_stride_elems * 2, static_cast<cuuint64_t>(plane)};
-  cuuint32_t box[4] = {64, box_rows, 1, 2};
+  cuuint32_t box[4] = {box_cols, box_rows, 1, 2};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   if ((strides[0] & 15) || (strides[1] & 15)) return fail(PK_ERR_INVALID_ARG, "TMA strides must be multiples of 16 bytes");
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(hi), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(PK_ERR_CUDA, "cuTensorMapEncodeTiled (4-D planes) failed (%d): cols=%llu rows=%llu batches=%llu ld=%llu bs=%llu plane=%lld",

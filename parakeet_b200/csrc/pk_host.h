@@ -28,10 +28,11 @@ int fail(int code, const char* fmt, ...);
 int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t batches,
                         uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows);
 
-// Both planes of a split-bf16 tensor as ONE 4-D map: dims {cols, rows, batches, 2}, box {64, box_rows, 1, 2} - a single TMA
+// Both planes of a split-bf16 tensor as ONE 4-D map: dims {cols, rows, batches, 2}, box {box_cols, box_rows, 1, 2} - one TMA
 // load then delivers [hi tile | lo tile] back to back.  Requires lo = hi + a positive 16-byte multiple (one allocation).
+// box_cols 64 / 16 selects a 128 / 32-byte swizzle (the box row is exactly one swizzle atom wide).
 int encode_tmap_bf16_planes(CUtensorMap* out, const void* hi, const void* lo, uint64_t cols, uint64_t rows, uint64_t batches,
-                            uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows);
+                            uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols = 64);
 
 int sm_count();
 void count_launch(int n = 1);

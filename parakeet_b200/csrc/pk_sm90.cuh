@@ -61,6 +61,15 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
   return d;
 }
 __device__ __forceinline__ uint64_t desc_kstep(int k) { return static_cast<uint64_t>((k * kWgmmaK * 2) >> 4); }
+// The same for a tile of ONE K-step: rows of 32 B (16 bf16), SWIZZLE_32B, 8-row groups 256 B apart, 256-B aligned.
+__device__ __forceinline__ uint64_t make_smem_desc_sw32(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;             // LBO (unused: the K extent is one swizzle atom)
+  d |= static_cast<uint64_t>(256 >> 4) << 32;      // SBO: 8 rows * 32 B
+  d |= static_cast<uint64_t>(3) << 62;             // SWIZZLE_32B
+  return d;
+}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -80,6 +89,10 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 // named barrier over `threads` threads (a warpgroup: 128)
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// arrive without waiting: the other `threads` - 128 threads of the barrier wait on it with named_bar_sync
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // wgmma.mma_async m64nNk16, bf16 x bf16 -> f32, K-major operands; d (N / 2 floats per thread) is accumulated in place.
@@ -158,6 +171,9 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 
 // mbarrier / TMA helpers taking shared-space addresses
 __device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
@@ -198,6 +214,20 @@ __device__ __forceinline__ void tma_load_4d_a(uint32_t smem_dst, const CUtensorM
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// TMA store of a box (rows outside the tensor are not written); the smem source may be reused after bulk_wait_read<0>.
+// The generic-proxy writes that filled the source must be made visible first (fence_proxy_async_all + a barrier).
+__device__ __forceinline__ void tma_store_4d_a(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+// asynchronous prefetch of `bytes` (a multiple of 16) contiguous global bytes into L2
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gptr, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
 
 // ----------------------------------------------------------------------------------------------------------------

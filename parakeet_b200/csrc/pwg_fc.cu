@@ -6,14 +6,18 @@
 // resident W_aux) become ONE K-step: A = the tile-relative band table of U (constants of the model,
 // models/_pwg_frame_cond.py), B = the 16-frame window of P = W_aux m' that the tile touches (frame rate, L2 resident).
 //
-// Hopper structure: persistent CTAs over 128-sample tiles (the two halves of the 256-sample window that one band-table /
-// P-window pair describes), 384 threads:
-//   * warps 8-11 (producer warpgroup, one TMA lane): per tile 4 A chunks (tap -d, tap +d, conditioning, centre tap) through a
-//     2-deep ring of 32 KB stages, plus the P window of the tile; W1 (three tap chunks) and W2 stay resident (128 KB);
-//   * warps 0-7 (two consumer warpgroups, 64 samples each): GEMM1 (wgmma, accumulator in registers), the gate in registers,
-//     z as the register A operand of GEMM2 - z never touches shared memory - and the stores straight from the fragments.
-//     The residual add `+ x` is folded in by starting GEMM2's accumulator at [0 | x], read from the centre-tap chunk
-//     while it is in shared memory.
+// Hopper structure: persistent CTAs over 128-sample half tiles of the 256-sample windows that one band-table / P-window pair
+// describes; each half tile is two 64-row tiles, one per consumer warpgroup ("ping-pong": while one warpgroup gates and
+// stores, the other keeps the tensor cores busy).  384 threads:
+//   * warps 8-11 (producer warpgroup, one TMA lane): per 64-row tile 4 A chunks (tap -d, tap +d, conditioning, centre tap)
+//     through one 6-deep ring of 16 KB stages, the two warpgroups' tiles alternating; the conditioning stage holds a
+//     16-column box of the band table and the 16-frame P window of the tile (32-byte swizzle).  W1 (three tap chunks) and
+//     W2 stay resident (128 KB);
+//   * warps 0-7 (two consumer warpgroups, one 64-row tile each): GEMM1 (wgmma, accumulator in registers, one commit group
+//     in flight), the gate in registers, z as the register A operand of GEMM2 - z never touches shared memory.  The residual
+//     add `+ x` is folded in by starting GEMM2's accumulator at [0 | x], read from the centre-tap chunk while it is in
+//     shared memory; that stage then holds y for one TMA store of the tile, and the skip sum is red.add-ed from the
+//     fragments (its rows were prefetched into L2 by the producer).  An ordering barrier alternates the warpgroups' GEMM1s.
 #include <stdlib.h>
 #include <string.h>
 
@@ -27,16 +31,19 @@ namespace fc {
 
 constexpr int kPwgR = 64;
 constexpr int kPwgG = 128;
-constexpr int kATile = 128 * kSwizzleBytes;                  // 16 KB: one plane of a 128-row K-chunk
+constexpr int kATile = 128 * kSwizzleBytes;                  // 16 KB: one plane of a resident 128-row weight chunk
+constexpr int kQTile = 64 * kSwizzleBytes;                   // 8 KB: one plane of a 64-row K-chunk of x
 constexpr int kConsumerThreads = 256;
 constexpr int kThreads = kConsumerThreads + 128;
 constexpr int kFcG1Chunks = 4;                               // tap -d, tap +d, conditioning, centre tap
-constexpr int kFcStages = 2;
-constexpr int kFcStageBytes = 2 * kATile;                    // A hi, A lo
+constexpr int kFcStages = 6;
+constexpr int kFcStageBytes = 2 * kQTile;                    // A hi, A lo
+constexpr int kFcUBytes = 2 * 64 * 32;                       // 4 KB: hi | lo of 16 band-table columns x 64 rows
+constexpr int kFcPBytes = 2 * 128 * 32;                      // 8 KB: hi | lo of 16 P frames x 128 output channels
 constexpr int kFcW1Bytes = 3 * 2 * kATile;                   // 96 KB: three tap chunks x 128 output channels
 constexpr int kFcW2Bytes = 2 * kATile;                       // 32 KB: 128 outputs (skip | out) x 64
-constexpr int kFcPBytes = 2 * kATile;                        // 32 KB: hi | lo of the P window of 128 output channels
-constexpr int kFcSmem = kFcStages * kFcStageBytes + kFcW1Bytes + kFcW2Bytes + kFcPBytes + 1024 + 256;
+constexpr int kFcSmem = kFcW1Bytes + kFcW2Bytes + kFcStages * kFcStageBytes + 1024 + 256;
+static_assert(kFcUBytes + kFcPBytes <= kFcStageBytes, "the conditioning operands share one ring stage");
 static_assert(kFcSmem <= 227 * 1024, "shared memory budget");
 
 struct FcLayerArgs {
@@ -49,8 +56,6 @@ struct FcLayerArgs {
   float k_a, k_g;
   float* skip;
   int skip_init;
-  __nv_bfloat16* y_hi;
-  __nv_bfloat16* y_lo;
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -98,13 +103,13 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
                     const __grid_constant__ CUtensorMap tm_p,          // 4-D maps: both planes of a tile in one TMA box
                     const __grid_constant__ CUtensorMap tm_w1_hi, const __grid_constant__ CUtensorMap tm_w1_lo,
                     const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
-                    const FcLayerArgs p) {
+                    const __grid_constant__ CUtensorMap tm_y, const FcLayerArgs p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w1 = smem + kFcStages * kFcStageBytes;        // [tap chunk][hi | lo] 128-row tiles, resident
+  const uint32_t w1 = smem;                                    // [tap chunk][hi | lo] 128-row tiles, resident
   const uint32_t w2 = w1 + kFcW1Bytes;                         // [hi | lo]
-  const uint32_t pbuf = w2 + kFcW2Bytes;                       // [hi | lo] P window of the current tile
-  const uint32_t bars = pbuf + kFcPBytes;
+  const uint32_t ring = w2 + kFcW2Bytes;                       // [stages] 64-row chunks [hi | lo]
+  const uint32_t bars = ring + kFcStages * kFcStageBytes;
   const uint32_t full_bar = bars;                              // [stages]
   const uint32_t empty_bar = full_bar + 8 * kFcStages;         // [stages]
   const uint32_t w_bar = empty_bar + 8 * kFcStages;
@@ -115,7 +120,9 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
   if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_u); tma_prefetch_desc(&tm_p);
     tma_prefetch_desc(&tm_w1_hi); tma_prefetch_desc(&tm_w1_lo); tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kFcStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
+    tma_prefetch_desc(&tm_y);
+    // a stage is read by one consumer warpgroup: one arrival per warp
+    for (int s = 0; s < kFcStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 4); }
     mbar_init_a(w_bar, 1);
     fence_barrier_init();
   }
@@ -138,65 +145,80 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
       int b, m0, half;
       while (ti.next(b, m0, half)) {
         const int mh = m0 + 128 * half;
-        for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
-          const int s = it % kFcStages;
-          mbar_wait_a(empty_bar + 8 * s, ((it / kFcStages) & 1) ^ 1);
-          const uint32_t st = smem + s * kFcStageBytes;
-          const uint32_t fb = full_bar + 8 * s;
-          // chunk order: tap -d, tap +d, conditioning, centre tap (last: it also supplies the residual x)
-          if (j == 2) {
-            // conditioning as U (W_aux m'): A = tile-relative band table rows (K window = 16 frames inside a 64-wide box),
-            // B = the same 16 frames of P for the 128 output channels; frames outside the utterance are out of bounds of
-            // the tensor map and read as zero.  The P buffer's previous reader (this chunk of the previous tile) finished
-            // before the stage now being refilled was handed back.
-            mbar_arrive_expect_tx_a(fb, kFcStageBytes + kFcPBytes);
-            // band rows of this half tile: first 128 rows of an utterance, the half tiles touching its last 128 rows
-            // (per-utterance block; 2 * 128 clamps halves lying wholly past the end onto the zero block), else interior
-            const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
-            const int m1 = ((len - 128) >> 7) << 7;
-            const int urow = mh == 0 ? p.u_start_row
-                             : (mh + 128 > len - 128) ? p.u_end_base + 384 * b + min(mh - m1, 256)
-                                                      : mh % p.u_period;
-            tma_load_4d_a(st, &tm_u, fb, 0, urow, 0, 0);
-            // one K window per 256-sample window: it starts at the frame of the window's first row, aligned down to
-            // 8 frames (16 B) - TMA faults on an unaligned innermost coordinate
-            const int j0 = (m0 / p.hop - 2) & ~7;
-            tma_load_4d_a(pbuf, &tm_p, fb, j0, p.p_row0, b, 0);
-          } else {
-            mbar_arrive_expect_tx_a(fb, kFcStageBytes);
-            const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
-            tma_load_4d_a(st, &tm_x, fb, 0, mh + (wj - 1) * p.dil, b, 0);
+        // band rows of this half tile: first 128 rows of an utterance, the half tiles touching its last 128 rows
+        // (per-utterance block; 2 * 128 clamps halves lying wholly past the end onto the zero block), else interior
+        const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
+        const int m1 = ((len - 128) >> 7) << 7;
+        const int urow = mh == 0 ? p.u_start_row
+                         : (mh + 128 > len - 128) ? p.u_end_base + 384 * b + min(mh - m1, 256)
+                                                  : mh % p.u_period;
+        // one K window per 256-sample window: it starts at the frame of the window's first row, aligned down to
+        // 8 frames (16 B) - TMA faults on an unaligned innermost coordinate
+        const int j0 = (m0 / p.hop - 2) & ~7;
+        for (int wg = 0; wg < 2; ++wg) {                       // the 64-row tiles of consumer warpgroups 0 and 1
+          // the tile's rows of the skip sum go to L2 now, so that the red.add of its epilogue does not wait for HBM
+          const int rows = min(64, p.t - (mh + 64 * wg));
+          if (!p.skip_init && rows > 0)
+            bulk_prefetch_l2(p.skip + (static_cast<long long>(b) * p.t + mh + 64 * wg) * 64, rows * 64 * 4);
+          for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
+            const int s = it % kFcStages;
+            mbar_wait_a(empty_bar + 8 * s, ((it / kFcStages) & 1) ^ 1);
+            const uint32_t st = ring + s * kFcStageBytes;
+            const uint32_t fb = full_bar + 8 * s;
+            // chunk order: tap -d, tap +d, conditioning, centre tap (last: it also supplies the residual x)
+            if (j == 2) {
+              // conditioning as U (W_aux m'): A = the tile's 64 band-table rows (K window = columns 0..15), B = the same 16
+              // frames of P for the 128 output channels; frames outside the utterance are out of bounds of the tensor map
+              // and read as zero
+              mbar_arrive_expect_tx_a(fb, kFcUBytes + kFcPBytes);
+              tma_load_4d_a(st, &tm_u, fb, 0, urow + 64 * wg, 0, 0);
+              tma_load_4d_a(st + kFcUBytes, &tm_p, fb, j0, p.p_row0, b, 0);
+            } else {
+              mbar_arrive_expect_tx_a(fb, kFcStageBytes);
+              const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
+              tma_load_4d_a(st, &tm_x, fb, 0, mh + 64 * wg + (wj - 1) * p.dil, b, 0);
+            }
           }
         }
       }
     }
   } else {
-    // ------------------------------ consumers: 64 samples per warpgroup ------------------------------
+    // ------------------------------ consumers: one 64-row tile per warpgroup ------------------------------
     setmaxnreg_inc<232>();
     const int wg = warp >> 2;
     const int rl = 16 * (warp & 3) + (lane >> 2);              // this thread's rows: rl and rl + 8 of the warpgroup's 64
     const int cq = 2 * (lane & 3);                             // and columns 8 j + cq, + 1
     const float kSqrtHalf = 0.70710678118654752440f;
     mbar_wait_a(w_bar, 0);
-    uint32_t it = 0;
+    uint32_t it = wg * kFcG1Chunks;                            // ring position of this warpgroup's first chunk
     FcTileIter ti(p);
     int b, m0, half;
-    while (ti.next(b, m0, half)) {
+    bool more = ti.next(b, m0, half);
+    bool first = true;
+    while (more) {
       const int mh = m0 + 128 * half;
       float acc1[64], acc2[64];
-      for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
-        const int s = it % kFcStages;
-        mbar_wait_a(full_bar + 8 * s, (it / kFcStages) & 1);
-        const uint32_t st = smem + s * kFcStageBytes + wg * 64 * kSwizzleBytes;
-        const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kATile);
+      // ordering barrier: the warpgroups take turns at GEMM1 (warpgroup 0 first), so that one of them gates and stores while
+      // the other's GEMM1 has the tensor cores
+      if (wg == 1 || !first) named_bar_sync(1 + wg, kConsumerThreads);
+      first = false;
+      // fully unrolled: the chunk kind is a compile-time case, so the wgmma chains of consecutive chunks stay asynchronous
+      // (one commit group in flight; the stage of chunk j - 1 goes back to the producer once chunk j has been issued)
+#pragma unroll
+      for (int j = 0; j < kFcG1Chunks; ++j) {
+        const int s = (it + j) % kFcStages;
+        mbar_wait_a(full_bar + 8 * s, ((it + j) / kFcStages) & 1);
+        const uint32_t st = ring + s * kFcStageBytes;
         wgmma_fence();
         if (j == 2) {                                          // one K-step: 16 frames of band table x P window
-          const uint64_t b_hi = make_smem_desc_sw128(pbuf), b_lo = make_smem_desc_sw128(pbuf + kATile);
+          const uint64_t a_hi = make_smem_desc_sw32(st), a_lo = make_smem_desc_sw32(st + kFcUBytes / 2);
+          const uint64_t b_hi = make_smem_desc_sw32(st + kFcUBytes), b_lo = make_smem_desc_sw32(st + kFcUBytes + kFcPBytes / 2);
           wgmma_ss_n128(acc1, a_hi, b_hi, 1);
           wgmma_ss_n128(acc1, a_lo, b_hi, 1);
           wgmma_ss_n128(acc1, a_hi, b_lo, 1);
         } else {
           const int wj = j == 0 ? 0 : j == 1 ? 2 : 1;
+          const uint64_t a_hi = make_smem_desc_sw128(st), a_lo = make_smem_desc_sw128(st + kQTile);
           const uint64_t b_hi = make_smem_desc_sw128(w1 + wj * 2 * kATile), b_lo = make_smem_desc_sw128(w1 + wj * 2 * kATile + kATile);
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
@@ -214,7 +236,7 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
             for (int hh = 0; hh < 2; ++hh) {
               const int r = rl + 8 * hh;
               const uint32_t off = r * kSwizzleBytes + ((((8 * jj + cq) >> 3) ^ (r & 7)) << 4) + (cq & 7) * 2;
-              const uint32_t xh = lds_u32(st + off), xl = lds_u32(st + kATile + off);
+              const uint32_t xh = lds_u32(st + off), xl = lds_u32(st + kQTile + off);
               acc2[4 * jj + 2 * hh] = 0.f;
               acc2[4 * jj + 2 * hh + 1] = 0.f;
               acc2[32 + 4 * jj + 2 * hh] = __uint_as_float(xh << 16) + __uint_as_float(xl << 16);
@@ -222,11 +244,22 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
             }
           }
         }
-        wgmma_wait<0>();
-        reg_fence(acc1);
-        __syncwarp();
-        if (lane == 0) mbar_arrive_a(empty_bar + 8 * s);
+        if (j > 0) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive_a(empty_bar + 8 * ((it + j - 1) % kFcStages));
+        }
       }
+      wgmma_wait<0>();
+      reg_fence(acc1);
+      // the centre-tap stage stays with this warpgroup: it becomes the staging tile of y (same rows, same layout as x)
+      const int cs = (it + kFcG1Chunks - 1) % kFcStages;
+      const uint32_t ystage = ring + cs * kFcStageBytes;
+      it += 2 * kFcG1Chunks;                                   // the other warpgroup's tile sits in between
+      // hand GEMM1 to the other warpgroup (warpgroup 1 skips this after its last tile: warpgroup 0 waits for no more turns)
+      int nb, nm0, nhalf;
+      const bool next = ti.next(nb, nm0, nhalf);
+      if (wg == 0 || next) named_bar_arrive(2 - wg, kConsumerThreads);
       // gate: z = tanh(a + ba) * sigmoid(g + bg) = (1 - e1) / ((1 + e1)(1 + e2)), e1 = exp(-2(a+ba)), e2 = exp(-(g+bg))
       // (one reciprocal; the exp2 argument of e1 is clamped at 60 so that the product cannot overflow where z != 0).
       // a column c and its g column 64 + c sit in the same thread (fragments j and j + 8).
@@ -259,30 +292,53 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(acc2);
-      // stores: skip half -> fp32 skip sum (write or red.add), out half -> (out + b_out) * sqrt(1/2) as split planes
+      // stores: out half -> (out + b_out) * sqrt(1/2) as split planes into the staging tile, then one TMA store of the 64 rows
+      // (rows past t lie outside the tensor map: not written); skip half -> fp32 skip sum (write or red.add) from the
+      // fragments while the TMA engine reads the staging tile
       const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = rl + 8 * hh;
+        const bool live = mh + wg * 64 + r < len;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int c = 8 * jj + cq;
+          const float y0 = live ? (acc2[32 + 4 * jj + 2 * hh] + p.out_b[c]) * kSqrtHalf : 0.f;
+          const float y1 = live ? (acc2[32 + 4 * jj + 2 * hh + 1] + p.out_b[c + 1]) * kSqrtHalf : 0.f;
+          uint32_t oh, ol;
+          split2(y0, y1, oh, ol);
+          const uint32_t off = r * kSwizzleBytes + (((c >> 3) ^ (r & 7)) << 4) + (cq & 7) * 2;   // where x was read
+          sts_u32(ystage + off, oh);
+          sts_u32(ystage + kQTile + off, ol);
+        }
+      }
+      fence_proxy_async_all();
+      named_bar_sync(3 + wg, 128);
+      const bool store_lane = (threadIdx.x & 127) == 0;
+      if (store_lane) {
+        tma_store_4d_a(&tm_y, ystage, 0, mh + wg * 64, b, 0);
+        bulk_commit();
+      }
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int trow = mh + wg * 64 + rl + 8 * hh;
         if (trow < p.t) {
           const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-          const bool live = trow < len;
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj) {
-            const int c = 8 * jj + cq;
-            float* d2 = p.skip + row_off + c;
+            float* d2 = p.skip + row_off + 8 * jj + cq;
             const float s0 = acc2[4 * jj + 2 * hh], s1 = acc2[4 * jj + 2 * hh + 1];
             if (p.skip_init) *reinterpret_cast<float2*>(d2) = make_float2(s0, s1);
             else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d2), "f"(s0), "f"(s1) : "memory");
-            const float y0 = live ? (acc2[32 + 4 * jj + 2 * hh] + p.out_b[c]) * kSqrtHalf : 0.f;
-            const float y1 = live ? (acc2[32 + 4 * jj + 2 * hh + 1] + p.out_b[c + 1]) * kSqrtHalf : 0.f;
-            uint32_t oh, ol;
-            split2(y0, y1, oh, ol);
-            *reinterpret_cast<uint32_t*>(p.y_hi + row_off + c) = oh;
-            *reinterpret_cast<uint32_t*>(p.y_lo + row_off + c) = ol;
           }
         }
       }
+      if (store_lane) {
+        bulk_wait_read<0>();                                   // the stage has been read: back to the producer
+#pragma unroll
+        for (int w = 0; w < 4; ++w) mbar_arrive_a(empty_bar + 8 * cs);   // the arrivals of the warpgroup's 4 warps
+      }
+      b = nb; m0 = nm0; half = nhalf; more = next;
     }
   }
 }
@@ -302,16 +358,18 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
                a->u_rows >= a->u_end_base + 384 * a->batch, "bad compact band table layout");
   PK_CHECK_ARG(a->p_rows > 0 && a->p_row0 >= 0 && a->p_row0 + 128 <= a->p_rows && (a->p_ld % 8) == 0 && a->p_ld >= 64 && a->p_frames > 0 &&
                a->p_frames <= a->p_ld, "bad P plane geometry");
-  CUtensorMap tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo;
+  CUtensorMap tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty;
   int rc;
   const uint64_t T = a->t, B = a->batch;
-  if ((rc = encode_tmap_bf16_planes(&tx, a->x_hi, a->x_lo, kPwgR, T, B, kPwgR, T * kPwgR, 128))) return rc;
-  // compact band table planes (u_rows, 64): the K window sits in columns 0..15
-  if ((rc = encode_tmap_bf16_planes(&tu, a->u_hi, a->u_lo, 64, a->u_rows, 1, 64, 0, 128))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&tx, a->x_hi, a->x_lo, kPwgR, T, B, kPwgR, T * kPwgR, 64))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&ty, a->y_hi, a->y_lo, kPwgR, T, B, kPwgR, T * kPwgR, 64))) return rc;
+  // compact band table planes (u_rows, 64): the K window sits in columns 0..15, a 16-column box of 64 rows
+  if ((rc = encode_tmap_bf16_planes(&tu, a->u_hi, a->u_lo, 64, a->u_rows, 1, 64, 0, 64, 16))) return rc;
   // P planes (batch, p_rows, p_ld): frames are the K axis; columns >= p_frames (and < 0) read as zero
   const uint64_t prow = a->p_rows, pld = a->p_ld;
   // (the extent is the padded row length p_ld >= 64: columns [p_frames, p_ld) hold zeros in memory, frames < 0 are out of bounds)
-  if ((rc = encode_tmap_bf16_planes(&tp, a->p_hi, a->p_lo, pld, prow, B, pld, prow * pld, 128))) return rc;
+  // (16-frame box of the 128 output channels of the layer)
+  if ((rc = encode_tmap_bf16_planes(&tp, a->p_hi, a->p_lo, pld, prow, B, pld, prow * pld, 128, 16))) return rc;
   const uint64_t k1 = 5 * kChunkK;     // row pitch of the packed W1 (pk_pwg_residual_layer layout); only the 3 tap chunks are read
   if ((rc = encode_tmap_bf16_3d(&tw1_hi, a->w1_hi, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 128))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw1_lo, a->w1_lo, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 128))) return rc;
@@ -334,11 +392,10 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
     p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
     p.out_b[i] = a->bias2[64 + i];
   }
-  p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int tiles = ((a->t + 255) / 256) * 2 * a->batch;
   const int grid = std::min(tiles, sm_count());
-  pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
+  pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

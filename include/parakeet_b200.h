@@ -406,6 +406,70 @@ typedef struct pk_waveflow_flow_args {
 } pk_waveflow_flow_args;
 int pk_waveflow_flow(const pk_waveflow_flow_args* args, pk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * WaveFlow density estimation: ConditionalWaveFlow.forward (:759-783) = WaveFlow.forward (:627-672) on the untrimmed encoder
+ * output, and WaveFlowLoss (:855-891).  Flow.forward (:465-494) is not autoregressive: every layer runs over all
+ * n_group - 1 net rows of all utterances at once.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* One ResidualBlock.forward (:197-226) over every (utterance, net row r in [0, n_group - 1), column) position, for 64 or 128
+ * channels: a | g = conv2d(x, kernel 3x3, dilation (1, dilation), padding causal [2, 0] x same) + condition_proj(condition)
+ * + bias1; z = tanh(a) sigmoid(g); skip | res = out_proj(z) + bias2; skip (=|+=) skip; y = x + res.
+ * x / y planes (batch * (n_group + 1), width, channels): rows [b (n_group + 1), b (n_group + 1) + 2) stay ZERO (the causal
+ * padding), net row r of utterance b is row b (n_group + 1) + 2 + r.  y must be another buffer (neighbouring positions read
+ * x), NULL on the last layer; its zero rows are not written.  cond planes (batch, n_group, width, n_mels); cond_rows[h]
+ * (HOST [n_group]) = the condition height that height h of this flow reads (the previous flows' permutations, composed):
+ * net row r uses height r + 1.  w1 / w2 / bias1 / bias2: the operands of pk_waveflow_flow for ONE layer, row-step variant 0
+ * (ring slot s = kernel row s): w1 planes (2 channels, 9 channels + 128), w2 planes (2 channels, channels), biases HOST.
+ * skip fp32 (batch, n_group - 1, width, channels).  Every pair of planes comes from ONE allocation (lo after hi). */
+typedef struct pk_waveflow_forward_layer_args {
+  int32_t batch, width, channels, n_mels, n_group, dilation;
+  const int32_t* cond_rows;
+  const void* x_hi;
+  const void* x_lo;
+  const void* cond_hi;
+  const void* cond_lo;
+  const void* w1_hi;
+  const void* w1_lo;
+  const void* w2_hi;
+  const void* w2_lo;
+  const float* bias1;
+  const float* bias2;
+  void* y_hi;
+  void* y_lo;
+  float* skip;
+  int32_t skip_init;
+} pk_waveflow_forward_layer_args;
+int pk_waveflow_forward_layer(const pk_waveflow_forward_layer_args* args, pk_stream_t stream);
+
+/* The tail of one Flow.forward plus the height permutation after it (:661-665), and the next flow's input_proj:
+ *   (logs, b) = output_proj(skip) (out_w [2][channels], out_b [2], HOST); z[:, 0] = x[:, 0], z[:, h] = x[:, h] exp(logs) + b
+ *   (:459-463); x_next[:, i] = z[:, perm[i]] (perm HOST [n_group]); *log_det += sum of logs over all positions, summed in a
+ *   fixed order (repeated calls give identical bits); the next flow's input_proj (in_w / in_b HOST [channels]) of x_next rows
+ *   0 .. n_group - 2 into the next layer input planes (the x planes of pk_waveflow_forward_layer).
+ * skip == NULL: z = x (no output_proj, log_det untouched) - the first flow's input_proj.  x_next, next_hi / next_lo may be
+ * NULL (not written).  x / x_next fp32 (batch, n_group, width), distinct.  partials: device fp32 [1024] scratch; counter:
+ * device uint32, zero before the first call and left zero by every call. */
+typedef struct pk_waveflow_forward_tail_args {
+  int32_t batch, width, channels, n_group;
+  const float* skip;
+  const float* out_w;
+  const float* out_b;
+  const float* x;
+  const int32_t* perm;
+  float* x_next;
+  const float* in_w;
+  const float* in_b;
+  void* next_hi;
+  void* next_lo;
+  float* log_det;
+  float* partials;
+  uint32_t* counter;
+} pk_waveflow_forward_tail_args;
+int pk_waveflow_forward_tail(const pk_waveflow_forward_tail_args* args, pk_stream_t stream);
+/* WaveFlowLoss.forward: loss[0] = (sq_sum[0] / (2 sigma^2) - log_det[0]) / n + log(2 pi) / 2 + log(sigma), with sq_sum the
+ * device double sum of z^2 from pk_sq_sum and n = numel(z). */
+int pk_waveflow_nll(const double* sq_sum, const float* log_det, int64_t n, float sigma, float* loss, pk_stream_t stream);
+
 /* FastSpeech2Loss.forward with use_masking=True (models/fastspeech2/fastspeech2.py:701-812; DurationPredictorLoss
  * duration_predictor.py:140-184): out4 = { l1_loss = L1(before, ys) + L1(after, ys) over valid frames,
  * duration_loss = MSE(d_outs, log(ds + 1)), pitch_loss = MSE(p_outs, ps), energy_loss = MSE(e_outs, es) over valid tokens }.

@@ -94,6 +94,25 @@ class WaveflowFlowArgs(C.Structure):
                 ("flags_len", C.c_int64)]
 
 
+class WaveflowForwardLayerArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32), ("n_mels", C.c_int32),
+                ("n_group", C.c_int32), ("dilation", C.c_int32), ("cond_rows", C.c_void_p), ("x_hi", C.c_void_p),
+                ("x_lo", C.c_void_p), ("cond_hi", C.c_void_p), ("cond_lo", C.c_void_p), ("w1_hi", C.c_void_p),
+                ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p), ("bias1", C.c_void_p),
+                ("bias2", C.c_void_p), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("skip", C.c_void_p),
+                ("skip_init", C.c_int32)]
+
+
+class WaveflowForwardTailArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32), ("n_group", C.c_int32),
+                ("skip", C.c_void_p), ("out_w", C.c_void_p), ("out_b", C.c_void_p), ("x", C.c_void_p), ("perm", C.c_void_p),
+                ("x_next", C.c_void_p), ("in_w", C.c_void_p), ("in_b", C.c_void_p), ("next_hi", C.c_void_p),
+                ("next_lo", C.c_void_p), ("log_det", C.c_void_p), ("partials", C.c_void_p), ("counter", C.c_void_p)]
+
+
+WAVEFLOW_TAIL_PARTIALS = 1024      # fp32 scratch elements pk_waveflow_forward_tail needs
+
+
 def _declare(L):
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     sigs = {
@@ -109,6 +128,9 @@ def _declare(L):
         "pk_pwg_residual_layer_fc": [C.POINTER(PwgLayerFcArgs), vp],
         "pk_waveflow_layer": [C.POINTER(WaveflowLayerArgs), vp],
         "pk_waveflow_flow": [C.POINTER(WaveflowFlowArgs), vp],
+        "pk_waveflow_forward_layer": [C.POINTER(WaveflowForwardLayerArgs), vp],
+        "pk_waveflow_forward_tail": [C.POINTER(WaveflowForwardTailArgs), vp],
+        "pk_waveflow_nll": [vp, vp, i64, f32, vp, vp],
         "pk_pwg_tail": [vp, vp, vp, vp, vp, vp, f32, i64, vp, vp],
         "pk_embed_pe": [vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp],
         "pk_layer_norm": [vp, vp, vp, f32, vp, i32, i32, i32, vp, vp, vp, vp],

@@ -506,6 +506,128 @@ waveflow_flow_kernel(const __grid_constant__ FlowArgs<C> p) {
   }
 }
 
+
+// ------------------------------------------------------------------------------------------------------------------------
+// pk_waveflow_forward_layer: one ResidualBlock.forward (:197-226) of Flow.forward (:465-494) over ALL n_group - 1 net rows
+// of all utterances in one launch - no row dependency, so it is a plain 2-D gated convolution over 128-position tiles along
+// the width of one (utterance, net row).  Input / output are (batch * (n_group + 1), w, C) split planes: two zero rows per
+// utterance, then its net rows, so that kernel row kh of net row r reads buffer row r + kh (= net row r - 2 + kh, the causal
+// padding [2, 0]) and never the previous utterance; the width taps read columns w + (tap - 1) 2^l, and TMA's out-of-bounds
+// fill is the "same" padding.  GEMM1 chunk j = (tap, kh, channel block) reads weight columns [64 j, 64 j + 64) of the row
+// step variant 0 of the inverse's packed weight (slot s = kernel row s).  Consumer side and epilogue as pk_waveflow_flow.
+// ------------------------------------------------------------------------------------------------------------------------
+template <int C>
+struct FwdLayerArgs {
+  int w, n_group, dil, tiles_per_row, total_tiles, cond_ksteps_last, skip_init;
+  int cmap[kMaxGroup];                   // condition row (after the previous flows' permutations) of height h
+  float gate_c[2 * C];                   // accumulator order, pre-scaled
+  float out_b[2 * C];
+  float k_a, k_g;
+  float* skip;                           // (batch, n_group - 1, w, C)
+  const __nv_bfloat16* x_hi;             // (batch * (n_group + 1), w, C): the residual reads the net row itself
+  const __nv_bfloat16* x_lo;
+  __nv_bfloat16* y_hi;                   // same layout; NULL on the last layer
+  __nv_bfloat16* y_lo;
+};
+
+template <int C>
+__global__ void __launch_bounds__(kThreads, 1)
+waveflow_forward_layer_kernel(const __grid_constant__ CUtensorMap tm_x,    // input planes (batch * (n_group + 1), w, C)
+                              const __grid_constant__ CUtensorMap tm_c,    // condition planes (batch * n_group, w, n_mels)
+                              const __grid_constant__ CUtensorMap tm_w1,   // GEMM1 weight planes (2C, 64 G1), box = all rows
+                              const __grid_constant__ CUtensorMap tm_w2,   // out_proj planes (2C, C)
+                              const __grid_constant__ FwdLayerArgs<C> p) {
+  using G = Geo<C>;
+  constexpr int kPer = C / 64;                                 // 64-channel blocks
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t full_bar = smem + kStages * G::kStageBytes;   // [stages]
+  const uint32_t empty_bar = full_bar + 8 * kStages;           // [stages]
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int rows = p.n_group - 1;
+
+  if (threadIdx.x == kConsumerThreads) {
+    tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_c); tma_prefetch_desc(&tm_w1); tma_prefetch_desc(&tm_w2);
+    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= kConsumerThreads / 32) {
+    setmaxnreg_dec<40>();
+    if (warp == kConsumerThreads / 32 && lane == 0) {
+      // ------------------------------ TMA producer ------------------------------
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+        const int br = tile / p.tiles_per_row, w0 = (tile - br * p.tiles_per_row) * 128;
+        const int b = br / rows, r = br - b * rows;
+        const int xrow = b * (p.n_group + 1) + r;              // + kh: net row r - 2 + kh
+        const int crow = b * p.n_group + p.cmap[r + 1];        // Flow.forward conditions net row r on height r + 1
+        for (int j = 0; j < G::kG1Chunks + G::kG2Chunks; ++j, ++it) {
+          const int s = it % kStages;
+          mbar_wait_a(empty_bar + 8 * s, ((it / kStages) & 1) ^ 1);
+          const uint32_t st = smem + s * G::kStageBytes;
+          const uint32_t fb = full_bar + 8 * s;
+          if (j < 9 * kPer) {
+            const int tap = j / (3 * kPer), rem = j - 3 * kPer * tap;
+            const int kh = rem / kPer, hb = rem - kPer * kh;
+            mbar_arrive_expect_tx_a(fb, G::kStageBytes);
+            tma_load_4d_a(st, &tm_x, fb, hb * 64, w0 + (tap - 1) * p.dil, xrow + kh, 0);   // columns outside [0, w) read as zero
+            tma_load_4d_a(st + 2 * kATile, &tm_w1, fb, j * kChunkK, 0, 0, 0);
+          } else if (j < G::kG1Chunks) {
+            mbar_arrive_expect_tx_a(fb, G::kStageBytes);
+            tma_load_4d_a(st, &tm_c, fb, (j - 9 * kPer) * kChunkK, w0, crow, 0);              // channels >= n_mels read as zero
+            tma_load_4d_a(st + 2 * kATile, &tm_w1, fb, j * kChunkK, 0, 0, 0);
+          } else {
+            mbar_arrive_expect_tx_a(fb, G::kWBytes);                                         // out_proj K-chunk: weights only
+            tma_load_4d_a(st + 2 * kATile, &tm_w2, fb, (j - G::kG1Chunks) * kChunkK, 0, 0, 0);
+          }
+        }
+      }
+    }
+  } else {
+    // ------------------------------ consumers ------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int rl = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const int br = tile / p.tiles_per_row, w0 = (tile - br * p.tiles_per_row) * 128;
+      const int b = br / rows, r = br - b * rows;
+      const long long srow = static_cast<long long>(br) * p.w;                             // skip row (b, r)
+      const long long xrow = (static_cast<long long>(b) * (p.n_group + 1) + 2 + r) * p.w;  // buffer row of net row r
+      consume_tile<C>(smem, full_bar, empty_bar, it, wg, lane, p.gate_c, p.k_a, p.k_g, p.cond_ksteps_last,
+                      [&](int blk, const float (&acc2)[64]) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int col = w0 + rl + 8 * hh;
+          if (col >= p.w) continue;                            // positions past the end of the row: nothing to store
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int c = 64 * blk + 8 * jj + cq;              // channel inside C
+            const int ca = 128 * blk + 8 * jj + cq;            // accumulator column of its skip value
+            float* dst = p.skip + (srow + col) * C + c;
+            const float o0 = acc2[4 * jj + 2 * hh] + p.out_b[ca], o1 = acc2[4 * jj + 2 * hh + 1] + p.out_b[ca + 1];
+            if (p.skip_init) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
+            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(o0), "f"(o1) : "memory");
+            if (p.y_hi != nullptr) {
+              // ResidualBlock.forward: res = x_in + res, into the other buffer (neighbouring tiles still read this one)
+              const long long off = (xrow + col) * C + c;
+              const float2 x = ld_split2(p.x_hi, p.x_lo, off);
+              uint32_t oh, ol;
+              split2(acc2[4 * (8 + jj) + 2 * hh] + p.out_b[ca + 64] + x.x, acc2[4 * (8 + jj) + 2 * hh + 1] + p.out_b[ca + 65] + x.y, oh, ol);
+              *reinterpret_cast<uint32_t*>(p.y_hi + off) = oh;
+              *reinterpret_cast<uint32_t*>(p.y_lo + off) = ol;
+            }
+          }
+        }
+      });
+    }
+  }
+}
+
 }  // namespace wf
 }  // namespace pk
 
@@ -640,4 +762,69 @@ extern "C" int pk_waveflow_flow(const pk_waveflow_flow_args* a, pk_stream_t stre
                a->bias1 && a->bias2 && a->in_w && a->in_b && a->out_w && a->out_b && a->z && a->x && a->skip && a->flags,
                "NULL pointer in pk_waveflow_flow_args");
   return a->channels == 128 ? flow_launch<128>(a, stream) : flow_launch<64>(a, stream);
+}
+
+template <int C>
+static int forward_layer_launch(const pk_waveflow_forward_layer_args* a, pk_stream_t stream) {
+  using namespace pk;
+  using namespace pk::wf;
+  using G = Geo<C>;
+  static std::once_flag attr_once;
+  static cudaError_t attr_err = cudaSuccess;
+  std::call_once(attr_once, [] {
+    attr_err = cudaFuncSetAttribute(waveflow_forward_layer_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem);
+  });
+  PK_CHECK_CUDA(attr_err);
+  const uint64_t W = a->width, B = a->batch, NG = a->n_group;
+  CUtensorMap tx, tc, tw1, tw2;
+  int rc;
+  if ((rc = encode_tmap_bf16_planes(&tx, a->x_hi, a->x_lo, C, W, B * (NG + 1), C, W * C, 128))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&tc, a->cond_hi, a->cond_lo, a->n_mels, W, B * NG, a->n_mels, W * a->n_mels, 128))) return rc;
+  if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, G::kG1Chunks * kChunkK, 2 * C, 1, G::kG1Chunks * kChunkK, 0, 2 * C)))
+    return rc;
+  if ((rc = encode_tmap_bf16_planes(&tw2, a->w2_hi, a->w2_lo, C, 2 * C, 1, C, 0, 2 * C))) return rc;
+  FwdLayerArgs<C> p;
+  p.w = a->width; p.n_group = a->n_group; p.dil = a->dilation; p.skip_init = a->skip_init;
+  p.tiles_per_row = (a->width + 127) / 128;
+  const long long total = static_cast<long long>(p.tiles_per_row) * a->batch * (a->n_group - 1);
+  PK_CHECK_ARG(total < (1ll << 31), "too many tiles (%lld)", total);
+  p.total_tiles = static_cast<int>(total);
+  p.cond_ksteps_last = (a->n_mels - 64 + kWgmmaK - 1) / kWgmmaK;
+  for (int i = 0; i < a->n_group; ++i) {
+    PK_CHECK_ARG(a->cond_rows[i] >= 0 && a->cond_rows[i] < a->n_group, "cond_rows[%d] out of range", i);
+    p.cmap[i] = a->cond_rows[i];
+  }
+  constexpr float kLog2e = 1.4426950408889634f;
+  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
+  for (int blk = 0; blk < C / 64; ++blk) {
+    for (int i = 0; i < 64; ++i) {
+      p.gate_c[128 * blk + i] = -2.f * kLog2e * a->bias1[128 * blk + i];
+      p.gate_c[128 * blk + 64 + i] = -kLog2e * a->bias1[128 * blk + 64 + i];
+    }
+  }
+  for (int i = 0; i < 2 * C; ++i) p.out_b[i] = a->bias2[i];
+  p.skip = a->skip;
+  p.x_hi = static_cast<const __nv_bfloat16*>(a->x_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->x_lo);
+  p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
+  const int grid = std::min(p.total_tiles, sm_count());
+  waveflow_forward_layer_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tx, tc, tw1, tw2, p);
+  PK_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PK_OK;
+}
+
+extern "C" int pk_waveflow_forward_layer(const pk_waveflow_forward_layer_args* a, pk_stream_t stream) {
+  using namespace pk;
+  using namespace pk::wf;
+  PK_CHECK_ARG(a != nullptr, "args is NULL");
+  PK_CHECK_ARG(a->batch > 0 && a->width > 0 && a->dilation >= 1 && a->dilation <= 128, "bad batch/width/dilation");
+  PK_CHECK_ARG(a->channels == 64 || a->channels == 128,
+               "the WaveFlow forward layer is built for 64 or 128 residual channels (got %d)", a->channels);
+  PK_CHECK_ARG(a->n_mels > 64 && a->n_mels <= 128 && (a->n_mels % 8) == 0, "n_mels must be in (64, 128], a multiple of 8");
+  PK_CHECK_ARG(a->n_group >= 2 && a->n_group <= kMaxGroup, "n_group must be 2..16");
+  PK_CHECK_ARG(a->cond_rows && a->x_hi && a->x_lo && a->cond_hi && a->cond_lo && a->w1_hi && a->w1_lo && a->w2_hi && a->w2_lo &&
+               a->bias1 && a->bias2 && a->skip, "NULL pointer in pk_waveflow_forward_layer_args");
+  PK_CHECK_ARG((a->y_hi == nullptr) == (a->y_lo == nullptr), "y_hi / y_lo: both or neither");
+  PK_CHECK_ARG(a->y_hi == nullptr || (a->y_hi != a->x_hi && a->y_lo != a->x_lo), "the layer cannot write its input in place");
+  return a->channels == 128 ? forward_layer_launch<128>(a, stream) : forward_layer_launch<64>(a, stream);
 }

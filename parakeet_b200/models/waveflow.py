@@ -1,12 +1,15 @@
-"""ConditionalWaveFlow inference on H100 - host side (reference parakeet/models/waveflow.py:714-909).
+"""ConditionalWaveFlow inference and density estimation on H100 - host side (reference parakeet/models/waveflow.py:714-909).
 
 Same constructor as the reference (`upsample_factors, n_flows, n_layers, n_group, channels, n_mels, kernel_size`), same
 state-dict keys (`encoder.{i}.{weight_g,weight_v,bias}`, `decoder.{f}.input_proj.*`,
 `decoder.{f}.resnet.{l}.{conv,condition_proj,out_proj}.*`, `decoder.{f}.output_proj.{weight,bias}`), `infer(mel)` and
-`predict(mel)`.  All arithmetic is in libparakeet_b200.so; fold / permute / row slicing are torch views and gathers.
+`predict(mel)`, `forward(audio, mel)` and WaveFlowLoss.  All arithmetic is in libparakeet_b200.so; fold / permute / row
+slicing are torch views and gathers.
 
 Supported this round: kernel_size (3, 3) and n_group in {8, 16} (height dilation 1 -> a 3-row causal buffer), which
-covers the shipped config (examples/waveflow/config.py).  Training (`forward`, WaveFlowLoss) is not implemented.
+covers the shipped config (examples/waveflow/config.py).  The density direction (`forward`: audio -> z, log-det, the
+held-out negative log-likelihood with WaveFlowLoss) runs for 64 or 128 channels and n_mels in (64, 128]; its backward (the
+training step) is not implemented.
 """
 import ctypes as C_
 import os
@@ -279,6 +282,91 @@ class ConditionalWaveFlow(Layer):
             z = x
         return z.transpose(1, 2).reshape(B, -1)
 
+    def _check_forward(self, audio_len, cond_len):
+        if not self._eligible():
+            raise NotImplementedError("ConditionalWaveFlow.forward needs 64 or 128 channels, 64 < n_mels <= 128 (a multiple of 8) "
+                                      "and at most 8 layers per flow")
+        if audio_len > cond_len:
+            raise ValueError(f"audio ({audio_len} samples) is longer than its condition ({cond_len} samples)")
+
+    def decoder_forward(self, audio, condition):
+        """WaveFlow.forward (:627-672): audio (B, T), upsampled condition (B, n_mels, T_c >= T) ->
+        (z (B, T // n_group * n_group), log_det_jacobian (1,)).  The counterpart of inverse(z, condition)."""
+        self._check_forward(audio.shape[-1], condition.shape[-1])
+        ops._require_cuda(audio, condition)
+        pk = self._pack()
+        L = _lib.lib()
+        G, C, NL = self.n_group, self.channels, self.n_layers
+        pruned = audio.shape[-1] // G * G                                                 # _trim (:617-625)
+        B, W, dev = audio.shape[0], pruned // G, audio.device
+        x = audio[:, :pruned].float().reshape(B, W, G).transpose(1, 2).contiguous()     # (B, H, W): sample t = w*G + h
+        cond = condition[:, :, :pruned].float().reshape(B, self.n_mels, W, G).permute(0, 3, 2, 1).contiguous()
+        cond_s = Split.from_f32(cond)                                                     # (B, H, W, n_mels), never permuted
+        bufs = [Split.zeros((B * (G + 1), W, C), dev) for _ in range(2)]                  # 2 zero rows + G - 1 net rows each
+        skip = torch.empty(B, G - 1, W, C, device=dev)
+        log_det = torch.zeros(1, device=dev)
+        partials = torch.empty(_lib.WAVEFLOW_TAIL_PARTIALS, device=dev)
+        counter = torch.zeros(1, dtype=torch.int32, device=dev)
+        x_next = torch.empty_like(x)
+        st = _stream()
+        i32 = lambda v: (C_.c_int32 * G)(*v)
+
+        def tail(fw, perm, nxt, x_in, x_out):
+            a = _lib.WaveflowForwardTailArgs()
+            a.batch, a.width, a.channels, a.n_group = B, W, C, G
+            keep = dict(perm=i32(perm))
+            a.perm = C_.cast(keep["perm"], C_.c_void_p)
+            a.x, a.x_next = _ptr(x_in), _ptr(x_out)
+            if fw is not None:
+                h = fw["host"]
+                a.skip, a.out_w, a.out_b = _ptr(skip), h["out_w"].ctypes.data, h["out_b"].ctypes.data
+                a.log_det, a.partials, a.counter = _ptr(log_det), _ptr(partials), _ptr(counter)
+            if nxt is not None:
+                a.in_w, a.in_b = nxt["host"]["in_w"].ctypes.data, nxt["host"]["in_b"].ctypes.data
+                a.next_hi, a.next_lo = _ptr(bufs[0].hi), _ptr(bufs[0].lo)
+            _lib.check(L.pk_waveflow_forward_tail(C_.byref(a), st), "pk_waveflow_forward_tail")
+
+        flows = pk["flows"]
+        tail(None, list(range(G)), flows[0], x, None)                                    # input_proj of the first flow
+        cmap = list(range(G))                                                             # condition height of height h
+        for fi, fw in enumerate(flows):
+            rows = i32(cmap)
+            src, dst = bufs
+            for l, lay in enumerate(fw["layers"]):
+                f = lay["fused"]
+                a = _lib.WaveflowForwardLayerArgs()
+                a.batch, a.width, a.channels, a.n_mels, a.n_group, a.dilation = B, W, C, self.n_mels, G, 2 ** l
+                a.cond_rows = C_.cast(rows, C_.c_void_p)
+                a.x_hi, a.x_lo = _ptr(src.hi), _ptr(src.lo)
+                a.cond_hi, a.cond_lo = _ptr(cond_s.hi), _ptr(cond_s.lo)
+                w1 = f["w1"][0]                                                           # variant 0: ring slot s = kernel row s
+                a.w1_hi, a.w1_lo, a.w2_hi, a.w2_lo = _ptr(w1[0]), _ptr(w1[1]), _ptr(f["w2"][0]), _ptr(f["w2"][1])
+                a.bias1, a.bias2 = f["b1"].ctypes.data, f["b2"].ctypes.data
+                if l + 1 < NL:
+                    a.y_hi, a.y_lo = _ptr(dst.hi), _ptr(dst.lo)
+                a.skip, a.skip_init = _ptr(skip), 1 if l == 0 else 0
+                _lib.check(L.pk_waveflow_forward_layer(C_.byref(a), st), "pk_waveflow_forward_layer")
+                src, dst = dst, src
+            # output_proj, z, log-det, the permutation of the heights and the next flow's input_proj (into bufs[0])
+            tail(fw, self.perms[fi], flows[fi + 1] if fi + 1 < len(flows) else None, x, x_next)
+            x, x_next = x_next, x
+            cmap = [cmap[j] for j in self.perms[fi]]                                      # geo.shuffle_dim(condition, 2, perm)
+        return x.transpose(1, 2).reshape(B, -1), log_det
+
+    def forward(self, audio, mel):
+        """ConditionalWaveFlow.forward (:759-783): audio (B, T), mel (B, n_mels, T') -> (z (B, T // n_group * n_group),
+        log_det_jacobian (1,)), the condition being the encoder output WITHOUT the trim of infer (256 T' samples)."""
+        t_cond = mel.shape[-1]
+        for f in self.upsample_factors:
+            t_cond *= f
+        self._check_forward(audio.shape[-1], t_cond)
+        if not (audio.is_cuda and mel.is_cuda):
+            raise _lib.PkError("ConditionalWaveFlow needs CUDA tensors (no CPU fallback)")
+        audio, mel = audio.contiguous().float(), mel.contiguous().float()
+        fn = lambda a_, m_: self.decoder_forward(a_, self.encode(m_, trim_conv_artifact=False))
+        z, log_det = self._graphs.run(("forward", audio.shape[0], audio.shape[-1], mel.shape[-1]), fn, [audio, mel])
+        return z.clone(), log_det.clone()
+
     def infer(self, mel, z=None):
         """reference :784-805; the noise z (B, T_c) may be supplied (parity tests), else torch.randn."""
         if not mel.is_cuda:
@@ -318,3 +406,27 @@ class ConditionalWaveFlow(Layer):
         """reference :807-825: numpy mel (n_mels, T') -> numpy audio."""
         mel = torch.as_tensor(np.asarray(mel), dtype=torch.float32, device=self.device).unsqueeze(0)
         return self.infer(mel)[0].cpu().numpy()
+
+
+class WaveFlowLoss:
+    """WaveFlowLoss (reference :855-891): (sum z^2 / (2 sigma^2) - log_det_jacobian) / numel(z) + log(2 pi) / 2 + log(sigma),
+    shape (1,) - the negative log-likelihood per sample of a Gaussian prior.  sum z^2 is pk_sq_sum (double accumulator)."""
+
+    def __init__(self, sigma=1.0):
+        if not sigma > 0:
+            raise ValueError("sigma must be positive")
+        self.sigma = float(sigma)
+
+    def forward(self, z, log_det_jacobian):
+        ops._require_cuda(z, log_det_jacobian)
+        L = _lib.lib()
+        z = z.contiguous().float()
+        log_det_jacobian = log_det_jacobian.contiguous().float()
+        sq = torch.zeros(1, dtype=torch.float64, device=z.device)
+        loss = torch.empty(1, device=z.device)
+        st = _stream()
+        _lib.check(L.pk_sq_sum(_ptr(z), z.numel(), _ptr(sq), st), "pk_sq_sum")
+        _lib.check(L.pk_waveflow_nll(_ptr(sq), _ptr(log_det_jacobian), z.numel(), self.sigma, _ptr(loss), st), "pk_waveflow_nll")
+        return loss
+
+    __call__ = forward

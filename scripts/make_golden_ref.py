@@ -9,6 +9,7 @@ into them (which also checks every state-dict key and shape against the referenc
 REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to these vectors.
 
     python scripts/make_golden_ref.py        # needs /root/reference; writes tests/golden/ref_executed*.npz
+    python scripts/make_golden_ref.py waveflow_forward   # only tests/golden/ref_executed_waveflow_forward.npz
 """
 import importlib.util
 import os
@@ -261,6 +262,31 @@ def waveflow(out):
         out["wf128_x"] = ref128.decoder.inverse(T(z3), cond3).numpy()
 
 
+def waveflow_forward(out):
+    """The density direction: the reference's own ConditionalWaveFlow.forward (encoder without trim, WaveFlow.forward with its
+    permutations and log-det sum) and WaveFlowLoss at two sigmas.  (a) 64 channels, seed-4 parameters, B = 2, 22 mel frames,
+    audio of 22 * 256 - 5 samples (shorter than the condition, not a multiple of 16: W = 351); (b) the shipped 128-channel
+    config, seed-5 parameters, B = 1, 22 frames."""
+    from oracle import waveflow as owf
+    from parakeet.models.waveflow import ConditionalWaveFlow, WaveFlowLoss
+    g = torch.Generator().manual_seed(46)
+    for tag, channels, seed, batch, samples in (("a", 64, 4, 2, 22 * 256 - 5), ("b", 128, 5, 1, 22 * 256)):
+        ref = ConditionalWaveFlow(upsample_factors=[16, 16], n_flows=8, n_layers=8, n_group=16, channels=channels, n_mels=80,
+                                  kernel_size=[3, 3])
+        ref.eval()
+        params = owf.synth_params(seed, channels=channels)
+        check_keys(ref, params, f"ConditionalWaveFlow({channels})")
+        ref.set_state_dict(params)
+        mel = torch.randn(batch, 80, 22, generator=g) * 0.5 - 3
+        audio = (torch.rand(batch, samples, generator=g) * 2 - 1) * 0.5
+        with torch.no_grad():
+            z, log_det = ref(T(audio), T(mel))
+            out[f"{tag}_mel"], out[f"{tag}_audio"] = mel.numpy(), audio.numpy()
+            out[f"{tag}_z"], out[f"{tag}_log_det"] = z.numpy(), log_det.numpy().reshape(1)
+            for sigma in (1.0, 0.7):
+                out[f"{tag}_loss_sigma{sigma}"] = np.asarray(WaveFlowLoss(sigma)(z, log_det).numpy(), dtype=np.float32).reshape(1)
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -331,6 +357,16 @@ def sampled(models):
 
 
 def main():
+    if sys.argv[1:] == ["waveflow_forward"]:
+        uninstall = loader.install(paddle_standin.build())
+        try:
+            fwd = {}
+            waveflow_forward(fwd)
+        finally:
+            uninstall()
+        np.savez_compressed(os.path.join(GOLD, "ref_executed_waveflow_forward.npz"), **fwd)
+        print("ref_executed_waveflow_forward.npz", os.path.getsize(os.path.join(GOLD, "ref_executed_waveflow_forward.npz")) // 1024, "KB")
+        return
     uninstall = loader.install(paddle_standin.build())
     try:
         small, models = {}, {}

@@ -268,6 +268,9 @@ def build():
 
         def forward(self, x):
             s, p, d, g = self.args
+            if isinstance(p, tuple) and len(p) == 4:            # paddle: [top, bottom, left, right] (asymmetric, e.g. causal)
+                x = TF.pad(x, (p[2], p[3], p[0], p[1]))
+                p = 0
             return TF.conv2d(x, self.weight, self.bias, s, p, d, g)
     nn.Conv2D = Conv2D
 

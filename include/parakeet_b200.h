@@ -587,6 +587,46 @@ int pk_stft_loss_grad(const float* xre, const float* xim, const float* yre, cons
 int pk_frames_overlap_add(const float* frames_grad, const float* window, int32_t batch, int32_t frames, int32_t n_fft, int32_t hop,
                           int32_t t, float* dx, pk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * SpeedySpeech (reference: parakeet/models/speedyspeech/speedyspeech.py).  Everything but the residual blocks reuses the
+ * kernels above (pk_conv_gemm, pk_duration_post, pk_length_regulate, pk_embed_pe, pk_leaky_relu).
+ * ------------------------------------------------------------------------------------------------------------ */
+/* One ResidualBlock.forward (speedyspeech.py:21-39) in eval mode: h_0 = x, h_i = relu(conv_i(h_{i-1}) + bias_i) * scale_i +
+ * shift_i for i = 1..n_convs, y = x + h_n.  scale / shift are the BatchNorm1D affine (gamma / sqrt(var + eps), beta - mean *
+ * scale).  The convs are undilated with pad_left zero rows before the sequence and taps - 1 - pad_left after it (Paddle's
+ * padding="same").  x fp32 (batch, t, channels) and its split planes; w*_hi / w*_lo the packed weight planes [channels,
+ * taps * channels] (ops.pack_weight of the Paddle [out, in, k] weight); bias / scale / shift fp32 [channels].  lens (device
+ * int32 [batch], or NULL = t): each utterance is computed as if it were alone - the intermediate is zero outside [0, lens[b])
+ * and rows t >= lens[b] of y are written as 0; rows of x at t >= lens[b] must already be 0.  y fp32 and split planes, not
+ * aliasing x.  The intermediate of a two-conv block stays in shared memory.  channels must be 128 (PK_ERR_UNSUPPORTED
+ * otherwise), taps 1..4, n_convs 1 or 2. */
+typedef struct pk_ss_residual_block_args {
+  int32_t batch;
+  int32_t t;
+  int32_t channels;
+  int32_t n_convs;
+  int32_t taps;
+  int32_t pad_left;
+  const int32_t* lens;
+  const float* x;
+  const void* x_hi;
+  const void* x_lo;
+  const void* w1_hi;
+  const void* w1_lo;
+  const float* bias1;
+  const float* scale1;
+  const float* shift1;
+  const void* w2_hi;
+  const void* w2_lo;
+  const float* bias2;
+  const float* scale2;
+  const float* shift2;
+  float* y;
+  void* y_hi;
+  void* y_lo;
+} pk_ss_residual_block_args;
+int pk_ss_residual_block(const pk_ss_residual_block_args* args, pk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

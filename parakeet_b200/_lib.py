@@ -113,6 +113,14 @@ class WaveflowForwardTailArgs(C.Structure):
 WAVEFLOW_TAIL_PARTIALS = 1024      # fp32 scratch elements pk_waveflow_forward_tail needs
 
 
+class SsResidualBlockArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("t", C.c_int32), ("channels", C.c_int32), ("n_convs", C.c_int32), ("taps", C.c_int32),
+                ("pad_left", C.c_int32), ("lens", C.c_void_p), ("x", C.c_void_p), ("x_hi", C.c_void_p), ("x_lo", C.c_void_p),
+                ("w1_hi", C.c_void_p), ("w1_lo", C.c_void_p), ("bias1", C.c_void_p), ("scale1", C.c_void_p), ("shift1", C.c_void_p),
+                ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p), ("bias2", C.c_void_p), ("scale2", C.c_void_p), ("shift2", C.c_void_p),
+                ("y", C.c_void_p), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p)]
+
+
 def _declare(L):
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     sigs = {
@@ -131,6 +139,7 @@ def _declare(L):
         "pk_waveflow_forward_layer": [C.POINTER(WaveflowForwardLayerArgs), vp],
         "pk_waveflow_forward_tail": [C.POINTER(WaveflowForwardTailArgs), vp],
         "pk_waveflow_nll": [vp, vp, i64, f32, vp, vp],
+        "pk_ss_residual_block": [C.POINTER(SsResidualBlockArgs), vp],
         "pk_pwg_tail": [vp, vp, vp, vp, vp, vp, f32, i64, vp, vp],
         "pk_embed_pe": [vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp],
         "pk_layer_norm": [vp, vp, vp, f32, vp, i32, i32, i32, vp, vp, vp, vp],

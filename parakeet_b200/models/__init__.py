@@ -1,3 +1,4 @@
 from .fastspeech2 import FastSpeech2, FastSpeech2Inference, FastSpeech2Loss  # noqa: F401
 from .parallel_wavegan import PWGDiscriminator, PWGGenerator, PWGInference  # noqa: F401
+from .speedyspeech import SpeedySpeech, SpeedySpeechInference  # noqa: F401
 from .waveflow import ConditionalWaveFlow, WaveFlowLoss  # noqa: F401

@@ -304,6 +304,38 @@ def variance_embed_add(hs, pitch, energy, wp, bp, we, be, lens=None):
     return y
 
 
+def ss_residual_block(x, xs, convs, taps, pad_left, lens=None):
+    """SpeedySpeech ResidualBlock (pk_ss_residual_block): x fp32 (B, T, 128) and its Split xs -> (y fp32, y Split).
+    convs: one or two dicts(w=packed Split, b=bias, s=BN scale, t=BN shift), each fp32 [128] on the device."""
+    _require_cuda(x, xs.hi)
+    B, T, Cc = x.shape
+    y = torch.empty_like(x)
+    ys = Split.empty((B, T, Cc), x.device)
+    a = _lib.SsResidualBlockArgs()
+    a.batch, a.t, a.channels, a.n_convs, a.taps, a.pad_left = B, T, Cc, len(convs), taps, pad_left
+    a.lens = lens.data_ptr() if lens is not None else None
+    a.x, a.x_hi, a.x_lo = x.data_ptr(), xs.hi.data_ptr(), xs.lo.data_ptr()
+    c1 = convs[0]
+    a.w1_hi, a.w1_lo, a.bias1, a.scale1, a.shift1 = c1["w"].hi.data_ptr(), c1["w"].lo.data_ptr(), c1["b"].data_ptr(), \
+        c1["s"].data_ptr(), c1["t"].data_ptr()
+    if len(convs) == 2:
+        c2 = convs[1]
+        a.w2_hi, a.w2_lo, a.bias2, a.scale2, a.shift2 = c2["w"].hi.data_ptr(), c2["w"].lo.data_ptr(), c2["b"].data_ptr(), \
+            c2["s"].data_ptr(), c2["t"].data_ptr()
+    a.y, a.y_hi, a.y_lo = y.data_ptr(), ys.hi.data_ptr(), ys.lo.data_ptr()
+    _lib.check(_lib.lib().pk_ss_residual_block(C.byref(a), _stream()), "pk_ss_residual_block")
+    return y, ys
+
+
+def relu_split(x):
+    """ReLU of an fp32 tensor into split planes (pk_leaky_relu with slope 0)."""
+    _require_cuda(x)
+    x = x.contiguous()
+    ys = Split.empty(tuple(x.shape), x.device)
+    _lib.check(_lib.lib().pk_leaky_relu(_ptr(x), x.numel(), 0.0, None, _ptr(ys.hi), _ptr(ys.lo), _stream()), "pk_leaky_relu")
+    return ys
+
+
 def zscore(x, mu, sigma, inverse=False):
     x = x.contiguous().float()
     y = torch.empty_like(x)

@@ -10,6 +10,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
 
     python scripts/make_golden_ref.py        # needs /root/reference; writes tests/golden/ref_executed*.npz
     python scripts/make_golden_ref.py waveflow_forward   # only tests/golden/ref_executed_waveflow_forward.npz
+    python scripts/make_golden_ref.py speedyspeech       # only tests/golden/ref_executed_speedyspeech.npz
 """
 import importlib.util
 import os
@@ -287,6 +288,46 @@ def waveflow_forward(out):
                 out[f"{tag}_loss_sigma{sigma}"] = np.asarray(WaveFlowLoss(sigma)(z, log_det).numpy(), dtype=np.float32).reshape(1)
 
 
+def speedyspeech(out):
+    """The reference's own SpeedySpeech (eval), SpeedySpeechInference (+ ZScore) and expand: (small) 3 encoder / 2 decoder
+    blocks with tones - inference with and without tones, the wrapper, and the batched teacher-forced forward over padded
+    tokens; (shipped) the baker yaml's 10 / 18 blocks at one short utterance."""
+    from oracle import speedyspeech as oss
+    from parakeet.models.speedyspeech.speedyspeech import SpeedySpeech, SpeedySpeechInference
+    from parakeet.modules.normalizer import ZScore
+    g = torch.Generator().manual_seed(31)
+    for tag, cfg, seed, tone_size in (("small", oss.SMALL_CFG, 6, 7), ("shipped", oss.SHIPPED_CFG, 7, None)):
+        ref = SpeedySpeech(vocab_size=40, tone_size=tone_size, **cfg)
+        ref.eval()
+        params = oss.synth_params(seed, cfg, tone_size=tone_size)
+        keys = check_keys(ref, params, f"SpeedySpeech({tag})")
+        out[f"{tag}_keys"] = np.asarray(keys)
+        out[f"{tag}_shapes"] = np.asarray([",".join(map(str, params[k].shape)) for k in keys])
+        ref.set_state_dict(params)
+        text = torch.randint(1, 40, (12 if tag == "shipped" else 23,), generator=g)
+        out[f"{tag}_inf_text"] = text.numpy()
+        with torch.no_grad():
+            out[f"{tag}_inf_mel"] = ref.inference(T(text)).numpy()
+            if tone_size:
+                tones = torch.randint(1, tone_size, tuple(text.shape), generator=g)
+                out[f"{tag}_inf_tones"] = tones.numpy()
+                out[f"{tag}_inf_tone_mel"] = ref.inference(T(text), T(tones)).numpy()
+                mu, sigma = torch.randn(80, generator=g), torch.rand(80, generator=g) + 0.5
+                out[f"{tag}_wr_mu"], out[f"{tag}_wr_sigma"] = mu.numpy(), sigma.numpy()
+                out[f"{tag}_wr_logmel"] = SpeedySpeechInference(ZScore(T(mu), T(sigma)), ref)(T(text), T(tones)).numpy()
+                lengths = [17, 9, 14]
+                text_b = torch.zeros(3, 17, dtype=torch.int64)
+                tones_b = torch.zeros(3, 17, dtype=torch.int64)
+                dur_b = torch.zeros(3, 17, dtype=torch.int64)
+                for i, n in enumerate(lengths):
+                    text_b[i, :n] = torch.randint(1, 40, (n,), generator=g)
+                    tones_b[i, :n] = torch.randint(1, tone_size, (n,), generator=g)
+                    dur_b[i, :n] = torch.randint(0, 7, (n,), generator=g)
+                decoded, pred = ref(T(text_b), T(tones_b), T(dur_b))
+                out[f"{tag}_fwd_text"], out[f"{tag}_fwd_tones"], out[f"{tag}_fwd_durations"] = text_b.numpy(), tones_b.numpy(), dur_b.numpy()
+                out[f"{tag}_fwd_decoded"], out[f"{tag}_fwd_pred_durations"] = decoded.numpy(), pred.numpy()
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -357,15 +398,17 @@ def sampled(models):
 
 
 def main():
-    if sys.argv[1:] == ["waveflow_forward"]:
+    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech}
+    if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:
-            fwd = {}
-            waveflow_forward(fwd)
+            vecs = {}
+            single[sys.argv[1]](vecs)
         finally:
             uninstall()
-        np.savez_compressed(os.path.join(GOLD, "ref_executed_waveflow_forward.npz"), **fwd)
-        print("ref_executed_waveflow_forward.npz", os.path.getsize(os.path.join(GOLD, "ref_executed_waveflow_forward.npz")) // 1024, "KB")
+        name = f"ref_executed_{sys.argv[1]}.npz"
+        np.savez_compressed(os.path.join(GOLD, name), **vecs)
+        print(name, os.path.getsize(os.path.join(GOLD, name)) // 1024, "KB")
         return
     uninstall = loader.install(paddle_standin.build())
     try:

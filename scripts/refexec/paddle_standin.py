@@ -235,26 +235,37 @@ def build():
     nn.Linear = Linear
 
     def _pad(p, k, d):
+        """-> (dilation, left, right).  padding="same" is Paddle's rule (models/speedyspeech.py `paddle_same_conv`): undilated,
+        the extra row of an even kernel on the right."""
         if isinstance(p, str):
             assert p.lower() == "same"
-            return (k - 1) // 2 * d
+            from parakeet_b200.models.speedyspeech import paddle_same_conv
+            return paddle_same_conv(k, d)
         if isinstance(p, (list, tuple)):
             assert len(p) == 1 or p[0] == p[1]
-            return int(p[0])
-        return int(p)
+            return d, int(p[0]), int(p[0])
+        return d, int(p), int(p)
 
     class Conv1D(Layer):
         def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, padding_mode="zeros",
                      weight_attr=None, bias_attr=None, data_format="NCL"):
             super().__init__()
-            assert data_format == "NCL" and padding_mode == "zeros"
+            assert data_format in ("NCL", "NLC") and padding_mode == "zeros"
             self.weight = torch.nn.Parameter(torch.zeros(out_channels, in_channels // groups, kernel_size))
             self.bias = torch.nn.Parameter(torch.zeros(out_channels)) if bias_attr is not False else None
-            self.args = (stride, _pad(padding, kernel_size, dilation), dilation, groups)
+            d, left, right = _pad(padding, kernel_size, dilation)
+            self.args = (stride, (left, right), d, groups)
+            self._nlc = data_format == "NLC"
 
         def forward(self, x):
-            s, p, d, g = self.args
-            return TF.conv1d(x, self.weight, self.bias, s, p, d, g)
+            s, (left, right), d, g = self.args
+            if self._nlc:
+                x = x.transpose(1, 2)
+            if left == right:
+                y = TF.conv1d(x, self.weight, self.bias, s, left, d, g)
+            else:
+                y = TF.conv1d(TF.pad(x, (left, right)), self.weight, self.bias, s, 0, d, g)
+            return y.transpose(1, 2) if self._nlc else y
     nn.Conv1D = Conv1D
 
     class Conv2D(Layer):
@@ -311,8 +322,14 @@ def build():
             self.register_buffer("_mean", torch.zeros(num_features))
             self.register_buffer("_variance", torch.ones(num_features))
             self._eps, self._momentum = epsilon, momentum
+            self._nlc = data_format == "NLC"
 
         def forward(self, x):
+            if self._nlc:
+                return self._ncl(x.transpose(1, 2)).transpose(1, 2)
+            return self._ncl(x)
+
+        def _ncl(self, x):
             if self.training:
                 # restated Paddle semantics (oracle/README.md): normalise with the biased batch variance; running statistics
                 # move by (1 - momentum) with momentum 0.9 and keep the BIASED variance

@@ -17,7 +17,27 @@ import torch.nn.functional as F
 
 TILE = 256          # rows of a band-table window: both 128-row tiles of the window multiply with the SAME 16-frame window of P
 KWIN = 16
-EDGE = 128          # rows next to either end of an utterance that carry their own coefficients (edge effects reach < 128)
+EDGE = 128          # rows next to either end of an utterance that carry their own coefficients (exact while edge_reach <= EDGE)
+
+
+def edge_reach(scales):
+    """Samples next to either end of an utterance whose upsampled conditioning depends on the zero padding of the FIR stages
+    after the first: sum over i >= 1 of s_i * prod_{k > i} s_k.  The first stage's padding needs no table rows of its own:
+    it is the same as zero frames outside [0, frames), which the kernel reads as zero."""
+    reach = 0
+    for s in scales[1:]:
+        reach = (reach + 1) * s
+    return reach
+
+
+def frame_rate_exact(scales):
+    """True when the compact band tables reproduce the upsampled conditioning exactly: a 256-row tile touches at most two
+    frames, so the 8-frame windows of its rows fit its 16-frame K window (hop >= 256, which pk_pwg_residual_layer_fc also
+    requires), and the padding effects stay inside the EDGE rows that carry their own coefficients."""
+    hop = 1
+    for s in scales:
+        hop *= s
+    return hop >= TILE and edge_reach(scales) <= EDGE
 
 
 def window_start(t0, hop):

@@ -192,7 +192,7 @@ class PWGGenerator(Layer):
             self._graphs.clear()          # captured forwards point into the old workspace
             dev = self.device
             ws = dict(xa=Split.zeros((B, T, 64), dev), xb=Split.zeros((B, T, 64), dev),
-                      c=Split.empty((B, T, self.aux_channels), dev) if not self._frame_cond() else None,   # sample-rate planes: legacy path only
+                      c=Split.empty((B, T, self.aux_channels), dev) if not self._uses_frame_cond() else None,   # sample-rate path only
                       skip=torch.empty(B, T, 64, dtype=torch.float32, device=dev),
                       conv_in=torch.empty(B, T // self.upsample_factor, self.aux_channels, dtype=torch.float32, device=dev))
             self._ws[key] = ws
@@ -203,6 +203,13 @@ class PWGGenerator(Layer):
         """Frame-rate conditioning (csrc/pwg_fc.cu) is the default; PK_PWG_FRAME_COND=0 selects the round-1 kernel that
         streams the sample-rate conditioning planes (kept for A/B measurements)."""
         return os.environ.get("PK_PWG_FRAME_COND", "1") != "0"
+
+    def _uses_frame_cond(self):
+        """Whether this generator runs the frame-rate path: the switch above is on and the compact band tables are exact for
+        its upsample_scales (hop >= 256 and the upsampler's padding reaches at most EDGE samples into an utterance;
+        _pwg_frame_cond.frame_rate_exact).  Other configs, e.g. [2, 16, 8] or a hop of 64, run the sample-rate kernel."""
+        from ._pwg_frame_cond import frame_rate_exact
+        return self._frame_cond() and frame_rate_exact(self.upsample_scales)
 
     # -- forward (reference :445-472) ------------------------------------------------------------------------------
     def forward(self, x, c, lens=None):
@@ -224,9 +231,15 @@ class PWGGenerator(Layer):
         if lens is not None:
             assert lens.dtype == torch.int32 and lens.is_cuda
             # host copy of the lengths: they select the band-table end blocks (lengths are host data in the reference's callers
-            # too, synthesize.py:96-104)
-            lens_key = tuple(int(v) for v in torch.div(lens, self.upsample_factor, rounding_mode="floor").cpu().tolist())
-        eager = not self._frame_cond() or getattr(self, "_layer_events", None) is not None
+            # too, synthesize.py:96-104).  An utterance is a whole number of frames: a length that is not, or one past T, would
+            # give band tables and conditioning that disagree with the rows the layer kernels treat as live.
+            hop = self.upsample_factor
+            lens_h = lens.cpu().tolist() if lens.dim() == 1 and lens.shape[0] == B else None
+            if lens_h is None or any(v < 0 or v > T or v % hop for v in lens_h):
+                raise _lib.PkError(f"lens must hold {B} lengths in samples, each a multiple of hop {hop} in [0, {T}] "
+                                   f"(got {lens.cpu().tolist()})")
+            lens_key = tuple(v // hop for v in lens_h)
+        eager = not self._uses_frame_cond() or getattr(self, "_layer_events", None) is not None
         if eager:
             return self._forward_impl(x, c, lens, lens_key)
         fn = lambda x_, c_, *l_: self._forward_impl(x_, c_, l_[0] if l_ else None, lens_key)   # noqa: E731
@@ -238,7 +251,7 @@ class PWGGenerator(Layer):
         pk = self._pack()
         B, _, T = x.shape
         frames = c.shape[-1] - 2 * self.aux_context_window
-        fcond = self._frame_cond()
+        fcond = self._uses_frame_cond()
         if self._ws and (next(iter(self._ws.values()))["c"] is None) != fcond:
             self._ws.clear()                                         # the toggle changed between calls
             self._graphs.clear()

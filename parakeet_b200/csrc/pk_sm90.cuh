@@ -36,6 +36,8 @@ __device__ __forceinline__ void fence_barrier_init() {
 // ----------------------------------------------------------------------------------------------------------------
 // all generic-proxy writes of this thread -> visible to later async-proxy (TMA / wgmma) reads
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// the same for this thread's shared-memory writes only (e.g. a tile staged for a TMA store); global writes are not waited for
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------------------------
 // TMA

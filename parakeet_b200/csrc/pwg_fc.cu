@@ -312,7 +312,8 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
           sts_u32(ystage + kQTile + off, ol);
         }
       }
-      fence_proxy_async_all();
+      // (shared memory only: a fence over all of the thread's writes would also wait for the previous tile's skip red.adds)
+      fence_proxy_async_shared();
       named_bar_sync(3 + wg, 128);
       const bool store_lane = (threadIdx.x & 127) == 0;
       if (store_lane) {

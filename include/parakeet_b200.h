@@ -627,6 +627,95 @@ typedef struct pk_ss_residual_block_args {
 } pk_ss_residual_block_args;
 int pk_ss_residual_block(const pk_ss_residual_block_args* args, pk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * WaveFlow training step (reference: examples/waveflow/train.py:95-118 Experiment.train_batch; ConditionalWaveFlow.forward
+ * models/waveflow.py:759-783, Flow.forward :465-494, ResidualBlock.forward :209-226, UpsampleNet.forward :103-132,
+ * WaveFlowLoss :855-891; loss.backward() and paddle.optimizer.Adam).  The GEMMs run through pk_conv_gemm; these kernels sit
+ * between them.  "Net layout": fp32 or split planes (batch * (n_group + 1), width, ld), utterance b's net row j (the flow's
+ * height j + 1, j < n_group - 1) at row b * (n_group + 1) + j, its last two rows zero.  "Input layout": the same rows two
+ * further down, i.e. two zero rows before each utterance's net rows (the causal height padding of the 3x3 conv).  Flow
+ * inputs / outputs x fp32 (batch, n_group, width), sample t = w * n_group + h.  No reduction uses atomics: repeated calls give
+ * identical bits.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* dst[i] = split(idx[i] >= 0 ? src[idx[i]] : 0), i < n: packs GEMM operands from the flat folded weights. */
+int pk_waveflow_train_gather_split(const float* src, const int32_t* idx, int64_t n, void* dst_hi, void* dst_lo, pk_stream_t stream);
+/* input_proj (Flow._predict_parameters :453, 1x1 Conv2D 1 -> c) of flow input rows 0 .. n_group - 2: h fp32 (net layout, c; pad rows 0) and
+ * x_hi / x_lo split planes (input layout, c; only net rows written).  w, bias device fp32 [c]. */
+int pk_waveflow_train_input_fwd(const float* x, const float* w, const float* bias, int32_t batch, int32_t n_group, int32_t width, int32_t c,
+                                float* h, void* x_hi, void* x_lo, pk_stream_t stream);
+/* ResidualBlock.forward (:197-226) after out_proj, and ResidualNet.forward's skip sum (:355-360): out fp32 (net layout, 2c) = (res | skip); h += res; skip = skip_part (skip_init)
+ * or skip += skip_part; x_hi / x_lo (input layout, or NULL): the next layer's input planes of h's net rows. */
+int pk_waveflow_train_update(const float* out, int32_t batch, int32_t n_group, int32_t width, int32_t c, float* h, float* skip, int32_t skip_init,
+                             void* x_hi, void* x_lo, pk_stream_t stream);
+/* Flow._predict_parameters / _transform (:455-463) + WaveFlow.forward's permutation (:664): (logs, b) = output_proj(skip) (out_w device [2][c],
+ * out_b device [2]); z = x for height 0, x exp(logs) + b above; x_next[:, inv_perm[h]] = z[:, h] (inv_perm device int32
+ * [n_group], the inverse of the reference's perm); logs fp32 (batch, n_group - 1, width). */
+int pk_waveflow_train_tail_fwd(const float* skip, const float* out_w, const float* out_b, const float* x, const int32_t* inv_perm, int32_t batch,
+                               int32_t n_group, int32_t width, int32_t c, float* x_next, float* logs, pk_stream_t stream);
+/* Backward of pk_waveflow_train_tail_fwd.  The gradient of x_next is dy, or y_coef * y when dy is NULL (the last flow: y = z
+ * and y_coef = 1 / (sigma^2 numel(z)) from WaveFlowLoss); dlogs is added to every logs gradient (-1 / numel(z): the log-det
+ * term).  Writes dx (batch, n_group, width) - the direct path only, overwritten - dparams fp32 (net layout, 2) = d(logs, b),
+ * dskip fp32 (net layout, c) and the same as split planes at ds[row * ds_ld + ds_col0 + c].  Pad rows are not written. */
+int pk_waveflow_forward_tail_bwd(const float* skip, const float* out_w, const float* out_b, const float* x, const int32_t* inv_perm, const float* dy,
+                                 const float* y, float y_coef, float dlogs, int32_t batch, int32_t n_group, int32_t width, int32_t c, float* dx,
+                                 float* dparams, float* dskip, void* ds_hi, void* ds_lo, int32_t ds_ld, int32_t ds_col0, pk_stream_t stream);
+/* Backward of input_proj's data path: dx[b, j, w] += sum_c w[c] dh[(b, j), w, c] for j < n_group - 1 (dh net layout); xcol
+ * fp32 (net layout, 1) <- x[b, j, w] on net rows (pad rows not written), the operand of the input_proj weight gradient. */
+int pk_waveflow_train_input_bwd(const float* dh, const float* x, const float* w, int32_t batch, int32_t n_group, int32_t width, int32_t c,
+                                float* dx, float* xcol, pk_stream_t stream);
+/* out[i * os_i + j * os_j] (+)= sum_r a[r * lda + i] * (b ? b[r * ldb + j] : 1), i < ka, j < kb, ka * kb <= 256: bias and small
+ * weight gradients in a fixed order (per-block partials in scratch, then their sum). */
+int pk_waveflow_train_outer_sum(const float* a, int32_t lda, int32_t ka, const float* b, int32_t ldb, int32_t kb, int64_t rows, float* scratch,
+                                int64_t scratch_len, float* out, int64_t os_i, int64_t os_j, int32_t accumulate, pk_stream_t stream);
+/* Backward of one untrimmed UpsampleNet stage (:103-132): y = leaky_relu(Conv2DTranspose(x; w [3][2 factor], bias), slope), x
+ * (batch, c, t_in), y / dy (batch, c, t_in * factor).  dpre: scratch of y's size; dx (or NULL) (batch, c, t_in); dw [3 * 2 factor]
+ * and db [1] overwritten; scratch fp32 for the fixed-order partials. */
+int pk_waveflow_upsample_bwd(const float* x, const float* y, const float* dy, const float* w, int32_t batch, int32_t c, int32_t t_in,
+                             int32_t factor, float slope, float* dpre, float* dx, float* scratch, int64_t scratch_len, float* dw, float* db,
+                             pk_stream_t stream);
+/* The condition of one flow in the net layout: row (b, j) = height rows[j + 1] (rows device int32 [n_group], the composed
+ * permutation of the flows before it) of cond fp32 (batch, n_mels, t_cond) -> split planes (net layout, n_mels), pad rows 0. */
+int pk_waveflow_train_cond_gather(const float* cond, const int32_t* rows, int32_t batch, int32_t n_group, int32_t width, int32_t n_mels,
+                                  int32_t t_cond, void* hi, void* lo, pk_stream_t stream);
+/* Its adjoint, accumulated: dcond[b, m, w * n_group + rows[j + 1]] += dc[(b, j), w, m] (dc fp32 net layout). */
+int pk_waveflow_train_cond_scatter(const float* dc, const int32_t* rows, int32_t batch, int32_t n_group, int32_t width, int32_t n_mels,
+                                   int32_t t_cond, float* dcond, pk_stream_t stream);
+/* One layer boundary of the residual net's backward (ResidualBlock.forward :197-226 and ResidualNet.forward :339-360,
+ * differentiated), the mirror image of pk_waveflow_forward_layer, for channels C = 64 or 128, all net rows of all utterances:
+ *   has_gemm1: dx = dx + conv2d^T(dh_in) (the 3x3 conv of layer l, width dilation `dilation`; dh_in rows q + 1, q + 2 below the
+ *              last net row are the two zero rows of the net layout, so dh_in needs batch * (n_group + 1) + 2 rows), else dx = 0;
+ *              dx fp32 (net layout, C) is read and written in place and also written as split planes into columns [0, C) of a2.
+ *   has_gemm2: dz = a2 . W2 (K = 2C, a2 = [dx | dskip] split planes (net layout, 2C) whose columns [C, 2C) hold dskip);
+ *              dh_out = gate backward of dz with the pre-gate h fp32 (net layout, 2C) of layer l - 1, as split planes.
+ * dh_in / dh_out: split planes with row pitch dh_ld (2C columns each; e.g. column blocks of one (rows, W, n_layers * 2C)
+ * allocation).  w1: conv^T planes (C, 18 C), column ((s * 3 + t) * 2C + o) = conv.weight[o, c, 2 - s, 2 - t] of row c;
+ * w2: out_proj^T planes (C, 2C) = out_proj.weight[o, c] at (c, o).  Pad rows are not written. */
+typedef struct pk_waveflow_backward_layer_args {
+  int32_t batch;
+  int32_t width;
+  int32_t channels;
+  int32_t n_group;
+  int32_t dilation;
+  int32_t has_gemm1;
+  int32_t has_gemm2;
+  int32_t dh_ld;
+  const void* dh_in_hi;
+  const void* dh_in_lo;
+  const void* w1_hi;
+  const void* w1_lo;
+  const void* w2_hi;
+  const void* w2_lo;
+  float* dx;
+  void* a2_hi;
+  void* a2_lo;
+  const float* h;
+  void* dh_out_hi;
+  void* dh_out_lo;
+} pk_waveflow_backward_layer_args;
+int pk_waveflow_backward_layer(const pk_waveflow_backward_layer_args* args, pk_stream_t stream);
+/* WaveFlowLoss (:855-891) in a fixed order: loss[0] = (sum z^2 / (2 sigma^2) - sum logs) / n + log(2 pi) / 2 + log(sigma). */
+int pk_waveflow_train_loss(const float* z, int64_t n, const float* logs, int64_t n_logs, float sigma, float* loss, pk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -110,6 +110,13 @@ class WaveflowForwardTailArgs(C.Structure):
                 ("next_lo", C.c_void_p), ("log_det", C.c_void_p), ("partials", C.c_void_p), ("counter", C.c_void_p)]
 
 
+class WaveflowBackwardLayerArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32), ("n_group", C.c_int32), ("dilation", C.c_int32),
+                ("has_gemm1", C.c_int32), ("has_gemm2", C.c_int32), ("dh_ld", C.c_int32), ("dh_in_hi", C.c_void_p), ("dh_in_lo", C.c_void_p),
+                ("w1_hi", C.c_void_p), ("w1_lo", C.c_void_p), ("w2_hi", C.c_void_p), ("w2_lo", C.c_void_p), ("dx", C.c_void_p),
+                ("a2_hi", C.c_void_p), ("a2_lo", C.c_void_p), ("h", C.c_void_p), ("dh_out_hi", C.c_void_p), ("dh_out_lo", C.c_void_p)]
+
+
 WAVEFLOW_TAIL_PARTIALS = 1024      # fp32 scratch elements pk_waveflow_forward_tail needs
 
 
@@ -191,6 +198,18 @@ def _declare(L):
         "pk_waveflow_row_out": [vp, vp, vp, vp, i64, i32, i32, i32, vp, i64, vp],
         "pk_spectral_loss_sums": [vp, vp, i64, f32, vp, vp],
         "pk_stft": [vp, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp, i32, f32, vp, i32, vp, i32, f32, vp, f32, vp],
+        "pk_waveflow_train_gather_split": [vp, vp, i64, vp, vp, vp],
+        "pk_waveflow_train_input_fwd": [vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp],
+        "pk_waveflow_train_update": [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, vp],
+        "pk_waveflow_train_tail_fwd": [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp],
+        "pk_waveflow_forward_tail_bwd": [vp, vp, vp, vp, vp, vp, vp, f32, f32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp],
+        "pk_waveflow_train_input_bwd": [vp, vp, vp, i32, i32, i32, i32, vp, vp, vp],
+        "pk_waveflow_train_outer_sum": [vp, i32, i32, vp, i32, i32, i64, vp, i64, vp, i64, i64, i32, vp],
+        "pk_waveflow_upsample_bwd": [vp, vp, vp, vp, i32, i32, i32, i32, f32, vp, vp, vp, i64, vp, vp, vp],
+        "pk_waveflow_train_cond_gather": [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp],
+        "pk_waveflow_train_cond_scatter": [vp, vp, i32, i32, i32, i32, i32, vp, vp],
+        "pk_waveflow_train_loss": [vp, i64, vp, i64, f32, vp, vp],
+        "pk_waveflow_backward_layer": [C.POINTER(WaveflowBackwardLayerArgs), vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(L, name)

@@ -8,8 +8,8 @@ slicing are torch views and gathers.
 
 Supported this round: kernel_size (3, 3) and n_group in {8, 16} (height dilation 1 -> a 3-row causal buffer), which
 covers the shipped config (examples/waveflow/config.py).  The density direction (`forward`: audio -> z, log-det, the
-held-out negative log-likelihood with WaveFlowLoss) runs for 64 or 128 channels and n_mels in (64, 128]; its backward (the
-training step) is not implemented.
+held-out negative log-likelihood with WaveFlowLoss) runs for 64 or 128 channels and n_mels in (64, 128]; its training step is
+parakeet_b200.training.WaveFlowTrainStep.
 """
 import ctypes as C_
 import os

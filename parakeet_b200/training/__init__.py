@@ -1,3 +1,4 @@
 from .fs2_step import FastSpeech2TrainStep  # noqa: F401
 from .flat import FlatBuffers  # noqa: F401
 from .pwg_step import PWGTrainStep  # noqa: F401
+from .waveflow_step import WaveFlowTrainStep  # noqa: F401

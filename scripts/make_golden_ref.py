@@ -11,6 +11,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py        # needs /root/reference; writes tests/golden/ref_executed*.npz
     python scripts/make_golden_ref.py waveflow_forward   # only tests/golden/ref_executed_waveflow_forward.npz
     python scripts/make_golden_ref.py speedyspeech       # only tests/golden/ref_executed_speedyspeech.npz
+    python scripts/make_golden_ref.py waveflow_train     # only tests/golden/ref_executed_waveflow_train.npz
 """
 import importlib.util
 import os
@@ -288,6 +289,32 @@ def waveflow_forward(out):
                 out[f"{tag}_loss_sigma{sigma}"] = np.asarray(WaveFlowLoss(sigma)(z, log_det).numpy(), dtype=np.float32).reshape(1)
 
 
+def waveflow_train(out):
+    """The training gradients: torch autograd through the reference's own ConditionalWaveFlow.forward (its weight-normed
+    Conv2D / Conv2DTranspose layers, so the gradients are those of weight_g / weight_v) and WaveFlowLoss (sigma 1), as
+    examples/waveflow/train.py:95-118 runs them.  64 channels, 2 flows x 8 layers (the reference's Flow takes its height
+    dilations from a table of 8), n_group 16, 2 clips x 6 frames of 6 * 256 - 3 samples (W = 95).  Tensors of up to 4096
+    elements are stored in full, larger ones as every stride-th element (stride = numel // 4096) plus their L2 norm."""
+    from oracle import waveflow as owf
+    from parakeet.models.waveflow import ConditionalWaveFlow, WaveFlowLoss
+    g = torch.Generator().manual_seed(47)
+    ref = ConditionalWaveFlow(upsample_factors=[16, 16], n_flows=2, n_layers=8, n_group=16, channels=64, n_mels=80, kernel_size=[3, 3])
+    params = owf.synth_params(6, n_flows=2, n_layers=8, channels=64)
+    check_keys(ref, params, "ConditionalWaveFlow(64, 2 flows)")
+    ref.set_state_dict(params)
+    mel = torch.randn(2, 80, 6, generator=g) * 0.5 - 3
+    audio = (torch.rand(2, 6 * 256 - 3, generator=g) * 2 - 1) * 0.5
+    z, log_det = ref(T(audio), T(mel))
+    loss = WaveFlowLoss(1.0)(z, log_det)
+    loss.backward()
+    out["mel"], out["audio"] = mel.numpy(), audio.numpy()
+    out["loss"] = np.asarray(loss.detach().numpy(), dtype=np.float32).reshape(1)
+    for k, v in ref.named_parameters():
+        gk = (v.grad if v.grad is not None else torch.zeros_like(v)).detach().reshape(-1)
+        out["grad/" + k] = gk[::max(1, gk.numel() // 4096)].numpy().astype(np.float32)
+        out["gradnorm/" + k] = np.asarray(float(gk.double().norm()))
+
+
 def speedyspeech(out):
     """The reference's own SpeedySpeech (eval), SpeedySpeechInference (+ ZScore) and expand: (small) 3 encoder / 2 decoder
     blocks with tones - inference with and without tones, the wrapper, and the batched teacher-forced forward over padded
@@ -398,7 +425,7 @@ def sampled(models):
 
 
 def main():
-    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech}
+    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

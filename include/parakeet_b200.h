@@ -545,6 +545,27 @@ int pk_dropout(const float* x, const void* x_hi, const void* x_lo, int64_t n, fl
                float* y, void* y_hi, void* y_lo, pk_stream_t stream);
 int pk_adam(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
             int32_t step, float grad_scale, pk_stream_t stream);
+/* Speaker conditioning of the multi-speaker training step (fastspeech2.py:148-152 spk_embedding_table = nn.Embedding(num_speakers,
+ * D, padding_idx=0); :395-401 and _integrate_with_spk_embed :560-590: F.normalize(p=2, axis=1, epsilon) then the "concat" / "add"
+ * projection, whose GEMMs run through pk_conv_gemm).  Speaker ids are int64 on the device and never read on the host; ids equal
+ * to padding_idx, or outside [0, num_speakers), embed to zeros and receive no gradient.  No atomics: fixed summation orders. */
+/* e[b] = table[ids[b]] / max(||table[ids[b]]||, eps) (batch, d); norms[b] = ||table[ids[b]]|| (0 for padding ids), saved for
+ * pk_spk_normalize_bwd. */
+int pk_spk_embed_fwd(const float* table, int32_t num_speakers, int32_t d, const int64_t* ids, int32_t batch, int32_t padding_idx,
+                     float eps, float* e, float* norms, pk_stream_t stream);
+/* out[b, j] = sum over ALL t rows of dx[b, row, col0 + j], j < ncols, dx (batch, t, c) fp32: the gradient of a per-utterance
+ * vector broadcast over time.  dhs (or NULL): columns [0, dhs_cols) of dx copied to a contiguous (batch, t, dhs_cols) in the
+ * same pass (the hs part of the concat projection's input gradient). */
+int pk_spk_time_sum(const float* dx, int32_t batch, int32_t t, int32_t c, int32_t col0, int32_t ncols, float* dhs, int32_t dhs_cols,
+                    float* out, pk_stream_t stream);
+/* backward of pk_spk_embed_fwd's normalisation: dx = (g - e (e . g)) / ||x|| (g / eps where ||x|| <= eps); rows of padding ids
+ * are exact zeros. */
+int pk_spk_normalize_bwd(const float* e, const float* norms, const float* g, const int64_t* ids, int32_t batch, int32_t num_speakers,
+                         int32_t padding_idx, int32_t d, float eps, float* dx, pk_stream_t stream);
+/* dense embedding gradient (Paddle's sparse=False): dtable[r] = sum over b ascending with ids[b] == r of de[b], every row written
+ * (absent speakers and padding_idx as zeros), e.g. straight into the table's slice of a flat gradient buffer. */
+int pk_spk_table_grad(const float* de, const int64_t* ids, int32_t batch, int32_t num_speakers, int32_t d, int32_t padding_idx,
+                      float* dtable, pk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Parallel WaveGAN training step (reference: PWGUpdater.update_core, models/parallel_wavegan/parallel_wavegan_updater.py:76-153;

@@ -175,6 +175,10 @@ def _declare(L):
         "pk_length_regulate_bwd": [vp, vp, i32, i32, i32, i32, vp, vp],
         "pk_scalar_conv_wgrad": [vp, vp, i32, i32, i32, i32, vp, vp, vp],
         "pk_adam": [vp, vp, vp, vp, i64, f32, f32, f32, f32, i32, f32, vp],
+        "pk_spk_embed_fwd": [vp, i32, i32, vp, i32, i32, f32, vp, vp, vp],
+        "pk_spk_time_sum": [vp, i32, i32, i32, i32, i32, vp, i32, vp, vp],
+        "pk_spk_normalize_bwd": [vp, vp, vp, vp, i32, i32, i32, i32, f32, vp, vp],
+        "pk_spk_table_grad": [vp, vp, i32, i32, i32, i32, vp, vp],
         "pk_gate_fwd": [vp, i64, i32, vp, vp, vp, vp],
         "pk_gate_bwd": [vp, vp, i64, i32, vp, vp],
         "pk_leaky_relu": [vp, i64, f32, vp, vp, vp, vp],

@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 FS2_FIELDS = ("text", "text_lengths", "speech", "speech_lengths", "durations", "pitch", "energy")
+FS2_MS_FIELDS = FS2_FIELDS + ("spk_id",)          # the multi-speaker recipes (train.py:66-71)
 
 
 def read_metadata(path):
@@ -64,10 +65,27 @@ def batch_sequences(sequences, pad_value=0):
     return out
 
 
+def read_speaker_id_map(path):
+    """The recipe's `speaker_id_map.txt` (one `<speaker> <id>` pair per line; examples/fastspeech2/train.py:67-71, which takes
+    num_speakers = the number of lines) -> dict speaker name -> int id, in file order.  num_speakers = len(result)."""
+    out = {}
+    with open(path, "rt", encoding="utf-8") as f:
+        for n, line in enumerate(f, 1):
+            parts = line.strip().split()
+            if not parts:
+                continue
+            if len(parts) != 2:
+                raise ValueError(f"{path}:{n}: expected '<speaker> <id>', got {line.strip()!r}")
+            out[parts[0]] = int(parts[1])
+    return out
+
+
 def fastspeech2_batch(examples, device=None):
     """fastspeech2_single_spk_batch_fn (am_batch_fn.py:60-99): list of examples -> dict of tensors
     text (B, Tmax) i64, text_lengths (B,) i64, durations (B, Tmax) i64, speech (B, Lmax, n_mels) f32, speech_lengths (B,) i64,
-    pitch / energy (B, Tmax, 1) f32 (a trailing feature axis is added to 1-D pitch / energy, the shape the model expects)."""
+    pitch / energy (B, Tmax, 1) f32 (a trailing feature axis is added to 1-D pitch / energy, the shape the model expects).
+    When the examples carry `spk_id` (FeatureTable(..., fields=FS2_MS_FIELDS)) this is fastspeech2_multi_spk_batch_fn
+    (am_batch_fn.py:102-145) and the dict also holds spk_id (B,) i64."""
     def feat(name):
         arrs = [np.asarray(e[name], dtype=np.float32) for e in examples]
         return [a[:, None] if a.ndim == 1 else a for a in arrs]
@@ -79,6 +97,8 @@ def fastspeech2_batch(examples, device=None):
         "speech_lengths": np.asarray([e["speech_lengths"] for e in examples], dtype=np.int64),
         "pitch": batch_sequences(feat("pitch")), "energy": batch_sequences(feat("energy")),
     }
+    if "spk_id" in examples[0]:
+        batch["spk_id"] = np.asarray([e["spk_id"] for e in examples], dtype=np.int64).reshape(len(examples))
     out = {k: torch.from_numpy(v) for k, v in batch.items()}
     if device is not None:
         out = {k: v.to(device, non_blocking=True) for k, v in out.items()}

@@ -399,6 +399,47 @@ def axpy_(a, x, y):
     _lib.check(_lib.lib().pk_axpy(float(a), _ptr(x), x.numel(), _ptr(y), _stream()), "pk_axpy")
 
 
+def spk_embed_fwd(table, ids, padding_idx=0, eps=1e-12):
+    """Speaker-table lookup + F.normalize (pk_spk_embed_fwd): table fp32 (N, D), ids int64 (B,) on the device ->
+    (e fp32 (B, D), norms fp32 (B,) for spk_normalize_bwd)."""
+    _require_cuda(table, ids)
+    table, ids = table.contiguous(), ids.contiguous()
+    B, (N, D) = ids.numel(), table.shape
+    e = torch.empty(B, D, dtype=torch.float32, device=table.device)
+    norms = torch.empty(B, dtype=torch.float32, device=table.device)
+    _lib.check(_lib.lib().pk_spk_embed_fwd(_ptr(table), N, D, _ptr(ids), B, padding_idx, float(eps), _ptr(e), _ptr(norms), _stream()),
+               "pk_spk_embed_fwd")
+    return e, norms
+
+
+def spk_time_sum(dx, col0, ncols, dhs_cols=0):
+    """dx fp32 (B, T, C) -> (sum over all T rows of dx[..., col0:col0 + ncols] (B, ncols), dx[..., :dhs_cols] contiguous or None)."""
+    _require_cuda(dx)
+    assert dx.is_contiguous() and dx.dtype == torch.float32
+    B, T, Cc = dx.shape
+    out = torch.empty(B, ncols, dtype=torch.float32, device=dx.device)
+    dhs = torch.empty(B, T, dhs_cols, dtype=torch.float32, device=dx.device) if dhs_cols else None
+    _lib.check(_lib.lib().pk_spk_time_sum(_ptr(dx), B, T, Cc, col0, ncols, _ptr(dhs), dhs_cols, _ptr(out), _stream()), "pk_spk_time_sum")
+    return out, dhs
+
+
+def spk_normalize_bwd(e, norms, g, ids, num_speakers, padding_idx=0, eps=1e-12):
+    """Backward of spk_embed_fwd's normalisation: (B, D) gradient w.r.t. the looked-up table rows (zeros for padding ids)."""
+    B, D = e.shape
+    dx = torch.empty_like(e)
+    _lib.check(_lib.lib().pk_spk_normalize_bwd(_ptr(e), _ptr(norms), _ptr(g), _ptr(ids), B, num_speakers, padding_idx, D, float(eps),
+                                               _ptr(dx), _stream()), "pk_spk_normalize_bwd")
+    return dx
+
+
+def spk_table_grad(de, ids, out, padding_idx=0):
+    """Dense table gradient (pk_spk_table_grad) written into out (N, D), e.g. a view of a flat gradient buffer."""
+    assert out.is_contiguous() and de.is_contiguous()
+    N, D = out.shape
+    _lib.check(_lib.lib().pk_spk_table_grad(_ptr(de), _ptr(ids), ids.numel(), N, D, padding_idx, _ptr(out), _stream()), "pk_spk_table_grad")
+    return out
+
+
 def dropout(x, p, seed, site, step, out_f32=True, out_split=False, inplace=False, step_dev=None):
     """pk_dropout: x fp32 tensor or Split (any shape, contiguous) -> (y fp32 or None, y Split or None).  p == 0 is not a
     special case here (callers skip the call)."""

@@ -57,8 +57,11 @@ class FastSpeech2TrainStep:
         launches of 10-40 us); bucketing samplers repeat shapes, so do synthetic benchmarks."""
         if not model.device.type == "cuda":
             raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
-        if model.spk_embed_dim is not None or model.tone_embed_dim is not None:
-            raise NotImplementedError("the training step covers the single-speaker recipe (speaker / tone conditioning is inference-only)")
+        if model.tone_embed_dim is not None:
+            raise NotImplementedError("the training step does not cover tone conditioning (tone_embed_dim): no recipe trains with tones")
+        # multi-speaker recipes (aishell3, vctk): batch["spk_id"] -> spk_embedding_table -> F.normalize -> spk_projection
+        self.spk = model.spk_embed_dim is not None
+        self._order = self._BATCH_ORDER + (("spk_id",) if self.spk else ())
         self.m = model
         self.lr, self.b1, self.b2, self.eps = learning_rate, beta1, beta2, epsilon
         self.sg_pitch = model.stop_gradient_from_pitch_predictor if stop_gradient_from_pitch_predictor is None else stop_gradient_from_pitch_predictor
@@ -394,6 +397,41 @@ class FastSpeech2TrainStep:
         return g
 
     # ------------------------------------------------------------------------------------------------------------
+    # speaker conditioning (fastspeech2.py:395-401, _integrate_with_spk_embed :560-590): hs' is computed on every Tmax row -
+    # the padded rows are live (bias + projected speaker), the predictors' convolutions read them and they get gradient
+    # ------------------------------------------------------------------------------------------------------------
+    def spk_fwd(self, hs, hs_split, spk_id):
+        m = self.m
+        B, T, A = hs.shape
+        e, norms = ops.spk_embed_fwd(self.P("spk_embedding_table.weight"), spk_id, m.padding_idx)
+        S = dict(ids=spk_id, e=e, norms=norms)
+        if m.spk_embed_integration_type == "add":
+            S["e_split"] = Split.from_f32(e.reshape(B, 1, -1))
+            proj, _ = self.layer_fwd(S["e_split"], "spk_projection.weight", "spk_projection.bias", "lin")
+            hs2 = hs.clone()
+            ops.axpy_(1.0, proj.expand(B, T, A).contiguous(), hs2)
+            return hs2, Split.from_f32(hs2), S
+        S["cat"] = Split.from_f32(torch.cat([hs, e.unsqueeze(1).expand(B, T, e.shape[1])], dim=-1))          # layout only
+        hs2, hs2_split = self.layer_fwd(S["cat"], "spk_projection.weight", "spk_projection.bias", "lin", f32=True, split=True)
+        return hs2, hs2_split, S
+
+    def spk_bwd(self, dhs2, S):
+        """dhs2: gradient w.r.t. hs' (fp32 (B, T, A)).  Writes the projection's and the table's gradients, returns d hs."""
+        m = self.m
+        B, T, A = dhs2.shape
+        D = m.spk_embed_dim
+        if m.spk_embed_integration_type == "add":
+            dproj, _ = ops.spk_time_sum(dhs2, 0, A)                                  # the broadcast over time, all Tmax rows
+            de = self.layer_bwd(dproj.reshape(B, 1, A), S["e_split"], "spk_projection.weight", "spk_projection.bias", "lin")
+            dhs = dhs2
+        else:
+            dcat = self.layer_bwd(dhs2, S["cat"], "spk_projection.weight", "spk_projection.bias", "lin")
+            de, dhs = ops.spk_time_sum(dcat, A, D, dhs_cols=A)                       # one pass over the (B, T, A + D) gradient
+        dx = ops.spk_normalize_bwd(S["e"], S["norms"], de.reshape(B, D).contiguous(), S["ids"], m.num_speakers, m.padding_idx)
+        ops.spk_table_grad(dx, S["ids"], self.grads["spk_embedding_table.weight"], m.padding_idx)
+        return dhs
+
+    # ------------------------------------------------------------------------------------------------------------
     # one training step
     # ------------------------------------------------------------------------------------------------------------
     def forward_backward(self, batch):
@@ -412,6 +450,13 @@ class FastSpeech2TrainStep:
         ps = batch["pitch"].to(dev, torch.float32).reshape(B, T).contiguous()
         es = batch["energy"].to(dev, torch.float32).reshape(B, T).contiguous()
         ys = batch["speech"].to(dev, torch.float32).contiguous()
+        if batch.get("spembs") is not None:
+            raise NotImplementedError("training with utterance-level speaker embeddings (spembs) is not supported: the recipes pass spk_id")
+        spk_id = None
+        if self.spk:
+            if batch.get("spk_id") is None:
+                raise ValueError("this model has a speaker embedding table: the batch needs spk_id (int64, (B,))")
+            spk_id = batch["spk_id"].to(dev, torch.int64).reshape(B).contiguous()
         A, odim = m.adim, m.odim
         # ---- forward (train mode) ----
         R = self.rates
@@ -419,6 +464,8 @@ class FastSpeech2TrainStep:
         if R["transformer_enc_positional_dropout_rate"] > 0:
             self.drop(x, R["transformer_enc_positional_dropout_rate"], self.site(0, 0, 0), inplace=True)
         hs, hs_split, S_enc = self.stack_fwd(x, "encoder.", m.elayers, ilens)
+        if self.spk:
+            hs, hs_split, S_spk = self.spk_fwd(hs, hs_split, spk_id)
         p_raw, S_p = self.pred_fwd("pitch_predictor.", m.cfg["pitch"][0], hs_split)
         e_raw, S_e = self.pred_fwd("energy_predictor.", m.cfg["energy"][0], hs_split)
         d_raw, S_d = self.pred_fwd("duration_predictor.", m.cfg["dur"][0], hs_split)
@@ -523,6 +570,8 @@ class FastSpeech2TrainStep:
         gp = self.pred_bwd(g_p, S_p, need_dx=not self.sg_pitch)
         if not self.sg_pitch:
             ops.axpy_(1.0, gp, dhs)
+        if self.spk:
+            dhs = self.spk_bwd(dhs, S_spk)
         dx = self.stack_bwd(dhs, S_enc)
         if R["transformer_enc_positional_dropout_rate"] > 0:
             self.drop(dx, R["transformer_enc_positional_dropout_rate"], self.site(0, 0, 0), inplace=True)
@@ -533,14 +582,17 @@ class FastSpeech2TrainStep:
 
     _BATCH_ORDER = ("text", "text_lengths", "speech", "speech_lengths", "durations", "pitch", "energy")
 
-    @classmethod
-    def _batch_key(cls, batch):
-        return tuple(tuple(batch[k].shape) for k in cls._BATCH_ORDER)
+    def _batch_key(self, batch):
+        return tuple(tuple(batch[k].shape) for k in self._order)
 
     def _forward_backward_graphed(self, batch):
         dev = self.m.device
-        order = self._BATCH_ORDER
-        dtypes = (torch.int64, torch.int64, torch.float32, torch.int64, torch.int64, torch.float32, torch.float32)
+        order = self._order            # + spk_id for speaker models: a replay reads the ids of the current batch
+        if self.spk and batch.get("spk_id") is None:
+            raise ValueError("this model has a speaker embedding table: the batch needs spk_id (int64, (B,))")
+        if batch.get("spembs") is not None:
+            raise NotImplementedError("training with utterance-level speaker embeddings (spembs) is not supported: the recipes pass spk_id")
+        dtypes = (torch.int64, torch.int64, torch.float32, torch.int64, torch.int64, torch.float32, torch.float32, torch.int64)
         tensors = [batch[k].to(dev, dt).contiguous() for k, dt in zip(order, dtypes)]
         key = tuple(tuple(t.shape) for t in tensors)
         self._zp.touch(key)                      # a replay does not pass through forward_backward: keep the LRU order honest

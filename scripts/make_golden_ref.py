@@ -12,6 +12,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py waveflow_forward   # only tests/golden/ref_executed_waveflow_forward.npz
     python scripts/make_golden_ref.py speedyspeech       # only tests/golden/ref_executed_speedyspeech.npz
     python scripts/make_golden_ref.py waveflow_train     # only tests/golden/ref_executed_waveflow_train.npz
+    python scripts/make_golden_ref.py fs2ms_train        # only tests/golden/ref_executed_fs2ms_train.npz
 """
 import importlib.util
 import os
@@ -184,6 +185,50 @@ def fastspeech2_training(out):
     bufs = dict(ref.named_buffers())
     for k in ("postnet.postnet.0.1._mean", "postnet.postnet.0.1._variance", "postnet.postnet.4.1._variance"):
         out["fs2_train_stat/" + k] = bufs[k].detach().numpy()
+
+
+FS2MS_TRAIN_SPK = (3, 0, 3)          # a repeated speaker and the padding id 0; speakers 1, 2, 4, 5 are absent
+FS2MS_TRAIN_KEEP = ("encoder.embed.0.weight", "encoder.encoders.3.feed_forward.w_2.weight", "encoder.after_norm.weight",
+                    "encoder.after_norm.bias", "duration_predictor.conv.0.0.weight", "pitch_predictor.conv.0.0.bias",
+                    "energy_predictor.conv.0.0.weight", "pitch_embed.0.weight", "decoder.encoders.0.self_attn.linear_q.weight",
+                    "feat_out.weight", "postnet.postnet.0.0.weight")
+
+
+def fastspeech2_multispeaker_training(out):
+    """The multi-speaker training gradients (aishell3 / vctk: spk_embed_dim 256, conf/default.yaml:76-77): the reference in
+    TRAIN mode (dropout 0), forward(..., spk_id=) as fastspeech2_updater.py:51-99 calls it, its FastSpeech2Loss and the sum of
+    the four losses, differentiated by autograd through the reference's code, for "concat" (a) and "add" (b).  3 utterances,
+    spk_id = FS2MS_TRAIN_SPK of 6 speakers.  The gradients of the speaker table and the projection bias are stored in full; the
+    projection weight and the tensors in FS2MS_TRAIN_KEEP as every stride-th element (stride = numel // 2048) plus their L2 norm."""
+    from oracle import fastspeech2 as ofs
+    from parakeet.models.fastspeech2.fastspeech2 import FastSpeech2, FastSpeech2Loss
+    zero = {k: 0.0 for k in ofs.DROPOUT_DEFAULTS}
+    for tag, st in (("a", "concat"), ("b", "add")):
+        ref = FastSpeech2(idim=80, odim=80, **ofs.LJSPEECH_MODEL_CFG, **zero, num_speakers=6, spk_embed_dim=256,
+                          spk_embed_integration_type=st, stop_gradient_from_pitch_predictor=True, stop_gradient_from_energy_predictor=False)
+        ref.train()
+        params = {k: v for k, v in ofs.add_speaker_tone_params(ofs.synth_params(1), 1, spk_type=st).items() if not k.startswith("tone_")}
+        check_keys(ref, params, f"FastSpeech2(spk {st})")
+        ref.set_state_dict(params)
+        b = ofs.synth_train_batch(13, [19, 27, 22])
+        spk = torch.tensor(FS2MS_TRAIN_SPK, dtype=torch.int64)
+        for k, v in b.items():
+            out[f"{tag}_{k}"] = v.numpy()
+        out[f"{tag}_spk_id"] = spk.numpy()
+        before, after, d_outs, p_outs, e_outs, ys, olens = ref(T(b["text"]), T(b["text_lengths"]), T(b["speech"]), T(b["speech_lengths"]),
+                                                               T(b["durations"]), T(b["pitch"]), T(b["energy"]), spk_id=T(spk))
+        l1, dur, pitch, energy = FastSpeech2Loss()(after_outs=after, before_outs=before, d_outs=d_outs, p_outs=p_outs, e_outs=e_outs,
+                                                   ys=ys, ds=T(b["durations"]), ps=T(b["pitch"]), es=T(b["energy"]),
+                                                   ilens=T(b["text_lengths"]), olens=olens)
+        (l1 + dur + pitch + energy).backward()
+        out[f"{tag}_loss"] = np.asarray([float(l1), float(dur), float(pitch), float(energy)], dtype=np.float64)
+        named = dict(ref.named_parameters())
+        for k in ("spk_embedding_table.weight", "spk_projection.weight", "spk_projection.bias") + FS2MS_TRAIN_KEEP:
+            gk = named[k].grad
+            gk = (gk if gk is not None else torch.zeros_like(named[k])).detach().reshape(-1)
+            stride = 1 if k in ("spk_embedding_table.weight", "spk_projection.bias") else max(1, gk.numel() // 2048)
+            out[f"{tag}_grad/{k}"] = gk[::stride].numpy().astype(np.float32)
+            out[f"{tag}_gradnorm/{k}"] = np.asarray(float(gk.double().norm()))
 
 
 def parallel_wavegan(out):
@@ -425,7 +470,8 @@ def sampled(models):
 
 
 def main():
-    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train}
+    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
+              "fs2ms_train": fastspeech2_multispeaker_training}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

@@ -648,6 +648,37 @@ typedef struct pk_ss_residual_block_args {
 } pk_ss_residual_block_args;
 int pk_ss_residual_block(const pk_ss_residual_block_args* args, pk_stream_t stream);
 
+/* SpeedySpeech training step (reference: SpeedySpeechUpdater.update_core, models/speedyspeech/speedyspeech_updater.py:48-85, with
+ * the model in train() mode).  The Conv1D / Linear forwards, data gradients and weight gradients run through pk_conv_gemm; these
+ * are the train-mode BatchNorm1D of the Conv1D -> ReLU -> BatchNorm1D units (speedyspeech.py:21-39) and the losses.  Every sum is
+ * taken over per-block partials in a fixed order (no atomics): repeated calls give identical bits.  c must be 128
+ * (PK_ERR_UNSUPPORTED otherwise).  scratch: fp32 workspace of at least 256 * ceil(rows / 128) elements. */
+/* BatchNorm1D in training mode on r (rows, c), r = relu(conv(x) + bias) as pk_conv_gemm wrote it: batch mean and biased variance
+ * over all rows, y = gamma * (r - mean) * rstd + beta (+ residual, the block input, on the last unit of a ResidualBlock) as fp32
+ * and / or split planes; run_mean / run_var (or both NULL) updated as momentum * running + (1 - momentum) * batch (Paddle's
+ * convention); save_mean / save_rstd [c] are kept for the backward. */
+int pk_ss_bn_train_fwd(const float* r, int64_t rows, int32_t c, const float* gamma, const float* beta, float eps, float momentum,
+                       float* run_mean, float* run_var, const float* residual, float* scratch, float* y, void* y_hi, void* y_lo,
+                       float* save_mean, float* save_rstd, pk_stream_t stream);
+/* Backward of ReLU -> BatchNorm1D in one go: from dy and the saved r / mean / rstd, dbeta = sum dy, dgamma = sum dy * xhat
+ * (overwritten), dr = gamma * rstd * (dy - mean(dy) - xhat * mean(dy * xhat)) * [r > 0] - the gradient at the conv's output -
+ * as fp32 and / or split planes (the operand of the data and weight gradient GEMMs), and dbias = sum dr (or NULL). */
+int pk_ss_bn_relu_bwd(const float* dy, const float* r, const float* mean, const float* rstd, const float* gamma, int64_t rows,
+                      int32_t c, float* scratch, float* dgamma, float* dbeta, float* dbias, float* dr, void* dr_hi, void* dr_lo,
+                      pk_stream_t stream);
+/* The losses of update_core :57-80 and their gradients.  decoded / feats fp32 (batch, l, odim), odim <= 80; num_frames /
+ * num_phones device int32 [batch]; pred_durations fp32 and durations int64 (batch, t).
+ *   l1       = sum |decoded - feats| * mask / (sum mask * odim)                              (modules/losses.py:60-100)
+ *   duration = sum huber(pred, log(max(durations, 1)), delta 1) * token mask / sum token mask (fluid.layers.huber_loss)
+ *   ssim     = 1 - mean over all batch * l * odim positions of the SSIM map of (decoded * mask, feats * mask): 11 x 11 Gaussian
+ *              window, sigma 1.5, zero padding 5 (modules/ssim.py:21-80), evaluated as two 1-D passes
+ * losses[4] = { l1 + ssim + duration, l1, duration, ssim }.  g_decoded (batch, l, odim) and g_durations (batch, t) receive
+ * d losses[0] / d decoded and / d pred_durations; both NULL computes the losses only (the evaluator, :110-157).
+ * scratch: fp32, at least 2 * batch * ceil(l / 16) elements, plus 3 * batch * l * odim when gradients are requested. */
+int pk_ss_loss(const float* decoded, const float* feats, const int32_t* num_frames, int32_t batch, int32_t l, int32_t odim,
+               const float* pred_durations, const int64_t* durations, const int32_t* num_phones, int32_t t, float* scratch,
+               float* losses, float* g_decoded, float* g_durations, pk_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * WaveFlow training step (reference: examples/waveflow/train.py:95-118 Experiment.train_batch; ConditionalWaveFlow.forward
  * models/waveflow.py:759-783, Flow.forward :465-494, ResidualBlock.forward :209-226, UpsampleNet.forward :103-132,

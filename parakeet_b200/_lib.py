@@ -147,6 +147,9 @@ def _declare(L):
         "pk_waveflow_forward_tail": [C.POINTER(WaveflowForwardTailArgs), vp],
         "pk_waveflow_nll": [vp, vp, i64, f32, vp, vp],
         "pk_ss_residual_block": [C.POINTER(SsResidualBlockArgs), vp],
+        "pk_ss_bn_train_fwd": [vp, i64, i32, vp, vp, f32, f32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp],
+        "pk_ss_bn_relu_bwd": [vp, vp, vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp, vp],
+        "pk_ss_loss": [vp, vp, vp, i32, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp],
         "pk_pwg_tail": [vp, vp, vp, vp, vp, vp, f32, i64, vp, vp],
         "pk_embed_pe": [vp, vp, i32, i32, vp, vp, vp, i32, i32, i32, vp, vp],
         "pk_layer_norm": [vp, vp, vp, f32, vp, i32, i32, i32, vp, vp, vp, vp],

@@ -11,8 +11,9 @@ encoder's last BatchNorm through pk_leaky_relu (slope 0), duration rounding thro
 through pk_length_regulate, the sinusoid position encoding through pk_embed_pe (alpha 1).  The embedding lookups are gathers
 (no arithmetic), as in FastSpeech2.  There is one device->host copy per call: the frame counts that size the decoder.
 
-Scope: eval-mode arithmetic only (BatchNorm uses its running statistics).  Training (train-mode BatchNorm, the losses of
-speedyspeech_updater.py) is not implemented: a forward in training mode raises PkError.  Every hidden size must be 128.
+Scope: eval-mode arithmetic only (BatchNorm uses its running statistics): a forward in training mode raises PkError.  The
+train-mode forward, the losses of speedyspeech_updater.py and the update live in training/speedyspeech_step.py
+(SpeedySpeechTrainStep), which does not go through this class's forward.  Every hidden size must be 128.
 """
 import math
 

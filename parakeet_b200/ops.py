@@ -440,6 +440,57 @@ def spk_table_grad(de, ids, out, padding_idx=0):
     return out
 
 
+def ss_scratch_elems(rows, batch=0, l=0, odim=0):
+    """fp32 elements of workspace the SpeedySpeech training kernels need for `rows` BatchNorm rows and a (batch, l, odim) loss."""
+    return max(256 * ((rows + 127) // 128), 2 * batch * ((l + 15) // 16) + 3 * batch * l * odim, 256)
+
+
+def ss_bn_train_fwd(r, gamma, beta, run_mean, run_var, scratch, residual=None, want_f32=True, want_split=True, eps=1e-5, momentum=0.9):
+    """Train-mode BatchNorm1D on r fp32 (..., 128) (pk_ss_bn_train_fwd) -> (y fp32 or None, y Split or None, mean, rstd);
+    run_mean / run_var are updated in place, residual (same shape as r) is added to y."""
+    _require_cuda(r, gamma, beta, scratch)
+    assert r.is_contiguous() and (residual is None or residual.is_contiguous())
+    c = r.shape[-1]
+    rows = r.numel() // c
+    y = torch.empty_like(r) if want_f32 else None
+    ys = Split.empty(tuple(r.shape), r.device) if want_split else None
+    mean = torch.empty(c, dtype=torch.float32, device=r.device)
+    rstd = torch.empty(c, dtype=torch.float32, device=r.device)
+    _lib.check(_lib.lib().pk_ss_bn_train_fwd(_ptr(r), rows, c, _ptr(gamma), _ptr(beta), eps, momentum, _ptr(run_mean), _ptr(run_var),
+                                             _ptr(residual), _ptr(scratch), _ptr(y), _ptr(ys.hi if ys else None),
+                                             _ptr(ys.lo if ys else None), _ptr(mean), _ptr(rstd), _stream()), "pk_ss_bn_train_fwd")
+    return y, ys, mean, rstd
+
+
+def ss_bn_relu_bwd(dy, r, mean, rstd, gamma, scratch, dgamma, dbeta, dbias=None, want_f32=False, want_split=True):
+    """Backward of ReLU -> train-mode BatchNorm1D (pk_ss_bn_relu_bwd): writes dgamma / dbeta / dbias [128] (views of a gradient
+    buffer) and returns (dr fp32 or None, dr Split or None), the gradient at the conv's output."""
+    _require_cuda(dy, r, scratch)
+    assert dy.is_contiguous() and r.is_contiguous() and dy.shape == r.shape
+    c = r.shape[-1]
+    dr = torch.empty_like(r) if want_f32 else None
+    drs = Split.empty(tuple(r.shape), r.device) if want_split else None
+    _lib.check(_lib.lib().pk_ss_bn_relu_bwd(_ptr(dy), _ptr(r), _ptr(mean), _ptr(rstd), _ptr(gamma), r.numel() // c, c, _ptr(scratch),
+                                            _ptr(dgamma), _ptr(dbeta), _ptr(dbias), _ptr(dr), _ptr(drs.hi if drs else None),
+                                            _ptr(drs.lo if drs else None), _stream()), "pk_ss_bn_relu_bwd")
+    return dr, drs
+
+
+def ss_loss(decoded, feats, num_frames, pred_durations, durations, num_phones, scratch, want_grads=True):
+    """SpeedySpeech's L1 + SSIM + duration losses (pk_ss_loss) -> (losses fp32 [4] = loss, l1, duration, ssim; d loss / d decoded
+    or None; d loss / d pred_durations or None).  num_frames / num_phones int32, durations int64, all on the device."""
+    _require_cuda(decoded, feats, num_frames, pred_durations, durations, num_phones, scratch)
+    assert decoded.is_contiguous() and feats.is_contiguous() and pred_durations.is_contiguous() and durations.is_contiguous()
+    B, L, odim = decoded.shape
+    T = pred_durations.shape[1]
+    losses = torch.empty(4, dtype=torch.float32, device=decoded.device)
+    g_dec = torch.empty_like(decoded) if want_grads else None
+    g_dur = torch.empty_like(pred_durations) if want_grads else None
+    _lib.check(_lib.lib().pk_ss_loss(_ptr(decoded), _ptr(feats), _ptr(num_frames), B, L, odim, _ptr(pred_durations), _ptr(durations),
+                                     _ptr(num_phones), T, _ptr(scratch), _ptr(losses), _ptr(g_dec), _ptr(g_dur), _stream()), "pk_ss_loss")
+    return losses, g_dec, g_dur
+
+
 def dropout(x, p, seed, site, step, out_f32=True, out_split=False, inplace=False, step_dev=None):
     """pk_dropout: x fp32 tensor or Split (any shape, contiguous) -> (y fp32 or None, y Split or None).  p == 0 is not a
     special case here (callers skip the call)."""

@@ -13,6 +13,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py speedyspeech       # only tests/golden/ref_executed_speedyspeech.npz
     python scripts/make_golden_ref.py waveflow_train     # only tests/golden/ref_executed_waveflow_train.npz
     python scripts/make_golden_ref.py fs2ms_train        # only tests/golden/ref_executed_fs2ms_train.npz
+    python scripts/make_golden_ref.py speedyspeech_train # only tests/golden/ref_executed_speedyspeech_train.npz
 """
 import importlib.util
 import os
@@ -400,6 +401,56 @@ def speedyspeech(out):
                 out[f"{tag}_fwd_decoded"], out[f"{tag}_fwd_pred_durations"] = decoded.numpy(), pred.numpy()
 
 
+def speedyspeech_train(out):
+    """The training gradients: torch autograd through the reference's own SpeedySpeech in train() mode (batch-statistics
+    BatchNorm1D, encodings.detach() in front of the duration predictor) and the reference's own masked_l1_loss, weighted_mean
+    and ssim, composed exactly as SpeedySpeechUpdater.update_core does (speedyspeech_updater.py:52-80; the updater class itself
+    needs the Trainer runtime and is not imported).  Small config (3 encoder / 2 decoder blocks), two tone table sizes
+    and batches with padded tokens, zero durations and utterances shorter than the longest; always with tones, because the
+    reference's forward casts `tones` unconditionally (speedyspeech.py:169) and cannot run without them.  Stored: the batch, the four losses,
+    every parameter gradient (tensors of up to 1024 elements in full, larger ones as every stride-th element, stride = numel //
+    1024, plus their L2 norm) and the new running statistics."""
+    import paddle
+    import paddle.nn.functional as F
+    from paddle.fluid.layers import huber_loss
+    from oracle import speedyspeech as oss
+    from oracle import speedyspeech_train as ost
+    from parakeet.models.speedyspeech.speedyspeech import SpeedySpeech
+    from parakeet.modules.losses import masked_l1_loss, weighted_mean
+    from parakeet.modules.ssim import ssim
+    cfg = oss.SMALL_CFG
+    for tag, seed, tone_size, lens in (("a", 8, 7, [13, 7, 10]), ("b", 9, 5, [16, 9, 12, 14])):
+        ref = SpeedySpeech(vocab_size=40, tone_size=tone_size, **cfg)
+        ref.train()
+        params = oss.synth_params(seed, cfg, tone_size=tone_size)
+        check_keys(ref, params, f"SpeedySpeech(train, {tag})")
+        ref.set_state_dict(params)
+        out[f"{tag}/seed"], out[f"{tag}/tone_size"] = np.asarray(seed), np.asarray(tone_size)
+        batch = ost.synth_batch(seed + 100, lens, tone_size=tone_size)
+        for k, v in batch.items():
+            out[f"{tag}/batch/{k}"] = v.numpy()
+        decoded, predicted_durations = ref(text=T(batch["phones"]), tones=T(batch["tones"]),
+                                           durations=T(batch["durations"]))
+        target_mel = T(batch["feats"])
+        spec_mask = F.sequence_mask(T(batch["num_frames"]), dtype=target_mel.dtype).unsqueeze(-1)
+        text_mask = F.sequence_mask(T(batch["num_phones"]), dtype=predicted_durations.dtype)
+        l1_loss = masked_l1_loss(decoded, target_mel, spec_mask)
+        target_durations = paddle.maximum(T(batch["durations"]).astype(predicted_durations.dtype), paddle.to_tensor([1.0]))
+        duration_loss = weighted_mean(huber_loss(predicted_durations, paddle.log(target_durations), delta=1.0), text_mask)
+        ssim_loss = 1.0 - ssim((decoded * spec_mask).unsqueeze(1), (target_mel * spec_mask).unsqueeze(1))
+        loss = l1_loss + ssim_loss + duration_loss
+        loss.backward()
+        for k, v in dict(loss=loss, l1_loss=l1_loss, duration_loss=duration_loss, ssim_loss=ssim_loss).items():
+            out[f"{tag}/{k}"] = np.asarray(float(v.detach().reshape(-1)[0]))
+        for k, v in ref.named_parameters():
+            gk = (v.grad if v.grad is not None else torch.zeros_like(v)).detach().reshape(-1)
+            out[f"{tag}/grad/{k}"] = gk[::max(1, gk.numel() // 1024)].numpy().astype(np.float32)
+            out[f"{tag}/gradnorm/{k}"] = np.asarray(float(gk.double().norm()))
+        for k, v in ref.named_buffers():
+            if k.endswith(("_mean", "_variance")):
+                out[f"{tag}/stat/{k}"] = v.detach().numpy().astype(np.float32)
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -471,7 +522,7 @@ def sampled(models):
 
 def main():
     single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
-              "fs2ms_train": fastspeech2_multispeaker_training}
+              "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

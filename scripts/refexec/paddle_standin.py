@@ -59,7 +59,17 @@ class Tensor(torch.Tensor):
         return torch.Tensor.repeat(self, *reps)
 
     def unsqueeze(self, axis):
+        if isinstance(axis, (list, tuple)):                 # paddle accepts a list of axes, applied in order
+            out = self
+            for a in axis:
+                out = torch.Tensor.unsqueeze(out, a)
+            return out
         return torch.Tensor.unsqueeze(self, axis)
+
+    @property
+    def size(self):
+        """paddle: Tensor.size is the element count (an int); torch: Tensor.size(dim) is a method.  Both spellings work."""
+        return _Size(self)
 
     def squeeze(self, axis=None):
         return torch.Tensor.squeeze(self) if axis is None else torch.Tensor.squeeze(self, axis)
@@ -96,6 +106,16 @@ class Tensor(torch.Tensor):
 
 
 Tensor._counter = 0
+
+
+class _Size(int):
+    def __new__(cls, t):
+        obj = super().__new__(cls, t.numel())
+        obj._shape = t.shape
+        return obj
+
+    def __call__(self, dim=None):
+        return self._shape if dim is None else self._shape[dim]
 
 
 def T(x):
@@ -171,6 +191,7 @@ def build():
     sig.stft = p_stft
     P.signal = sig
     P.subtract = lambda a, b: T(a - b)
+    P.maximum = lambda a, b: T(torch.maximum(a, b))
     P.get_default_dtype = lambda: "float32"
     P.multiply = lambda a, b: T(a * b)
     P.add = lambda a, b: T(a + b)
@@ -473,6 +494,20 @@ def build():
     F.normalize = lambda x, p=2, axis=1, epsilon=1e-12: T(TF.normalize(x, p=p, dim=axis, eps=epsilon))
     F.pad = lambda x, pad, mode="constant", value=0.0, data_format="NCL": T(TF.pad(x, tuple(pad), mode=mode, value=value) if mode == "constant" else TF.pad(x, tuple(pad), mode=mode))
     F.interpolate = lambda x, size=None, scale_factor=None, mode="nearest", **k: T(TF.interpolate(x, size=size, scale_factor=scale_factor, mode=mode))
+    def sequence_mask(x, maxlen=None, dtype="int64", name=None):
+        """fluid.layers.sequence_mask / F.sequence_mask: mask[..., j] = j < x[...], maxlen defaults to max(x)."""
+        n = int(x.max()) if maxlen is None else int(maxlen)
+        return T((torch.arange(n) < torch.as_tensor(x).unsqueeze(-1)).to(_dt(dtype)))
+    F.sequence_mask = sequence_mask
+
+    def huber_loss(input, label, delta):
+        """fluid.layers.huber_loss (huber_loss_op.h): r = label - input; 0.5 r^2 where |r| <= delta, else delta (|r| - 0.5 delta)."""
+        r = label - input
+        return T(torch.where(r.abs() <= delta, 0.5 * r * r, delta * (r.abs() - 0.5 * delta)))
+    fluid = types.ModuleType("paddle.fluid")
+    fluid.layers = types.ModuleType("paddle.fluid.layers")
+    fluid.layers.sequence_mask, fluid.layers.huber_loss = sequence_mask, huber_loss
+    P.fluid = fluid
     nn.functional = F
 
     utils = types.ModuleType("paddle.nn.utils")
@@ -520,4 +555,4 @@ def build():
     librosa.util.pad_center = pad_center
     tg = types.ModuleType("typeguard")                 # the installed typeguard rejects the reference's `x: int = None` defaults
     tg.check_argument_types = lambda *a, **k: True
-    return {"typeguard": tg, "librosa": librosa, "librosa.util": librosa.util, "paddle": P, "paddle.distributed": dist, "paddle.signal": sig, "paddle.nn": nn, "paddle.nn.functional": F, "paddle.nn.initializer": init, "paddle.nn.utils": utils}
+    return {"paddle.fluid": fluid, "paddle.fluid.layers": fluid.layers, "typeguard": tg, "librosa": librosa, "librosa.util": librosa.util, "paddle": P, "paddle.distributed": dist, "paddle.signal": sig, "paddle.nn": nn, "paddle.nn.functional": F, "paddle.nn.initializer": init, "paddle.nn.utils": utils}

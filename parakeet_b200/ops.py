@@ -80,6 +80,37 @@ def pack_weight(w, device=None):
     return Split(hi.to(dev).contiguous(), lo.to(dev).contiguous())
 
 
+def ceil_to(n, m):
+    return (n + m - 1) // m * m
+
+
+def pack_dev(w):
+    """[n, k, taps] (or [n, k]) fp32 CUDA tensor -> K-major split planes [n, taps * Kp] (pack_weight on the device: the training
+    steps pack the weights of every step)."""
+    if w.dim() == 2:
+        w = w.unsqueeze(-1)
+    n, k, taps = w.shape
+    kp = ceil_to(k, 64)
+    packed = torch.zeros(n, taps, kp, dtype=torch.float32, device=w.device)
+    packed[:, :, :k] = w.permute(0, 2, 1)
+    return Split.from_f32(packed.reshape(n, taps * kp))
+
+
+def pad8(t):
+    """(..., C) -> (..., ceil_to(C, 8)) zero padded: TMA row pitches are multiples of 16 bytes."""
+    c = t.shape[-1]
+    if c % 8 == 0:
+        return t.contiguous()
+    out = torch.zeros(t.shape[:-1] + (ceil_to(c, 8),), dtype=t.dtype, device=t.device)
+    out[..., :c] = t
+    return out
+
+
+def split_pad8(dy):
+    """fp32 gradient (..., C) -> its split planes, the channel axis padded to a multiple of 8 (a GEMM operand)."""
+    return Split.from_f32(pad8(dy))
+
+
 def _operand(s, rows, cols, ld, batch_stride, batches, bmul=1, hmul=0, col0=0, colh=0):
     return Operand(hi=s.hi.data_ptr(), lo=s.lo.data_ptr(), batch_stride=batch_stride, ld=ld, rows=rows, cols=cols,
                    batches=batches, bmul=bmul, hmul=hmul, col0=col0, colh=colh)

@@ -2,14 +2,21 @@
 
 The reference wraps the model in `paddle.DataParallel` (examples/fastspeech2/*/train.py:117-119), which all-reduces
 gradients bucket by bucket.  Here every trainable tensor is a view into ONE flat fp32 buffer (and its gradient into a second
-one), so the exchange step of the path is a single `all_reduce(SUM)` of the flat gradient and the optimiser is a single
-kernel over the flat buffers; the 1/world scale of the DataParallel mean is applied by the optimiser.
-Device-agnostic on purpose: the CPU tests run it over gloo (tests/test_dist_cpu.py).
+one), so the exchange step of the path is a single `all_reduce(SUM)` of the flat gradient and the optimiser (`FlatAdam`, the
+one every training step uses) is a single kernel over the flat buffers; it also applies the 1/world scale of the DataParallel
+mean.
+Device-agnostic on purpose: the CPU tests run the buffers over gloo (tests/test_dist_cpu.py) and the optimiser's checkpoint
+entries on the CPU (tests/test_flat_adam_cpu.py); only `FlatAdam.update` needs the library.
 """
 from collections import OrderedDict
 
 import torch
 import torch.distributed as dist
+
+from .. import _lib
+from ..ops import _ptr, _stream
+
+BUFFERS = ("_mean", "_variance")      # BatchNorm running statistics: state-dict entries that are not trained
 
 
 class FlatBuffers:
@@ -34,3 +41,52 @@ class FlatBuffers:
         """The one exchange step of the path: SUM over ranks (the optimiser divides by the world size)."""
         if dist.is_initialized() and dist.get_world_size(group) > 1:
             dist.all_reduce(self.gflat, op=dist.ReduceOp.SUM, group=group)
+
+
+class FlatAdam:
+    """paddle.optimizer.Adam (with ClipGradByGlobalNorm when `clip_norm` is given) over one FlatBuffers: both moments are flat
+    buffers of the same layout and one kernel updates everything.  `clip_norm` 0.0 keeps the clipping kernels and never clips."""
+
+    def __init__(self, params, names, device, beta1=0.9, beta2=0.999, epsilon=1e-8, clip_norm=None):
+        self.buffers = FlatBuffers(params, names, device)
+        self.flat, self.gflat, self.grads = self.buffers.flat, self.buffers.gflat, self.buffers.grads
+        self.m = torch.zeros_like(self.flat)
+        self.v = torch.zeros_like(self.flat)
+        self.beta1, self.beta2, self.epsilon, self.clip_norm = beta1, beta2, epsilon, clip_norm
+        self.sq = torch.zeros(1, dtype=torch.float64, device=device) if clip_norm is not None else None    # squared gradient norm
+        self.steps = 0
+
+    def update(self, lr, world=1, group=None):
+        """One update from the gradient in `gflat`: SUM over the ranks and the DataParallel mean when world > 1, then Adam."""
+        L, n = _lib.lib(), self.flat.numel()
+        if world > 1:
+            self.buffers.all_reduce_grads(group)
+        self.steps += 1
+        if self.clip_norm is None:
+            _lib.check(L.pk_adam(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), n, lr, self.beta1, self.beta2, self.epsilon,
+                                 self.steps, 1.0 / world, _stream()), "pk_adam")
+            return
+        if world > 1:
+            self.gflat.mul_(1.0 / world)                 # the mean comes before the clip, like paddle
+        self.sq.zero_()
+        _lib.check(L.pk_sq_sum(_ptr(self.gflat), n, _ptr(self.sq), _stream()), "pk_sq_sum")
+        _lib.check(L.pk_adam_clip(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), n, lr, self.beta1, self.beta2, self.epsilon,
+                                  self.steps, _ptr(self.sq), float(self.clip_norm), _stream()), "pk_adam_clip")
+
+    def _views(self):
+        b = self.buffers
+        for k, o, n in zip(b.names, b.offsets, b.sizes):
+            shape = b.grads[k].shape
+            yield k + "_moment1_0", self.m[o:o + n].view(shape)
+            yield k + "_moment2_0", self.v[o:o + n].view(shape)
+
+    def moments(self):
+        """The moments per parameter under Paddle's accumulator suffixes (`<name>_moment1_0`, `<name>_moment2_0`; Paddle prefixes
+        them with its internal tensor names, which do not exist here, so the structured names are used)."""
+        return {key: view.clone() for key, view in self._views()}
+
+    def load_moments(self, opt):
+        """The reverse of moments(); entries that `opt` lacks keep their values."""
+        for key, view in self._views():
+            if key in opt:
+                view.copy_(torch.as_tensor(opt[key]).reshape(view.shape).to(view.device, view.dtype))

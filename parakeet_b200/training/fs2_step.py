@@ -8,9 +8,10 @@ fastspeech2_updater.py:51-99; data-parallel set-up examples/fastspeech2/train.py
 
 All parameters live in ONE flat fp32 buffer (the model's state-dict entries are views into it), all gradients in a second
 flat buffer: the data-parallel exchange is a single NCCL all-reduce of that buffer per step over NVLink, the 1/world
-scale is folded into the fused Adam kernel (pk_adam).  Every FLOP runs in libparakeet_b200.so: GEMM-shaped gradients
-(dgrad = conv with flipped taps, wgrad = dY^T X over the flattened batch x time axis, attention dQ/dK/dV/dP) reuse
-pk_conv_gemm on transposed split planes (pk_transpose_planes); the rest are the row-wise kernels of train.cu.
+scale is folded into the fused Adam kernel (pk_adam; training/flat.py: FlatAdam).  Every FLOP runs in libparakeet_b200.so:
+GEMM-shaped gradients (dgrad = conv with flipped taps, wgrad = dY^T X over the flattened batch x time axis - training/wgrad.py:
+splitk_wgrad -, attention dQ/dK/dV/dP) reuse pk_conv_gemm on transposed split planes (pk_transpose_planes); the rest are the
+row-wise kernels of train.cu.
 torch is used for buffers, views, permutes / copies (layout plumbing) and torch.distributed.
 """
 import ctypes as C
@@ -22,27 +23,10 @@ import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.fastspeech2 import FastSpeech2, _i32
-from ..ops import Split, _ptr, _stream
+from ..ops import Split, _ptr, _stream, ceil_to, pack_dev
 from ..graph import GraphRunner
 from . import wgrad
-from .flat import FlatBuffers
-
-BUFFERS = ("_mean", "_variance")
-
-
-def _ceil64(n):
-    return (n + 63) // 64 * 64
-
-
-def pack_dev(w):
-    """[n, k, taps] (or [n, k]) fp32 CUDA tensor -> K-major split planes [n, taps * Kp] (device-side ops.pack_weight)."""
-    if w.dim() == 2:
-        w = w.unsqueeze(-1)
-    n, k, taps = w.shape
-    kp = _ceil64(k)
-    packed = torch.zeros(n, taps, kp, dtype=torch.float32, device=w.device)
-    packed[:, :, :k] = w.permute(0, 2, 1)
-    return Split.from_f32(packed.reshape(n, taps * kp))
+from .flat import BUFFERS, FlatAdam
 
 
 class FastSpeech2TrainStep:
@@ -63,7 +47,7 @@ class FastSpeech2TrainStep:
         self.spk = model.spk_embed_dim is not None
         self._order = self._BATCH_ORDER + (("spk_id",) if self.spk else ())
         self.m = model
-        self.lr, self.b1, self.b2, self.eps = learning_rate, beta1, beta2, epsilon
+        self.lr = learning_rate
         self.sg_pitch = model.stop_gradient_from_pitch_predictor if stop_gradient_from_pitch_predictor is None else stop_gradient_from_pitch_predictor
         self.sg_energy = model.stop_gradient_from_energy_predictor if stop_gradient_from_energy_predictor is None else stop_gradient_from_energy_predictor
         self.group = process_group
@@ -73,12 +57,9 @@ class FastSpeech2TrainStep:
         self.overlap = os.environ.get("PK_TRAIN_OVERLAP", "1") != "0"      # parameter gradients on a side stream (on_side)
         self._side, self._side_used, self._keep = None, False, []
         names = [k for k in model._params if not k.endswith(BUFFERS)]
-        self.buffers = FlatBuffers(model._params, names, dev)      # the model's tensors become views of one flat buffer
-        self.flat, self.gflat, self.grads = self.buffers.flat, self.buffers.gflat, self.buffers.grads
-        self.adam_m = torch.zeros(self.buffers.total, dtype=torch.float32, device=dev)
-        self.adam_v = torch.zeros(self.buffers.total, dtype=torch.float32, device=dev)
+        self.opt = opt = FlatAdam(model._params, names, dev, beta1, beta2, epsilon)   # the model's tensors become views of one flat buffer
+        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
         model._packed = None
-        self.step_count = 0
         if dropout is True:
             self.rates = dict(model.dropout_rates)
         elif isinstance(dropout, dict):
@@ -107,6 +88,8 @@ class FastSpeech2TrainStep:
     # ------------------------------------------------------------------------------------------------------------
     # GEMM-shaped forward / backward pieces
     # ------------------------------------------------------------------------------------------------------------
+    step_count = property(lambda self: self.opt.steps)
+
     def P(self, name):
         return self.m._params[name]
 
@@ -149,12 +132,8 @@ class FastSpeech2TrainStep:
         """dy fp32 (B,T,cout), x_saved split (B,T,cin): accumulates grads of weight / bias, returns dx fp32 (B,T,cin)."""
         cin, cout, taps = self.dims(wname, kind)
         B, T = dy.shape[0], dy.shape[1]
-        if cout % 8:
-            dy8 = torch.zeros(B, T, (cout + 7) // 8 * 8, dtype=torch.float32, device=dy.device)   # TMA row pitch: 16 bytes
-            dy8[..., :cout] = dy
-            dys = Split.from_f32(dy8)
-        else:
-            dys = Split.from_f32(dy)
+        dys = ops.split_pad8(dy)
+
         def param_grads():
             if bname:      # from the split copy: dy itself may be the residual-stream gradient, which LayerNorm backward updates in place
                 ops.colsum_split_(dys, cout, self.grads[bname])
@@ -196,24 +175,12 @@ class FastSpeech2TrainStep:
         return self._zp.get(role, shape, self.dev)
 
     def wgrad(self, x, dys, wname, kind, cin, cout, taps):
-        """dW = X^T dY over the flattened (batch, time) axis, split-K (training/wgrad.py)."""
-        B, T = x.hi.shape[0], x.hi.shape[1]
-        dev = x.hi.device
-        Tp, S, ks, KKp = wgrad.plan(B, T, cout, cin)
-        dyt = self.zbuf(("dyt", B, T), (cout, KKp))
-        ops.transpose_planes(dys, z=B, rows=T, src_zstride=T * dys.hi.shape[2], ld_src=dys.hi.shape[2], c0=0, cols=cout, shift=0,
-                             r_out=T, dst=dyt, dst_zstride=Tp, ld_dst=KKp)
-        pad = (taps - 1) // 2
-        tmp = torch.empty(taps, cout, cin, dtype=torch.float32, device=dev) if kind == "conv" else None
-        for tap in range(taps):
-            xt = self.zbuf(("xt", B, T), (cin, KKp))
-            ops.transpose_planes(x, z=B, rows=T, src_zstride=x.hi.stride(0), ld_src=x.hi.stride(1), c0=0, cols=cin, shift=tap - pad,
-                                 r_out=T, dst=xt, dst_zstride=Tp, ld_dst=KKp)
-            if kind == "lin":    # Paddle Linear weight [in, out]
-                wgrad.nt_splitk(xt, dyt, cin, cout, S, ks, KKp, out=self.grads[wname])
-            else:                # Conv1D weight [out, in, k]
-                wgrad.nt_splitk(dyt, xt, cout, cin, S, ks, KKp, out=tmp[tap])
-        if kind == "conv":
+        """dW = X^T dY over the flattened (batch, time) axis, split-K (wgrad.splitk_wgrad); 'same' padding centres the taps."""
+        if kind == "lin":    # Paddle Linear weight [in, out]
+            wgrad.splitk_wgrad(self._zp, x, dys, cout, cin, [0], x_first=True, out=self.grads[wname])
+        else:                # Conv1D weight [out, in, k]
+            pad = (taps - 1) // 2
+            tmp = wgrad.splitk_wgrad(self._zp, x, dys, cout, cin, [tap - pad for tap in range(taps)])
             self.grads[wname].copy_(tmp.permute(1, 2, 0))
 
     # ------------------------------------------------------------------------------------------------------------
@@ -226,7 +193,7 @@ class FastSpeech2TrainStep:
         r_layer, r_attn = self.rates[f"transformer_{tag}_dropout_rate"], self.rates[f"transformer_{tag}_attn_dropout_rate"]
         B, T, A = x.shape
         H, dk = m.aheads, A // m.aheads
-        Tp = _ceil64(T)
+        Tp = ceil_to(T, 64)
         ctxs = []
         kind = "lin" if m._linear_ffn else "conv"
         for i in range(n_layers):
@@ -281,7 +248,7 @@ class FastSpeech2TrainStep:
         pre = S["pre"]
         B, T, A = dy.shape
         H, dk = m.aheads, A // m.aheads
-        Tp = _ceil64(T)
+        Tp = ceil_to(T, 64)
         dev = dy.device
         kind = "lin" if m._linear_ffn else "conv"
         dx = torch.empty_like(dy)
@@ -349,13 +316,7 @@ class FastSpeech2TrainStep:
                 ops.colsum_(dqkv.reshape(B * T, ld), bsum)
                 for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
                     self.grads[q + "self_attn." + nm + ".bias"].copy_(bsum[j * A:(j + 1) * A])
-                Tq, Sq, ksq, KKq = wgrad.plan(B, T, A, ld)
-                xt = self.zbuf(("xt", B, T), (A, KKq))
-                ops.transpose_planes(h1, z=B, rows=T, src_zstride=T * A, ld_src=A, c0=0, cols=A, shift=0, r_out=T, dst=xt, dst_zstride=Tq, ld_dst=KKq)
-                dyt = self.zbuf(("dyt", B, T), (ld, KKq))
-                ops.transpose_planes(dqs, z=B, rows=T, src_zstride=T * ld, ld_src=ld, c0=0, cols=ld, shift=0, r_out=T, dst=dyt, dst_zstride=Tq,
-                                     ld_dst=KKq)
-                gw = wgrad.nt_splitk(xt, dyt, A, ld, Sq, ksq, KKq)
+                gw = wgrad.splitk_wgrad(self._zp, h1, dqs, ld, A, [0], x_first=True)
                 for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
                     self.grads[q + "self_attn." + nm + ".weight"].copy_(gw[:, j * A:(j + 1) * A])
 
@@ -606,13 +567,8 @@ class FastSpeech2TrainStep:
     # ------------------------------------------------------------------------------------------------------------
     def state_dict(self, epoch=0):
         """{"main_params", "main_optimizer", "epoch", "iteration"}: Adam moments per parameter under Paddle's accumulator
-        suffixes (`<name>_moment1_0`, `<name>_moment2_0`; Paddle prefixes them with its internal tensor names, which do not
-        exist here, so the structured names are used) plus the step count the bias correction needs."""
-        opt = {}
-        for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-            shape = self.m._params[k].shape
-            opt[k + "_moment1_0"] = self.adam_m[o:o + n].view(shape).clone()
-            opt[k + "_moment2_0"] = self.adam_v[o:o + n].view(shape).clone()
+        suffixes (FlatAdam.moments) plus the step count the bias correction needs."""
+        opt = self.opt.moments()
         opt["step_count"] = self.step_count
         opt["LR_Scheduler"] = {"last_lr": self.lr}
         return {"main_params": self.m.state_dict(), "main_optimizer": opt, "epoch": int(epoch), "iteration": int(self.step_count)}
@@ -620,22 +576,15 @@ class FastSpeech2TrainStep:
     def set_state_dict(self, state):
         self.m.set_state_dict(state["main_params"])                  # in place: the parameters stay views of self.flat
         opt = state.get("main_optimizer", {})
-        for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-            for suffix, buf in (("_moment1_0", self.adam_m), ("_moment2_0", self.adam_v)):
-                if k + suffix in opt:
-                    buf[o:o + n].copy_(torch.as_tensor(opt[k + suffix]).reshape(-1).to(buf.device, buf.dtype))
-        self.step_count = int(opt.get("step_count", state.get("iteration", self.step_count)))
+        self.opt.load_moments(opt)
+        self.opt.steps = int(opt.get("step_count", state.get("iteration", self.step_count)))
         self.step_dev.fill_(self.step_count)
         self._packs = {}
 
     def step(self, batch):
         """One update: returns the four loss values (device tensor: l1, duration, pitch, energy)."""
         losses = self._forward_backward_graphed(batch) if self.use_graphs else self.forward_backward(batch)
-        if self.world > 1:
-            self.buffers.all_reduce_grads(self.group)                                # the one exchange step of the path
-        self.step_count += 1
-        _lib.check(_lib.lib().pk_adam(_ptr(self.flat), _ptr(self.gflat), _ptr(self.adam_m), _ptr(self.adam_v), self.flat.numel(),
-                                      self.lr, self.b1, self.b2, self.eps, self.step_count, 1.0 / self.world, _stream()), "pk_adam")
+        self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
         self.step_dev += 1
         self.m._packed = None
         return losses

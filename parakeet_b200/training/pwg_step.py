@@ -10,52 +10,41 @@ This is the training-mode formulation of the generator: every intermediate the b
 z, the layer inputs, the upsampling stages) is kept, so the residual stack runs as separate wgmma GEMMs (`pk_conv_gemm`:
 dilated conv + aux 1x1 accumulated through the residual operand, skip|out 1x1) around the element-wise kernels of csrc/gan.cu
 instead of the fused inference kernel (csrc/pwg_fc.cu), which keeps nothing.  Data gradients are convolutions with flipped taps,
-weight gradients NT matmuls over the flattened batch x time axis on transposed split planes - the scheme of training/fs2_step.py
-with dilation.  The STFT losses differentiate through pk_stft's re / im outputs: the adjoint of the windowed DFT is a GEMM with the
-DFT basis followed by an overlap-add through the reflect padding.  Weight norm (g, v) is re-folded every step and its backward
-maps dw to (dg, dv).  Parameters, gradients and Adam moments of each network live in flat buffers (one NCCL all-reduce per network
-and step under data parallelism, like paddle.DataParallel's gradient mean).
+weight gradients NT matmuls over the flattened batch x time axis on transposed split planes (training/wgrad.py: splitk_wgrad, the
+tap shifts scaled by the dilation).  The STFT losses differentiate through pk_stft's re / im outputs: the adjoint of the windowed
+DFT is a GEMM with the DFT basis followed by an overlap-add through the reflect padding.  Weight norm (g, v) is re-folded every
+step and its backward maps dw to (dg, dv).  Parameters, gradients and Adam moments of each network live in flat buffers
+(training/flat.py: FlatAdam; one NCCL all-reduce per network and step under data parallelism, like paddle.DataParallel's gradient
+mean).
 torch is used for buffers, views / copies (layout) and torch.distributed only.
 """
 import math
+import os
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from .. import _lib, ops
-from ..ops import Split, _ptr, _stream
+from ..graph import GraphRunner
+from ..ops import Split, _ptr, _stream, ceil_to, pack_dev, pad8
 from ..modules.audio import STFT
 from . import wgrad
-from .flat import FlatBuffers
-from .fs2_step import pack_dev
-
-
-def _pad8(t):
-    """(..., C) -> (..., ceil8(C)) zero padded: TMA row pitches are multiples of 16 bytes."""
-    c = t.shape[-1]
-    if c % 8 == 0:
-        return t.contiguous()
-    out = torch.zeros(t.shape[:-1] + ((c + 7) // 8 * 8,), dtype=t.dtype, device=t.device)
-    out[..., :c] = t
-    return out
+from .flat import FlatAdam
 
 
 class _Net:
     """Weight-normed conv parameters of one network in flat buffers + the folded weights of the current step."""
 
-    def __init__(self, layer, device):
+    def __init__(self, layer, device, eps, clip):
         self.layer = layer
-        names = list(layer._params.keys())
-        self.buffers = FlatBuffers(layer._params, names, device)
-        self.flat, self.gflat, self.grads = self.buffers.flat, self.buffers.gflat, self.buffers.grads
-        self.m = torch.zeros_like(self.flat)
-        self.v = torch.zeros_like(self.flat)
-        self.sq = torch.zeros(1, dtype=torch.float64, device=device)
+        self.opt = opt = FlatAdam(layer._params, list(layer._params.keys()), device, epsilon=eps, clip_norm=clip)
+        self.buffers, self.flat, self.gflat, self.grads = opt.buffers, opt.flat, opt.gflat, opt.grads
         self.w = {}                     # folded weights (fp32, Paddle layouts) of the current step
         self.dw = {}                    # gradients w.r.t. the folded weights
-        self.steps = 0
         layer._packed = None
+
+    steps = property(lambda self: self.opt.steps)
 
     def P(self, k):
         return self.layer._params[k]
@@ -87,27 +76,16 @@ class _Net:
                 _lib.check(L.pk_weight_norm_bwd(_ptr(v), _ptr(self.P(name + "_g")), _ptr(self.dw[name]), v.shape[0], v.numel() // v.shape[0],
                                                 _ptr(self.grads[name + "_g"]), _ptr(self.grads[k]), _stream()), "pk_weight_norm_bwd")
 
-    def adam(self, lr, eps, clip, world, group=None):
-        if world > 1:
-            self.buffers.all_reduce_grads(group)
-            self.gflat.mul_(1.0 / world)                 # DataParallel mean (before the clip, like paddle)
-        self.sq.zero_()
-        L = _lib.lib()
-        _lib.check(L.pk_sq_sum(_ptr(self.gflat), self.gflat.numel(), _ptr(self.sq), _stream()), "pk_sq_sum")
-        self.steps += 1
-        _lib.check(L.pk_adam_clip(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), self.flat.numel(), lr, 0.9, 0.999, eps,
-                                  self.steps, _ptr(self.sq), float(clip), _stream()), "pk_adam_clip")
+    def update(self, lr, world, group=None):
+        self.opt.update(lr, world, group)
         self.layer._packed = None
 
 
 class _ConvOps:
     """Channels-last Conv1D forward / backward through pk_conv_gemm (dilation, 'same' zero padding via TMA bounds)."""
 
-    @staticmethod
-    def _wgrad(dys, x, cout, cin, k, shifts):
-        return _wgrad_splitk(dys, x, cout, cin, k, shifts)
-
-    def __init__(self):
+    def __init__(self, zp):
+        self.zp = zp                    # the step's ZeroPlanes
         self.packs = {}
 
     def reset(self):
@@ -138,43 +116,32 @@ class _ConvOps:
         (B, T, Cin) or None."""
         cout, cin, k = w.shape
         B, T = dy.shape[0], dy.shape[1]
-        dev = dy.device
-        dy8 = _pad8(dy)
-        cout_p = dy8.shape[-1]
-        dys = Split.from_f32(dy8)
+        dys = ops.split_pad8(dy)
         if db is not None:
             ops.colsum_(dy.reshape(B * T, cout), db)       # pk_colsum ACCUMULATES: bias gradients start from the zeroed flat buffer
-        dx = None
-        if need_dx:
-            wb = self._pk(("b", name), lambda: pack_dev(_pad8(w.flip(-1).permute(1, 2, 0)).permute(0, 2, 1)))   # [Cin, Cout_p, k]
-            dx, _ = ops.conv_gemm(dys, wb, n=cin, k=cout_p, taps=k, dil=dil)
+        dx = self.dgrad(dys, name, w, dil) if need_dx else None
         # weight gradient: dW[:, :, tap] = dY^T . shift(X, (tap - pad) * dil) over the flattened (batch, time) axis
         pad = (k - 1) // 2
-        g = self._wgrad(dys, x, cout, cin, k, [(tap - pad) * dil for tap in range(k)])
+        g = self.wgrad(dys, x, w, [(tap - pad) * dil for tap in range(k)])
         if accumulate:
             ops.axpy_(1.0, g.contiguous(), dw)
         else:
             dw.copy_(g)
         return dx
 
+    def dgrad(self, dys, name, w, dil):
+        """dys Split (B, T, Cout_p) -> dx fp32 (B, T, Cin): the conv with flipped taps."""
+        cout, cin, k = w.shape
+        wb = self._pk(("b", name), lambda: pack_dev(pad8(w.flip(-1).permute(1, 2, 0)).permute(0, 2, 1)))   # [Cin, Cout_p, k]
+        return ops.conv_gemm(dys, wb, n=cin, k=dys.hi.shape[-1], taps=k, dil=dil)[0]
 
-def _wgrad_splitk(dys, x, cout, cin, k, shifts):
-    """dW (cout, cin, k): dW[:, :, j] = sum_{b, t} dY[b, t, :]^T X[b, t + shifts[j], :], split-K (training/wgrad.py: the reduction
-    runs over batch * time = 10^5 .. 10^6 rows while the output is one or two tiles)."""
-    B, T = dys.hi.shape[0], dys.hi.shape[1]
-    dev = dys.hi.device
-    cout_p, cin_p = dys.hi.shape[-1], x.hi.shape[-1]
-    Tp, S, ks, KKp = wgrad.plan(B, T, cout_p, cin_p)
-    dyt = wgrad.zero_planes(("dyt", B, T), (cout_p, KKp), dev, geom=("pwg", B, T))
-    ops.transpose_planes(dys, z=B, rows=T, src_zstride=T * cout_p, ld_src=cout_p, c0=0, cols=cout_p, shift=0, r_out=T, dst=dyt,
-                         dst_zstride=Tp, ld_dst=KKp)
-    out = torch.empty(len(shifts), cout_p, cin_p, dtype=torch.float32, device=dev)
-    for j, sh in enumerate(shifts):
-        xt = wgrad.zero_planes(("xt", B, T), (cin_p, KKp), dev, geom=("pwg", B, T))
-        ops.transpose_planes(x, z=B, rows=T, src_zstride=x.hi.stride(0), ld_src=x.hi.stride(1), c0=0, cols=cin_p, shift=sh, r_out=T, dst=xt,
-                             dst_zstride=Tp, ld_dst=KKp)
-        wgrad.nt_splitk(dyt, xt, cout_p, cin_p, S, ks, KKp, out=out[j])
-    return out[:, :cout, :cin].permute(1, 2, 0)
+    def wgrad(self, dys, x, w, shifts):
+        """-> dW (Cout, Cin, k), dW[:, :, j] = sum_{b, t} dY[b, t, :]^T X[b, t + shifts[j], :] (a view of the GEMMs' padded result: the
+        reduction runs over batch * time = 10^5 .. 10^6 rows while the output is one or two tiles)."""
+        cout, cin, _ = w.shape
+        B, T = dys.hi.shape[0], dys.hi.shape[1]
+        self.zp.begin(("pwg", B, T))    # one step visits two or three geometries (sample rate, frame rate)
+        return wgrad.splitk_wgrad(self.zp, x, dys, dys.hi.shape[-1], x.hi.shape[-1], shifts)[:, :cout, :cin].permute(1, 2, 0)
 
 
 class PWGTrainStep:
@@ -190,9 +157,8 @@ class PWGTrainStep:
         self.G, self.D = generator, discriminator
         if not generator._weight_norm:
             generator.apply_weight_norm()
-        self.g, self.d = _Net(generator, dev), _Net(discriminator, dev)
-        self.lr_g, self.lr_d, self.eps = lr_g, lr_d, eps
-        self.clip_g, self.clip_d, self.step_size, self.gamma = grad_norm_g, grad_norm_d, step_size, gamma
+        self.g, self.d = _Net(generator, dev, eps, grad_norm_g), _Net(discriminator, dev, eps, grad_norm_d)
+        self.lr_g, self.lr_d, self.step_size, self.gamma = lr_g, lr_d, step_size, gamma
         self.lambda_adv, self.d_start = lambda_adv, discriminator_train_start_steps
         self.iteration = 0
         self.group = process_group
@@ -203,24 +169,20 @@ class PWGTrainStep:
         for nf, hop, wl in zip(sp["fft_sizes"], sp["hop_sizes"], sp["win_lengths"]):
             st = STFT(nf, hop, wl, sp["window"], device=dev)
             bins = nf // 2 + 1
-            bins_p = (bins + 63) // 64 * 64
+            bins_p = ceil_to(bins, 64)
             n = torch.arange(nf, dtype=torch.float64)[:, None]
             k = torch.arange(bins, dtype=torch.float64)[None, :]
             basis = torch.zeros(nf, 2 * bins_p, dtype=torch.float64)
             basis[:, :bins] = torch.cos(2 * math.pi * k * n / nf)              # d re[k] / d frame[n]
             basis[:, bins_p:bins_p + bins] = -torch.sin(2 * math.pi * k * n / nf)   # d im[k] / d frame[n]
             self.res.append(dict(stft=st, n_fft=nf, hop=hop, bins=bins, bins_p=bins_p, basis=pack_dev(basis.float().to(dev))))
-        self.conv = _ConvOps()
         # forward + backward of each half of update_core replay as a CUDA graph per batch shape (the step is ~2 500 small launches;
         # the Adam kernels stay outside: their bias correction is a host-computed scalar).  PK_TRAIN_GRAPH=0 disables.
-        import os
-        from ..graph import GraphRunner
         self._graphs = GraphRunner(max_graphs=8)
-        # the weight-gradient operand planes (wgrad.zero_planes) are shared per batch geometry and baked into the captured graphs:
-        # if a geometry is evicted (more than 16 distinct (batch, length) geometries), every graph of this step is dropped and captured again
-        import weakref
-        ref = weakref.ref(self)
-        wgrad.on_default_evict(lambda geom: ref() is not None and ref()._graphs.clear())
+        # the weight-gradient operand planes are filed per (batch, length) geometry and baked into the captured graphs: if a geometry
+        # is evicted (more than 16 distinct ones), every graph of this step is dropped and captured again
+        self._zp = wgrad.ZeroPlanes(max_geoms=16, on_evict=lambda _: self._graphs.clear())
+        self.conv = _ConvOps(self._zp)
         self.use_graphs = (os.environ.get("PK_TRAIN_GRAPH", "1") != "0") if use_graphs is None else bool(use_graphs)
         if self.world > 1:
             for net in (self.g, self.d):
@@ -276,16 +238,9 @@ class PWGTrainStep:
                 dx = self.conv.bwd(g, h_in, "d" + name, w, self.D.dilations[i], net.dw[name + ".weight"], net.dw.get(name + ".bias"),
                                    need_dx=(not last) or need_dx, accumulate=accumulate)
             else:
-                dx = self._data_grad(g, "d" + name, w, self.D.dilations[i]) if ((not last) or need_dx) else None
+                dx = self.conv.dgrad(ops.split_pad8(g), "d" + name, w, self.D.dilations[i]) if ((not last) or need_dx) else None
             g = dx
         return g[:, :, 0].contiguous() if (need_dx and g is not None) else None
-
-    def _data_grad(self, dy, name, w, dil):
-        cout, cin, k = w.shape
-        dys = Split.from_f32(_pad8(dy))
-        wb = self.conv._pk(("b", name), lambda: pack_dev(_pad8(w.flip(-1).permute(1, 2, 0)).permute(0, 2, 1)))
-        dx, _ = ops.conv_gemm(dys, wb, n=cin, k=dys.hi.shape[-1], taps=k, dil=dil)
-        return dx
 
     def _mse(self, x, target, dx_coef=None):
         """MSELoss (mean) of logits (B, T, 1) against a constant; returns (loss 0-d tensor, d loss / dx * dx_coef or None)."""
@@ -453,11 +408,7 @@ class PWGTrainStep:
         dm1 = torch.zeros(B, frames + kin - 1, A, dtype=torch.float32, device=dev)    # rows past `frames` carried no output
         dm1[:, :frames] = g.reshape(B, A, frames).transpose(1, 2)
         # conv_in ran with pad = 0 (taps at +0 .. +kin-1): weight gradient with the matching shifts
-        self._wgrad_nopad(dm1, S["mel_cl"], w_in, net.dw["upsample_net.conv_in.weight"])
-
-    def _wgrad_nopad(self, dy, x, w, dw):
-        cout, cin, k = w.shape
-        dw.copy_(_wgrad_splitk(Split.from_f32(_pad8(dy)), x, cout, cin, k, list(range(k))))
+        net.dw["upsample_net.conv_in.weight"].copy_(self.conv.wgrad(ops.split_pad8(dm1), S["mel_cl"], w_in, range(kin)))
 
     # ------------------------------------------------------------------------------------------------------------
     # one update_core
@@ -527,9 +478,9 @@ class PWGTrainStep:
             return {k: v.clone() for k, v in zip(names, vals)}
         g_names = ("spectral_convergence_loss", "log_stft_magnitude_loss") + (("adversarial_loss",) if adversarial else ()) + ("generator_loss",)
         losses = run("g", self.generator_losses_and_grads, g_names)
-        self.g.adam(self._lr(self.lr_g, self.g.steps), self.eps, self.clip_g, self.world, self.group)
+        self.g.update(self._lr(self.lr_g, self.g.steps), self.world, self.group)
         if adversarial:
             losses.update(run("d", self.discriminator_losses_and_grads, ("real_loss", "fake_loss", "discriminator_loss")))
-            self.d.adam(self._lr(self.lr_d, self.d.steps), self.eps, self.clip_d, self.world, self.group)
+            self.d.update(self._lr(self.lr_d, self.d.steps), self.world, self.group)
         self.iteration += 1
         return losses

@@ -4,17 +4,17 @@ parakeet/models/speedyspeech/speedyspeech_updater.py:48-85, :110-157; baker reci
     forward in train mode (every BatchNorm1D takes its batch statistics over ALL B*T or B*L rows: nothing is masked, padded
     tokens and frames are live; the duration predictor reads encodings.detach())
     -> masked L1 + SSIM + Huber-on-log-durations -> backward -> mean all-reduce of the flat gradient over ranks
-    -> paddle.optimizer.Adam with ClipGradByGlobalNorm (pk_sq_sum + pk_adam_clip).
+    -> paddle.optimizer.Adam with ClipGradByGlobalNorm (training/flat.py: FlatAdam).
 
 The model's own forward / inference keep refusing training mode; the train-mode forward lives here, and the step neither reads
-nor changes `model.training`.  Parameters, gradients and Adam moments are flat buffers (training/flat.py); the BatchNorm running
+nor changes `model.training`.  Parameters, gradients and Adam moments are flat buffers (FlatAdam); the BatchNorm running
 statistics stay the model's own tensors and are updated in place by pk_ss_bn_train_fwd.
 
 Every Conv1D -> ReLU -> BatchNorm1D unit is pk_conv_gemm (bias + ReLU in its epilogue) followed by pk_ss_bn_train_fwd (statistics,
 normalisation, the block's residual add, fp32 + split planes); its backward is pk_ss_bn_relu_bwd (dgamma, dbeta, the conv's bias
 gradient, and the gradient at the conv's output as split planes), then the data gradient (pk_conv_gemm with flipped taps, the
-block's residual gradient added in its epilogue) and the split-K weight gradient (training/wgrad.py).  The losses and their
-gradients are pk_ss_loss; the embedding tables' dense gradients are pk_spk_table_grad over the B*T tokens.
+block's residual gradient added in its epilogue) and the split-K weight gradient (training/wgrad.py: splitk_wgrad).  The losses and
+their gradients are pk_ss_loss; the embedding tables' dense gradients are pk_spk_table_grad over the B*T tokens.
 """
 import torch
 import torch.distributed as dist
@@ -22,10 +22,9 @@ import torch.distributed as dist
 from .. import _lib, ops
 from ..graph import GraphRunner
 from ..models.speedyspeech import CHANNELS, SpeedySpeech, _i32, paddle_same_conv
-from ..ops import Split, _ptr, _stream
+from ..ops import Split, _ptr, _stream, pack_dev
 from . import wgrad
-from .flat import FlatBuffers
-from .fs2_step import BUFFERS, pack_dev
+from .flat import BUFFERS, FlatAdam
 
 _KEYS = ("phones", "tones", "num_phones", "num_frames", "feats", "durations")
 
@@ -41,18 +40,15 @@ class SpeedySpeechTrainStep:
         if model.device.type != "cuda":
             raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
         self.m, self.dev, self.group = model, model.device, process_group
-        self.lr, self.clip, self.b1, self.b2, self.eps = learning_rate, max_grad_norm, beta1, beta2, epsilon
+        self.lr = learning_rate
         self.check_durations = check_durations
         self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
         names = [k for k in model._params if not k.endswith(BUFFERS)]
-        self.buffers = FlatBuffers(model._params, names, self.dev)       # the model's tensors become views of one flat buffer
-        self.flat, self.gflat, self.grads = self.buffers.flat, self.buffers.gflat, self.buffers.grads
-        self.adam_m = torch.zeros_like(self.flat)
-        self.adam_v = torch.zeros_like(self.flat)
-        self.sqnorm = torch.zeros(1, dtype=torch.float64, device=self.dev)
+        # the model's tensors become views of one flat buffer; a falsy max_grad_norm never clips
+        self.opt = opt = FlatAdam(model._params, names, self.dev, beta1, beta2, epsilon, clip_norm=max_grad_norm or 0.0)
+        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
         self.one = torch.ones(1, device=self.dev)
         model._packed = None
-        self.step_count = 0
         self._graphs = GraphRunner(max_graphs=4)          # a graph pins every saved activation of its batch shape
         self._zp = wgrad.ZeroPlanes(max_geoms=4, on_evict=self._graphs.drop)
         if self.world > 1:      # paddle.DataParallel broadcasts rank 0's parameters and buffers at construction
@@ -101,6 +97,8 @@ class SpeedySpeechTrainStep:
     # ------------------------------------------------------------------------------------------------------------
     # GEMM-shaped pieces
     # ------------------------------------------------------------------------------------------------------------
+    step_count = property(lambda self: self.opt.steps)
+
     def P(self, name):
         return self.m._params[name]
 
@@ -124,38 +122,12 @@ class SpeedySpeechTrainStep:
         """dy fp32 (B, T, out) or its Split; x_saved Split (B, T, in): writes the weight / bias gradients, returns dx fp32."""
         w = self.P(name + ".weight")
         cin, cout = w.shape
-        if isinstance(dy, Split):
-            dys = dy
-        elif cout % 8:
-            dy8 = torch.zeros(dy.shape[0], dy.shape[1], (cout + 7) // 8 * 8, dtype=torch.float32, device=self.dev)   # TMA row pitch: 16 bytes
-            dy8[..., :cout] = dy
-            dys = Split.from_f32(dy8)
-        else:
-            dys = Split.from_f32(dy)
+        dys = dy if isinstance(dy, Split) else ops.split_pad8(dy)
         ops.colsum_split_(dys, cout, self.grads[name + ".bias"])
-        self.wgrad(x_saved, dys, self.grads[name + ".weight"], cin, cout, 1, 0)
+        wgrad.splitk_wgrad(self._zp, x_saved, dys, cout, cin, [0], x_first=True, out=self.grads[name + ".weight"])
         if not need_dx:
             return None
         return ops.conv_gemm(dys, self._pack(("b", name), lambda: pack_dev(w)), n=cin, k=cout)[0]
-
-    def wgrad(self, x, dys, out, cin, cout, taps, left):
-        """dW = X^T dY over the flattened (batch, time) axis, split-K; tap q pairs dY[t] with X[t + q - left]."""
-        B, T = x.hi.shape[0], x.hi.shape[1]
-        Tp, S, ks, KKp = wgrad.plan(B, T, cout, cin)
-        dyt = self._zp.get(("dyt", B, T), (cout, KKp), self.dev)
-        ops.transpose_planes(dys, z=B, rows=T, src_zstride=T * dys.hi.shape[2], ld_src=dys.hi.shape[2], c0=0, cols=cout, shift=0, r_out=T,
-                             dst=dyt, dst_zstride=Tp, ld_dst=KKp)
-        tmp = torch.empty(taps, cout, cin, dtype=torch.float32, device=self.dev) if taps > 1 or out.dim() == 3 else None
-        for tap in range(taps):
-            xt = self._zp.get(("xt", B, T), (cin, KKp), self.dev)
-            ops.transpose_planes(x, z=B, rows=T, src_zstride=x.hi.stride(0), ld_src=x.hi.stride(1), c0=0, cols=cin, shift=tap - left, r_out=T,
-                                 dst=xt, dst_zstride=Tp, ld_dst=KKp)
-            if tmp is None:      # Linear weight [in, out]
-                wgrad.nt_splitk(xt, dyt, cin, cout, S, ks, KKp, out=out)
-            else:                # Conv1D weight [out, in, k]
-                wgrad.nt_splitk(dyt, xt, cout, cin, S, ks, KKp, out=tmp[tap])
-        if tmp is not None:
-            out.copy_(tmp.permute(1, 2, 0))
 
     # ------------------------------------------------------------------------------------------------------------
     # ResidualBlock (speedyspeech.py:21-39) in training mode
@@ -187,7 +159,9 @@ class SpeedySpeechTrainStep:
             q = u["q"]
             _, drs = ops.ss_bn_relu_bwd(g, u["r"], u["mean"], u["rstd"], self.P(q + "2.weight"), sc, self.grads[q + "2.weight"],
                                         self.grads[q + "2.bias"], dbias=self.grads[q + "0.bias"])
-            self.wgrad(u["x"], drs, self.grads[q + "0.weight"], CHANNELS, CHANNELS, k, left)
+            # tap pairs dY[t] with X[t + tap - left]: the 4-tap kernel pads one more row on the right
+            dw = wgrad.splitk_wgrad(self._zp, u["x"], drs, CHANNELS, CHANNELS, [tap - left for tap in range(k)])
+            self.grads[q + "0.weight"].copy_(dw.permute(1, 2, 0))
             if j == 0 and not need_dx:
                 return None
             w = self.P(q + "0.weight")
@@ -303,16 +277,7 @@ class SpeedySpeechTrainStep:
         tensors, key = self._prepare(batch)
         self._zp.touch(key)
         losses = self._graphs.run(key, self._forward_backward, tensors).clone()
-        L_ = _lib.lib()
-        if self.world > 1:
-            self.buffers.all_reduce_grads(self.group)                       # the one exchange step: SUM, then the DataParallel mean
-            ops.axpy_(1.0 / self.world - 1.0, self.gflat, self.gflat)
-        self.step_count += 1
-        self.sqnorm.zero_()
-        n = self.flat.numel()
-        _lib.check(L_.pk_sq_sum(_ptr(self.gflat), n, _ptr(self.sqnorm), _stream()), "pk_sq_sum")
-        _lib.check(L_.pk_adam_clip(_ptr(self.flat), _ptr(self.gflat), _ptr(self.adam_m), _ptr(self.adam_v), n, self.lr, self.b1, self.b2,
-                                   self.eps, self.step_count, _ptr(self.sqnorm), float(self.clip or 0.0), _stream()), "pk_adam_clip")
+        self.opt.update(self.lr, self.world, self.group)
         self.m._packed = None            # inference re-packs the updated weights and running statistics, and drops its graphs
         return self._named(losses)
 
@@ -320,11 +285,7 @@ class SpeedySpeechTrainStep:
     # snapshot / resume: the container of StandardUpdater.state_dict, as FastSpeech2TrainStep writes it
     # ------------------------------------------------------------------------------------------------------------
     def state_dict(self, epoch=0):
-        opt = {}
-        for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-            shape = self.m._params[k].shape
-            opt[k + "_moment1_0"] = self.adam_m[o:o + n].view(shape).clone()
-            opt[k + "_moment2_0"] = self.adam_v[o:o + n].view(shape).clone()
+        opt = self.opt.moments()
         opt["step_count"] = self.step_count
         opt["LR_Scheduler"] = {"last_lr": self.lr}
         return {"main_params": self.m.state_dict(), "main_optimizer": opt, "epoch": int(epoch), "iteration": int(self.step_count)}
@@ -332,11 +293,8 @@ class SpeedySpeechTrainStep:
     def set_state_dict(self, state):
         self.m.set_state_dict(state["main_params"])                  # in place: the parameters stay views of self.flat
         opt = state.get("main_optimizer", {})
-        for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-            for suffix, buf in (("_moment1_0", self.adam_m), ("_moment2_0", self.adam_v)):
-                if k + suffix in opt:
-                    buf[o:o + n].copy_(torch.as_tensor(opt[k + suffix]).reshape(-1).to(buf.device, buf.dtype))
-        self.step_count = int(opt.get("step_count", state.get("iteration", self.step_count)))
+        self.opt.load_moments(opt)
+        self.opt.steps = int(opt.get("step_count", state.get("iteration", self.step_count)))
 
     def save(self, path, epoch=0):
         from .. import checkpoint

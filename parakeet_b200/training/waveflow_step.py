@@ -8,7 +8,7 @@ backward of the residual net is one `pk_waveflow_backward_layer` launch per laye
 gradient, out_proj^T with dx as the register operand, gate backward); the forward's convs are `pk_conv_gemm` (the 3x3 conv as
 three launches, one per kernel row, over the "net layout" of csrc/waveflow_train.cu); the weight gradients are split-K NT
 matmuls (`wgrad.nt_splitk`) over transposed planes, the conv bias gradient riding along as a ones row.  Parameters,
-gradients and Adam moments live in flat buffers (`FlatBuffers`); the model's tensors are views of the parameter buffer.
+gradients and Adam moments live in flat buffers (`training/flat.py: FlatAdam`); the model's tensors are views of the parameter buffer.
 torch only allocates, views, copies and all-reduces.
 """
 import ctypes as C_
@@ -20,16 +20,12 @@ import torch.distributed as dist
 
 from .. import _lib, ops
 from ..graph import GraphRunner
-from ..ops import Split, _ptr, _stream
+from ..ops import Split, _ptr, _stream, ceil_to
 from . import wgrad
-from .flat import FlatBuffers
+from .flat import FlatAdam
 
 SLOPE = 0.4            # UpsampleNet's leaky_relu (waveflow.py:130)
 _SCRATCH = 1024 * 256  # fp32 partials of pk_waveflow_train_outer_sum / pk_waveflow_upsample_bwd
-
-
-def _c64(n):
-    return (n + 63) // 64 * 64
 
 
 class WaveFlowTrainStep:
@@ -42,16 +38,14 @@ class WaveFlowTrainStep:
         if not sigma > 0:
             raise ValueError("sigma must be positive")
         self.m = model
-        self.lr, self.sigma, self.b1, self.b2, self.eps = learning_rate, float(sigma), beta1, beta2, epsilon
+        self.lr, self.sigma = learning_rate, float(sigma)
         self.group = process_group
         self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
         dev = self.dev = model.device
         names = list(model._params)
-        self.buffers = FlatBuffers(model._params, names, dev)      # the model's tensors become views of one flat buffer
-        self.flat, self.gflat, self.grads = self.buffers.flat, self.buffers.gflat, self.buffers.grads
+        self.opt = opt = FlatAdam(model._params, names, dev, beta1, beta2, epsilon)      # the model's tensors become views of one flat buffer
+        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
         self.off = dict(zip(names, self.buffers.offsets))
-        self.adam_m = torch.zeros_like(self.flat)
-        self.adam_v = torch.zeros_like(self.flat)
         self.weff = torch.zeros_like(self.flat)     # weights as the forward uses them: weight norm folded into the weight_v slots
         self.dweff = torch.zeros_like(self.flat)    # gradients with respect to weff
         self._wn = []                                # (v offset, g offset, rows, inner) of every weight-normed tensor
@@ -68,7 +62,6 @@ class WaveFlowTrainStep:
         self.cmaps = [i32(c) for c in cmaps]                                   # condition height of each height, per flow
         self.inv_perms = [i32(np.argsort(pm).tolist()) for pm in self.perms]
         self._build_packs()
-        self.step_count = 0
         # a captured graph pins its own memory pool: ~20 GB at the recipe's batch and 128 channels, so only a few shapes are kept
         self._graphs = GraphRunner(max_graphs=2)
         self.use_graphs = os.environ.get("PK_TRAIN_GRAPH", "1") != "0"
@@ -77,6 +70,8 @@ class WaveFlowTrainStep:
         if self.world > 1:
             # paddle.DataParallel broadcasts rank 0's parameters at construction
             dist.broadcast(self.flat, src=0, group=process_group)
+
+    step_count = property(lambda self: self.opt.steps)
 
     # ------------------------------------------------------------------------------------------------------------
     # weights: offsets into the flat buffers and the packed GEMM operands
@@ -100,7 +95,7 @@ class WaveFlowTrainStep:
             ix = ix.reshape(ix.shape[0], -1)
             segs.append((total, ix))
             o = total
-            total += _c64(ix.numel())
+            total += ceil_to(ix.numel(), 64)
             return (o, tuple(ix.shape))
 
         for fl in range(m.n_flows):
@@ -110,7 +105,7 @@ class WaveFlowTrainStep:
                 w1 = self._idx(q + "conv", (2 * C, C, 3, 3))
                 wc = self._idx(q + "condition_proj", (2 * C, M))
                 w2 = self._idx(q + "out_proj", (2 * C, C))
-                wcp = torch.full((2 * C, _c64(M)), -1, dtype=torch.int64)
+                wcp = torch.full((2 * C, ceil_to(M, 64)), -1, dtype=torch.int64)
                 wcp[:, :M] = wc
                 layers.append(dict(
                     w1f=[add(w1[:, :, kh, :].permute(0, 2, 1)) for kh in range(3)],             # (o, kw, c): output row q reads input row q + kh
@@ -356,11 +351,7 @@ class WaveFlowTrainStep:
         self._check(wav, mel)
         wav, mel = wav.contiguous().float(), mel.contiguous().float()
         loss = self.forward_backward_graphed(wav, mel)
-        if self.world > 1:
-            self.buffers.all_reduce_grads(self.group)                                # the one exchange step of the path
-        self.step_count += 1
-        _lib.check(_lib.lib().pk_adam(_ptr(self.flat), _ptr(self.gflat), _ptr(self.adam_m), _ptr(self.adam_v), self.flat.numel(),
-                                      self.lr, self.b1, self.b2, self.eps, self.step_count, 1.0 / self.world, _stream()), "pk_adam")
+        self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
         self.m._packed = None                                                        # inference weights are re-packed on demand
         return loss.clone()
 
@@ -370,24 +361,18 @@ class WaveFlowTrainStep:
     def state_dict(self):
         """(params, opt): the model's state dict and the Adam state under Paddle's accumulator suffixes (`<name>_moment1_0`,
         `<name>_moment2_0`, `<name>_beta1_pow_acc_0`, `<name>_beta2_pow_acc_0`)."""
-        opt = {}
-        for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-            shape = self.m._params[k].shape
-            opt[k + "_moment1_0"] = self.adam_m[o:o + n].view(shape).clone()
-            opt[k + "_moment2_0"] = self.adam_v[o:o + n].view(shape).clone()
-            opt[k + "_beta1_pow_acc_0"] = torch.tensor([self.b1 ** self.step_count])
-            opt[k + "_beta2_pow_acc_0"] = torch.tensor([self.b2 ** self.step_count])
+        opt = self.opt.moments()
+        for k in self.buffers.names:
+            opt[k + "_beta1_pow_acc_0"] = torch.tensor([self.opt.beta1 ** self.step_count])
+            opt[k + "_beta2_pow_acc_0"] = torch.tensor([self.opt.beta2 ** self.step_count])
         opt["step_count"] = self.step_count
         return self.m.state_dict(), opt
 
     def set_state_dict(self, params, opt=None):
         self.m.set_state_dict(params)                # in place: the parameters stay views of self.flat
         if opt:
-            for k, o, n in zip(self.buffers.names, self.buffers.offsets, self.buffers.sizes):
-                for suffix, buf in (("_moment1_0", self.adam_m), ("_moment2_0", self.adam_v)):
-                    if k + suffix in opt:
-                        buf[o:o + n].copy_(torch.as_tensor(opt[k + suffix]).reshape(-1).to(buf.device, buf.dtype))
-            self.step_count = int(opt.get("step_count", self.step_count))
+            self.opt.load_moments(opt)
+            self.opt.steps = int(opt.get("step_count", self.step_count))
 
     def save(self, checkpoint_dir, iteration=None):
         """Write step-N.pdparams and step-N.pdopt (N = iteration or the completed steps) and record it in checkpoint_dir/checkpoint."""

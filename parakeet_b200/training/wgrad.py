@@ -1,6 +1,7 @@
 """Split-K weight gradients: dW = A^T-style NT matmuls whose reduction axis is the flattened (batch, time) axis (10^4 .. 10^6)
 while the output is a handful of 128 x N tiles.  K is cut into S slices so that tiles x S fills the machine: S independent NT
-matmuls (`pk_conv_gemm` batched over the slices) whose fp32 partial results are summed by `pk_sum_slices`."""
+matmuls (`pk_conv_gemm` batched over the slices) whose fp32 partial results are summed by `pk_sum_slices`.  `splitk_wgrad` is the
+weight gradient of a Conv1D or Linear layer as the FastSpeech2, SpeedySpeech and Parallel WaveGAN steps compute it."""
 import torch
 
 from .. import ops
@@ -49,30 +50,6 @@ class ZeroPlanes:
         return len(self._geoms)
 
 
-_EVICT_HOOKS = []
-
-
-def _default_evicted(geom):
-    for hook in list(_EVICT_HOOKS):
-        hook(geom)
-
-
-_DEFAULT_PLANES = ZeroPlanes(max_geoms=16, on_evict=_default_evicted)   # one PWG step uses 2-3 geometries (sample rate, frame rate)
-
-
-def on_default_evict(hook):
-    """Register hook(geom) for evictions from the module-level cache (a training step that captures CUDA graphs over these planes
-    drops its graphs there: their buffer addresses are baked in)."""
-    _EVICT_HOOKS.append(hook)
-
-
-def zero_planes(role, shape, dev, geom=None):
-    """Module-level cache for callers without their own ZeroPlanes (the PWG training step: fixed batch geometry)."""
-    if geom is not None and geom != _DEFAULT_PLANES._cur:
-        _DEFAULT_PLANES.begin(geom)
-    return _DEFAULT_PLANES.get(role, shape, dev)
-
-
 def plan(batch, t, m, n, max_slices=128):
     """-> (Tp, S, ks, KKp): padded time, number of K slices, slice length (multiple of 64), padded reduction length S * ks."""
     tp = (t + 63) // 64 * 64
@@ -105,3 +82,32 @@ def nt_splitk(at, bt, m, n, s, ks, kkp, out=None):
         out.copy_(y)
         return out
     return y
+
+
+def splitk_wgrad(zp, x, dys, rows_dy, rows_x, shifts, x_first=False, out=None):
+    """Conv1D weight gradient, one plane per tap: -> fp32 (len(shifts), rows_dy, rows_x),
+    [j] = sum over (b, t) of dY[b, t, :rows_dy]^T X[b, t + shifts[j], :rows_x].
+    x, dys: Split (B, T, >= rows_x) saved input (may be a view) and (B, T, >= rows_dy) output gradient; zp: the caller's ZeroPlanes.
+    (rows_dy, rows_x) also fix the number of K slices, i.e. the summation order.
+    x_first (Paddle Linear weight [in, out]; one shift): the operands swapped, (rows_x, rows_dy) written into `out`.
+    Allocates and launches on the current stream only."""
+    B, T = x.hi.shape[0], x.hi.shape[1]
+    dev = x.hi.device
+    Tp, S, ks, KKp = plan(B, T, rows_dy, rows_x)
+    ld = dys.hi.shape[2]
+    dyt = zp.get(("dyt", B, T), (rows_dy, KKp), dev)
+    ops.transpose_planes(dys, z=B, rows=T, src_zstride=T * ld, ld_src=ld, c0=0, cols=rows_dy, shift=0, r_out=T, dst=dyt, dst_zstride=Tp,
+                         ld_dst=KKp)
+
+    def shifted(sh):                                          # ONE plane, rewritten per tap
+        xt = zp.get(("xt", B, T), (rows_x, KKp), dev)
+        ops.transpose_planes(x, z=B, rows=T, src_zstride=x.hi.stride(0), ld_src=x.hi.stride(1), c0=0, cols=rows_x, shift=sh, r_out=T, dst=xt,
+                             dst_zstride=Tp, ld_dst=KKp)
+        return xt
+
+    if x_first:
+        return nt_splitk(shifted(shifts[0]), dyt, rows_x, rows_dy, S, ks, KKp, out=out)
+    res = torch.empty(len(shifts), rows_dy, rows_x, dtype=torch.float32, device=dev)
+    for j, sh in enumerate(shifts):
+        nt_splitk(dyt, shifted(sh), rows_dy, rows_x, S, ks, KKp, out=res[j])
+    return res

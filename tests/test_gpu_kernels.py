@@ -169,10 +169,13 @@ def test_fused_attention_vs_fp64(cuda):
 def test_sum_slices_and_splitk_wgrad(cuda):
     """pk_sum_slices (split-K reduction, overwrites its output): the float4 path, the scalar path (n % 4 != 0 or a misaligned
     view of the flat gradient buffer), and wgrad.nt_splitk writing into a non-contiguous destination; the persistent zero
-    planes of the transposed operands give the same gradient on a second use with other data."""
+    planes of the transposed operands give the same gradient on a second use with other data.  wgrad.splitk_wgrad, the weight
+    gradient the training steps share: a dilated 3-tap conv over padded channel counts and a view of a wider input, and the
+    Linear orientation."""
     from parakeet_b200 import ops
     from parakeet_b200.training import wgrad
     g = torch.Generator().manual_seed(21)
+    zp = wgrad.ZeroPlanes()
     for s, n, off in ((7, 4096, 0), (128, 384 * 3, 0), (5, 1001, 0), (3, 64, 1)):
         part = torch.randn(s, n, generator=g).to(cuda)
         flat = torch.full((n + 8,), 7.0, device=cuda)            # garbage the call must overwrite
@@ -187,8 +190,8 @@ def test_sum_slices_and_splitk_wgrad(cuda):
         dy = torch.randn(B, T, cout, generator=g).to(cuda)
         Tp, S, ks, KKp = wgrad.plan(B, T, cin, cout)
         xs, dys = ops.Split.from_f32(x), ops.Split.from_f32(dy)
-        xt = wgrad.zero_planes(("test_xt", B, T), (cin, KKp), cuda)
-        dyt = wgrad.zero_planes(("test_dyt", B, T), (cout, KKp), cuda)
+        xt = zp.get(("test_xt", B, T), (cin, KKp), cuda)
+        dyt = zp.get(("test_dyt", B, T), (cout, KKp), cuda)
         ops.transpose_planes(xs, z=B, rows=T, src_zstride=T * cin, ld_src=cin, c0=0, cols=cin, shift=0, r_out=T, dst=xt, dst_zstride=Tp, ld_dst=KKp)
         ops.transpose_planes(dys, z=B, rows=T, src_zstride=T * cout, ld_src=cout, c0=0, cols=cout, shift=0, r_out=T, dst=dyt, dst_zstride=Tp,
                              ld_dst=KKp)
@@ -199,3 +202,23 @@ def test_sum_slices_and_splitk_wgrad(cuda):
         err = (got.double().cpu() - ref).abs().max().item() / ref.abs().max().item()
         assert err < 2e-5, (rep, S, err)
         assert rep != 2 or S > 1
+    # the shared weight gradient, twice over the same planes: dW[j] = dY^T shift(X, shifts[j]), rows past either end of an utterance are zero
+    B, T, cin, cout, dil = 8, 700, 40, 20, 3                                      # S > 1
+    for rep in range(2):
+        wide = ops.Split.from_f32(torch.randn(B, T, cin + 8, generator=g).to(cuda))
+        xs = ops.Split(wide.hi[:, :, :cin], wide.lo[:, :, :cin])                  # a view: the source strides are the wide tensor's
+        dys = ops.split_pad8(torch.randn(B, T, cout, generator=g).to(cuda))       # 20 -> 24 columns, the last four zero
+        xd, dyd = xs.float().double().cpu(), dys.float().double().cpu()
+        shifts = [-dil, 0, dil]
+        got = wgrad.splitk_wgrad(zp, xs, dys, 24, cin, shifts)
+        assert got.shape == (3, 24, cin) and got[:, cout:].abs().max().item() == 0
+        for j, sh in enumerate(shifts):
+            xsh = torch.zeros_like(xd)
+            xsh[:, max(0, -sh):T - max(0, sh)] = xd[:, max(0, sh):T - max(0, -sh)]
+            ref = torch.einsum("btd,btc->dc", dyd, xsh)
+            assert (got[j].double().cpu() - ref).abs().max().item() / ref.abs().max().item() < 2e-5, (rep, sh)
+        big = torch.zeros(cin, cout + 4, device=cuda)
+        out = big[:, :cout] if rep else torch.empty(cin, cout, device=cuda)
+        lin = wgrad.splitk_wgrad(zp, xs, dys, cout, cin, [0], x_first=True, out=out)
+        ref = torch.einsum("btc,btd->cd", xd, dyd[..., :cout])
+        assert lin is out and (lin.double().cpu() - ref).abs().max().item() / ref.abs().max().item() < 2e-5, rep

@@ -6,7 +6,7 @@ events around the captured graph.
 warm-up that packs weights and sets kernel attributes), captures it into a CUDA graph the second time, and replays the
 graph afterwards: inputs are copied into the graph's static input tensors, outputs are the graph's static output tensors
 (valid until the next replay of the same key - callers clone what they hand out).  `fn` must not synchronise with the
-host.  Set PK_CUDA_GRAPHS=0 to run everything eagerly.
+host.  `enabled=False`, or PK_CUDA_GRAPHS=0 for every runner, runs everything eagerly.
 """
 import os
 
@@ -22,8 +22,8 @@ def _tensors(obj):
 
 
 class GraphRunner:
-    def __init__(self, max_graphs=32):
-        self.enabled = os.environ.get("PK_CUDA_GRAPHS", "1") != "0"
+    def __init__(self, max_graphs=32, enabled=True):
+        self.enabled = enabled and os.environ.get("PK_CUDA_GRAPHS", "1") != "0"
         self.max_graphs = max_graphs
         self._seen = set()
         self._disabled = set()

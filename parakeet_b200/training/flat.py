@@ -7,16 +7,52 @@ one every training step uses) is a single kernel over the flat buffers; it also 
 mean.
 Device-agnostic on purpose: the CPU tests run the buffers over gloo (tests/test_dist_cpu.py) and the optimiser's checkpoint
 entries on the CPU (tests/test_flat_adam_cpu.py); only `FlatAdam.update` needs the library.
+The rest is what every training step shares around its buffers: rank 0's broadcast at construction, the snapshot container of
+`StandardUpdater` and the switch of the step's CUDA graphs.
 """
+import os
 from collections import OrderedDict
 
 import torch
 import torch.distributed as dist
 
 from .. import _lib
+from ..graph import GraphRunner
 from ..ops import _ptr, _stream
 
 BUFFERS = ("_mean", "_variance")      # BatchNorm running statistics: state-dict entries that are not trained
+
+
+def step_graphs(max_graphs, use_graphs=None):
+    """The GraphRunner that replays a training step's forward + backward: on when `use_graphs` says so, else unless
+    PK_TRAIN_GRAPH=0 (PK_CUDA_GRAPHS=0 turns every graph off)."""
+    on = os.environ.get("PK_TRAIN_GRAPH", "1") != "0" if use_graphs is None else bool(use_graphs)
+    return GraphRunner(max_graphs=max_graphs, enabled=on)
+
+
+def broadcast_from_rank0(flat, params, group=None):
+    """paddle.DataParallel broadcasts rank 0's parameters and buffers at construction (examples/fastspeech2/*/train.py:117-119):
+    the flat parameter buffer, then every BUFFERS entry of `params`."""
+    dist.broadcast(flat, src=0, group=group)
+    for k, v in params.items():
+        if k.endswith(BUFFERS):
+            dist.broadcast(v, src=0, group=group)
+
+
+def updater_state(model, opt, lr, epoch=0):
+    """StandardUpdater.state_dict's container {"main_params", "main_optimizer", "epoch", "iteration"}: Adam moments per
+    parameter under Paddle's accumulator suffixes (FlatAdam.moments) plus the step count the bias correction needs."""
+    o = opt.moments()
+    o["step_count"] = opt.steps
+    o["LR_Scheduler"] = {"last_lr": lr}
+    return {"main_params": model.state_dict(), "main_optimizer": o, "epoch": int(epoch), "iteration": int(opt.steps)}
+
+
+def load_updater_state(model, opt, state):
+    model.set_state_dict(state["main_params"])                  # in place: the parameters stay views of the flat buffer
+    o = state.get("main_optimizer", {})
+    opt.load_moments(o)
+    opt.steps = int(o.get("step_count", state.get("iteration", opt.steps)))
 
 
 class FlatBuffers:

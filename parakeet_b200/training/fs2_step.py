@@ -23,10 +23,10 @@ import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.fastspeech2 import FastSpeech2, _i32
-from ..ops import Split, _ptr, _stream, ceil_to, pack_dev
-from ..graph import GraphRunner
+from ..ops import Split, _ptr, _stream, ceil_to
 from . import wgrad
-from .flat import BUFFERS, FlatAdam
+from .conv import ConvOps
+from .flat import BUFFERS, FlatAdam, broadcast_from_rank0, load_updater_state, step_graphs, updater_state
 
 
 class FastSpeech2TrainStep:
@@ -70,20 +70,16 @@ class FastSpeech2TrainStep:
         # completed steps, on the device: the dropout kernels add it to their step argument, so a captured graph of forward +
         # backward draws new masks on every replay
         self.step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._fb_graphs = GraphRunner(max_graphs=16)
+        self._fb_graphs = step_graphs(16, use_graphs)
         self._zp = wgrad.ZeroPlanes(max_geoms=16, on_evict=self._fb_graphs.drop)     # planes and graph of a batch shape go together
-        self.use_graphs = (os.environ.get("PK_TRAIN_GRAPH", "1") != "0") if use_graphs is None else bool(use_graphs)
+        self.conv = ConvOps(self._zp)
         # workspace of the BatchNorm / LayerNorm reductions: 2 floats per channel (pk_batch_norm_train / _bwd)
         widest = max([model.odim, model.adim] + [int(v.shape[0]) for k, v in model._params.items() if k.startswith("postnet.")])
         self.sums = torch.zeros(max(4096, 2 * widest), dtype=torch.float32, device=dev)
         if model.adim > 512:
             raise NotImplementedError("pk_layer_norm_bwd supports rows of at most 512 channels (adim)")
         if self.world > 1:
-            # paddle.DataParallel broadcasts rank 0's parameters and buffers at construction (train.py:117-119)
-            dist.broadcast(self.flat, src=0, group=process_group)
-            for k, v in model._params.items():
-                if k.endswith(BUFFERS):
-                    dist.broadcast(v, src=0, group=process_group)
+            broadcast_from_rank0(self.flat, model._params, process_group)
 
     # ------------------------------------------------------------------------------------------------------------
     # GEMM-shaped forward / backward pieces
@@ -92,12 +88,6 @@ class FastSpeech2TrainStep:
 
     def P(self, name):
         return self.m._params[name]
-
-    def _pack(self, key, fn):
-        v = self._packs.get(key)
-        if v is None:
-            v = self._packs[key] = fn()
-        return v
 
     @staticmethod
     def site(stack, layer, kind):
@@ -111,40 +101,22 @@ class FastSpeech2TrainStep:
         """Forward AND backward: the mask depends only on (seed, step, site, element index)."""
         return ops.dropout(x, p, self.seed, site, 1, step_dev=self.step_dev, **kw)      # step = 1 + completed steps (device counter)
 
-    def w_fwd(self, name, kind):
-        w = self.P(name)
-        return self._pack(("f", name), lambda: pack_dev(w.t().contiguous() if kind == "lin" else w))
-
-    def w_bwd(self, name, kind):
-        w = self.P(name)
-        return self._pack(("b", name), lambda: pack_dev(w if kind == "lin" else w.flip(-1).permute(1, 0, 2).contiguous()))
-
-    def dims(self, name, kind):
-        w = self.P(name)
-        return (w.shape[0], w.shape[1], 1) if kind == "lin" else (w.shape[1], w.shape[0], w.shape[2])   # (cin, cout, taps)
-
-    def layer_fwd(self, x, wname, bname, kind, act=None, residual=None, f32=True, split=False):
-        cin, cout, taps = self.dims(wname, kind)
-        return ops.conv_gemm(x, self.w_fwd(wname, kind), n=cout, k=cin, taps=taps, bias=self.P(bname) if bname else None, act=act,
-                             residual=residual, out_f32=f32, out_split=split)
+    def layer_fwd(self, x, wname, bname, kind, **kw):
+        return self.conv.fwd(x, wname, self.P(wname), linear=kind == "lin", bias=self.P(bname) if bname else None, **kw)
 
     def layer_bwd(self, dy, x_saved, wname, bname, kind, need_dx=True):
-        """dy fp32 (B,T,cout), x_saved split (B,T,cin): accumulates grads of weight / bias, returns dx fp32 (B,T,cin)."""
-        cin, cout, taps = self.dims(wname, kind)
-        B, T = dy.shape[0], dy.shape[1]
+        """dy fp32 (B,T,cout), x_saved split (B,T,cin): writes the grads of weight / bias, returns dx fp32 (B,T,cin)."""
+        w, linear = self.P(wname), kind == "lin"
         dys = ops.split_pad8(dy)
 
         def param_grads():
             if bname:      # from the split copy: dy itself may be the residual-stream gradient, which LayerNorm backward updates in place
-                ops.colsum_split_(dys, cout, self.grads[bname])
-            self.wgrad(x_saved, dys, wname, kind, cin, cout, taps)
+                ops.colsum_split_(dys, dy.shape[-1], self.grads[bname])
+            self.conv.wgrad(x_saved, dys, w, linear=linear, out=self.grads[wname])
 
         # the parameter gradients are leaves of the backward graph: they run beside the dx chain (the critical path)
         self.on_side(param_grads, dys, x_saved)
-        dx = None
-        if need_dx:
-            dx, _ = ops.conv_gemm(dys, self.w_bwd(wname, kind), n=cin, k=cout, taps=taps)
-        return dx
+        return self.conv.dgrad(dys, wname, w, linear=linear) if need_dx else None
 
     def on_side(self, fn, *keep):
         """Run fn() on the side stream, after everything issued so far on the current stream (fork); join_side() is the join.
@@ -174,14 +146,10 @@ class FastSpeech2TrainStep:
         """Persistent zero-initialised operand planes of the current batch shape (training/wgrad.py: ZeroPlanes)."""
         return self._zp.get(role, shape, self.dev)
 
-    def wgrad(self, x, dys, wname, kind, cin, cout, taps):
-        """dW = X^T dY over the flattened (batch, time) axis, split-K (wgrad.splitk_wgrad); 'same' padding centres the taps."""
-        if kind == "lin":    # Paddle Linear weight [in, out]
-            wgrad.splitk_wgrad(self._zp, x, dys, cout, cin, [0], x_first=True, out=self.grads[wname])
-        else:                # Conv1D weight [out, in, k]
-            pad = (taps - 1) // 2
-            tmp = wgrad.splitk_wgrad(self._zp, x, dys, cout, cin, [tap - pad for tap in range(taps)])
-            self.grads[wname].copy_(tmp.permute(1, 2, 0))
+    def wqkv(self, q):
+        """The fused Q | K | V projection of layer prefix `q` as one Paddle Linear weight [A, 3A]."""
+        return torch.cat([self.P(q + "self_attn.linear_q.weight"), self.P(q + "self_attn.linear_k.weight"),
+                          self.P(q + "self_attn.linear_v.weight")], dim=1)
 
     # ------------------------------------------------------------------------------------------------------------
     # FFT-block stack (Encoder.forward after the embedding) with saved context
@@ -200,10 +168,8 @@ class FastSpeech2TrainStep:
             q = f"{pre}encoders.{i}."
             c = dict(x0=x)
             _, c["h1"] = ops.layer_norm(x, self.P(q + "norm1.weight"), self.P(q + "norm1.bias"))
-            wqkv = self._pack(("f", q + "qkv"), lambda: pack_dev(torch.cat([self.P(q + "self_attn.linear_q.weight"), self.P(q + "self_attn.linear_k.weight"),
-                                                                          self.P(q + "self_attn.linear_v.weight")], dim=1).t().contiguous()))
             bqkv = torch.cat([self.P(q + "self_attn.linear_q.bias"), self.P(q + "self_attn.linear_k.bias"), self.P(q + "self_attn.linear_v.bias")])
-            _, qkv = ops.conv_gemm(c["h1"], wqkv, n=3 * A, k=A, bias=bqkv, out_f32=False, out_split=True)
+            _, qkv = self.conv.fwd(c["h1"], q + "qkv", self.wqkv(q), linear=True, bias=bqkv, out_f32=False, out_split=True)
             c["qkv"] = qkv
             ld = 3 * A
             s_buf = torch.empty(B * H, T, Tp, dtype=torch.float32, device=x.device)
@@ -229,7 +195,7 @@ class FastSpeech2TrainStep:
                 x1, _ = self.layer_fwd(ctx, q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin", residual=x)
             c["x1"] = x1
             _, c["h2"] = ops.layer_norm(x1, self.P(q + "norm2.weight"), self.P(q + "norm2.bias"))
-            _, c["u"] = self.layer_fwd(c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind, act="relu", f32=False, split=True)
+            _, c["u"] = self.layer_fwd(c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind, act="relu", out_f32=False, out_split=True)
             c["ud"] = self.drop(c["u"], r_layer, self.site(sid, i, 3), out_f32=False, out_split=True)[1] if r_layer > 0 else c["u"]
             if r_layer > 0:
                 f_out, _ = self.layer_fwd(c["ud"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", kind)
@@ -308,20 +274,19 @@ class FastSpeech2TrainStep:
                                   y_batch_stride=T * ld, y_head_stride=dk, y_ld=ld)                               # dK = dS^T Q
             # fused QKV projection: h1 [A] -> [3A]
             dqs = Split.from_f32(dqkv)
-            wq_b = self._pack(("b", q + "qkv"), lambda: pack_dev(torch.cat([self.P(q + "self_attn.linear_q.weight"), self.P(q + "self_attn.linear_k.weight"),
-                                                                           self.P(q + "self_attn.linear_v.weight")], dim=1).contiguous()))
+            wqkv = self.wqkv(q)
 
-            def qkv_param_grads(q=q, dqkv=dqkv, dqs=dqs, h1=c["h1"]):
+            def qkv_param_grads(q=q, dqkv=dqkv, dqs=dqs, h1=c["h1"], wqkv=wqkv):
                 bsum = torch.zeros(ld, dtype=torch.float32, device=dev)
                 ops.colsum_(dqkv.reshape(B * T, ld), bsum)
                 for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
                     self.grads[q + "self_attn." + nm + ".bias"].copy_(bsum[j * A:(j + 1) * A])
-                gw = wgrad.splitk_wgrad(self._zp, h1, dqs, ld, A, [0], x_first=True)
+                gw = self.conv.wgrad(h1, dqs, wqkv, linear=True)
                 for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
                     self.grads[q + "self_attn." + nm + ".weight"].copy_(gw[:, j * A:(j + 1) * A])
 
             self.on_side(qkv_param_grads, dqkv, dqs, c["h1"])
-            dh1, _ = ops.conv_gemm(dqs, wq_b, n=A, k=ld)
+            dh1 = self.conv.dgrad(dqs, q + "qkv", wqkv, linear=True)
             ops.layer_norm_bwd(c["x0"], self.P(q + "norm1.weight"), dh1, dx, True, self.grads[q + "norm1.weight"], self.grads[q + "norm1.bias"])
         return dx
 
@@ -333,7 +298,7 @@ class FastSpeech2TrainStep:
                      "duration_predictor.": (4, self.rates["duration_predictor_dropout_rate"])}[pre]
         saved, h = [], hs_split
         for i in range(n_layers):
-            y, ys = self.layer_fwd(h, f"{pre}conv.{i}.0.weight", f"{pre}conv.{i}.0.bias", "conv", act="relu", f32=True, split=True)
+            y, ys = self.layer_fwd(h, f"{pre}conv.{i}.0.weight", f"{pre}conv.{i}.0.bias", "conv", act="relu", out_split=True)
             _, hn = ops.layer_norm(y, self.P(f"{pre}conv.{i}.2.weight"), self.P(f"{pre}conv.{i}.2.bias"))
             if rate > 0:
                 hn = self.drop(hn, rate, self.site(sid, i, 5), out_f32=False, out_split=True)[1]
@@ -373,7 +338,7 @@ class FastSpeech2TrainStep:
             ops.axpy_(1.0, proj.expand(B, T, A).contiguous(), hs2)
             return hs2, Split.from_f32(hs2), S
         S["cat"] = Split.from_f32(torch.cat([hs, e.unsqueeze(1).expand(B, T, e.shape[1])], dim=-1))          # layout only
-        hs2, hs2_split = self.layer_fwd(S["cat"], "spk_projection.weight", "spk_projection.bias", "lin", f32=True, split=True)
+        hs2, hs2_split = self.layer_fwd(S["cat"], "spk_projection.weight", "spk_projection.bias", "lin", out_split=True)
         return hs2, hs2_split, S
 
     def spk_bwd(self, dhs2, S):
@@ -400,7 +365,7 @@ class FastSpeech2TrainStep:
         L = _lib.lib()
         st = _stream()
         dev = m.device
-        self._packs = {}
+        self.conv.reset()
         self._zp.begin(self._batch_key(batch))
         self.gflat.zero_()
         text = batch["text"].to(dev, torch.int64).contiguous()
@@ -458,7 +423,7 @@ class FastSpeech2TrainStep:
         if R["transformer_dec_positional_dropout_rate"] > 0:
             self.drop(xd, R["transformer_dec_positional_dropout_rate"], self.site(1, 0, 0), inplace=True)
         zs, zs_split, S_dec = self.stack_fwd(xd, "decoder.", m.dlayers, olens)
-        before, before_split = self.layer_fwd(zs_split, "feat_out.weight", "feat_out.bias", "lin", f32=True, split=True)
+        before, before_split = self.layer_fwd(zs_split, "feat_out.weight", "feat_out.bias", "lin", out_split=True)
         post, h = [], before_split
         rows = B * t_dec
         for i in range(m.postnet_layers):
@@ -566,24 +531,16 @@ class FastSpeech2TrainStep:
     # updater first and loading afterwards - which is why Layer.set_state_dict copies IN PLACE into the flat buffer)
     # ------------------------------------------------------------------------------------------------------------
     def state_dict(self, epoch=0):
-        """{"main_params", "main_optimizer", "epoch", "iteration"}: Adam moments per parameter under Paddle's accumulator
-        suffixes (FlatAdam.moments) plus the step count the bias correction needs."""
-        opt = self.opt.moments()
-        opt["step_count"] = self.step_count
-        opt["LR_Scheduler"] = {"last_lr": self.lr}
-        return {"main_params": self.m.state_dict(), "main_optimizer": opt, "epoch": int(epoch), "iteration": int(self.step_count)}
+        return updater_state(self.m, self.opt, self.lr, epoch)
 
     def set_state_dict(self, state):
-        self.m.set_state_dict(state["main_params"])                  # in place: the parameters stay views of self.flat
-        opt = state.get("main_optimizer", {})
-        self.opt.load_moments(opt)
-        self.opt.steps = int(opt.get("step_count", state.get("iteration", self.step_count)))
+        load_updater_state(self.m, self.opt, state)
         self.step_dev.fill_(self.step_count)
-        self._packs = {}
+        self.conv.reset()
 
     def step(self, batch):
         """One update: returns the four loss values (device tensor: l1, duration, pitch, energy)."""
-        losses = self._forward_backward_graphed(batch) if self.use_graphs else self.forward_backward(batch)
+        losses = self._forward_backward_graphed(batch)
         self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
         self.step_dev += 1
         self.m._packed = None

@@ -19,18 +19,17 @@ mean).
 torch is used for buffers, views / copies (layout) and torch.distributed only.
 """
 import math
-import os
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from .. import _lib, ops
-from ..graph import GraphRunner
-from ..ops import Split, _ptr, _stream, ceil_to, pack_dev, pad8
+from ..ops import Split, _ptr, _stream, ceil_to, pack_dev
 from ..modules.audio import STFT
 from . import wgrad
-from .flat import FlatAdam
+from .conv import ConvOps
+from .flat import FlatAdam, broadcast_from_rank0, step_graphs
 
 
 class _Net:
@@ -81,69 +80,6 @@ class _Net:
         self.layer._packed = None
 
 
-class _ConvOps:
-    """Channels-last Conv1D forward / backward through pk_conv_gemm (dilation, 'same' zero padding via TMA bounds)."""
-
-    def __init__(self, zp):
-        self.zp = zp                    # the step's ZeroPlanes
-        self.packs = {}
-
-    def reset(self):
-        self.packs = {}
-
-    def _pk(self, key, fn):
-        v = self.packs.get(key)
-        if v is None:
-            v = self.packs[key] = fn()
-        return v
-
-    def fwd(self, x, name, w, b, dil=1, residual=None, f32=True, split=False):
-        """x Split (B, T, Cin_p >= Cin); w (Cout, Cin, k) -> (B, T, Cout)."""
-        cout, cin, k = w.shape
-        cin_p = x.hi.shape[-1]
-
-        def packed():
-            if cin_p == cin:
-                return pack_dev(w)
-            wp_ = torch.zeros(cout, cin_p, k, dtype=torch.float32, device=w.device)      # zero weights for the padding channels
-            wp_[:, :cin] = w
-            return pack_dev(wp_)
-        return ops.conv_gemm(x, self._pk(("f", name), packed), n=cout, k=cin_p, taps=k, dil=dil, bias=b, residual=residual, out_f32=f32,
-                             out_split=split)
-
-    def bwd(self, dy, x, name, w, dil, dw, db, need_dx=True, accumulate=False):
-        """dy fp32 (B, T, Cout); x Split saved input (B, T, Cin_p).  Writes dw (Cout, Cin, k) / db (or accumulates); returns dx fp32
-        (B, T, Cin) or None."""
-        cout, cin, k = w.shape
-        B, T = dy.shape[0], dy.shape[1]
-        dys = ops.split_pad8(dy)
-        if db is not None:
-            ops.colsum_(dy.reshape(B * T, cout), db)       # pk_colsum ACCUMULATES: bias gradients start from the zeroed flat buffer
-        dx = self.dgrad(dys, name, w, dil) if need_dx else None
-        # weight gradient: dW[:, :, tap] = dY^T . shift(X, (tap - pad) * dil) over the flattened (batch, time) axis
-        pad = (k - 1) // 2
-        g = self.wgrad(dys, x, w, [(tap - pad) * dil for tap in range(k)])
-        if accumulate:
-            ops.axpy_(1.0, g.contiguous(), dw)
-        else:
-            dw.copy_(g)
-        return dx
-
-    def dgrad(self, dys, name, w, dil):
-        """dys Split (B, T, Cout_p) -> dx fp32 (B, T, Cin): the conv with flipped taps."""
-        cout, cin, k = w.shape
-        wb = self._pk(("b", name), lambda: pack_dev(pad8(w.flip(-1).permute(1, 2, 0)).permute(0, 2, 1)))   # [Cin, Cout_p, k]
-        return ops.conv_gemm(dys, wb, n=cin, k=dys.hi.shape[-1], taps=k, dil=dil)[0]
-
-    def wgrad(self, dys, x, w, shifts):
-        """-> dW (Cout, Cin, k), dW[:, :, j] = sum_{b, t} dY[b, t, :]^T X[b, t + shifts[j], :] (a view of the GEMMs' padded result: the
-        reduction runs over batch * time = 10^5 .. 10^6 rows while the output is one or two tiles)."""
-        cout, cin, _ = w.shape
-        B, T = dys.hi.shape[0], dys.hi.shape[1]
-        self.zp.begin(("pwg", B, T))    # one step visits two or three geometries (sample rate, frame rate)
-        return wgrad.splitk_wgrad(self.zp, x, dys, dys.hi.shape[-1], x.hi.shape[-1], shifts)[:, :cout, :cin].permute(1, 2, 0)
-
-
 class PWGTrainStep:
     def __init__(self, generator, discriminator, lr_g=1e-4, lr_d=5e-5, eps=1e-6, grad_norm_g=10.0, grad_norm_d=1.0, step_size=200000,
                  gamma=0.5, lambda_adv=4.0, discriminator_train_start_steps=100000, stft_loss_params=None, process_group=None,
@@ -178,15 +114,30 @@ class PWGTrainStep:
             self.res.append(dict(stft=st, n_fft=nf, hop=hop, bins=bins, bins_p=bins_p, basis=pack_dev(basis.float().to(dev))))
         # forward + backward of each half of update_core replay as a CUDA graph per batch shape (the step is ~2 500 small launches;
         # the Adam kernels stay outside: their bias correction is a host-computed scalar).  PK_TRAIN_GRAPH=0 disables.
-        self._graphs = GraphRunner(max_graphs=8)
+        self._graphs = step_graphs(8, use_graphs)
         # the weight-gradient operand planes are filed per (batch, length) geometry and baked into the captured graphs: if a geometry
         # is evicted (more than 16 distinct ones), every graph of this step is dropped and captured again
         self._zp = wgrad.ZeroPlanes(max_geoms=16, on_evict=lambda _: self._graphs.clear())
-        self.conv = _ConvOps(self._zp)
-        self.use_graphs = (os.environ.get("PK_TRAIN_GRAPH", "1") != "0") if use_graphs is None else bool(use_graphs)
+        self.conv = ConvOps(self._zp)
         if self.world > 1:
             for net in (self.g, self.d):
-                dist.broadcast(net.flat, src=0, group=process_group)
+                broadcast_from_rank0(net.flat, net.layer._params, process_group)
+
+    def conv_bwd(self, dy, x, key, w, dil, dw, db, need_dx=True, accumulate=False):
+        """dy fp32 (B, T, Cout); x Split saved input (B, T, >= Cin).  Writes dw (Cout, Cin, k) / db (or accumulates); returns dx fp32
+        (B, T, Cin) or None."""
+        B, T, cout = dy.shape
+        dys = ops.split_pad8(dy)
+        if db is not None:
+            ops.colsum_(dy.reshape(B * T, cout), db)       # pk_colsum ACCUMULATES: bias gradients start from the zeroed flat buffer
+        dx = self.conv.dgrad(dys, key, w, dil=dil) if need_dx else None
+        self._zp.begin(("pwg", B, T))    # one step visits two or three geometries (sample rate, frame rate)
+        g = self.conv.wgrad(x, dys, w, dil=dil)
+        if accumulate:
+            ops.axpy_(1.0, g.contiguous(), dw)
+        else:
+            dw.copy_(g)
+        return dx
 
     # ------------------------------------------------------------------------------------------------------------
     # schedules
@@ -209,7 +160,7 @@ class PWGTrainStep:
         for i in range(n_layers):
             name = f"conv_layers.{2 * i}"
             w, b = net.w[name + ".weight"], net.w.get(name + ".bias")
-            y, _ = self.conv.fwd(h, "d" + name, w, b, dil=self.D.dilations[i])
+            y, _ = self.conv.fwd(h, "d" + name, w, bias=b, dil=self.D.dilations[i])
             if i < n_layers - 1:
                 a = Split.empty(tuple(y.shape), y.device)
                 _lib.check(L.pk_leaky_relu(_ptr(y), y.numel(), self.D.slope, None, _ptr(a.hi), _ptr(a.lo), _stream()), "pk_leaky_relu")
@@ -235,10 +186,10 @@ class PWGTrainStep:
             w = net.w[name + ".weight"]
             last = i == 0
             if param_grads:
-                dx = self.conv.bwd(g, h_in, "d" + name, w, self.D.dilations[i], net.dw[name + ".weight"], net.dw.get(name + ".bias"),
+                dx = self.conv_bwd(g, h_in, "d" + name, w, self.D.dilations[i], net.dw[name + ".weight"], net.dw.get(name + ".bias"),
                                    need_dx=(not last) or need_dx, accumulate=accumulate)
             else:
-                dx = self.conv.dgrad(ops.split_pad8(g), "d" + name, w, self.D.dilations[i]) if ((not last) or need_dx) else None
+                dx = self.conv.dgrad(ops.split_pad8(g), "d" + name, w, dil=self.D.dilations[i]) if ((not last) or need_dx) else None
             g = dx
         return g[:, :, 0].contiguous() if (need_dx and g is not None) else None
 
@@ -295,7 +246,7 @@ class PWGTrainStep:
         mel_cl = Split.from_f32(mel.transpose(1, 2).contiguous())                     # (B, frames + 2w, aux)
         w_in = net.w["upsample_net.conv_in.weight"]
         kin = w_in.shape[-1]
-        cin_full, _ = ops.conv_gemm(mel_cl, self.conv._pk(("f", "conv_in"), lambda: pack_dev(w_in)), n=A, k=A, taps=kin, pad=0)
+        cin_full, _ = self.conv.fwd(mel_cl, "conv_in", w_in, pad=0)
         frames = mel.shape[-1] - (kin - 1)
         m1 = cin_full[:, :frames].contiguous()                                        # taps at +0 .. +kin-1: valid for the first `frames` rows
         ups = [m1.transpose(1, 2).reshape(B * A, frames).contiguous()]
@@ -312,20 +263,20 @@ class PWGTrainStep:
         n8 = torch.zeros(B, T, 8, dtype=torch.float32, device=dev)
         n8[:, :, 0] = noise[:, 0]
         n8s = Split.from_f32(n8)
-        x, xs = self.conv.fwd(n8s, "first", net.w["first_conv.weight"], net.w["first_conv.bias"], f32=True, split=True)
+        x, xs = self.conv.fwd(n8s, "first", net.w["first_conv.weight"], bias=net.w["first_conv.bias"], out_split=True)
         skips = torch.empty(B, T, 64, dtype=torch.float32, device=dev)
         layers = []
         lps = G.layers // G.stacks
         for i in range(G.layers):
             pre = f"conv_layers.{i}."
             d = 2 ** (i % lps)
-            h1, _ = self.conv.fwd(xs, "g" + pre + "conv", net.w[pre + "conv.weight"], net.w.get(pre + "conv.bias"), dil=d)
-            h, _ = self.conv.fwd(c, "g" + pre + "aux", net.w[pre + "conv1x1_aux.weight"], None, residual=h1)
+            h1, _ = self.conv.fwd(xs, "g" + pre + "conv", net.w[pre + "conv.weight"], bias=net.w.get(pre + "conv.bias"), dil=d)
+            h, _ = self.conv.fwd(c, "g" + pre + "aux", net.w[pre + "conv1x1_aux.weight"], residual=h1)
             z = Split.empty((B, T, 64), dev)
             _lib.check(L.pk_gate_fwd(_ptr(h), B * T, 64, None, _ptr(z.hi), _ptr(z.lo), _stream()), "pk_gate_fwd")
             w2 = torch.cat([net.w[pre + "conv1x1_skip.weight"], net.w[pre + "conv1x1_out.weight"]], dim=0)
             b2 = torch.cat([net.w[pre + "conv1x1_skip.bias"], net.w[pre + "conv1x1_out.bias"]])
-            so, _ = ops.conv_gemm(z, self.conv._pk(("f", "g" + pre + "so"), lambda: pack_dev(w2)), n=128, k=64, bias=b2)
+            so, _ = self.conv.fwd(z, "g" + pre + "so", w2, bias=b2)
             xo = torch.empty(B, T, 64, dtype=torch.float32, device=dev)
             xos = Split.empty((B, T, 64), dev)
             _lib.check(L.pk_pwg_res_update(_ptr(so), _ptr(x), B * T, _ptr(skips), 1 if i == 0 else 0, _ptr(xo), _ptr(xos.hi), _ptr(xos.lo),
@@ -340,10 +291,10 @@ class PWGTrainStep:
         u0s = Split.from_f32(u0)
         w1t = net.w["last_conv_layers.1.weight"]
         # relu(s * k) = k * relu(s) for k > 0: the scale is folded into the 1x1 weights of this step
-        v1, _ = ops.conv_gemm(u0s, self.conv._pk(("f", "tail1"), lambda: pack_dev(w1t * scale)), n=64, k=64, bias=net.w["last_conv_layers.1.bias"])
+        v1, _ = self.conv.fwd(u0s, "tail1", w1t * scale, bias=net.w["last_conv_layers.1.bias"])
         u1 = Split.empty(tuple(v1.shape), dev)
         _lib.check(L.pk_leaky_relu(_ptr(v1), v1.numel(), 0.0, None, _ptr(u1.hi), _ptr(u1.lo), _stream()), "pk_leaky_relu")
-        out, _ = self.conv.fwd(u1, "tail3", net.w["last_conv_layers.3.weight"], net.w["last_conv_layers.3.bias"])
+        out, _ = self.conv.fwd(u1, "tail3", net.w["last_conv_layers.3.weight"], bias=net.w["last_conv_layers.3.bias"])
         if keep:
             save.update(mel_cl=mel_cl, frames=frames, ups=ups, c=c, n8s=n8s, layers=layers, skips=skips, u0s=u0s, v1=v1, u1=u1, scale=scale)
         return out[:, :, 0].contiguous()
@@ -354,13 +305,13 @@ class PWGTrainStep:
         B, T = dwav.shape
         A, dev = G.aux_channels, dwav.device
         dout = dwav.reshape(B, T, 1).contiguous()
-        du1 = self.conv.bwd(dout, S["u1"], "tail3", net.w["last_conv_layers.3.weight"], 1, net.dw["last_conv_layers.3.weight"],
+        du1 = self.conv_bwd(dout, S["u1"], "tail3", net.w["last_conv_layers.3.weight"], 1, net.dw["last_conv_layers.3.weight"],
                             net.dw["last_conv_layers.3.bias"])
         dv1 = torch.empty_like(du1)
         _lib.check(L.pk_leaky_relu_bwd(_ptr(S["v1"]), _ptr(du1), du1.numel(), 0.0, _ptr(dv1), _stream()), "pk_leaky_relu_bwd")
         w1s = net.w["last_conv_layers.1.weight"] * S["scale"]
         dws = torch.empty_like(w1s)
-        du0 = self.conv.bwd(dv1, S["u0s"], "tail1", w1s, 1, dws, net.dw["last_conv_layers.1.bias"])
+        du0 = self.conv_bwd(dv1, S["u0s"], "tail1", w1s, 1, dws, net.dw["last_conv_layers.1.bias"])
         net.dw["last_conv_layers.1.weight"].copy_(dws * S["scale"])
         dskips = torch.empty_like(du0)
         _lib.check(L.pk_leaky_relu_bwd(_ptr(S["skips"]), _ptr(du0), du0.numel(), 0.0, _ptr(dskips), _stream()), "pk_leaky_relu_bwd")
@@ -374,21 +325,21 @@ class PWGTrainStep:
             _lib.check(L.pk_pwg_res_update_bwd(_ptr(dskips), _ptr(dx), B * T, _ptr(dso), _ptr(dx_res), _stream()), "pk_pwg_res_update_bwd")
             dw2 = torch.empty_like(c_["w2"])
             db2 = torch.zeros(128, dtype=torch.float32, device=dev)
-            dz = self.conv.bwd(dso, c_["z"], "g" + pre + "so", c_["w2"], 1, dw2, db2)
+            dz = self.conv_bwd(dso, c_["z"], "g" + pre + "so", c_["w2"], 1, dw2, db2)
             net.dw[pre + "conv1x1_skip.weight"].copy_(dw2[:64])
             net.dw[pre + "conv1x1_out.weight"].copy_(dw2[64:])
             net.dw[pre + "conv1x1_skip.bias"].copy_(db2[:64])
             net.dw[pre + "conv1x1_out.bias"].copy_(db2[64:])
             dh = torch.empty(B, T, 128, dtype=torch.float32, device=dev)
             _lib.check(L.pk_gate_bwd(_ptr(c_["h"]), _ptr(dz), B * T, 64, _ptr(dh), _stream()), "pk_gate_bwd")
-            dci = self.conv.bwd(dh, S["c"], "g" + pre + "aux", net.w[pre + "conv1x1_aux.weight"], 1, net.dw[pre + "conv1x1_aux.weight"], None)
+            dci = self.conv_bwd(dh, S["c"], "g" + pre + "aux", net.w[pre + "conv1x1_aux.weight"], 1, net.dw[pre + "conv1x1_aux.weight"], None)
             ops.axpy_(1.0, dci, dc)
-            dxi = self.conv.bwd(dh, c_["xs"], "g" + pre + "conv", net.w[pre + "conv.weight"], c_["d"], net.dw[pre + "conv.weight"],
+            dxi = self.conv_bwd(dh, c_["xs"], "g" + pre + "conv", net.w[pre + "conv.weight"], c_["d"], net.dw[pre + "conv.weight"],
                                 net.dw.get(pre + "conv.bias"))
             ops.axpy_(1.0, dx_res, dxi)
             dx = dxi
         # first conv (input is noise: no data gradient)
-        self.conv.bwd(dx, S["n8s"], "first", net.w["first_conv.weight"], 1, net.dw["first_conv.weight"], net.dw["first_conv.bias"], need_dx=False)
+        self.conv_bwd(dx, S["n8s"], "first", net.w["first_conv.weight"], 1, net.dw["first_conv.weight"], net.dw["first_conv.bias"], need_dx=False)
         # upsampling net: stages in reverse, then conv_in
         g = dc.transpose(1, 2).reshape(B * A, T).contiguous()
         tin = T
@@ -408,7 +359,8 @@ class PWGTrainStep:
         dm1 = torch.zeros(B, frames + kin - 1, A, dtype=torch.float32, device=dev)    # rows past `frames` carried no output
         dm1[:, :frames] = g.reshape(B, A, frames).transpose(1, 2)
         # conv_in ran with pad = 0 (taps at +0 .. +kin-1): weight gradient with the matching shifts
-        net.dw["upsample_net.conv_in.weight"].copy_(self.conv.wgrad(ops.split_pad8(dm1), S["mel_cl"], w_in, range(kin)))
+        self._zp.begin(("pwg", B, frames + kin - 1))
+        self.conv.wgrad(S["mel_cl"], ops.split_pad8(dm1), w_in, pad=0, out=net.dw["upsample_net.conv_in.weight"])
 
     # ------------------------------------------------------------------------------------------------------------
     # one update_core
@@ -469,8 +421,6 @@ class PWGTrainStep:
         shape = (tuple(noise.shape), tuple(mel.shape))
 
         def run(tag, fn, names):
-            if not self.use_graphs:
-                return fn(noise, mel, wav)
             def once(n_, m_, w_):
                 res = fn(n_, m_, w_)
                 return tuple(res[k] for k in names)

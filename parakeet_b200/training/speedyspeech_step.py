@@ -20,11 +20,11 @@ import torch
 import torch.distributed as dist
 
 from .. import _lib, ops
-from ..graph import GraphRunner
 from ..models.speedyspeech import CHANNELS, SpeedySpeech, _i32, paddle_same_conv
-from ..ops import Split, _ptr, _stream, pack_dev
+from ..ops import Split, _ptr, _stream
 from . import wgrad
-from .flat import BUFFERS, FlatAdam
+from .conv import ConvOps
+from .flat import BUFFERS, FlatAdam, broadcast_from_rank0, load_updater_state, step_graphs, updater_state
 
 _KEYS = ("phones", "tones", "num_phones", "num_frames", "feats", "durations")
 
@@ -49,13 +49,11 @@ class SpeedySpeechTrainStep:
         self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
         self.one = torch.ones(1, device=self.dev)
         model._packed = None
-        self._graphs = GraphRunner(max_graphs=4)          # a graph pins every saved activation of its batch shape
+        self._graphs = step_graphs(4)          # a graph pins every saved activation of its batch shape
         self._zp = wgrad.ZeroPlanes(max_geoms=4, on_evict=self._graphs.drop)
-        if self.world > 1:      # paddle.DataParallel broadcasts rank 0's parameters and buffers at construction
-            dist.broadcast(self.flat, src=0, group=process_group)
-            for k, v in model._params.items():
-                if k.endswith(BUFFERS):
-                    dist.broadcast(v, src=0, group=process_group)
+        self.conv = ConvOps(self._zp)
+        if self.world > 1:
+            broadcast_from_rank0(self.flat, model._params, process_group)
 
     # ------------------------------------------------------------------------------------------------------------
     # batch checks (host side; nothing here can fault on the device)
@@ -102,32 +100,21 @@ class SpeedySpeechTrainStep:
     def P(self, name):
         return self.m._params[name]
 
-    def _pack(self, key, fn):
-        v = self._packs.get(key)
-        if v is None:
-            v = self._packs[key] = fn()
-        return v
-
     def workspace(self, rows, batch=0, l=0):
         """The kernels' fp32 workspace for one call.  Allocated by the call that uses it, never kept across calls: inside a graph
         capture it then belongs to that graph's memory pool and lives as long as the graph whose kernels hold its address."""
         return torch.empty(ops.ss_scratch_elems(rows, batch, l, self.m.odim), dtype=torch.float32, device=self.dev)
 
-    def lin_fwd(self, xs, name, act=None, residual=None, split=False):
-        w = self.P(name + ".weight")                                   # Paddle Linear: [in, out]
-        wp = self._pack(("f", name), lambda: pack_dev(w.t().contiguous()))
-        return ops.conv_gemm(xs, wp, n=w.shape[1], k=w.shape[0], bias=self.P(name + ".bias"), act=act, residual=residual, out_split=split)
+    def lin_fwd(self, xs, name, **kw):
+        return self.conv.fwd(xs, name, self.P(name + ".weight"), linear=True, bias=self.P(name + ".bias"), **kw)
 
     def lin_bwd(self, dy, x_saved, name, need_dx=True):
         """dy fp32 (B, T, out) or its Split; x_saved Split (B, T, in): writes the weight / bias gradients, returns dx fp32."""
         w = self.P(name + ".weight")
-        cin, cout = w.shape
         dys = dy if isinstance(dy, Split) else ops.split_pad8(dy)
-        ops.colsum_split_(dys, cout, self.grads[name + ".bias"])
-        wgrad.splitk_wgrad(self._zp, x_saved, dys, cout, cin, [0], x_first=True, out=self.grads[name + ".weight"])
-        if not need_dx:
-            return None
-        return ops.conv_gemm(dys, self._pack(("b", name), lambda: pack_dev(w)), n=cin, k=cout)[0]
+        ops.colsum_split_(dys, w.shape[1], self.grads[name + ".bias"])
+        self.conv.wgrad(x_saved, dys, w, linear=True, out=self.grads[name + ".weight"])
+        return self.conv.dgrad(dys, name, w, linear=True) if need_dx else None
 
     # ------------------------------------------------------------------------------------------------------------
     # ResidualBlock (speedyspeech.py:21-39) in training mode
@@ -139,19 +126,17 @@ class SpeedySpeechTrainStep:
         units, hs = [], xs
         for j in range(n):
             q = f"{pre}blocks.{j}."
-            w = self.P(q + "0.weight")
-            r, _ = ops.conv_gemm(hs, self._pack(("f", q), lambda: pack_dev(w)), n=CHANNELS, k=CHANNELS, taps=k, pad=left,
-                                 bias=self.P(q + "0.bias"), act="relu")
+            r, _ = self.conv.fwd(hs, q, self.P(q + "0.weight"), bias=self.P(q + "0.bias"), pad=left, act="relu")
             last = j == n - 1
             y, ys, mean, rstd = ops.ss_bn_train_fwd(r, self.P(q + "2.weight"), self.P(q + "2.bias"), self.P(q + "2._mean"),
                                                     self.P(q + "2._variance"), sc, residual=x if last else None, want_f32=last)
             units.append(dict(q=q, x=hs, r=r, mean=mean, rstd=rstd))
             hs = ys
-        return y, hs, dict(units=units, k=k, left=left)
+        return y, hs, dict(units=units, left=left)
 
     def block_bwd(self, dy, ctx, need_dx=True):
         """dy fp32: gradient at the block's output -> gradient at its input (the residual path included)."""
-        k, left = ctx["k"], ctx["left"]
+        left = ctx["left"]
         sc = self._ws
         g = dy
         for j in reversed(range(len(ctx["units"]))):
@@ -160,13 +145,11 @@ class SpeedySpeechTrainStep:
             _, drs = ops.ss_bn_relu_bwd(g, u["r"], u["mean"], u["rstd"], self.P(q + "2.weight"), sc, self.grads[q + "2.weight"],
                                         self.grads[q + "2.bias"], dbias=self.grads[q + "0.bias"])
             # tap pairs dY[t] with X[t + tap - left]: the 4-tap kernel pads one more row on the right
-            dw = wgrad.splitk_wgrad(self._zp, u["x"], drs, CHANNELS, CHANNELS, [tap - left for tap in range(k)])
-            self.grads[q + "0.weight"].copy_(dw.permute(1, 2, 0))
+            w = self.P(q + "0.weight")
+            self.conv.wgrad(u["x"], drs, w, pad=left, out=self.grads[q + "0.weight"])
             if j == 0 and not need_dx:
                 return None
-            w = self.P(q + "0.weight")
-            wb = self._pack(("b", q), lambda: pack_dev(w.flip(-1).permute(1, 0, 2).contiguous()))
-            g, _ = ops.conv_gemm(drs, wb, n=CHANNELS, k=CHANNELS, taps=k, pad=k - 1 - left, residual=dy if j == 0 else None)
+            g = self.conv.dgrad(drs, q, w, pad=left, residual=dy if j == 0 else None)
         return g
 
     # ------------------------------------------------------------------------------------------------------------
@@ -178,7 +161,7 @@ class SpeedySpeechTrainStep:
         B, T = phones.shape
         L = feats.shape[1]
         C = CHANNELS
-        self._packs = {}
+        self.conv.reset()
         self._ws = sc = self.workspace(max(B * T, B * L), B, L)
         self._zp.begin((B, T, L, tones is not None))
         self.gflat.zero_()
@@ -190,7 +173,7 @@ class SpeedySpeechTrainStep:
             tone_w = self.P("encoder.embedding.tone_embedding.weight")
             ops.axpy_(1.0, m._embed_ids(tone_w, tones), emb)
         emb_s = Split.from_f32(emb)
-        pre, pre_s = self.lin_fwd(emb_s, "encoder.prenet.0", act="relu", split=True)
+        pre, pre_s = self.lin_fwd(emb_s, "encoder.prenet.0", act="relu", out_split=True)
         x, xs, enc_ctx = pre, pre_s, []
         for i in range(len(m.encoder_dilations)):
             x, xs, c = self.block_fwd(x, xs, f"encoder.res_blocks.{i}.", ek, 2)
@@ -202,7 +185,7 @@ class SpeedySpeechTrainStep:
         q = "encoder.postnet2.1"
         _, bn_s, mean1, rstd1 = ops.ss_bn_train_fwd(r1, self.P(q + ".weight"), self.P(q + ".bias"), self.P(q + "._mean"),
                                                     self.P(q + "._variance"), sc, want_f32=False)
-        enc, enc_s = self.lin_fwd(bn_s, "encoder.postnet2.2", split=True)
+        enc, enc_s = self.lin_fwd(bn_s, "encoder.postnet2.2", out_split=True)
         # ---- duration predictor on encodings.detach() (:109-118, :178) ----
         h, hs, dur_ctx = enc, enc_s, []
         for i, k in enumerate((4, 3, 1)):
@@ -217,7 +200,7 @@ class SpeedySpeechTrainStep:
         for i in range(len(m.decoder_dilations)):
             x, xs, c = self.block_fwd(x, xs, f"decoder.res_blocks.{i}.", dk, 2)
             dec_ctx.append(c)
-        x2, x2s = self.lin_fwd(xs, "decoder.postnet1.0", residual=x0, split=True)
+        x2, x2s = self.lin_fwd(xs, "decoder.postnet1.0", residual=x0, out_split=True)
         _, hs2, post_ctx = self.block_fwd(x2, x2s, "decoder.postnet2.0.", dk, 2)
         decoded, _ = self.lin_fwd(hs2, "decoder.postnet2.1")
         # ---- losses and their gradients (update_core :57-80) ----
@@ -285,16 +268,10 @@ class SpeedySpeechTrainStep:
     # snapshot / resume: the container of StandardUpdater.state_dict, as FastSpeech2TrainStep writes it
     # ------------------------------------------------------------------------------------------------------------
     def state_dict(self, epoch=0):
-        opt = self.opt.moments()
-        opt["step_count"] = self.step_count
-        opt["LR_Scheduler"] = {"last_lr": self.lr}
-        return {"main_params": self.m.state_dict(), "main_optimizer": opt, "epoch": int(epoch), "iteration": int(self.step_count)}
+        return updater_state(self.m, self.opt, self.lr, epoch)
 
     def set_state_dict(self, state):
-        self.m.set_state_dict(state["main_params"])                  # in place: the parameters stay views of self.flat
-        opt = state.get("main_optimizer", {})
-        self.opt.load_moments(opt)
-        self.opt.steps = int(opt.get("step_count", state.get("iteration", self.step_count)))
+        load_updater_state(self.m, self.opt, state)
 
     def save(self, path, epoch=0):
         from .. import checkpoint

@@ -19,10 +19,9 @@ import torch
 import torch.distributed as dist
 
 from .. import _lib, ops
-from ..graph import GraphRunner
 from ..ops import Split, _ptr, _stream, ceil_to
 from . import wgrad
-from .flat import FlatAdam
+from .flat import FlatAdam, broadcast_from_rank0, step_graphs
 
 SLOPE = 0.4            # UpsampleNet's leaky_relu (waveflow.py:130)
 _SCRATCH = 1024 * 256  # fp32 partials of pk_waveflow_train_outer_sum / pk_waveflow_upsample_bwd
@@ -63,13 +62,11 @@ class WaveFlowTrainStep:
         self.inv_perms = [i32(np.argsort(pm).tolist()) for pm in self.perms]
         self._build_packs()
         # a captured graph pins its own memory pool: ~20 GB at the recipe's batch and 128 channels, so only a few shapes are kept
-        self._graphs = GraphRunner(max_graphs=2)
-        self.use_graphs = os.environ.get("PK_TRAIN_GRAPH", "1") != "0"
+        self._graphs = step_graphs(2)
         self._lens = {}
         model._packed = None
         if self.world > 1:
-            # paddle.DataParallel broadcasts rank 0's parameters at construction
-            dist.broadcast(self.flat, src=0, group=process_group)
+            broadcast_from_rank0(self.flat, model._params, process_group)
 
     step_count = property(lambda self: self.opt.steps)
 
@@ -326,8 +323,6 @@ class WaveFlowTrainStep:
 
     def forward_backward_graphed(self, audio, mel):
         lens = self._net_lens(audio.shape[0], audio.shape[-1] // self.m.n_group)
-        if not self.use_graphs:
-            return self.forward_backward(audio, mel, lens)
         key = (audio.shape[0], audio.shape[-1], mel.shape[-1])
         return self._graphs.run(key, lambda a_, m_: self.forward_backward(a_, m_, lens), [audio, mel])
 

@@ -70,6 +70,7 @@ def _train_exchange_worker(rank, world, port, q):
 
     from oracle.fastspeech2 import adam_step
     from parakeet_b200.training import FlatBuffers
+    from parakeet_b200.training.flat import broadcast_from_rank0
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
@@ -78,6 +79,14 @@ def _train_exchange_worker(rank, world, port, q):
                              w2=torch.randn(2, 5, 3, generator=g))
         fb = FlatBuffers(params, ["w1", "b1", "w2"], "cpu")           # buffers (bn_mean) stay out of the flat buffer
         assert params["w1"].data_ptr() == fb.flat.data_ptr() and fb.total == 16 + 8 + 32
+        params["bn_variance"] = torch.ones(5)
+        w1 = params["w1"].clone()
+        if rank:                                                      # rank 0's parameters and BatchNorm buffers win
+            fb.flat.add_(1.0)
+            params["bn_mean"].fill_(3.0)
+            params["bn_variance"].fill_(3.0)
+        broadcast_from_rank0(fb.flat, params)
+        bcast_ok = torch.equal(params["w1"], w1) and not params["bn_mean"].any() and params["bn_variance"].eq(1.0).all()
         grads = {}
         for r in range(world):                                        # what each rank's backward would have produced
             gr = torch.Generator().manual_seed(100 + r)
@@ -86,7 +95,7 @@ def _train_exchange_worker(rank, world, port, q):
             fb.grads[k].copy_(grads[rank][k])
         fb.all_reduce_grads()
         mean = {k: sum(grads[r][k] for r in range(world)) / world for k in fb.names}
-        ok = all(torch.allclose(fb.grads[k] / world, mean[k], atol=1e-6) for k in fb.names)
+        ok = bool(bcast_ok) and all(torch.allclose(fb.grads[k] / world, mean[k], atol=1e-6) for k in fb.names)
         # Adam on the flat buffers with the DataParallel mean folded in as grad_scale = 1/world (what pk_adam does)
         new_p = adam_step({"flat": fb.flat}, {"flat": fb.gflat / world}, {}, 1e-3, 0.9, 0.999, 1e-8)["flat"]
         per_tensor = adam_step({k: params[k].clone() for k in fb.names}, mean, {}, 1e-3, 0.9, 0.999, 1e-8)

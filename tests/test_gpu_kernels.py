@@ -222,3 +222,60 @@ def test_sum_slices_and_splitk_wgrad(cuda):
         lin = wgrad.splitk_wgrad(zp, xs, dys, cout, cin, [0], x_first=True, out=out)
         ref = torch.einsum("btc,btd->cd", xd, dyd[..., :cout])
         assert lin is out and (lin.double().cpu() - ref).abs().max().item() / ref.abs().max().item() < 2e-5, rep
+
+
+@pytest.mark.parametrize("shape,linear,dil,pad", [
+    ((64, 1, 1), False, 1, None),      # PWG first_conv: 1-channel input
+    ((64, 1, 3), False, 1, None),      # PWG discriminator, first layer
+    ((1, 64, 3), False, 2, None),      # PWG discriminator, last layer: 1-channel output
+    ((1, 64, 1), False, 1, None),      # PWG last_conv_layers.3
+    ((1, 8, 3), False, 1, None),
+    ((128, 64, 3), False, 4, None),    # dilated
+    ((80, 80, 5), False, 1, None),
+    ((64, 80, 1), False, 1, None),
+    ((128, 128, 4), False, 1, 1),      # SpeedySpeech even kernel: one more row on the right
+    ((384, 1), True, 1, None),         # Paddle Linear [in, out]
+    ((96, 200), True, 1, None),
+])
+def test_conv_ops_equal_the_per_step_formulations(cuda, shape, linear, dil, pad):
+    """training/conv.py ConvOps against the packings it replaced, restated here: FastSpeech2 / SpeedySpeech (Linear transposed
+    for the forward, Conv1D taps flipped for the data gradient) and Parallel WaveGAN (Cin zero-padded to the operand width for
+    the forward, Cout padded to 8 in the data-gradient pack, the weight gradient over the padded widths, then sliced).  Packs
+    (both planes), GEMM outputs and weight gradients are compared bit for bit."""
+    from parakeet_b200 import ops
+    from parakeet_b200.ops import pack_dev, pad8
+    from parakeet_b200.training import wgrad
+    from parakeet_b200.training.conv import ConvOps
+    g = torch.Generator().manual_seed(sum(shape) + dil)
+    B, T = 3, 150
+    zp = wgrad.ZeroPlanes()
+    zp.begin(("test", B, T))
+    conv = ConvOps(zp)
+    w = torch.randn(*shape, generator=g).to(cuda)
+    cout, cin, taps = (shape[1], shape[0], 1) if linear else shape
+    x = ops.Split.from_f32(pad8(torch.randn(B, T, cin, generator=g)).to(cuda))        # a 1-channel input rides 8 wide
+    dys = ops.split_pad8(torch.randn(B, T, cout, generator=g).to(cuda))
+    same = lambda a, b: torch.equal(a.hi, b.hi) and torch.equal(a.lo, b.lo)
+    y = conv.fwd(x, "w", w, linear=linear, dil=dil, pad=pad)[0]
+    dx = conv.dgrad(dys, "w", w, linear=linear, dil=dil, pad=pad)
+    dw = conv.wgrad(x, dys, w, linear=linear, dil=dil, pad=pad)
+    pf, pb = conv.packs[("f", "w")], conv.packs[("b", "w")]
+    if linear:
+        old_f, old_b = pack_dev(w.t().contiguous()), pack_dev(w)                         # FastSpeech2 w_fwd / w_bwd, SpeedySpeech lin_*
+        assert same(pf, old_f) and same(pb, old_b)
+        assert torch.equal(y, ops.conv_gemm(x, old_f, n=cout, k=cin)[0])
+        assert torch.equal(dx, ops.conv_gemm(dys, old_b, n=cin, k=cout)[0])
+        assert torch.equal(dw, wgrad.splitk_wgrad(zp, x, dys, cout, cin, [0], x_first=True))
+        return
+    cin_p, cout_p = x.hi.shape[-1], dys.hi.shape[-1]
+    wp = torch.zeros(cout, cin_p, taps, device=cuda)
+    wp[:, :cin] = w
+    old_f = pack_dev(wp)                                                                   # PWG _ConvOps.fwd
+    old_b = pack_dev(pad8(w.flip(-1).permute(1, 2, 0)).permute(0, 2, 1))                 # PWG _ConvOps.dgrad
+    assert same(pf, pack_dev(w)) and same(pf, old_f)                                       # FastSpeech2 w_fwd, SpeedySpeech block_fwd
+    assert same(pb, pack_dev(w.flip(-1).permute(1, 0, 2).contiguous())) and same(pb, old_b)   # FastSpeech2 w_bwd, SpeedySpeech block_bwd
+    assert torch.equal(y, ops.conv_gemm(x, old_f, n=cout, k=cin_p, taps=taps, dil=dil, pad=pad)[0])
+    assert torch.equal(dx, ops.conv_gemm(dys, old_b, n=cin, k=cout_p, taps=taps, dil=dil, pad=None if pad is None else taps - 1 - pad)[0])
+    left = (taps - 1) // 2 if pad is None else pad
+    old_w = wgrad.splitk_wgrad(zp, x, dys, cout_p, cin_p, [(tap - left) * dil for tap in range(taps)])[:, :cout, :cin].permute(1, 2, 0)
+    assert dw.shape == w.shape and torch.equal(dw, old_w)

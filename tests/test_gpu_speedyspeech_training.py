@@ -161,7 +161,8 @@ def test_residual_block_forward_and_backward_alone_against_fp64(cuda, k, n, pre)
     stats = {}
     y_ref = sst.residual_block(q, pre, xd, n, stats)
     y_ref.backward(dy.double())
-    step._packs, step._ws = {}, step.workspace(3 * 37)
+    step.conv.reset()
+    step._ws = step.workspace(3 * 37)
     step._zp.begin(("block", k, n))
     xg = x.to(cuda)
     y, ys, ctx = step.block_fwd(xg, ops.Split.from_f32(xg), pre, k, n)

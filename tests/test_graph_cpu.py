@@ -43,6 +43,24 @@ def test_graph_runner_state_machine(monkeypatch):
     assert not r._graphs and not r._disabled and not r._seen
     r.enabled = False
     assert torch.equal(r.run("k", fn, [x]), x * 2) and not r._seen                     # PK_CUDA_GRAPHS=0: always eager
+    off = G.GraphRunner(enabled=False)
+    for _ in range(3):
+        assert torch.equal(off.run("k", fn, [x]), x * 2)
+    assert not off._seen and not off._graphs and off.replays == 0 and FakeGraph.replays == 2
+
+
+def test_training_steps_graph_switch(monkeypatch):
+    """One switch for every training step: use_graphs when given, else PK_TRAIN_GRAPH; PK_CUDA_GRAPHS=0 wins over both."""
+    from parakeet_b200.training.flat import step_graphs
+    monkeypatch.delenv("PK_CUDA_GRAPHS", raising=False)
+    monkeypatch.delenv("PK_TRAIN_GRAPH", raising=False)
+    assert step_graphs(4).enabled and not step_graphs(4, use_graphs=False).enabled and step_graphs(4).max_graphs == 4
+    monkeypatch.setenv("PK_TRAIN_GRAPH", "0")
+    assert not step_graphs(4).enabled and step_graphs(4, use_graphs=True).enabled
+    assert G.GraphRunner().enabled                                                      # the inference graphs do not follow it
+    monkeypatch.setenv("PK_CUDA_GRAPHS", "0")
+    monkeypatch.setenv("PK_TRAIN_GRAPH", "1")
+    assert not step_graphs(4).enabled and not step_graphs(4, use_graphs=True).enabled
 
 
 def test_zero_planes_lru_is_tied_to_the_graphs():

@@ -768,6 +768,42 @@ int pk_waveflow_backward_layer(const pk_waveflow_backward_layer_args* args, pk_s
 /* WaveFlowLoss (:855-891) in a fixed order: loss[0] = (sum z^2 / (2 sigma^2) - sum logs) / n + log(2 pi) / 2 + log(sigma). */
 int pk_waveflow_train_loss(const float* z, int64_t n, const float* logs, int64_t n_logs, float sigma, float* loss, pk_stream_t stream);
 
+/* ---- GE2E speaker encoder (parakeet/models/lstm_speaker_encoder.py; csrc/lstm.cu) ----
+ * One LSTM layer over all t steps as ONE persistent launch (Paddle nn.LSTM, gates i, f, g, o); the per-step GEMM is wgmma in
+ * bf16x3 with W_hh resident in shared memory and h_{t-1} read by TMA.  Time-major: row r of step s at s * rows + r.
+ * g_in (t, rows, 4H) = x W_ih^T + b_ih (one pk_conv_gemm); b_hh [4H] (or NULL) is added here.
+ * w_hi / w_lo: W_hh [4H, H] as split planes (one allocation, lo after hi) with its rows permuted: packed row
+ *   32 * 4 * s + 8 * (2 * (u / 4) + g / 2) + 2 * (u % 4) + g % 2  holds  W_hh row g * H + 32 * s + u  (slice s, local unit u < 32,
+ *   gate g < 4), so that one thread's accumulator fragment holds the four gates of its units.
+ * h_all ((t+1), rows, H) fp32 and h_hi / h_lo its split planes (one allocation): slab 0 holds h0 on entry (both forms), slab s+1
+ *   receives h_s.  c: (rows, H) updated in place when c_step == 0, else ((t+1), rows, H) with c0 in slab 0 and c_s in slab s+1
+ *   (c_step = rows * H, training).  gates (t, rows, 4H) receives the post-activation gates (or NULL).
+ * counters: >= t * ceil(rows / 64) uint32, zeroed on the stream by the call itself.  TMA operands 16-byte aligned.
+ * hidden in {64, 256}; any other size returns PK_ERR_UNSUPPORTED, as does a grid that cannot be co-resident. */
+int pk_lstm_fwd(const float* g_in, const float* b_hh, const void* w_hi, const void* w_lo, int32_t rows, int32_t t, int32_t hidden,
+                float* h_all, void* h_hi, void* h_lo, float* c, int64_t c_step, float* gates, uint32_t* counters,
+                int64_t counters_len, pk_stream_t stream);
+/* Backward through time of pk_lstm_fwd (training mode's gates and c_all), one persistent launch in reverse time, wgmma bf16x3:
+ * dh_s = dh_in[s] (or NULL) + (s == t-1 ? dh_last : 0) (or NULL) + dgates_{s+1} W_hh.  wt_hi / wt_lo: W_hh^T [H, 4H] split planes.
+ * dc: (rows, H) scratch.  dgates (t, rows, 4H) fp32 gradients of the pre-activation gates, dg_hi / dg_lo the same as split planes
+ * (one allocation; read back by TMA for the next step). */
+int pk_lstm_bwd(const void* wt_hi, const void* wt_lo, const float* gates, const float* c_all, const float* dh_in, const float* dh_last,
+                int32_t rows, int32_t t, int32_t hidden, float* dc, float* dgates, void* dg_hi, void* dg_lo, uint32_t* counters,
+                int64_t counters_len, pk_stream_t stream);
+/* doubles of scratch pk_ge2e_loss needs for embeds (n, m, c) */
+int64_t pk_ge2e_loss_scratch(int32_t n, int32_t m, int32_t c);
+/* LSTMSpeakerEncoder.similarity_matrix + loss on embeds (n, m, c) (m >= 2), one block in double: loss[0] (cross-entropy mean),
+ * sim (n*m, n) = (cosine to the inclusive centroids, own speaker: to the exclusive centroid) * w[0] + b[0] (or NULL).
+ * With d_embeds / dw / db (all or none): the gradient of the loss, dw and db times 0.01 (do_gradient_ops).  No atomics. */
+int pk_ge2e_loss(const float* embeds, int32_t n, int32_t m, int32_t c, const float* w, const float* b, double* scratch,
+                 int64_t scratch_len, float* loss, float* sim, float* d_embeds, float* dw, float* db, pk_stream_t stream);
+/* backward of F.normalize(relu(z)) (rows, n) given e = relu(z) and dy: dz (z > 0 read as e > 0). */
+int pk_ge2e_embed_bwd(const float* e, const float* dy, int32_t rows, int32_t n, float eps, float* dz, pk_stream_t stream);
+/* y[s] = F.normalize(mean(x[offsets[s] : offsets[s+1]], 0), axis=0) for s < segments (embed_utterance per utterance), n <= 8192;
+ * an empty segment yields zeros */
+int pk_segment_mean_normalize(const float* x, const int32_t* offsets, int32_t segments, int32_t n, float eps, float* y,
+                              pk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

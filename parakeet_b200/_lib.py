@@ -217,11 +217,18 @@ def _declare(L):
         "pk_waveflow_train_cond_scatter": [vp, vp, i32, i32, i32, i32, i32, vp, vp],
         "pk_waveflow_train_loss": [vp, i64, vp, i64, f32, vp, vp],
         "pk_waveflow_backward_layer": [C.POINTER(WaveflowBackwardLayerArgs), vp],
+        "pk_lstm_fwd": [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, i64, vp, vp, i64, vp],
+        "pk_lstm_bwd": [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp],
+        "pk_ge2e_loss": [vp, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
+        "pk_ge2e_embed_bwd": [vp, vp, i32, i32, f32, vp, vp],
+        "pk_segment_mean_normalize": [vp, vp, i32, i32, f32, vp, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(L, name)
         fn.argtypes = argtypes
         fn.restype = C.c_int
+    L.pk_ge2e_loss_scratch.argtypes = [i32, i32, i32]
+    L.pk_ge2e_loss_scratch.restype = i64
 
 
 def check(rc, what=""):

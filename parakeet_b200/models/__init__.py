@@ -2,3 +2,4 @@ from .fastspeech2 import FastSpeech2, FastSpeech2Inference, FastSpeech2Loss  # n
 from .parallel_wavegan import PWGDiscriminator, PWGGenerator, PWGInference  # noqa: F401
 from .speedyspeech import SpeedySpeech, SpeedySpeechInference  # noqa: F401
 from .waveflow import ConditionalWaveFlow, WaveFlowLoss  # noqa: F401
+from .lstm_speaker_encoder import LSTMSpeakerEncoder  # noqa: F401

@@ -535,3 +535,103 @@ def dropout(x, p, seed, site, step, out_f32=True, out_split=False, inplace=False
                                      float(p), int(seed) & 0xFFFFFFFFFFFFFFFF, int(site), int(step), _ptr(step_dev), _ptr(y), _ptr(ys.hi if ys else None),
                                      _ptr(ys.lo if ys else None), _stream()), "pk_dropout")
     return y, ys
+
+
+LSTM_ROWS, LSTM_SLICE = 64, 32          # csrc/lstm.cu: rows per tile, hidden units per CTA
+
+
+def lstm_schedule(rows, hidden, max_ctas):
+    """The grid of pk_lstm_fwd / pk_lstm_bwd (csrc/lstm.cu `schedule`): -> (slices, tiles, groups, grid).  CTA b serves hidden
+    slice b % slices and row tiles b // slices + k * groups; grid 0 means the launch is refused (not one CTA per slice fits)."""
+    slices, tiles = hidden // LSTM_SLICE, -(-rows // LSTM_ROWS)
+    groups = min(tiles, max_ctas // slices)
+    return slices, tiles, groups, groups * slices if groups >= 1 else 0
+
+
+def lstm_counters(rows, t, device):
+    return torch.empty(t * -(-rows // LSTM_ROWS), dtype=torch.int32, device=device)
+
+
+def lstm_gate_perm(hidden, device):
+    """Row order of the packed W_hh of pk_lstm_fwd: packed row 128 s + 8 (2 (u // 4) + g // 2) + 2 (u % 4) + g % 2 is W_hh row
+    g * H + 32 s + u, so that one thread's wgmma accumulator fragment holds the four gates (i, f, g, o) of its units."""
+    perm = torch.empty(4 * hidden, dtype=torch.int64)
+    for s in range(hidden // LSTM_SLICE):
+        for u in range(LSTM_SLICE):
+            for g in range(4):
+                perm[4 * LSTM_SLICE * s + 8 * (2 * (u // 4) + g // 2) + 2 * (u % 4) + g % 2] = g * hidden + LSTM_SLICE * s + u
+    return perm.to(device)
+
+
+def lstm_pack_fwd(w_hh, perm):
+    """W_hh [4H, H] fp32 -> the split planes pk_lstm_fwd keeps resident (rows in lstm_gate_perm order)."""
+    return Split.from_f32(w_hh.index_select(0, perm))
+
+
+def lstm_pack_bwd(w_hh):
+    """W_hh [4H, H] fp32 -> W_hh^T [H, 4H] split planes, the resident operand of pk_lstm_bwd."""
+    return Split.from_f32(w_hh.t())
+
+
+def lstm_fwd(g_in, b_hh, w_packed, h_all, h_split, c, gates=None, counters=None):
+    """One LSTM layer over all steps (pk_lstm_fwd).  g_in (T, rows, 4H) = x W_ih^T + b_ih; w_packed from lstm_pack_fwd;
+    h_all (T+1, rows, H) fp32 and h_split its Split planes, both with h0 in slab 0; c (rows, H) updated in place, or
+    (T+1, rows, H) with c0 in slab 0 (then every c_t is kept, with the gates, for the backward)."""
+    _require_cuda(g_in, b_hh, w_packed.hi, h_all, h_split.hi, c, gates, counters)
+    T, rows, H4 = g_in.shape
+    H = H4 // 4
+    counters = lstm_counters(rows, T, g_in.device) if counters is None else counters
+    c_step = 0 if c.dim() == 2 else rows * H
+    _lib.check(_lib.lib().pk_lstm_fwd(_ptr(g_in), _ptr(b_hh), _ptr(w_packed.hi), _ptr(w_packed.lo), rows, T, H, _ptr(h_all),
+                                      _ptr(h_split.hi), _ptr(h_split.lo), _ptr(c), c_step, _ptr(gates), _ptr(counters), counters.numel(),
+                                      _stream()), "pk_lstm_fwd")
+
+
+def lstm_bwd(wt_packed, gates, c_all, dh_in, dh_last, dgates, dg, dc=None, counters=None):
+    """Backward through time of one layer (pk_lstm_bwd): wt_packed from lstm_pack_bwd -> dgates (T, rows, 4H) fp32 and its split
+    planes `dg` (T * rows rows, 4H; one allocation)."""
+    _require_cuda(wt_packed.hi, gates, c_all, dh_in, dh_last, dgates, dg.hi, dc, counters)
+    T, rows, H4 = gates.shape
+    H = H4 // 4
+    dc = torch.empty(rows, H, dtype=torch.float32, device=gates.device) if dc is None else dc
+    counters = lstm_counters(rows, T, gates.device) if counters is None else counters
+    _lib.check(_lib.lib().pk_lstm_bwd(_ptr(wt_packed.hi), _ptr(wt_packed.lo), _ptr(gates), _ptr(c_all), _ptr(dh_in), _ptr(dh_last), rows,
+                                      T, H, _ptr(dc), _ptr(dgates), _ptr(dg.hi), _ptr(dg.lo), _ptr(counters), counters.numel(), _stream()),
+               "pk_lstm_bwd")
+    return dgates
+
+
+def ge2e_loss(embeds, n, m, c, w, b, want_grads=False):
+    """GE2E loss on embeds viewed as (n, m, c) -> (loss (1,), sim (n*m, n), d_embeds, dw (1,), db (1,)); the gradients are None
+    unless want_grads (dw, db already times 0.01)."""
+    _require_cuda(embeds, w, b)
+    dev = embeds.device
+    L = _lib.lib()
+    scratch = torch.empty(int(L.pk_ge2e_loss_scratch(n, m, c)), dtype=torch.float64, device=dev)
+    loss = torch.empty(1, dtype=torch.float32, device=dev)
+    sim = torch.empty(n * m, n, dtype=torch.float32, device=dev)
+    de = torch.empty_like(embeds) if want_grads else None
+    dw = torch.empty(1, dtype=torch.float32, device=dev) if want_grads else None
+    db = torch.empty(1, dtype=torch.float32, device=dev) if want_grads else None
+    _lib.check(L.pk_ge2e_loss(_ptr(embeds), n, m, c, _ptr(w), _ptr(b), _ptr(scratch), scratch.numel(), _ptr(loss), _ptr(sim), _ptr(de),
+                              _ptr(dw), _ptr(db), _stream()), "pk_ge2e_loss")
+    return loss, sim, de, dw, db
+
+
+def ge2e_embed_bwd(e, dy, eps=1e-12):
+    """backward of F.normalize(relu(z)) (rows, n), given e = relu(z)."""
+    _require_cuda(e, dy)
+    dz = torch.empty_like(e)
+    rows, n = e.shape
+    _lib.check(_lib.lib().pk_ge2e_embed_bwd(_ptr(e), _ptr(dy), rows, n, float(eps), _ptr(dz), _stream()), "pk_ge2e_embed_bwd")
+    return dz
+
+
+def segment_mean_normalize(x, offsets, eps=1e-12):
+    """x (rows, n), offsets int32 (S + 1,) on the device -> (S, n): F.normalize(mean of each segment's rows, axis=0)."""
+    _require_cuda(x, offsets)
+    s = offsets.numel() - 1
+    y = torch.empty(s, x.shape[1], dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().pk_segment_mean_normalize(_ptr(x), _ptr(offsets), s, x.shape[1], float(eps), _ptr(y), _stream()),
+               "pk_segment_mean_normalize")
+    return y

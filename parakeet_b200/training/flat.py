@@ -126,3 +126,48 @@ class FlatAdam:
         for key, view in self._views():
             if key in opt:
                 view.copy_(torch.as_tensor(opt[key]).reshape(view.shape).to(view.device, view.dtype))
+
+
+class PdCheckpoint:
+    """The old-style `step-N.pdparams` / `step-N.pdopt` pair of ExperimentBase (utils/checkpoint.py:61-138) for a training step
+    that holds its model as `self.m` and its optimiser as `self.opt` (a FlatAdam): the model's state dict, and the Adam state
+    under Paddle's accumulator suffixes (`<name>_moment1_0`, `<name>_moment2_0`, `<name>_beta1_pow_acc_0`, `<name>_beta2_pow_acc_0`)."""
+
+    step_count = property(lambda self: self.opt.steps)
+
+    def state_dict(self):
+        """(params, opt)."""
+        opt = self.opt.moments()
+        for k in self.opt.buffers.names:
+            opt[k + "_beta1_pow_acc_0"] = torch.tensor([self.opt.beta1 ** self.step_count])
+            opt[k + "_beta2_pow_acc_0"] = torch.tensor([self.opt.beta2 ** self.step_count])
+        opt["step_count"] = self.step_count
+        return self.m.state_dict(), opt
+
+    def set_state_dict(self, params, opt=None):
+        self.m.set_state_dict(params)                # in place: the parameters stay views of the flat buffer
+        if opt:
+            self.opt.load_moments(opt)
+            self.opt.steps = int(opt.get("step_count", self.step_count))
+
+    def save(self, checkpoint_dir, iteration=None):
+        """Write step-N.pdparams and step-N.pdopt (N = iteration or the completed steps) and record it in checkpoint_dir/checkpoint."""
+        from .. import checkpoint
+        it = self.step_count if iteration is None else int(iteration)
+        params, opt = self.state_dict()
+        os.makedirs(checkpoint_dir, exist_ok=True)
+        base = os.path.join(checkpoint_dir, f"step-{it}")
+        checkpoint.save(params, base + ".pdparams")
+        checkpoint.save(opt, base + ".pdopt")
+        with open(os.path.join(checkpoint_dir, "checkpoint"), "w") as fh:
+            fh.write(f"model_checkpoint_path: step-{it}")
+        return base
+
+    def load(self, checkpoint_dir, iteration=None):
+        from .. import checkpoint
+        if iteration is None:
+            with open(os.path.join(checkpoint_dir, "checkpoint")) as fh:
+                iteration = int(fh.read().strip().rsplit("-", 1)[-1])
+        base = os.path.join(checkpoint_dir, f"step-{iteration}")
+        self.set_state_dict(checkpoint.load(base + ".pdparams"), checkpoint.load(base + ".pdopt"))
+        return int(iteration)

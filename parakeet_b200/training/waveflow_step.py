@@ -12,7 +12,6 @@ gradients and Adam moments live in flat buffers (`training/flat.py: FlatAdam`); 
 torch only allocates, views, copies and all-reduces.
 """
 import ctypes as C_
-import os
 
 import numpy as np
 import torch
@@ -21,13 +20,13 @@ import torch.distributed as dist
 from .. import _lib, ops
 from ..ops import Split, _ptr, _stream, ceil_to
 from . import wgrad
-from .flat import FlatAdam, broadcast_from_rank0, step_graphs
+from .flat import FlatAdam, PdCheckpoint, broadcast_from_rank0, step_graphs
 
 SLOPE = 0.4            # UpsampleNet's leaky_relu (waveflow.py:130)
 _SCRATCH = 1024 * 256  # fp32 partials of pk_waveflow_train_outer_sum / pk_waveflow_upsample_bwd
 
 
-class WaveFlowTrainStep:
+class WaveFlowTrainStep(PdCheckpoint):
     def __init__(self, model, learning_rate=2e-4, sigma=1.0, beta1=0.9, beta2=0.999, epsilon=1e-8, process_group=None):
         if not model._eligible():
             raise NotImplementedError("the WaveFlow training step needs 64 or 128 channels, 64 < n_mels <= 128 (a multiple of 8) "
@@ -67,8 +66,6 @@ class WaveFlowTrainStep:
         model._packed = None
         if self.world > 1:
             broadcast_from_rank0(self.flat, model._params, process_group)
-
-    step_count = property(lambda self: self.opt.steps)
 
     # ------------------------------------------------------------------------------------------------------------
     # weights: offsets into the flat buffers and the packed GEMM operands
@@ -349,44 +346,3 @@ class WaveFlowTrainStep:
         self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
         self.m._packed = None                                                        # inference weights are re-packed on demand
         return loss.clone()
-
-    # ------------------------------------------------------------------------------------------------------------
-    # checkpoints: the old-style step-N.pdparams / step-N.pdopt pair (utils/checkpoint.py:61-138)
-    # ------------------------------------------------------------------------------------------------------------
-    def state_dict(self):
-        """(params, opt): the model's state dict and the Adam state under Paddle's accumulator suffixes (`<name>_moment1_0`,
-        `<name>_moment2_0`, `<name>_beta1_pow_acc_0`, `<name>_beta2_pow_acc_0`)."""
-        opt = self.opt.moments()
-        for k in self.buffers.names:
-            opt[k + "_beta1_pow_acc_0"] = torch.tensor([self.opt.beta1 ** self.step_count])
-            opt[k + "_beta2_pow_acc_0"] = torch.tensor([self.opt.beta2 ** self.step_count])
-        opt["step_count"] = self.step_count
-        return self.m.state_dict(), opt
-
-    def set_state_dict(self, params, opt=None):
-        self.m.set_state_dict(params)                # in place: the parameters stay views of self.flat
-        if opt:
-            self.opt.load_moments(opt)
-            self.opt.steps = int(opt.get("step_count", self.step_count))
-
-    def save(self, checkpoint_dir, iteration=None):
-        """Write step-N.pdparams and step-N.pdopt (N = iteration or the completed steps) and record it in checkpoint_dir/checkpoint."""
-        from .. import checkpoint
-        it = self.step_count if iteration is None else int(iteration)
-        params, opt = self.state_dict()
-        os.makedirs(checkpoint_dir, exist_ok=True)
-        base = os.path.join(checkpoint_dir, f"step-{it}")
-        checkpoint.save(params, base + ".pdparams")
-        checkpoint.save(opt, base + ".pdopt")
-        with open(os.path.join(checkpoint_dir, "checkpoint"), "w") as fh:
-            fh.write(f"model_checkpoint_path: step-{it}")
-        return base
-
-    def load(self, checkpoint_dir, iteration=None):
-        from .. import checkpoint
-        if iteration is None:
-            with open(os.path.join(checkpoint_dir, "checkpoint")) as fh:
-                iteration = int(fh.read().strip().rsplit("-", 1)[-1])
-        base = os.path.join(checkpoint_dir, f"step-{iteration}")
-        self.set_state_dict(checkpoint.load(base + ".pdparams"), checkpoint.load(base + ".pdopt"))
-        return int(iteration)

@@ -14,6 +14,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py waveflow_train     # only tests/golden/ref_executed_waveflow_train.npz
     python scripts/make_golden_ref.py fs2ms_train        # only tests/golden/ref_executed_fs2ms_train.npz
     python scripts/make_golden_ref.py speedyspeech_train # only tests/golden/ref_executed_speedyspeech_train.npz
+    python scripts/make_golden_ref.py ge2e               # only tests/golden/ref_executed_ge2e.npz
 """
 import importlib.util
 import os
@@ -451,6 +452,48 @@ def speedyspeech_train(out):
                 out[f"{tag}/stat/{k}"] = v.detach().numpy().astype(np.float32)
 
 
+def ge2e(out):
+    """The reference's own LSTMSpeakerEncoder (its nn.LSTM on the stand-in's LSTM, Paddle 2.1 keys): embed_sequences (also with
+    initial states and reduce=True), the forward's loss and EER (its reshape to [N, -1, N]), loss / similarity matrix on the plain
+    (N, M, C) grouping, and every parameter gradient after do_gradient_ops.  (small) 40 mels / 3 layers / hidden 64 / output 64
+    at 4 speakers x 3 utterances x 20 frames; (shipped) 40 / 3 / 256 / 256 at 4 x 5 x 160.  The weights and utterances are
+    regenerated from their seeds (oracle.ge2e); a sample of the utterances is stored to check that.  Gradients of up to 1024
+    elements are stored in full, larger ones as every stride-th element (stride = numel // 1024) plus their L2 norm.
+    The reference module imports scipy (interp1d, brentq) and sklearn (roc_curve) for its EER: regenerating this fixture needs
+    both installed (the stored EER comes from sklearn's roc_curve)."""
+    import numpy
+    from oracle import ge2e as og
+    from parakeet.models.lstm_speaker_encoder import LSTMSpeakerEncoder
+    if not hasattr(numpy, "int"):
+        numpy.int = int                  # inv_argmax's np.int (removed from numpy 1.24 on; the reference ran on older numpy)
+    for tag, (cfg, (N, M, T_), seed) in og.GOLDEN_CONFIGS.items():
+        ref = LSTMSpeakerEncoder(*cfg)
+        params = og.synth_params(seed, *cfg)
+        keys = check_keys(ref, params, f"LSTMSpeakerEncoder({tag})")
+        out[f"{tag}/keys"] = np.asarray(keys)
+        ref.set_state_dict(params)
+        x = og.synth_utterances(seed + 100, N * M, T_, cfg[0])
+        out[f"{tag}/x_sample"] = x.reshape(-1)[::97].numpy()
+        with torch.no_grad():
+            out[f"{tag}/embeds"] = ref.embed_sequences(T(x)).numpy()
+            out[f"{tag}/embed_reduce"] = ref.embed_utterance(T(x)).numpy()
+            h0, c0 = og.synth_states(seed + 200, cfg[1], N * M, cfg[2])
+            out[f"{tag}/embeds_init"] = ref.embed_sequences(T(x), (T(h0), T(c0))).numpy()
+            plain = ref.embed_sequences(T(x)).reshape([N, M, -1])
+            out[f"{tag}/plain_sim"] = ref.similarity_matrix(plain)[0].numpy()
+            out[f"{tag}/plain_loss"] = np.asarray(float(ref.loss(plain)[0]))
+            grouped = ref.embed_sequences(T(x)).reshape([N, -1, N])
+            out[f"{tag}/sim"] = ref.similarity_matrix(grouped)[0].numpy()
+        loss, eer = ref(T(x), N)
+        loss.backward()
+        ref.do_gradient_ops()
+        out[f"{tag}/loss"], out[f"{tag}/eer"] = np.asarray(float(loss)), np.asarray(float(eer))
+        for k, v in ref.named_parameters():
+            gk = v.grad.detach().reshape(-1)
+            out[f"{tag}/grad/{k}"] = gk[::max(1, gk.numel() // 1024)].numpy().astype(np.float32)
+            out[f"{tag}/gradnorm/{k}"] = np.asarray(float(gk.double().norm()))
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -522,7 +565,7 @@ def sampled(models):
 
 def main():
     single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
-              "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train}
+              "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

@@ -108,6 +108,11 @@ class Tensor(torch.Tensor):
 Tensor._counter = 0
 
 
+class Parameter(torch.nn.Parameter):
+    def _grad_ivar(self):                                # the gradient tensor itself (written in place by do_gradient_ops)
+        return self.grad
+
+
 class _Size(int):
     def __new__(cls, t):
         obj = super().__new__(cls, t.numel())
@@ -194,10 +199,18 @@ def build():
     P.maximum = lambda a, b: T(torch.maximum(a, b))
     P.get_default_dtype = lambda: "float32"
     P.multiply = lambda a, b: T(a * b)
+    P.bmm = lambda a, b: T(torch.bmm(a, b))
+    P.broadcast_to = lambda x, shape: T(torch.Tensor.expand(x, *shape))
+
+    def scatter(x, index, updates, overwrite=True):
+        """paddle.scatter along axis 0; overwrite=True: rows of `index` take the rows of `updates` (unique indices here)."""
+        assert overwrite
+        return T(x.index_put((index.reshape(-1).to(torch.int64),), updates))
+    P.scatter = scatter
     P.add = lambda a, b: T(a + b)
 
     def create_parameter(shape, dtype="float32", default_initializer=None, attr=None, is_bias=False):
-        p = torch.nn.Parameter(torch.zeros(tuple(shape), dtype=_dt(dtype) or torch.float32))
+        p = Parameter(torch.zeros(tuple(shape), dtype=_dt(dtype) or torch.float32))
         if default_initializer is not None:
             default_initializer(p)
         return p
@@ -458,6 +471,53 @@ def build():
             return list(self.children())[i]
     nn.LayerList = LayerList
 
+    class LSTMCell(Layer):
+        def __init__(self, input_size, hidden_size):
+            super().__init__()
+            self.weight_ih = torch.nn.Parameter(torch.zeros(4 * hidden_size, input_size))
+            self.weight_hh = torch.nn.Parameter(torch.zeros(4 * hidden_size, hidden_size))
+            self.bias_ih = torch.nn.Parameter(torch.zeros(4 * hidden_size))
+            self.bias_hh = torch.nn.Parameter(torch.zeros(4 * hidden_size))
+
+    class RNN(Layer):
+        def __init__(self, cell):
+            super().__init__()
+            self.cell = cell
+
+    class LSTM(Layer):
+        """paddle.nn.LSTM (2.1): a LayerList of RNN(LSTMCell), so the keys are `{l}.cell.weight_ih` ...; input (B, T, I)
+        (time_major=False), returns (out, (h, c)) with h, c [num_layers, B, H].  The cell is torch's lstm_cell (gates i, f, g, o,
+        both biases added)."""
+        def __init__(self, input_size, hidden_size, num_layers=1, direction="forward", time_major=False, dropout=0.0):
+            super().__init__()
+            assert direction == "forward" and not time_major and dropout == 0.0
+            for l in range(num_layers):
+                self.add_module(str(l), RNN(LSTMCell(input_size if l == 0 else hidden_size, hidden_size)))
+            self.num_layers, self.hidden_size = num_layers, hidden_size
+
+        def forward(self, inputs, initial_states=None):
+            B = inputs.shape[0]
+            x, hs, cs = inputs, [], []
+            for l, rnn in enumerate(self.children()):
+                if initial_states is None:
+                    h = c = torch.zeros(B, self.hidden_size, dtype=inputs.dtype)
+                else:
+                    h, c = initial_states[0][l], initial_states[1][l]
+                outs = []
+                for t in range(x.shape[1]):
+                    cell = rnn.cell
+                    h, c = torch._VF.lstm_cell(x[:, t], (h, c), cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh)
+                    outs.append(h)
+                x = torch.stack(outs, 1)
+                hs.append(h)
+                cs.append(c)
+            return T(x), (T(torch.stack(hs)), T(torch.stack(cs)))
+    nn.LSTMCell, nn.RNN, nn.LSTM = LSTMCell, RNN, LSTM
+
+    def cross_entropy_loss(weight=None, ignore_index=-100, reduction="mean", soft_label=False, axis=-1):
+        assert weight is None and not soft_label and axis == -1
+        return lambda x, label: T(TF.cross_entropy(x, label.reshape(-1), ignore_index=ignore_index, reduction=reduction))
+    nn.CrossEntropyLoss = cross_entropy_loss
     nn.MSELoss = lambda reduction="mean": (lambda a, b: T(TF.mse_loss(a, b, reduction=reduction)))
     nn.L1Loss = lambda reduction="mean": (lambda a, b: T(TF.l1_loss(a, b, reduction=reduction)))
 

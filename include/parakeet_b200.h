@@ -804,6 +804,57 @@ int pk_ge2e_embed_bwd(const float* e, const float* dy, int32_t rows, int32_t n, 
 int pk_segment_mean_normalize(const float* x, const int32_t* offsets, int32_t segments, int32_t n, float eps, float* y,
                               pk_stream_t stream);
 
+/* ---- Tacotron2 (csrc/tacotron2.cu) ----
+ * pk_taco2_decode: every step of Tacotron2Decoder.infer (teacher = 0) or of the teacher-forced Tacotron2Decoder.forward
+ * (teacher = 1) as one persistent launch, fp32.  Fixed sizes: d_attention_rnn = d_decoder_rnn = 1024, d_prenet 256,
+ * d_attention 128; d_enc 512 or 768, batch <= 32, dmr = d_mels * r a multiple of 4, odd loc_k <= 63 (else PK_ERR_UNSUPPORTED,
+ * as is a grid of fewer than 32 co-resident CTAs).  Weights are row-major [out, in]:
+ *   pre_w1 [256, dmr], pre_w2 [256, 256]; att_w [4096, 256 + d_enc + 1024] = [W_ih | W_hh] of the attention LSTMCell
+ *   (gates i, f, g, o), dec_w [4096, 1024 + d_enc + 1024] the same for the decoder LSTMCell, biases [4096] each;
+ *   q_w [128, 1024]; loc_w [128, 2, loc_k] = location_layer o location_conv; v_w [128]; proj_w [dmr, 1024 + d_enc], proj_b [dmr];
+ *   stop_w [1024 + d_enc], stop_b [1] or both NULL (no stop token).
+ * keys (batch, t_enc, d_enc) encoder outputs, pkeys (batch, t_enc, 128) = key_layer(keys); text_lens (int32, teacher only:
+ * energies of positions >= text_lens get -1e9); mels (batch, steps, dmr) teacher inputs.  The prenet dropout (ReLU, then
+ * p_prenet with pk_dropout's Philox: sites 0 and 1 for the two layers, step = decoder step, element b * 256 + j) is always on.
+ * Outputs (batch, steps, dmr) mel_out, (batch, steps, t_enc) align_out, (batch, steps) stop_out; frames[b] (int32) = frames
+ * produced.  infer stops on the device, after frame i when (stop token) sigmoid(stop_out[0, i]) > 0.5 (batch must be 1), or
+ * (no stop token) argmax(align[0, i]) == t_enc - 1 for an i > first such i + 20, or at i + 1 == steps; rows past the stop are
+ * zero.  The call zeroes the workspace (pk_taco2_workspace floats: counters and recurrent state) and the outputs on the stream. */
+typedef struct {
+  int32_t batch, t_enc, d_enc, dmr, steps, teacher, loc_k;
+  float p_prenet;
+  uint64_t seed;
+  const float* keys; const float* pkeys; const int32_t* text_lens; const float* mels;
+  const float* pre_w1; const float* pre_w2;
+  const float* att_w; const float* att_b_ih; const float* att_b_hh;
+  const float* q_w; const float* loc_w; const float* v_w;
+  const float* dec_w; const float* dec_b_ih; const float* dec_b_hh;
+  const float* proj_w; const float* proj_b; const float* stop_w; const float* stop_b;
+  float* workspace; int64_t workspace_len;
+  float* mel_out; float* align_out; float* stop_out; int32_t* frames;
+  uint64_t* prof; int64_t prof_len;   /* optional (NULL): per-CTA ns counters, [cta][0..5] time per phase incl. its hand-off,
+                                         [cta][6..11] wait from arrival to release; zeroed by the call; pk_taco2_prof_len() entries */
+} PkTaco2DecodeArgs;
+int64_t pk_taco2_workspace(int32_t batch, int32_t t_enc, int32_t d_enc);
+int64_t pk_taco2_prof_len(void);
+int pk_taco2_decode(const PkTaco2DecodeArgs* args, pk_stream_t stream);
+/* y (batch, t, channels) = table[ids] + (tones ? tone_table[tones], zero for tone 0 (padding_idx) : 0); ids / tones int64 */
+int pk_taco2_embed(const int64_t* ids, const float* table, const int64_t* tones, const float* tone_table, int32_t batch, int32_t t,
+                   int32_t channels, float* y, pk_stream_t stream);
+/* dst (t, batch, channels) = src (batch, t, channels) time-major; with reverse, row s < lens[b] (lens NULL: t) reads src row
+ * lens[b] - 1 - s (the backward direction of a bidirectional LSTM over ragged sequences) */
+int pk_taco2_time_major(const float* src, const int32_t* lens, int32_t reverse, int32_t batch, int32_t t, int32_t channels, float* dst,
+                        pk_stream_t stream);
+/* out (batch, t, 2 hidden + gc_dim) = [h_fwd[s] | h_bwd[lens - 1 - s] | gc[b]] for s < lens[b] (NULL: t), zero rows after;
+ * h_fwd / h_bwd (t, batch, hidden) time-major */
+int pk_taco2_bilstm_merge(const float* h_fwd, const float* h_bwd, const int32_t* lens, const float* gc, int32_t batch, int32_t t,
+                          int32_t hidden, int32_t gc_dim, float* out, pk_stream_t stream);
+/* Tacotron2Loss.forward, one block in double: out[5] = {loss, mel_loss, post_mel_loss, guided_attn_loss (align != NULL, else 0),
+ * stop_loss (stop_logits != NULL, else 0)}; mel / post / target (batch, t, channels), align (batch, t, t_enc), slens / plens int32 */
+int pk_taco2_loss(const float* mel, const float* post, const float* target, int32_t batch, int32_t t, int32_t channels, const float* align,
+                  int32_t t_enc, const int32_t* slens, const int32_t* plens, float sigma, const float* stop_logits, float* out,
+                  pk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -128,6 +128,16 @@ class SsResidualBlockArgs(C.Structure):
                 ("y", C.c_void_p), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p)]
 
 
+class Taco2DecodeArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("t_enc", C.c_int32), ("d_enc", C.c_int32), ("dmr", C.c_int32), ("steps", C.c_int32),
+                ("teacher", C.c_int32), ("loc_k", C.c_int32), ("p_prenet", C.c_float), ("seed", C.c_uint64)] + \
+        [(n, C.c_void_p) for n in ("keys", "pkeys", "text_lens", "mels", "pre_w1", "pre_w2", "att_w", "att_b_ih", "att_b_hh", "q_w",
+                                   "loc_w", "v_w", "dec_w", "dec_b_ih", "dec_b_hh", "proj_w", "proj_b", "stop_w", "stop_b",
+                                   "workspace")] + \
+        [("workspace_len", C.c_int64)] + [(n, C.c_void_p) for n in ("mel_out", "align_out", "stop_out", "frames")] + \
+        [("prof", C.c_void_p), ("prof_len", C.c_int64)]
+
+
 def _declare(L):
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     sigs = {
@@ -222,6 +232,11 @@ def _declare(L):
         "pk_ge2e_loss": [vp, i32, i32, i32, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
         "pk_ge2e_embed_bwd": [vp, vp, i32, i32, f32, vp, vp],
         "pk_segment_mean_normalize": [vp, vp, i32, i32, f32, vp, vp],
+        "pk_taco2_decode": [C.POINTER(Taco2DecodeArgs), vp],
+        "pk_taco2_embed": [vp, vp, vp, vp, i32, i32, i32, vp, vp],
+        "pk_taco2_time_major": [vp, vp, i32, i32, i32, i32, vp, vp],
+        "pk_taco2_bilstm_merge": [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp],
+        "pk_taco2_loss": [vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, f32, vp, vp, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(L, name)
@@ -229,6 +244,10 @@ def _declare(L):
         fn.restype = C.c_int
     L.pk_ge2e_loss_scratch.argtypes = [i32, i32, i32]
     L.pk_ge2e_loss_scratch.restype = i64
+    L.pk_taco2_workspace.argtypes = [i32, i32, i32]
+    L.pk_taco2_workspace.restype = i64
+    L.pk_taco2_prof_len.argtypes = []
+    L.pk_taco2_prof_len.restype = i64
 
 
 def check(rc, what=""):

@@ -593,20 +593,9 @@ extern "C" int pk_adam(float* params, const float* grads, float* m, float* v, in
 // inside the position-wise feed-forward, in the predictors and in the postnet - SURVEY.md 8a).
 // The mask is never stored: element i keeps iff word (i & 3) of Philox4x32-10(counter = {i >> 2 (64 bit), site, step},
 // key = seed) is >= p * 2^32, so the backward pass regenerates it from (seed, step, site) with the same kernel applied
-// to the gradient.  oracle/fastspeech2.py restates the generator in numpy for the parity tests.
+// to the gradient (philox4x32_10: pk_sm90.cuh).  oracle/fastspeech2.py restates the generator in numpy for the parity tests.
 // ----------------------------------------------------------------------------------------------------------------
 namespace pk {
-
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t* out) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
-  out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
 
 __global__ void dropout_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ x_hi, const __nv_bfloat16* __restrict__ x_lo,
                                long long n, uint32_t thresh, float scale, uint32_t seed_lo, uint32_t seed_hi, uint32_t site, uint32_t step,

@@ -3,3 +3,4 @@ from .parallel_wavegan import PWGDiscriminator, PWGGenerator, PWGInference  # no
 from .speedyspeech import SpeedySpeech, SpeedySpeechInference  # noqa: F401
 from .waveflow import ConditionalWaveFlow, WaveFlowLoss  # noqa: F401
 from .lstm_speaker_encoder import LSTMSpeakerEncoder  # noqa: F401
+from .tacotron2 import Tacotron2, Tacotron2Loss  # noqa: F401

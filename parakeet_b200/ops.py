@@ -635,3 +635,85 @@ def segment_mean_normalize(x, offsets, eps=1e-12):
     _lib.check(_lib.lib().pk_segment_mean_normalize(_ptr(x), _ptr(offsets), s, x.shape[1], float(eps), _ptr(y), _stream()),
                "pk_segment_mean_normalize")
     return y
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# Tacotron2 (csrc/tacotron2.cu)
+# ----------------------------------------------------------------------------------------------------------------
+TACO2_PRENET_SITES = (0, 1)          # Philox sites of the two prenet dropouts (pk_taco2_decode)
+
+
+def taco2_embed(ids, table, tones=None, tone_table=None):
+    """ids int64 (B, T) -> (B, T, C) = table[ids] (+ tone_table[tones], zero for tone 0)."""
+    _require_cuda(ids, table, tones, tone_table)
+    ids = ids.contiguous()
+    tones = tones.contiguous() if tones is not None else None
+    B, T = ids.shape
+    y = torch.empty(B, T, table.shape[1], dtype=torch.float32, device=ids.device)
+    _lib.check(_lib.lib().pk_taco2_embed(_ptr(ids), _ptr(table), _ptr(tones), _ptr(tone_table), B, T, table.shape[1], _ptr(y), _stream()),
+               "pk_taco2_embed")
+    return y
+
+
+def taco2_time_major(x, lens=None, reverse=False):
+    """x (B, T, C) -> (T, B, C); with reverse each sequence is reversed within its length (lens int32 or None = T)."""
+    x = x.contiguous()
+    B, T, Cc = x.shape
+    y = torch.empty(T, B, Cc, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().pk_taco2_time_major(_ptr(x), _ptr(lens), 1 if reverse else 0, B, T, Cc, _ptr(y), _stream()), "pk_taco2_time_major")
+    return y
+
+
+def taco2_bilstm_merge(h_fwd, h_bwd, lens=None, gc=None):
+    """h_fwd / h_bwd (T, B, H) -> (B, T, 2H + G): [forward | backward at its own position | gc], rows past lens zero."""
+    T, B, H = h_fwd.shape
+    G = 0 if gc is None else gc.shape[1]
+    gc = gc.contiguous().float() if gc is not None else None
+    out = torch.empty(B, T, 2 * H + G, dtype=torch.float32, device=h_fwd.device)
+    _lib.check(_lib.lib().pk_taco2_bilstm_merge(_ptr(h_fwd), _ptr(h_bwd), _ptr(lens), _ptr(gc), B, T, H, G, _ptr(out), _stream()),
+               "pk_taco2_bilstm_merge")
+    return out
+
+
+def taco2_decode(w, keys, pkeys, steps, *, teacher, mels=None, text_lens=None, p_prenet=0.5, seed=0, prof=None):
+    """pk_taco2_decode -> (mel_out (B, steps, dmr), align (B, steps, T_enc), stop (B, steps) or None, frames int32 (B,)); w is the
+    dict of packed decoder weights (models/tacotron2.py).  prof: optional int64 tensor of pk_taco2_prof_len() per-CTA phase
+    timers (scripts/time_tacotron2.py)."""
+    _require_cuda(keys, pkeys, mels, text_lens)
+    B, T_enc, d_enc = keys.shape
+    dmr = w["proj_w"].shape[0]
+    dev = keys.device
+    L = _lib.lib()
+    ws = torch.empty(int(L.pk_taco2_workspace(B, T_enc, d_enc)), dtype=torch.float32, device=dev)
+    mel = torch.empty(B, steps, dmr, dtype=torch.float32, device=dev)
+    align = torch.empty(B, steps, T_enc, dtype=torch.float32, device=dev)
+    stop = torch.empty(B, steps, dtype=torch.float32, device=dev) if w.get("stop_w") is not None else None
+    frames = torch.empty(B, dtype=torch.int32, device=dev)
+    a = _lib.Taco2DecodeArgs()
+    a.batch, a.t_enc, a.d_enc, a.dmr, a.steps, a.teacher, a.loc_k = B, T_enc, d_enc, dmr, steps, 1 if teacher else 0, w["loc_w"].shape[2]
+    a.p_prenet, a.seed = float(p_prenet), int(seed) & 0xFFFFFFFFFFFFFFFF
+    a.keys, a.pkeys, a.text_lens, a.mels = keys.data_ptr(), pkeys.data_ptr(), _ptr(text_lens).value, _ptr(mels).value
+    for n in ("pre_w1", "pre_w2", "att_w", "att_b_ih", "att_b_hh", "q_w", "loc_w", "v_w", "dec_w", "dec_b_ih", "dec_b_hh", "proj_w", "proj_b",
+              "stop_w", "stop_b"):
+        setattr(a, n, _ptr(w.get(n)).value)
+    a.workspace, a.workspace_len = ws.data_ptr(), ws.numel()
+    a.mel_out, a.align_out, a.stop_out, a.frames = mel.data_ptr(), align.data_ptr(), _ptr(stop).value, frames.data_ptr()
+    if prof is not None:
+        a.prof, a.prof_len = prof.data_ptr(), prof.numel()
+    _lib.check(L.pk_taco2_decode(C.byref(a), _stream()), "pk_taco2_decode")
+    return mel, align, stop, frames
+
+
+def taco2_loss(mel, post, target, align=None, slens=None, plens=None, sigma=0.2, stop_logits=None):
+    """Tacotron2Loss (pk_taco2_loss) -> fp32 (5,) = loss, mel_loss, post_mel_loss, guided_attn_loss, stop_loss."""
+    _require_cuda(mel, post, target, align, slens, plens, stop_logits)
+    mel, post, target = mel.contiguous().float(), post.contiguous().float(), target.contiguous().float()
+    align = align.contiguous().float() if align is not None else None
+    stop_logits = stop_logits.contiguous().float() if stop_logits is not None else None
+    slens = slens.to(torch.int32).contiguous() if slens is not None else None
+    plens = plens.to(torch.int32).contiguous() if plens is not None else None
+    B, T, Cc = mel.shape
+    out = torch.empty(5, dtype=torch.float32, device=mel.device)
+    _lib.check(_lib.lib().pk_taco2_loss(_ptr(mel), _ptr(post), _ptr(target), B, T, Cc, _ptr(align), align.shape[2] if align is not None else 0,
+                                        _ptr(slens), _ptr(plens), float(sigma), _ptr(stop_logits), _ptr(out), _stream()), "pk_taco2_loss")
+    return out

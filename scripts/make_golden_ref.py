@@ -15,6 +15,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py fs2ms_train        # only tests/golden/ref_executed_fs2ms_train.npz
     python scripts/make_golden_ref.py speedyspeech_train # only tests/golden/ref_executed_speedyspeech_train.npz
     python scripts/make_golden_ref.py ge2e               # only tests/golden/ref_executed_ge2e.npz
+    python scripts/make_golden_ref.py tacotron2          # only tests/golden/ref_executed_tacotron2.npz
 """
 import importlib.util
 import os
@@ -494,6 +495,55 @@ def ge2e(out):
             out[f"{tag}/gradnorm/{k}"] = np.asarray(float(gk.double().norm()))
 
 
+def tacotron2(out):
+    """The reference's own Tacotron2 (its BiRNN encoder LSTM on the stand-in, Paddle 2.1 keys) with p_prenet_dropout = 0 at the
+    configs of oracle.tacotron2.GOLDEN_CONFIGS: the teacher-forced forward with and without output_lens, Tacotron2Loss with the
+    guided attention term (and the stop term where the model has a stop token), and infer under both stop rules: the alignment
+    rule (no stop token; T_enc = 1 gives 22 frames, and a 7-token text), the stop token with its bias at +1e4 (fires at the
+    first frame).  Weights are regenerated from their seeds (oracle.tacotron2.synth_params), inputs are stored."""
+    from oracle import tacotron2 as ot
+    from parakeet.models.tacotron2 import Tacotron2, Tacotron2Loss
+    for tag, (cfg, seed) in ot.GOLDEN_CONFIGS.items():
+        kw = {k: v for k, v in cfg.items() if k != "vocab_size"}
+        ref = Tacotron2(cfg["vocab_size"], **kw)
+        params = ot.synth_params(seed, cfg)
+        out[f"{tag}/keys"] = np.asarray(check_keys(ref, params, f"Tacotron2({tag})"))
+        ref.set_state_dict(params)
+        ref.eval()
+        x = ot.golden_inputs(cfg, seed + 100)
+        for k, v in x.items():
+            if v is not None:
+                out[f"{tag}/in/{k}"] = v.numpy()
+        opt = lambda v: None if v is None else T(v)
+        with torch.no_grad():
+            for suffix, olens in (("", None), ("_olens", x["output_lens"])):
+                o = ref(T(x["text"]), T(x["text_lens"]), T(x["mels"]), opt(olens), opt(x["tones"]), opt(x["gc"]))
+                for k, v in o.items():
+                    out[f"{tag}/fwd{suffix}/{k}"] = v.numpy()
+            stop = cfg["use_stop_token"]
+            crit = Tacotron2Loss(use_stop_token_loss=stop, use_guided_attention_loss=True, sigma=0.2)
+            losses = crit(o["mel_output"], o["mel_outputs_postnet"], T(x["mels"]), o["alignments"], T(x["output_lens"]),
+                          T(x["text_lens"]), o.get("stop_logits"))
+            for k, v in losses.items():
+                out[f"{tag}/loss/{k}"] = np.asarray(float(v))
+            if stop:
+                p2 = dict(params)
+                p2["decoder.stop_layer.bias"] = torch.full((1,), 1e4)
+                ref.set_state_dict(p2)
+                o = ref.infer(T(x["text"][:1, :5]), max_decoder_steps=30, tones=opt(None if x["tones"] is None else x["tones"][:1, :5]),
+                              global_condition=opt(None if x["gc"] is None else x["gc"][:1]))
+                for k, v in o.items():
+                    out[f"{tag}/infer_stop/{k}"] = v.numpy()
+                ref.set_state_dict(params)
+            else:
+                for name, n in (("infer_t1", 1), ("infer", 7)):
+                    o = ref.infer(T(x["text"][:1, :n]), max_decoder_steps=60 if n == 1 else 30,
+                                  tones=opt(None if x["tones"] is None else x["tones"][:1, :n]),
+                                  global_condition=opt(None if x["gc"] is None else x["gc"][:1]))
+                    for k, v in o.items():
+                        out[f"{tag}/{name}/{k}"] = v.numpy()
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -565,7 +615,8 @@ def sampled(models):
 
 def main():
     single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
-              "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e}
+              "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e,
+              "tacotron2": tacotron2}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

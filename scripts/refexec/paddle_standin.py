@@ -181,7 +181,10 @@ def build():
     P.no_grad = torch.no_grad
     P.chunk = lambda x, chunks, axis=0: [T(t) for t in torch.chunk(x, chunks, dim=axis)]
     P.split = lambda x, n, axis=0: [T(t) for t in (torch.chunk(x, n, dim=axis) if isinstance(n, int) else torch.split(x, list(n), dim=axis))]
-    P.unsqueeze = lambda x, axis: T(torch.unsqueeze(x, axis))
+    P.unsqueeze = lambda x, axis: T(x).unsqueeze(axis)                           # an int or a list of axes
+    P.argmax = lambda x, axis=None: T(torch.argmax(x) if axis is None else torch.argmax(x, dim=axis))   # first index on ties
+    P.exp = lambda x: T(torch.exp(x))
+    P.tanh = lambda x: T(torch.tanh(x))
     P.squeeze = lambda x, axis=None: T(torch.squeeze(x) if axis is None else torch.squeeze(x, axis))
     P.shape = lambda x: list(x.shape)
     P.divide = lambda a, b: T(a / b)
@@ -479,6 +482,38 @@ def build():
             self.bias_ih = torch.nn.Parameter(torch.zeros(4 * hidden_size))
             self.bias_hh = torch.nn.Parameter(torch.zeros(4 * hidden_size))
 
+        def forward(self, inputs, states=None):
+            """paddle.nn.LSTMCell: -> (h, (h, c)); states default to zeros."""
+            if states is None:
+                z = torch.zeros(inputs.shape[0], self.weight_hh.shape[1], dtype=inputs.dtype)
+                states = (z, z)
+            h, c = torch._VF.lstm_cell(inputs, tuple(states), self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh)
+            return T(h), (T(h), T(c))
+
+    class BiRNN(Layer):
+        """paddle.nn.BiRNN (2.1): keys `cell_fw.*`, `cell_bw.*`."""
+        def __init__(self, cell_fw, cell_bw):
+            super().__init__()
+            self.cell_fw, self.cell_bw = cell_fw, cell_bw
+
+    def _run(cell, x, lens, reverse):
+        """Paddle 2.1's dynamic-graph RNN loop (rnn.py `_rnn_dynamic_graph`): the reverse direction runs over the whole padded
+        sequence flipped in time; with sequence_length, a step past a sequence's length keeps the previous state (the mask), and
+        every step's output is kept as computed."""
+        B, L = x.shape[0], x.shape[1]
+        H = cell.weight_hh.shape[1]
+        h = c = torch.zeros(B, H, dtype=x.dtype)
+        order = range(L - 1, -1, -1) if reverse else range(L)
+        outs = [None] * L
+        for t in order:
+            hn, cn = torch._VF.lstm_cell(x[:, t], (h, c), cell.weight_ih, cell.weight_hh, cell.bias_ih, cell.bias_hh)
+            outs[t] = hn
+            if lens is not None:
+                m = (t < lens).to(x.dtype).unsqueeze(-1)
+                hn, cn = m * hn + (1 - m) * h, m * cn + (1 - m) * c
+            h, c = hn, cn
+        return torch.stack(outs, 1), h, c
+
     class RNN(Layer):
         def __init__(self, cell):
             super().__init__()
@@ -490,12 +525,25 @@ def build():
         both biases added)."""
         def __init__(self, input_size, hidden_size, num_layers=1, direction="forward", time_major=False, dropout=0.0):
             super().__init__()
-            assert direction == "forward" and not time_major and dropout == 0.0
+            assert direction in ("forward", "bidirectional", "bidirect") and not time_major and dropout == 0.0
+            self.bidirectional = direction != "forward"
             for l in range(num_layers):
-                self.add_module(str(l), RNN(LSTMCell(input_size if l == 0 else hidden_size, hidden_size)))
+                if self.bidirectional:
+                    assert num_layers == 1
+                    self.add_module(str(l), BiRNN(LSTMCell(input_size, hidden_size), LSTMCell(input_size, hidden_size)))
+                else:
+                    self.add_module(str(l), RNN(LSTMCell(input_size if l == 0 else hidden_size, hidden_size)))
             self.num_layers, self.hidden_size = num_layers, hidden_size
 
-        def forward(self, inputs, initial_states=None):
+        def forward(self, inputs, initial_states=None, sequence_length=None):
+            if self.bidirectional:
+                assert initial_states is None
+                birnn = getattr(self, "0")
+                lens = None if sequence_length is None else torch.as_tensor(sequence_length).reshape(-1, 1).to(torch.int64).reshape(-1)
+                of, hf, cf = _run(birnn.cell_fw, inputs, lens, False)
+                ob, hb, cb = _run(birnn.cell_bw, inputs, lens, True)
+                return T(torch.cat([of, ob], -1)), (T(torch.stack([hf, hb])), T(torch.stack([cf, cb])))
+            assert sequence_length is None
             B = inputs.shape[0]
             x, hs, cs = inputs, [], []
             for l, rnn in enumerate(self.children()):
@@ -520,6 +568,8 @@ def build():
     nn.CrossEntropyLoss = cross_entropy_loss
     nn.MSELoss = lambda reduction="mean": (lambda a, b: T(TF.mse_loss(a, b, reduction=reduction)))
     nn.L1Loss = lambda reduction="mean": (lambda a, b: T(TF.l1_loss(a, b, reduction=reduction)))
+    nn.BCEWithLogitsLoss = lambda weight=None, reduction="mean", pos_weight=None: \
+        (lambda a, b: T(TF.binary_cross_entropy_with_logits(a, b.to(a.dtype), reduction=reduction)))
 
     init = types.ModuleType("paddle.nn.initializer")
     for name in ("XavierUniform", "XavierNormal", "KaimingUniform", "KaimingNormal", "Uniform", "Normal"):
@@ -541,6 +591,7 @@ def build():
     F.mse_loss = lambda a, b, reduction="mean": T(TF.mse_loss(a, b, reduction=reduction))
     F.leaky_relu = lambda x, negative_slope=0.01: T(TF.leaky_relu(x, negative_slope))
     F.sigmoid = lambda x: T(torch.sigmoid(x))
+    F.one_hot = lambda x, num_classes: T(TF.one_hot(torch.as_tensor(x).to(torch.int64), num_classes).to(torch.float32))
     F.tanh = lambda x: T(torch.tanh(x))
     F.conv1d = lambda x, w, bias=None, stride=1, padding=0, dilation=1, groups=1: T(TF.conv1d(x, w, bias, stride, padding, dilation, groups))
     def conv2d(x, w, bias=None, stride=1, padding=0, dilation=1, groups=1, data_format="NCHW"):

@@ -192,28 +192,27 @@ __global__ void __launch_bounds__(256) sum_slices_kernel(const float* __restrict
   }
 }
 
-// per-column sum and sum of squares (BatchNorm batch statistics): sums[c] += sum x, sums[C + c] += sum x^2
-__global__ void __launch_bounds__(256) col_stats_kernel(const float* __restrict__ x, long long rows, int c, float* __restrict__ sums) {
-  __shared__ float p1[4][64], p2[4][64];
+// BatchNorm batch statistics, second pass: sums[C + c] += sum (x - mean)^2 with mean = sums[c] / rows from the first pass (colsum_kernel).
+// Two passes rather than E[x^2] - mean^2: for a column whose mean is large against its spread (30 + N(0, 1)) the single-pass
+// difference cancels in fp32 and loses three decimal digits of the variance.
+__global__ void __launch_bounds__(256) col_centered_sq_kernel(const float* __restrict__ x, long long rows, int c, float* __restrict__ sums) {
+  __shared__ float p2[4][64];
   const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
   const int col = blockIdx.y * 64 + tx;
-  float s = 0.f, q = 0.f;
-  if (col < c)
+  float q = 0.f;
+  if (col < c) {
+    const float m = sums[col] / rows;
     for (long long r = blockIdx.x * 64LL + ty; r < rows && r < (blockIdx.x + 1) * 64LL; r += 4) {
-      const float v = x[r * c + col];
-      s += v;
-      q += v * v;
+      const float d = x[r * c + col] - m;
+      q = fmaf(d, d, q);
     }
-  p1[ty][tx] = s;
+  }
   p2[ty][tx] = q;
   __syncthreads();
-  if (ty == 0 && col < c) {
-    atomicAdd(sums + col, p1[0][tx] + p1[1][tx] + p1[2][tx] + p1[3][tx]);
-    atomicAdd(sums + c + col, p2[0][tx] + p2[1][tx] + p2[2][tx] + p2[3][tx]);
-  }
+  if (ty == 0 && col < c) atomicAdd(sums + c + col, p2[0][tx] + p2[1][tx] + p2[2][tx] + p2[3][tx]);
 }
 
-// BatchNorm1D training forward (given column sums): y = act(gamma * (x - mean) * rstd + beta); running stats updated by
+// BatchNorm1D training forward (given sum x and sum (x - mean)^2 per column): y = act(gamma * (x - mean) * rstd + beta); running stats updated by
 // thread block 0 (paddle momentum 0.9: running = 0.9 * running + 0.1 * batch, biased variance).  act: 0 none, 2 tanh.
 __global__ void bn_train_fwd_kernel(const float* __restrict__ x, const float* __restrict__ sums, const float* __restrict__ gamma,
                                     const float* __restrict__ beta, float eps, int act, long long rows, int c, float momentum,
@@ -225,7 +224,7 @@ __global__ void bn_train_fwd_kernel(const float* __restrict__ x, const float* __
   if (blockIdx.x == 0) {
     for (int col = threadIdx.x; col < c; col += blockDim.x) {
       const float mean = sums[col] / rows;
-      const float var = fmaxf(sums[c + col] / rows - mean * mean, 0.f);
+      const float var = sums[c + col] / rows;
       save_mean[col] = mean;
       save_rstd[col] = rsqrtf(var + eps);
       if (run_mean) {
@@ -237,7 +236,7 @@ __global__ void bn_train_fwd_kernel(const float* __restrict__ x, const float* __
   if (i >= n) return;
   const int col = i % c;
   const float mean = sums[col] / rows;
-  const float var = fmaxf(sums[c + col] / rows - mean * mean, 0.f);
+  const float var = sums[c + col] / rows;
   float v = (x[i] - mean) * rsqrtf(var + eps) * __ldg(gamma + col) + __ldg(beta + col);
   if (act == PK_ACT_TANH) v = tanhf(v);
   if (y) y[i] = v;
@@ -507,12 +506,13 @@ extern "C" int pk_batch_norm_train(const float* x, int64_t rows, int32_t c, cons
   PK_CHECK_ARG(y || y_hi, "no output requested");
   PK_CHECK_CUDA(cudaMemsetAsync(sums2c, 0, 2 * c * sizeof(float), PK_STREAM));
   dim3 grid(static_cast<unsigned>((rows + 63) / 64), (c + 63) / 64);
-  col_stats_kernel<<<grid, 256, 0, PK_STREAM>>>(x, rows, c, sums2c);
+  colsum_kernel<<<grid, 256, 0, PK_STREAM>>>(x, rows, c, sums2c);
+  col_centered_sq_kernel<<<grid, 256, 0, PK_STREAM>>>(x, rows, c, sums2c);
   bn_train_fwd_kernel<<<nblk(rows * c, 256), 256, 0, PK_STREAM>>>(x, sums2c, gamma, beta, eps, act, rows, c, momentum, run_mean, run_var, y,
                                                                   static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo),
                                                                   save_mean, save_rstd);
   PK_CHECK_CUDA(cudaGetLastError());
-  count_launch(2);
+  count_launch(3);
   return PK_OK;
 }
 

@@ -123,6 +123,10 @@ class FastSpeech2(Layer):
             unsupported.append("postnet without batch norm")
         if adim % 64 != 0 or adim % aheads != 0:
             unsupported.append("adim must be a multiple of 64 and of aheads")
+        elif (adim // aheads) % 64 != 0:
+            # the non-fused attention and the training step slice Q / K / V per head out of one (B, T, 3 adim) buffer, and the
+            # GEMM reads K in 64-column chunks: a head width that is not a multiple of 64 would read the next head's columns
+            unsupported.append(f"attention head width adim / aheads = {adim // aheads} (must be a multiple of 64)")
         if unsupported:
             raise NotImplementedError("not in this round's hot-path scope: " + ", ".join(unsupported))
         self.idim, self.odim, self.adim, self.aheads = idim, odim, adim, aheads

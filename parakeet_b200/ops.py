@@ -141,7 +141,9 @@ def conv_gemm(a, w, *, n, k, taps=1, dil=1, pad=None, bias=None, act=None, resid
     if out_split and y_split is None:
         y_split = Split.empty((B, T, n), dev)
     args = ConvGemmArgs()
-    args.a = _operand(a, rows=T, cols=Ctot, ld=a.hi.stride(1), batch_stride=a.hi.stride(0), batches=B)
+    # A's extent ends at k: the last 64-column K chunk is zero-filled past it instead of reading columns the weight has no
+    # taps for (a zero weight times a NaN or Inf there would still poison the output)
+    args.a = _operand(a, rows=T, cols=min(Ctot, k), ld=a.hi.stride(1), batch_stride=a.hi.stride(0), batches=B)
     args.b = _operand(w, rows=w.hi.shape[0], cols=w.hi.shape[1], ld=w.hi.stride(0), batch_stride=0, batches=1, bmul=0)
     args.batch, args.heads, args.m, args.n, args.k = B, 1, T, n, k
     args.taps, args.dil, args.pad = taps, dil, pad
@@ -182,10 +184,29 @@ def conv_gemm(a, w, *, n, k, taps=1, dil=1, pad=None, bias=None, act=None, resid
     return y_f32, y_split
 
 
+def k_tail_overlap(spec, heads, k):
+    """First head whose K slice [col0 + h * colh, + k) is followed, up to the next multiple of 64 columns, by columns inside
+    the operand's `cols`, or None.  pk_conv_gemm loads K in 64-column chunks bounded only by `cols`, so such columns would
+    enter the product (the SIMT path stops at k: the two paths would disagree)."""
+    if k % 64 == 0:
+        return None
+    for h in range(heads):
+        end = spec.get("col0", 0) + h * spec.get("colh", 0) + k
+        if end < spec["cols"]:
+            return h
+    return None
+
+
 def batched_matmul_nt(a, b, *, batch, heads, m, n, k, a_spec, b_spec, scale=1.0, y_f32=None, y_split=None,
                       y_batch_stride=None, y_head_stride=None, y_ld=None, lens=None, passes=3, simt=False):
     """y[b,h] = scale * A[b,h] (m x k) . B[b,h]^T (n x k); operand addressing given by a_spec / b_spec dicts
-    (rows, cols, ld, batch_stride, batches, bmul, hmul, col0, colh)."""
+    (rows, cols, ld, batch_stride, batches, bmul, hmul, col0, colh).  With k % 64 != 0 each operand's K slice must end at
+    its `cols` (k_tail_overlap): a head slice followed by live columns is refused."""
+    for name, spec in (("A", a_spec), ("B", b_spec)):
+        h = k_tail_overlap(spec, heads, k)
+        if h is not None:
+            raise _lib.PkError(f"batched_matmul_nt: k={k} is not a multiple of 64 and operand {name}'s K slice of head {h} is followed "
+                               f"by live columns (col0={spec.get('col0', 0)}, colh={spec.get('colh', 0)}, cols={spec['cols']})")
     args = ConvGemmArgs()
     args.a = _operand(a, **a_spec)
     args.b = _operand(b, **b_spec)

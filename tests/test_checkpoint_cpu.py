@@ -10,7 +10,7 @@ from parakeet_b200 import checkpoint
 
 def _fs2(device="cpu"):
     from parakeet_b200.models import FastSpeech2
-    return FastSpeech2(40, 80, adim=64, aheads=2, elayers=1, eunits=96, dlayers=1, dunits=96, positionwise_layer_type="conv1d",
+    return FastSpeech2(40, 80, adim=64, aheads=1, elayers=1, eunits=96, dlayers=1, dunits=96, positionwise_layer_type="conv1d",
                        positionwise_conv_kernel_size=3, duration_predictor_layers=1, duration_predictor_chans=32,
                        duration_predictor_kernel_size=3, postnet_layers=2, postnet_filts=5, postnet_chans=32,
                        pitch_predictor_layers=1, pitch_predictor_chans=32, pitch_predictor_kernel_size=3,

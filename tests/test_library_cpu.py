@@ -32,7 +32,7 @@ def test_no_cpu_fallback():
     with pytest.raises(_lib.PkError):
         ops.Split.from_f32(torch.zeros(4, 4))
     from parakeet_b200.models import FastSpeech2, PWGGenerator
-    m = FastSpeech2(20, 80, adim=64, aheads=2, elayers=1, dlayers=1, eunits=64, dunits=64, postnet_chans=64, device="cpu")
+    m = FastSpeech2(20, 80, adim=64, aheads=1, elayers=1, dlayers=1, eunits=64, dunits=64, postnet_chans=64, device="cpu")
     with pytest.raises(_lib.PkError):
         m.inference(torch.tensor([1, 2, 3]))
     g = PWGGenerator(layers=3, stacks=1, device="cpu")

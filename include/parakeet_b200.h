@@ -265,6 +265,19 @@ int pk_l2_normalize(const float* x, int32_t outer, int32_t n, int32_t inner, flo
 int pk_fused_attention(const void* qkv_hi, const void* qkv_lo, const void* vt_hi, const void* vt_lo, int32_t batch, int32_t t,
                        int32_t heads, int32_t dk, int32_t tp, const int32_t* key_lens, const int32_t* row_lens, float scale,
                        void* ctx_hi, void* ctx_lo, pk_stream_t stream);
+/* pk_fused_attention_ex: the generalised fused attention.  Q of head h = columns q_col0 + h dk of the split buffer q (batch, t_q,
+ * q_ld); K = columns k_col0 + h dk of k (batch, t_k, k_ld); V^T (batch * heads, dk, tp) from pk_transpose_heads, tp >= t_k.
+ * ctx (batch, t_q, heads dk) = softmax(scale q k^T, keys >= key_lens[b] masked, with `causal` also keys j > i) v.  Query rows
+ * >= row_lens[b] are written as zero (NULL: every row is computed, padded rows included).  causal needs t_q == t_k.  d_k 64 / 128 /
+ * 192; q_ld, k_ld multiples of 8. */
+typedef struct {
+  const void* q_hi; const void* q_lo; const void* k_hi; const void* k_lo; const void* vt_hi; const void* vt_lo;
+  int32_t batch, t_q, t_k, heads, dk, tp, q_ld, k_ld, q_col0, k_col0, causal;
+  const int32_t* key_lens; const int32_t* row_lens;
+  float scale;
+  void* ctx_hi; void* ctx_lo;
+} PkAttentionArgs;
+int pk_fused_attention_ex(const PkAttentionArgs* args, pk_stream_t stream);
 /* (batch, t, ld_src)[.., col0 + h*dk + d] -> (batch*heads, dk, ld_dst)[.., d, t] (zero-filled for t in [t, ld_dst)):
  * the value matrix in K-major form for the P.V product (attention.py:126). */
 int pk_transpose_heads(const void* src_hi, const void* src_lo, int32_t batch, int32_t t, int32_t ld_src, int32_t col0,
@@ -854,6 +867,45 @@ int pk_taco2_bilstm_merge(const float* h_fwd, const float* h_bwd, const int32_t*
 int pk_taco2_loss(const float* mel, const float* post, const float* target, int32_t batch, int32_t t, int32_t channels, const float* align,
                   int32_t t_enc, const int32_t* slens, const int32_t* plens, float sigma, const float* stop_logits, float* out,
                   pk_stream_t stream);
+
+/* ---- TransformerTTS (csrc/transformer_tts.cu) ---------------------------------------------------------------------------------
+ * pk_tts_decode: every step of TransformerTTS.inference's decoder loop (B = 1) in one persistent launch of a co-resident grid.
+ * Step t feeds the last of the r frames of step t - 1 (zeros at t = 0) through the prenet (Linear -> ReLU -> dropout p_prenet,
+ * Philox site = prenet layer, step = t, element j: pk_dropout's convention), the input Linear and + alpha pe[t], then `layers`
+ * pre-LN decoder layers on the new row (self-attention over the cached K / V of rows 0..t, source attention over mem_kv, the
+ * position-wise Linear feed-forward), after_norm, prob_out and feat_out.  It stops after step idx = t + 1 once
+ * (any sigmoid(prob) >= threshold or idx >= maxlen) and idx >= minlen.  fp32 FFMA, fixed summation order, no atomics.
+ *   mem_kv   (t_enc, layers * 2 adim) fp32: [K_0 | V_0 | K_1 | ...] of the source attentions over the encoder output
+ *   pre_w    prenet weights [out][in] row-major, layer 0 (prenet_units x odim) then the others; pre_b (prenet_layers, prenet_units)
+ *   in_w     (adim, prenet_units), in_b (adim); pe (steps, adim): alpha pe rows of the decoder's ScaledPositionalEncoding
+ *   layer_w  layers x pk_tts_layer_floats(adim, units) floats, each: wqkv (3 adim, adim), bqkv, wo_self (adim, adim), bo_self,
+ *            wq_src, bq_src, wo_src, bo_src, w1 (units, adim), b1, w2 (adim, units), b2, then gamma / beta of norm1, norm2, norm3
+ *   norm     after_norm gamma | beta; out_w (r + r odim, adim) = [prob_out rows | feat_out rows], out_b (r + r odim)
+ *   outs     (steps, r odim), probs (steps, r) sigmoid, att_ws (layers, heads, steps, t_enc): zeroed by the call, rows past the
+ *            stop stay zero; frames[0] = decoder steps run.  steps >= max(minlen, maxlen) sizes the caches and outputs.
+ * Refused with PK_ERR_UNSUPPORTED: head widths not a multiple of 32, adim / units / prenet_units / odim not multiples of 4,
+ * r > 16, max(steps, t_enc) past the shared-memory score buffer, fewer co-resident CTAs than heads. */
+typedef struct {
+  int32_t t_enc, adim, heads, units, odim, r, prenet_layers, prenet_units, layers, steps, minlen, maxlen;
+  float threshold, p_prenet;
+  uint64_t seed;
+  const float* mem_kv; const float* pre_w; const float* pre_b; const float* in_w; const float* in_b; const float* pe;
+  const float* layer_w; const float* norm; const float* out_w; const float* out_b;
+  float* workspace; int64_t workspace_len;   /* pk_tts_workspace() floats, 16-byte aligned */
+  float* outs; float* probs; float* att_ws; int32_t* frames;
+} PkTtsDecodeArgs;
+int64_t pk_tts_layer_floats(int32_t adim, int32_t units);
+int64_t pk_tts_workspace(int32_t adim, int32_t units, int32_t prenet_units, int32_t layers, int32_t steps);
+int pk_tts_decode(const PkTtsDecodeArgs* args, pk_stream_t stream);
+/* Glue of the teacher-forced forward.  pk_tts_text_eos: xs (batch, t + 1) = text with eos at column lens[b] and zeros after,
+ * ilens = lens + 1.  pk_tts_shift_frames: out (batch, l / r, odim)[b, 0] = 0, [b, i] = ys[b, i r - 1].  pk_tts_prenet_dropout: in
+ * place on (batch, l, units), element (b, i, j) kept with Philox site, step i, element b units + j (pk_tts_decode's masks), scaled
+ * 1 / (1 - p).  pk_tts_stop_labels: out (batch, width) = 1 where column >= olens[b] - 1 or column == width - 1, else 0. */
+int pk_tts_text_eos(const int64_t* text, const int32_t* lens, int32_t batch, int32_t t, int64_t eos, int64_t* xs, int32_t* ilens,
+                    pk_stream_t stream);
+int pk_tts_shift_frames(const float* ys, int32_t batch, int32_t l, int32_t odim, int32_t r, float* out, pk_stream_t stream);
+int pk_tts_prenet_dropout(float* x, int32_t batch, int32_t l, int32_t units, float p, uint64_t seed, int32_t site, pk_stream_t stream);
+int pk_tts_stop_labels(const int32_t* olens, int32_t batch, int32_t width, float* out, pk_stream_t stream);
 
 #ifdef __cplusplus
 }

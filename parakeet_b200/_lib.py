@@ -138,6 +138,20 @@ class Taco2DecodeArgs(C.Structure):
         [("prof", C.c_void_p), ("prof_len", C.c_int64)]
 
 
+class AttentionArgs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("q_hi", "q_lo", "k_hi", "k_lo", "vt_hi", "vt_lo")] + \
+        [(n, C.c_int32) for n in ("batch", "t_q", "t_k", "heads", "dk", "tp", "q_ld", "k_ld", "q_col0", "k_col0", "causal")] + \
+        [("key_lens", C.c_void_p), ("row_lens", C.c_void_p), ("scale", C.c_float), ("ctx_hi", C.c_void_p), ("ctx_lo", C.c_void_p)]
+
+
+class TtsDecodeArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("t_enc", "adim", "heads", "units", "odim", "r", "prenet_layers", "prenet_units", "layers", "steps",
+                                         "minlen", "maxlen")] + \
+        [("threshold", C.c_float), ("p_prenet", C.c_float), ("seed", C.c_uint64)] + \
+        [(n, C.c_void_p) for n in ("mem_kv", "pre_w", "pre_b", "in_w", "in_b", "pe", "layer_w", "norm", "out_w", "out_b", "workspace")] + \
+        [("workspace_len", C.c_int64)] + [(n, C.c_void_p) for n in ("outs", "probs", "att_ws", "frames")]
+
+
 def _declare(L):
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     sigs = {
@@ -237,6 +251,12 @@ def _declare(L):
         "pk_taco2_time_major": [vp, vp, i32, i32, i32, i32, vp, vp],
         "pk_taco2_bilstm_merge": [vp, vp, vp, vp, i32, i32, i32, i32, vp, vp],
         "pk_taco2_loss": [vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, f32, vp, vp, vp],
+        "pk_tts_decode": [C.POINTER(TtsDecodeArgs), vp],
+        "pk_fused_attention_ex": [C.POINTER(AttentionArgs), vp],
+        "pk_tts_text_eos": [vp, vp, i32, i32, i64, vp, vp],
+        "pk_tts_shift_frames": [vp, i32, i32, i32, i32, vp, vp],
+        "pk_tts_prenet_dropout": [vp, i32, i32, i32, f32, C.c_uint64, i32, vp],
+        "pk_tts_stop_labels": [vp, i32, i32, vp, vp],
     }
     for name, argtypes in sigs.items():
         fn = getattr(L, name)
@@ -248,6 +268,10 @@ def _declare(L):
     L.pk_taco2_workspace.restype = i64
     L.pk_taco2_prof_len.argtypes = []
     L.pk_taco2_prof_len.restype = i64
+    L.pk_tts_layer_floats.argtypes = [i32, i32]
+    L.pk_tts_layer_floats.restype = i64
+    L.pk_tts_workspace.argtypes = [i32, i32, i32, i32, i32]
+    L.pk_tts_workspace.restype = i64
 
 
 def check(rc, what=""):

@@ -22,13 +22,15 @@
 #include <mutex>
 
 #include "pk_host.h"
+#include "pk_decode.cuh"
 #include "pk_sm90.cuh"
 
 namespace pk {
 namespace taco2 {
 
-constexpr int kThreads = 512;
-constexpr int kWarps = kThreads / 32;
+using pdec::kThreads;
+using pdec::kWarps;
+using namespace pdec;
 constexpr int kH = 1024;          // d_attention_rnn = d_decoder_rnn
 constexpr int kPre = 256;         // d_prenet
 constexpr int kAtt = 128;         // d_attention
@@ -73,111 +75,7 @@ struct Params {
   unsigned long long* prof;
 };
 
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_inc(unsigned* p) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
-
-__device__ __forceinline__ unsigned long long globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
-// every CTA of the (co-resident) grid arrives; `target` advances by the grid size per hand-off (thread 0 keeps it).  With prof
-// (kPhases x 2 ns counters of this CTA), hand-off `phase` adds this CTA's time since the previous release (`last`) and its wait
-// from arrival to release: the smallest wait over the CTAs is the hand-off's own latency (the last CTA to arrive waits only for it).
 constexpr int kPhases = 6;
-__device__ __forceinline__ void grid_sync(unsigned* ctr, unsigned& target, int grid, unsigned long long* prof_all, int phase,
-                                          unsigned long long* last) {
-  unsigned long long* prof = prof_all ? prof_all + static_cast<long long>(blockIdx.x) * 2 * kPhases : nullptr;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned long long t_arrive = prof ? globaltimer() : 0ull;
-    target += grid;
-    __threadfence();
-    red_release_gpu_inc(ctr);
-    const long long t0 = clock64();
-    while (ld_acquire_gpu(ctr) < target) {
-      __nanosleep(20);
-      if (clock64() - t0 > (1ll << 33)) __trap();   // ~4 s: a CTA that never arrives is a scheduling bug - fail, do not hang
-    }
-    if (prof) {
-      const unsigned long long t_release = globaltimer();
-      prof[phase] += t_release - *last;
-      prof[kPhases + phase] += t_release - t_arrive;
-      *last = t_release;
-    }
-  }
-  __syncthreads();
-}
-
-struct Seg {
-  const float* p;   // row b at p + b * ld
-  int n;            // columns (multiple of 4)
-  long long ld;
-};
-
-// y[row][b] = W_row . [seg0 | seg1 | seg2][b] for the CTA's nrows rows and every b < B, in chunks of BC items staged in shared
-// memory (xs).  sink(rl, b, y) gets each result (lane 0 of the row's warp); after(b0) runs once per chunk after all its rows.
-template <int BC, class RowPtr, class Sink, class After>
-__device__ void matvec(int K, const Seg (&seg)[3], int B, int nrows, RowPtr row_ptr, Sink sink, After after, float* xs) {
-  const int K4 = K / 4, warp = threadIdx.x / 32, lane = threadIdx.x & 31;
-  float4* xs4 = reinterpret_cast<float4*>(xs);
-  for (int b0 = 0; b0 < B; b0 += BC) {
-    for (int idx = threadIdx.x; idx < BC * K4; idx += kThreads) {
-      const int bb = idx / K4, k = 4 * (idx - bb * K4), b = b0 + bb;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (b < B) {
-        const float* src;                 // constant indices only: seg stays in registers
-        if (k < seg[0].n) src = seg[0].p ? seg[0].p + b * seg[0].ld + k : nullptr;
-        else if (k < seg[0].n + seg[1].n) src = seg[1].p + b * seg[1].ld + (k - seg[0].n);
-        else src = seg[2].p + b * seg[2].ld + (k - seg[0].n - seg[1].n);
-        if (src) v = __ldcg(reinterpret_cast<const float4*>(src));
-      }
-      xs4[idx] = v;
-    }
-    __syncthreads();
-    for (int rl = warp; rl < nrows; rl += kWarps) {
-      const float4* w4 = reinterpret_cast<const float4*>(row_ptr(rl));
-      float acc[BC];
-#pragma unroll
-      for (int bb = 0; bb < BC; ++bb) acc[bb] = 0.f;
-#pragma unroll (BC == 1 ? 4 : 2)
-      for (int k4 = lane; k4 < K4; k4 += 32) {
-        const float4 w = __ldg(w4 + k4);
-#pragma unroll
-        for (int bb = 0; bb < BC; ++bb) {
-          const float4 x = xs4[bb * K4 + k4];
-          acc[bb] = fmaf(w.x, x.x, acc[bb]);
-          acc[bb] = fmaf(w.y, x.y, acc[bb]);
-          acc[bb] = fmaf(w.z, x.z, acc[bb]);
-          acc[bb] = fmaf(w.w, x.w, acc[bb]);
-        }
-      }
-#pragma unroll
-      for (int bb = 0; bb < BC; ++bb) acc[bb] = warp_sum(acc[bb]);
-      if (lane == 0) {
-#pragma unroll
-        for (int bb = 0; bb < BC; ++bb)
-          if (b0 + bb < B) sink(rl, b0 + bb, acc[bb]);
-      }
-    }
-    __syncthreads();
-    after(b0);
-    __syncthreads();
-  }
-}
 
 // ReLU then the prenet's always-on dropout: element b * 256 + j of site `site` at decoder step `step` (pk_dropout's convention)
 __device__ __forceinline__ float prenet_act(const Params& p, float v, int b, int j, uint32_t site, int step) {
@@ -359,7 +257,7 @@ __global__ void __launch_bounds__(kThreads, 1) taco2_decode_kernel(const __grid_
           dmr, sg, B, min(kWarps, kPre - r0), [&](int rl) { return p.pre_w1 + static_cast<long long>(r0 + rl) * dmr; },
           [&](int rl, int b, float y) { pre1[b * kPre + r0 + rl] = prenet_act(p, y, b, r0 + rl, kSitePrenet1, t); }, [](int) {}, xs);
     }
-    grid_sync(ctr, target, G, p.prof, 0, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 0, &s_last);
     // P2: prenet layer 2
     for (int r0 = cta * kWarps; r0 < kPre; r0 += G * kWarps) {
       const Seg sg[3] = {{pre1, kPre, kPre}, {nullptr, 0, 0}, {nullptr, 0, 0}};
@@ -367,25 +265,25 @@ __global__ void __launch_bounds__(kThreads, 1) taco2_decode_kernel(const __grid_
           kPre, sg, B, min(kWarps, kPre - r0), [&](int rl) { return p.pre_w2 + static_cast<long long>(r0 + rl) * kPre; },
           [&](int rl, int b, float y) { pre2[b * kPre + r0 + rl] = prenet_act(p, y, b, r0 + rl, kSitePrenet2, t); }, [](int) {}, xs);
     }
-    grid_sync(ctr, target, G, p.prof, 1, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 1, &s_last);
     // A: attention LSTMCell
     {
       const Seg sg[3] = {{pre2, kPre, kPre}, {ctx, p.d_enc, p.d_enc}, {h_att_prev, kH, kH}};
       lstm_phase<BC>(p, p.att_w, p.att_b_ih, p.att_b_hh, sg, p.ws + p.L.c_att, h_att, xs, gates);
     }
-    grid_sync(ctr, target, G, p.prof, 2, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 2, &s_last);
     // B: attention, one CTA per batch item
     for (int b = cta; b < B; b += G) {
       const int a = attention_phase<BC>(p, b, t, h_att, as, xs);
       if (b == 0 && threadIdx.x == 0) s_arg0 = a;
     }
-    grid_sync(ctr, target, G, p.prof, 3, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 3, &s_last);
     // C: decoder LSTMCell
     {
       const Seg sg[3] = {{h_att, kH, kH}, {ctx, p.d_enc, p.d_enc}, {h_dec_prev, kH, kH}};
       lstm_phase<BC>(p, p.dec_w, p.dec_b_ih, p.dec_b_hh, sg, p.ws + p.L.c_dec, h_dec, xs, gates);
     }
-    grid_sync(ctr, target, G, p.prof, 4, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 4, &s_last);
     // D: projection (and stop logit, output row 0 when present: CTA 0 evaluates the rule)
     for (int r0 = cta * kWarps; r0 < n_out; r0 += G * kWarps) {    // any dmr: row blocks of 16 strided over the grid
       const Seg sg[3] = {{h_dec, kH, kH}, {ctx, p.d_enc, p.d_enc}, {nullptr, 0, 0}};
@@ -414,7 +312,7 @@ __global__ void __launch_bounds__(kThreads, 1) taco2_decode_kernel(const __grid_
       }
       if (stop) *reinterpret_cast<volatile unsigned*>(done) = static_cast<unsigned>(t + 1);
     }
-    grid_sync(ctr, target, G, p.prof, 5, &s_last);
+    grid_sync(ctr, target, G, p.prof, kPhases, 5, &s_last);
     if (!p.teacher) {
       const unsigned d = ld_acquire_gpu(done);
       if (d) { frames = static_cast<int>(d); break; }

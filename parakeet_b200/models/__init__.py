@@ -4,3 +4,4 @@ from .speedyspeech import SpeedySpeech, SpeedySpeechInference  # noqa: F401
 from .waveflow import ConditionalWaveFlow, WaveFlowLoss  # noqa: F401
 from .lstm_speaker_encoder import LSTMSpeakerEncoder  # noqa: F401
 from .tacotron2 import Tacotron2, Tacotron2Loss  # noqa: F401
+from .transformer_tts import TransformerTTS, TransformerTTSInference  # noqa: F401

@@ -322,6 +322,25 @@ def fused_attention(qkv, heads, key_lens=None, row_lens=None, ctx=None):
     return ctx
 
 
+def fused_attention_ex(q, k, *, heads, q_col0, k_col0, v_col0, key_lens=None, row_lens=None, causal=False, ctx=None):
+    """pk_fused_attention_ex: ctx Split (B, T_q, heads d_k) = softmax(q k^T / sqrt(d_k), key mask[, causal]) v per head, with Q at
+    columns q_col0 + h d_k of the Split q (B, T_q, ·) and K / V at columns k_col0 / v_col0 + h d_k of the Split k (B, T_k, ·)."""
+    B, Tq, q_ld = q.hi.shape
+    Tk, k_ld = k.hi.shape[1], k.hi.shape[2]
+    dk = ctx.hi.shape[2] // heads                    # ctx (B, T_q, heads d_k) is given: its width fixes d_k
+    Tp = (Tk + 63) // 64 * 64
+    vt = transpose_heads(k, col0=v_col0, dk=dk, heads=heads, ld_dst=Tp)
+    a = _lib.AttentionArgs()
+    a.q_hi, a.q_lo, a.k_hi, a.k_lo, a.vt_hi, a.vt_lo = (t.data_ptr() for t in (q.hi, q.lo, k.hi, k.lo, vt.hi, vt.lo))
+    a.batch, a.t_q, a.t_k, a.heads, a.dk, a.tp, a.q_ld, a.k_ld = B, Tq, Tk, heads, dk, Tp, q_ld, k_ld
+    a.q_col0, a.k_col0, a.causal = q_col0, k_col0, 1 if causal else 0
+    a.key_lens, a.row_lens = _ptr(key_lens).value, _ptr(row_lens).value
+    a.scale = 1.0 / math.sqrt(dk)
+    a.ctx_hi, a.ctx_lo = ctx.hi.data_ptr(), ctx.lo.data_ptr()
+    _lib.check(_lib.lib().pk_fused_attention_ex(C.byref(a), _stream()), "pk_fused_attention_ex")
+    return ctx
+
+
 def duration_post(x, lens, offset=1.0):
     B, T = x.shape
     x = x.contiguous()
@@ -737,4 +756,67 @@ def taco2_loss(mel, post, target, align=None, slens=None, plens=None, sigma=0.2,
     out = torch.empty(5, dtype=torch.float32, device=mel.device)
     _lib.check(_lib.lib().pk_taco2_loss(_ptr(mel), _ptr(post), _ptr(target), B, T, Cc, _ptr(align), align.shape[2] if align is not None else 0,
                                         _ptr(slens), _ptr(plens), float(sigma), _ptr(stop_logits), _ptr(out), _stream()), "pk_taco2_loss")
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# TransformerTTS (csrc/transformer_tts.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def tts_decode(w, mem_kv, pe, *, heads, steps, minlen, maxlen, threshold, p_prenet=0.5, seed=0):
+    """pk_tts_decode -> (outs (steps, r * odim), probs (steps, r), att_ws (layers, heads, steps, T_enc), frames int32 (1,)); w is the
+    dict of packed decoder weights (models/transformer_tts.py), mem_kv (T_enc, layers * 2 adim) the source-attention K / V,
+    pe (steps, adim) the alpha-scaled positional encoding rows."""
+    _require_cuda(mem_kv, pe)
+    T_enc = mem_kv.shape[0]
+    A, U, Up, L, r, odim = w["adim"], w["units"], w["prenet_units"], w["layers"], w["r"], w["odim"]
+    dev = mem_kv.device
+    lib = _lib.lib()
+    ws = torch.empty(int(lib.pk_tts_workspace(A, U, Up, L, steps)), dtype=torch.float32, device=dev)
+    outs = torch.empty(steps, r * odim, dtype=torch.float32, device=dev)
+    probs = torch.empty(steps, r, dtype=torch.float32, device=dev)
+    att = torch.empty(L, heads, steps, T_enc, dtype=torch.float32, device=dev)
+    frames = torch.empty(1, dtype=torch.int32, device=dev)
+    a = _lib.TtsDecodeArgs()
+    a.t_enc, a.adim, a.heads, a.units, a.odim, a.r = T_enc, A, heads, U, odim, r
+    a.prenet_layers, a.prenet_units, a.layers, a.steps, a.minlen, a.maxlen = w["prenet_layers"], Up, L, steps, minlen, maxlen
+    a.threshold, a.p_prenet, a.seed = float(threshold), float(p_prenet), int(seed) & 0xFFFFFFFFFFFFFFFF
+    a.mem_kv, a.pe = mem_kv.data_ptr(), pe.data_ptr()
+    for n in ("pre_w", "pre_b", "in_w", "in_b", "layer_w", "norm", "out_w", "out_b"):
+        setattr(a, n, w[n].data_ptr())
+    a.workspace, a.workspace_len = ws.data_ptr(), ws.numel()
+    a.outs, a.probs, a.att_ws, a.frames = outs.data_ptr(), probs.data_ptr(), att.data_ptr(), frames.data_ptr()
+    _lib.check(lib.pk_tts_decode(C.byref(a), _stream()), "pk_tts_decode")
+    return outs, probs, att, frames
+
+
+def tts_text_eos(text, lens, eos):
+    """text int64 (B, T), lens int32 (B,) -> (xs int64 (B, T + 1): text with eos at column lens[b], zeros after; ilens int32 = lens + 1)."""
+    B, T = text.shape
+    xs = torch.empty(B, T + 1, dtype=torch.int64, device=text.device)
+    ilens = torch.empty(B, dtype=torch.int32, device=text.device)
+    _lib.check(_lib.lib().pk_tts_text_eos(_ptr(text), _ptr(lens), B, T, int(eos), _ptr(xs), _ptr(ilens), _stream()), "pk_tts_text_eos")
+    return xs, ilens
+
+
+def tts_shift_frames(ys, r):
+    """ys fp32 (B, L, odim) -> (B, L // r, odim): the frames thinned by r (the last of each group), a zero first frame, the last dropped."""
+    B, L, odim = ys.shape
+    out = torch.empty(B, L // r, odim, dtype=torch.float32, device=ys.device)
+    _lib.check(_lib.lib().pk_tts_shift_frames(_ptr(ys), B, L, odim, r, _ptr(out), _stream()), "pk_tts_shift_frames")
+    return out
+
+
+def tts_prenet_dropout_(x, p, seed, site):
+    """In place on fp32 (B, L, U): keep element (b, t, j) with Philox site `site`, step t, element b U + j, scale 1 / (1 - p)."""
+    B, L, U = x.shape
+    _lib.check(_lib.lib().pk_tts_prenet_dropout(_ptr(x), B, L, U, float(p), int(seed) & 0xFFFFFFFFFFFFFFFF, int(site), _stream()),
+               "pk_tts_prenet_dropout")
+    return x
+
+
+def tts_stop_labels(olens, width):
+    """olens int32 (B,) -> float (B, width): 1 at and after column olens[b] - 1 and in the last column, else 0."""
+    B = olens.numel()
+    out = torch.empty(B, width, dtype=torch.float32, device=olens.device)
+    _lib.check(_lib.lib().pk_tts_stop_labels(_ptr(olens), B, width, _ptr(out), _stream()), "pk_tts_stop_labels")
     return out

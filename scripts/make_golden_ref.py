@@ -16,6 +16,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py speedyspeech_train # only tests/golden/ref_executed_speedyspeech_train.npz
     python scripts/make_golden_ref.py ge2e               # only tests/golden/ref_executed_ge2e.npz
     python scripts/make_golden_ref.py tacotron2          # only tests/golden/ref_executed_tacotron2.npz
+    python scripts/make_golden_ref.py transformer_tts    # only tests/golden/ref_executed_transformer_tts.npz
 """
 import importlib.util
 import os
@@ -544,6 +545,110 @@ def tacotron2(out):
                         out[f"{tag}/{name}/{k}"] = v.numpy()
 
 
+def stop_threshold(probs, r, first=3):
+    """A threshold the stop rule crosses with the widest margin at a step >= first: -> (threshold, stop step, margin)."""
+    m = torch.from_numpy(np.asarray(probs.numpy())).reshape(-1, r).amax(1)
+    best = None
+    for s in range(first, len(m)):
+        gap = float(m[s] - m[:s].max())
+        if best is None or gap > best[2]:
+            best = (float(m[:s].max()) + gap / 2, s + 1, gap / 2)
+    return best
+
+
+class _ListEqShape(tuple):
+    def __eq__(self, other):
+        return tuple.__eq__(self, tuple(other) if isinstance(other, list) else other)
+
+    __hash__ = tuple.__hash__
+
+
+def minlen_threshold(probs, r):
+    """A threshold crossed first at step idx a and again at a later idx b >= a + 2 (before the run's end), with the widest margin:
+    -> (threshold, minlen = a + 2, margin).  With that minlen the early stop at a is held off and the loop ends at b by the rule."""
+    m = torch.from_numpy(np.asarray(probs.numpy())).reshape(-1, r).amax(1)
+    cands = sorted(set(float(v) for v in m))
+    best = None
+    for lo, hi in zip(cands, cands[1:]):
+        th = (lo + hi) / 2
+        idx = [i + 1 for i, v in enumerate(m.tolist()) if v >= th]
+        if len(idx) >= 2 and any(b >= idx[0] + 2 for b in idx[1:]) and max(idx) < len(m):
+            if best is None or (hi - lo) / 2 > best[2]:
+                best = (th, idx[0] + 2, (hi - lo) / 2)
+    assert best is not None, "no threshold gives a minlen case that stops by the rule"
+    return best
+
+
+def transformer_tts(out):
+    """The reference's own TransformerTTS.inference at oracle.transformer_tts.GOLDEN_CONFIGS, its prenet F.dropout supplied with
+    the position-keyed Philox masks (prenet layer i = site i, row = step, element b * units + j; oracle.transformer_tts.prenet_masks):
+    under maxlen (threshold 2), under the stop rule (a threshold placed from that run with the widest margin) and with minlenratio
+    holding an early stop off until the threshold is crossed again before maxlen; the eval forward on a ragged batch and
+    inference(use_teacher_forcing=True).  Weights regenerate from their seeds; inputs are stored."""
+    import types
+    from oracle import transformer_tts as ot
+    from parakeet.models.transformer_tts.transformer_tts import TransformerTTS
+    from parakeet.modules.tacotron2 import decoder as prenet_mod
+    for tag, (cfg, seed) in ot.GOLDEN_CONFIGS.items():
+        kw = {k: v for k, v in cfg.items() if k not in ("idim", "odim")}
+        ref = TransformerTTS(cfg["idim"], cfg["odim"], **kw)
+        params = ot.synth_params(seed, cfg)
+        out[f"{tag}/keys"] = np.asarray(check_keys(ref, params, f"TransformerTTS({tag})"))
+        ref.set_state_dict(params)
+        ref.eval()
+        text = ot.golden_text(cfg, seed + 100, 9 if tag == "small" else 12)
+        out[f"{tag}/text"] = text.numpy()
+        calls = [0]
+
+        def dropout(x, p=0.5, training=True, **k):
+            assert p == ot.P_PRENET and training and x.dim() == 3
+            i = calls[0] % cfg["dprenet_layers"]
+            calls[0] += 1
+            keep = ot.prenet_masks(seed, x.shape[1], x.shape[2], cfg["dprenet_layers"], batch=x.shape[0])[i]
+            return T(x * keep * (1.0 / (1.0 - p)))
+
+        saved = prenet_mod.F
+        prenet_mod.F = types.SimpleNamespace(dropout=dropout)
+        # DecoderLayer's cache check compares a shape with a list, as Paddle's list-valued shapes allow
+        paddle_standin.Tensor.shape = property(lambda self: _ListEqShape(torch.Tensor.shape.__get__(self)))
+        try:
+            with torch.no_grad():
+                T_in = len(text) + 1
+                mlr = 4.0 if tag == "small" else 2.0
+                cases = {"maxlen": dict(threshold=2.0, maxlenratio=mlr)}
+                o = ref.inference(T(text), threshold=2.0, maxlenratio=mlr)
+                th, stop, margin = stop_threshold(o[1], cfg["reduction_factor"])
+                cases["stop"] = dict(threshold=th, maxlenratio=mlr)
+                th2, minlen, m2 = minlen_threshold(o[1], cfg["reduction_factor"])
+                cases["minlen"] = dict(threshold=th2, maxlenratio=mlr, minlenratio=(minlen + 0.5) * cfg["reduction_factor"] / T_in)
+                out[f"{tag}/minlen/margin"] = np.asarray(m2)
+                for case, ckw in cases.items():
+                    calls[0] = 0
+                    o = ref.inference(T(text), **ckw)
+                    for k, v in ckw.items():
+                        out[f"{tag}/{case}/{k}"] = np.asarray(v)
+                    for k, v in zip(("outs", "probs", "att_ws"), o):
+                        out[f"{tag}/{case}/{k}"] = v.numpy()
+                out[f"{tag}/stop/margin"] = np.asarray(margin)
+                # the teacher-forced forward on a ragged batch (padded rows live) and inference(use_teacher_forcing=True)
+                text_b, tl, sp, sl = ot.golden_batch(cfg, seed + 200)
+                for k, v in (("text", text_b), ("text_lengths", tl), ("speech", sp), ("speech_lengths", sl)):
+                    out[f"{tag}/fwd/in/{k}"] = v.numpy()
+                calls[0] = 0
+                o = ref(T(text_b), T(tl), T(sp), T(sl))
+                for k, v in zip(("after_outs", "before_outs", "logits", "ys", "labels", "olens", "ilens"), o[:7]):
+                    out[f"{tag}/fwd/{k}"] = np.asarray(v.numpy())
+                out[f"{tag}/fwd/need_dict"] = np.asarray(sorted(k for k, v in o[7].items() if not hasattr(v, "parameters")))
+                calls[0] = 0
+                tf_speech = sp[0, :int(sl[0])]
+                o = ref.inference(T(text), speech=T(tf_speech), use_teacher_forcing=True)
+                out[f"{tag}/tf/speech"] = tf_speech.numpy()
+                out[f"{tag}/tf/outs"], out[f"{tag}/tf/att_ws"] = o[0].numpy(), o[2].numpy()
+        finally:
+            prenet_mod.F = saved
+            del paddle_standin.Tensor.shape
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -616,7 +721,7 @@ def sampled(models):
 def main():
     single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
               "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e,
-              "tacotron2": tacotron2}
+              "tacotron2": tacotron2, "transformer_tts": transformer_tts}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

@@ -166,6 +166,7 @@ def build():
     P.matmul = lambda a, b, transpose_x=False, transpose_y=False: T(torch.matmul(a.transpose(-1, -2) if transpose_x else a, torch.Tensor.transpose(b, -1, -2) if transpose_y else b))
     P.round = lambda x: T(torch.sign(x) * torch.floor(torch.abs(x) + 0.5))          # C round(): half away from zero
     P.logical_not = lambda x: T(torch.logical_not(x))
+    P.logical_and = lambda x, y: T(torch.logical_and(x, y))
     P.where = lambda c, a, b: T(torch.where(c, a, b))
     P.tril = lambda x, diagonal=0: T(torch.tril(x, diagonal))
     P.sin, P.cos, P.exp, P.log, P.sqrt, P.abs, P.tanh = (lambda f: (lambda x: T(f(x))))(torch.sin), None, None, None, None, None, None
@@ -237,6 +238,9 @@ def build():
         def add_parameter(self, name, p):
             self.register_parameter(name, p)
             return p
+
+        def named_sublayers(self, prefix="", include_self=False):
+            return [(n, m) for n, m in self.named_modules(prefix=prefix) if include_self or m is not self]
 
         def sublayers(self, include_self=False):
             return [m for m in self.modules() if include_self or m is not self]

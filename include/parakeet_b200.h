@@ -883,7 +883,7 @@ int pk_taco2_loss(const float* mel, const float* post, const float* target, int3
  *   norm     after_norm gamma | beta; out_w (r + r odim, adim) = [prob_out rows | feat_out rows], out_b (r + r odim)
  *   outs     (steps, r odim), probs (steps, r) sigmoid, att_ws (layers, heads, steps, t_enc): zeroed by the call, rows past the
  *            stop stay zero; frames[0] = decoder steps run.  steps >= max(minlen, maxlen) sizes the caches and outputs.
- * Refused with PK_ERR_UNSUPPORTED: head widths not a multiple of 32, adim / units / prenet_units / odim not multiples of 4,
+ * Refused with PK_ERR_UNSUPPORTED: head widths other than 64, 128 and 192, units / prenet_units / odim not multiples of 4,
  * r > 16, max(steps, t_enc) past the shared-memory score buffer, fewer co-resident CTAs than heads. */
 typedef struct {
   int32_t t_enc, adim, heads, units, odim, r, prenet_layers, prenet_units, layers, steps, minlen, maxlen;
@@ -898,7 +898,7 @@ int64_t pk_tts_layer_floats(int32_t adim, int32_t units);
 int64_t pk_tts_workspace(int32_t adim, int32_t units, int32_t prenet_units, int32_t layers, int32_t steps);
 int pk_tts_decode(const PkTtsDecodeArgs* args, pk_stream_t stream);
 /* Glue of the teacher-forced forward.  pk_tts_text_eos: xs (batch, t + 1) = text with eos at column lens[b] and zeros after,
- * ilens = lens + 1.  pk_tts_shift_frames: out (batch, l / r, odim)[b, 0] = 0, [b, i] = ys[b, i r - 1].  pk_tts_prenet_dropout: in
+ * ilens = lens + 1 (text may be NULL when t = 0).  pk_tts_shift_frames: out (batch, l / r, odim)[b, 0] = 0, [b, i] = ys[b, i r - 1].  pk_tts_prenet_dropout: in
  * place on (batch, l, units), element (b, i, j) kept with Philox site, step i, element b units + j (pk_tts_decode's masks), scaled
  * 1 / (1 - p).  pk_tts_stop_labels: out (batch, width) = 1 where column >= olens[b] - 1 or column == width - 1, else 0. */
 int pk_tts_text_eos(const int64_t* text, const int32_t* lens, int32_t batch, int32_t t, int64_t eos, int64_t* xs, int32_t* ilens,

@@ -2,7 +2,7 @@
 modules/fastspeech2_transformer/decoder.py `Decoder.forward_one_step`, decoder_layer.py `DecoderLayer.forward` with a cache,
 modules/tacotron2/decoder.py `Prenet` / `Postnet`).
 
-`inference` runs the reference's own step loop: every step re-embeds every earlier frame through the prenet, and each decoder layer
+`inference` is `encode`, then `decode`, the reference's own step loop on the encoder output: every step re-embeds every earlier frame through the prenet, and each decoder layer
 computes only the new query row over [its cached outputs | the new row], exactly as `forward_one_step` does; no K / V cache of its own.
 
 The prenet's `F.dropout` is always on with Paddle's default p = 0.5 (it ignores `dprenet_dropout_rate`).  Its masks cannot be
@@ -136,23 +136,35 @@ def embed_frames(p, cfg, ys, keep):
     h = ys
     for i in range(cfg["dprenet_layers"]):
         h = torch.relu(ofs.linear(p, f"decoder.embed.0.0.prenet.{i}.0", h))
-        h = h * keep[i, :, :h.shape[1]].to(h.dtype) * (1.0 / (1.0 - P_PRENET))
+        h = h * keep[i, :, :h.shape[1]].to(h) * (1.0 / (1.0 - P_PRENET))
     x = ofs.linear(p, "decoder.embed.0.1", h)
-    return x + p["decoder.embed.1.alpha"] * ofs.positional_encoding(x.shape[1], x.shape[2]).to(x.dtype)
+    return x + p["decoder.embed.1.alpha"] * ofs.positional_encoding(x.shape[1], x.shape[2]).to(x)
 
 
 def inference(p, cfg, text, threshold=0.5, minlenratio=0.0, maxlenratio=10.0, seed=0, dtype=torch.float64):
     """TransformerTTS.inference (no teacher forcing) on text (T,) int64 without eos -> (outs (L r, odim), probs (L r,),
     att_ws (dlayers, aheads, L, T + 1), the per-step decoder outputs before the postnet (L r, odim))."""
     p = {k: v.to(dtype) for k, v in p.items()}
-    r, odim, H = cfg["reduction_factor"], cfg["odim"], cfg["aheads"]
+    r = cfg["reduction_factor"]
     x = torch.cat([text.reshape(-1).long(), torch.tensor([cfg["idim"] - 1])]).unsqueeze(0)
     hs = encode(p, cfg, x)
     maxlen = int(hs.shape[1] * maxlenratio / r)
     minlen = int(hs.shape[1] * minlenratio / r)
+    before, probs, att_ws = decode(p, cfg, hs, minlen, maxlen, threshold, seed, dtype)
+    after = before + ofs.postnet(p, before.t().unsqueeze(0), cfg["postnet_layers"])[0].t()
+    return after, probs, att_ws, before
+
+
+def decode(p, cfg, hs, minlen, maxlen, threshold, seed, dtype=torch.float64):
+    """inference's decoder loop on the encoder output hs (1, T, adim), on hs's device -> (the decoder outputs before the postnet
+    (L r, odim), probs (L r,), att_ws (dlayers, aheads, L, T)); it stops after step idx once (any prob >= threshold or
+    idx >= maxlen) and idx >= minlen."""
+    p = {k: v.to(hs.device, dtype) for k, v in p.items()}
+    hs = hs.to(dtype)
+    r, odim, H = cfg["reduction_factor"], cfg["odim"], cfg["aheads"]
     cap = max(maxlen, minlen, 1)
     keep = prenet_masks(seed, cap, cfg["dprenet_units"], cfg["dprenet_layers"]) if P_PRENET > 0 else None
-    ys = torch.zeros(1, 1, odim, dtype=dtype)
+    ys = torch.zeros(1, 1, odim, dtype=dtype, device=hs.device)
     cache = [None] * cfg["dlayers"]
     outs, probs, att_ws = [], [], []
     idx = 0
@@ -182,9 +194,7 @@ def inference(p, cfg, text, threshold=0.5, minlenratio=0.0, maxlenratio=10.0, se
             if idx < minlen:
                 continue
             break
-    before = torch.cat(outs, 0)
-    after = before + ofs.postnet(p, before.t().unsqueeze(0), cfg["postnet_layers"])[0].t()
-    return after, torch.cat(probs, 0), torch.stack(att_ws, 2), before
+    return torch.cat(outs, 0), torch.cat(probs, 0), torch.stack(att_ws, 2)
 
 
 def golden_text(cfg, seed, n):

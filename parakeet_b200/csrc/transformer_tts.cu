@@ -403,10 +403,12 @@ extern "C" int pk_tts_decode(const PkTtsDecodeArgs* a, pk_stream_t stream) {
                    a->minlen >= 0 && a->maxlen >= 0, "t_enc, steps, layers, heads, prenet_layers and r must be >= 1");
   PK_CHECK_ARG(a->steps >= a->minlen && a->steps >= a->maxlen, "steps must hold max(minlen, maxlen) decoder steps");
   const int A = a->adim, H = a->heads;
-  if (A % H != 0 || (A / H) % 32 != 0 || A / H > kThreads || A % 4 || a->units % 4 || a->prenet_units % 4 || a->odim % 4 || a->r > kWarps)
-    return fail(PK_ERR_UNSUPPORTED, "pk_tts_decode supports head widths that are multiples of 32 (<= %d), adim, units, prenet units "
-                                    "and odim multiples of 4 and r <= %d (got adim %d, heads %d, units %d, prenet %d, odim %d, r %d)",
-                kThreads, kWarps, A, H, a->units, a->prenet_units, a->odim, a->r);
+  // head widths: the ones TransformerTTS can build (its teacher-forced path runs pk_fused_attention_ex, which takes 64, 128, 192)
+  const int dk = A % H == 0 ? A / H : 0;
+  if ((dk != 64 && dk != 128 && dk != 192) || a->units % 4 || a->prenet_units % 4 || a->odim % 4 || a->r > kWarps)
+    return fail(PK_ERR_UNSUPPORTED, "pk_tts_decode supports head widths 64, 128 and 192, units, prenet units and odim multiples of 4 "
+                                    "and r <= %d (got adim %d, heads %d, units %d, prenet %d, odim %d, r %d)",
+                kWarps, A, H, a->units, a->prenet_units, a->odim, a->r);
   PK_CHECK_ARG(a->mem_kv && a->pre_w && a->pre_b && a->in_w && a->in_b && a->pe && a->layer_w && a->norm && a->out_w && a->out_b &&
                    a->workspace && a->outs && a->probs && a->att_ws && a->frames, "NULL pointer in pk_tts_decode");
   PK_CHECK_ARG(a->p_prenet >= 0.f && a->p_prenet < 1.f, "prenet dropout must be in [0, 1)");
@@ -465,7 +467,8 @@ static unsigned blocks_for(long long n) { return static_cast<unsigned>((n + 255)
 
 extern "C" int pk_tts_text_eos(const int64_t* text, const int32_t* lens, int32_t batch, int32_t t, int64_t eos, int64_t* xs, int32_t* ilens,
                                pk_stream_t stream) {
-  PK_CHECK_ARG(text && lens && xs && ilens && batch > 0 && t >= 0, "bad arguments to pk_tts_text_eos");
+  // text may be NULL when t == 0 (an empty tensor has no storage): every row is then [eos] and text is never read
+  PK_CHECK_ARG((text || t == 0) && lens && xs && ilens && batch > 0 && t >= 0, "bad arguments to pk_tts_text_eos");
   text_eos_kernel<<<blocks_for(static_cast<long long>(batch) * (t + 1)), 256, 0, static_cast<cudaStream_t>(stream)>>>(text, lens, batch, t,
                                                                                                                        eos, xs, ilens);
   PK_CHECK_CUDA(cudaGetLastError());

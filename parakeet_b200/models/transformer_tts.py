@@ -63,6 +63,9 @@ class TransformerTTS(Layer):
             bad.append("postnet without batch norm")
         if adim % aheads or (adim // aheads) % 64:
             bad.append(f"attention head width adim / aheads = {adim / aheads:g} (must be a multiple of 64)")
+        elif adim // aheads > 192:
+            bad.append(f"attention head width adim / aheads = {adim // aheads} (the teacher-forced decoder's pk_fused_attention_ex "
+                       "takes 64, 128 or 192)")
         if odim % 4 or dprenet_units % 4 or dunits % 4 or reduction_factor < 1 or reduction_factor > 16:
             bad.append("odim, dprenet_units and dunits must be multiples of 4 and 1 <= reduction_factor <= 16")
         if postnet_layers and postnet_filts % 2 == 0:

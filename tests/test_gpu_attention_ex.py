@@ -23,14 +23,14 @@ PARENT_SHA256 = "0b50d53f15e679853ed6d711bd33e438fdc98ee29e522db6a9d18502b834a00
 
 
 def ref_attention(q, k, v, key_lens, causal):
-    """fp64: q (B, Tq, H, dk), k / v (B, Tk, H, dk) -> (B, Tq, H dk)."""
+    """fp64: q (B, Tq, H, dk), k / v (B, Tk, H, dk) -> (B, Tq, H dk), on q's device."""
     B, Tq, H, dk = q.shape
     Tk = k.shape[1]
     s = torch.einsum("bqhd,bkhd->bhqk", q, k) / math.sqrt(dk)
-    mask = torch.arange(Tk)[None, :] < key_lens[:, None]                                   # (B, Tk)
+    mask = torch.arange(Tk, device=q.device)[None, :] < key_lens.to(q.device)[:, None]   # (B, Tk)
     mask = mask[:, None, None, :].expand(B, 1, Tq, Tk)
     if causal:
-        mask = mask & torch.tril(torch.ones(Tq, Tk, dtype=torch.bool))[None, None]
+        mask = mask & torch.tril(torch.ones(Tq, Tk, dtype=torch.bool, device=q.device))[None, None]
     s = s.masked_fill(~mask, float("-inf"))
     p = torch.softmax(s, -1)
     return torch.einsum("bhqk,bkhd->bqhd", p, v).reshape(B, Tq, H * dk)
@@ -57,23 +57,36 @@ def test_causal_self_attention(T, dk):
     assert err < 3e-4 * v64.abs().max().item(), err
 
 
-@pytest.mark.parametrize("Tk", [1, 15, 128, 129, 700])
-def test_cross_attention(Tk):
-    H, dk, B, Tq = 8, 64, 3, 300
-    A, L = H * dk, 2
-    g = torch.Generator().manual_seed(Tk)
-    q = torch.randn(B, Tq, A, generator=g, dtype=torch.float64)
-    mem = torch.randn(B, Tk, L * 2 * A, generator=g, dtype=torch.float64)                 # [K_0 | V_0 | K_1 | V_1]
+def cross_cases():
+    """T_k x d_k x T_q x layers; the cases of 64-wide heads, 300 queries and 2 layers keep their T_k ids.  T_q = 1 is a
+    teacher-forced batch whose speech_lengths == r; 6 layers put k_col0 = 2 A l deep into the (B, T_k, 12 A) buffer."""
+    out = []
+    for Tk in (1, 15, 128, 129, 700):
+        for dk in (64, 128, 192):
+            for Tq in (300, 1):
+                for L in (2, 6):
+                    tag = str(Tk) if (dk, Tq, L) == (64, 300, 2) else f"{Tk}-dk{dk}-Tq{Tq}-L{L}"
+                    out.append(pytest.param(Tk, dk, Tq, L, id=tag))
+    return out
+
+
+@pytest.mark.parametrize("Tk,dk,Tq,L", cross_cases())
+def test_cross_attention(Tk, dk, Tq, L):
+    H, B = 8, 3
+    A = H * dk
+    g = torch.Generator().manual_seed(Tk * 1000 + dk * 10 + L + Tq)
+    q = torch.randn(B, Tq, A, generator=g)
+    mem = torch.randn(B, Tk, L * 2 * A, generator=g)                                      # [K_0 | V_0 | K_1 | V_1 | ...]
     lens = torch.tensor([Tk, max(1, Tk - 7), 1])
     qs, ms = split_of(q), split_of(mem)
-    qf, mf = qs.float().double().cpu(), ms.float().double().cpu()
+    qf, mf = qs.float().double(), ms.float().double()                                     # the reference on the device, in fp64
     for l in range(L):
         ctx = Split.empty((B, Tq, A), DEV)
         ops.fused_attention_ex(qs, ms, heads=H, q_col0=0, k_col0=2 * A * l, v_col0=2 * A * l + A, key_lens=lens.to(DEV, torch.int32), ctx=ctx)
         k = mf[..., 2 * A * l:2 * A * l + A].reshape(B, Tk, H, dk)
         v = mf[..., 2 * A * l + A:2 * A * (l + 1)].reshape(B, Tk, H, dk)
         want = ref_attention(qf.reshape(B, Tq, H, dk), k, v, lens, causal=False)
-        err = (ctx.float().double().cpu() - want).abs().max().item()
+        err = (ctx.float().double() - want).abs().max().item()
         assert err < 3e-4 * v.abs().max().item(), (l, err)
 
 

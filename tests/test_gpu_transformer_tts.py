@@ -88,10 +88,12 @@ def test_teacher_forced_inference_matches_the_fixture(tag):
     assert (att.double().sum(-1) - 1).abs().max().item() < 1e-4
 
 
-@pytest.mark.parametrize("n_text,r", [(0, 1), (1, 2), (150, 3), (512, 1), (150, 1)])
-def test_decoder_matches_the_fp64_oracle_at_every_step(n_text, r):
-    cfg = dict(ot.SMALL, reduction_factor=r, dlayers=3)
-    m, p, cfg = build(cfg, 20 + r)
+@pytest.mark.parametrize("n_text,r,adim", [pytest.param(n, r, 128, id=f"{n}-{r}") for n, r in [(0, 1), (1, 2), (150, 3), (512, 1), (150, 1)]]
+                         + [pytest.param(150, 2, adim, id=f"150-2-dk{adim // 2}") for adim in (256, 384)])
+def test_decoder_matches_the_fp64_oracle_at_every_step(n_text, r, adim):
+    """ot.SMALL's two heads at widths 64, 128 and 192."""
+    cfg = dict(ot.SMALL, reduction_factor=r, dlayers=3, adim=adim)
+    m, p, cfg = build(cfg, 20 + r + adim - 128)
     text = ot.golden_text(cfg, 30 + n_text, n_text)
     T = n_text + 1
     steps = 24
@@ -102,6 +104,29 @@ def test_decoder_matches_the_fp64_oracle_at_every_step(n_text, r):
     for name, ours, ref in (("outs", outs, a64), ("probs", probs, p64), ("att_ws", att, att64)):
         assert rel(ours, ref) < 2e-4, (name, rel(ours, ref))
     assert (att.double().sum(-1) - 1).abs().max().item() < 1e-5      # every source-attention row is a distribution
+
+
+@pytest.mark.parametrize("adim", [256, 384])
+def test_forward_matches_the_fp64_oracle_at_wide_heads(adim):
+    """The eval forward and teacher-forced inference on ot.golden_batch with two heads of 128 or 192 against ot.forward in fp64:
+    the causal and cross modes of pk_fused_attention_ex and the source weights of batched_matmul_nt at those widths.  1e-3
+    relative, the bound of the fixture comparisons (split-bf16 GEMMs over the same chain)."""
+    m, p, cfg = build(ot.SMALL, 130 + adim, adim=adim, aheads=2)
+    text, tl, speech, sl = ot.golden_batch(cfg, 140 + adim)
+    out = m(text.to(DEV), tl.to(DEV), speech.to(DEV), sl.to(DEV), seed=2 ** 62 - 1)
+    with torch.no_grad():
+        ref = ot.forward(p, cfg, text, tl, speech, sl, seed=2 ** 62 - 1)
+    for name, ours in zip(("after_outs", "before_outs", "logits", "ys", "labels", "olens", "ilens"), out[:7]):
+        assert tuple(ours.shape) == tuple(ref[name].shape), name
+        if name in ("ys", "labels", "olens", "ilens"):
+            assert torch.equal(ours.cpu().to(ref[name].dtype), ref[name]), name
+        else:
+            assert rel(ours, ref[name]) < 1e-3, (name, rel(ours, ref[name]))
+    n, f = int(tl[0]), int(sl[0])
+    outs, _, att = m.inference(text[0, :n].to(DEV), speech=speech[0, :f].to(DEV), use_teacher_forcing=True, seed=3)
+    with torch.no_grad():
+        one = ot.forward(p, cfg, text[:1, :n], tl[:1], speech[:1, :f], sl[:1], seed=3)
+    assert rel(outs, one["after_outs"][0]) < 1e-3 and rel(att, one["att_ws"][0]) < 1e-3
 
 
 def test_long_run_past_1000_steps():

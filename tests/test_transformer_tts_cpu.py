@@ -113,11 +113,11 @@ def test_state_dict_round_trip():
 @pytest.mark.parametrize("over", [dict(eprenet_conv_layers=3), dict(spk_embed_dim=64), dict(use_gst=True), dict(encoder_concat_after=True),
                                   dict(decoder_concat_after=True), dict(encoder_normalize_before=False),
                                   dict(decoder_normalize_before=False), dict(positionwise_layer_type="linear"), dict(dprenet_layers=0),
-                                  dict(aheads=4), dict(use_scaled_pos_enc=False), dict(use_batch_norm=False), dict(postnet_filts=4),
+                                  dict(aheads=4), dict(adim=256, aheads=1), dict(use_scaled_pos_enc=False), dict(use_batch_norm=False), dict(postnet_filts=4),
                                   dict(odim=10), dict(dprenet_units=30), dict(reduction_factor=17)],
                          ids=lambda d: next(iter(d)))
 def test_unsupported_configs_raise_in_the_constructor(over):
-    idim, odim, kw = model_kwargs(ot.SMALL, **over)             # aheads=4: 32-wide heads at adim 128
+    idim, odim, kw = model_kwargs(ot.SMALL, **over)             # aheads=4: 32-wide heads at adim 128; adim=256: one 256-wide head
     with pytest.raises(ValueError):
         TransformerTTS(idim, odim, device="cpu", **kw)
 

@@ -80,6 +80,27 @@ int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t cols, uint6
   return PK_OK;
 }
 
+int encode_tmap_f32_3d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t batches, uint64_t batch_stride_elems,
+                       uint32_t box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) return fail(PK_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
+  if (batches == 0) batches = 1;
+  if (batch_stride_elems == 0) batch_stride_elems = 32 * rows;
+  cuuint64_t dims[3] = {32, rows, batches};
+  cuuint64_t strides[2] = {32 * 4, batch_stride_elems * 4};  // bytes, dims 1..2
+  cuuint32_t box[3] = {32, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  if (strides[1] & 15) return fail(PK_ERR_INVALID_ARG, "TMA strides must be multiples of 16 bytes");
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(PK_ERR_CUDA, "cuTensorMapEncodeTiled (fp32) failed (%d): rows=%llu batches=%llu bs=%llu box_rows=%u",
+                static_cast<int>(r), (unsigned long long)rows, (unsigned long long)batches, (unsigned long long)batch_stride_elems,
+                box_rows);
+  return PK_OK;
+}
+
 int encode_tmap_bf16_planes(CUtensorMap* out, const void* hi, const void* lo, uint64_t cols, uint64_t rows, uint64_t batches,
                             uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols) {
   EncodeTiledFn fn = get_encode_fn();

@@ -34,6 +34,12 @@ int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t cols, uint6
 int encode_tmap_bf16_planes(CUtensorMap* out, const void* hi, const void* lo, uint64_t cols, uint64_t rows, uint64_t batches,
                             uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, uint32_t box_cols = 64);
 
+// A 3-D fp32 tiled tensor map of 128-byte lines (32 floats, one 128B-swizzle atom) with zero OOB fill:
+//   dims = {32, rows, batches}; batch stride in ELEMENTS (0: 32 * rows); box = {32, box_rows, 1}.  A tensor whose rows are
+//   wider than 32 floats is described with rows = its rows x (row width / 32).
+int encode_tmap_f32_3d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t batches, uint64_t batch_stride_elems,
+                       uint32_t box_rows);
+
 int sm_count();
 void count_launch(int n = 1);
 

@@ -188,6 +188,9 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
+__device__ __forceinline__ void sts_f2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
 
 // mbarrier / TMA helpers taking shared-space addresses
 __device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
@@ -235,9 +238,16 @@ __device__ __forceinline__ void tma_store_4d_a(const CUtensorMap* tm, uint32_t s
                ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-// asynchronous prefetch of `bytes` (a multiple of 16) contiguous global bytes into L2
-__device__ __forceinline__ void bulk_prefetch_l2(const void* gptr, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
+__device__ __forceinline__ void tma_store_3d_a(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+// The same, adding the box element-wise onto global memory (the add happens in L2; rows outside the tensor are left alone).
+__device__ __forceinline__ void tma_reduce_add_3d_a(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>

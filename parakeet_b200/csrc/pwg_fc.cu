@@ -10,14 +10,15 @@
 // describes; each half tile is two 64-row tiles, one per consumer warpgroup ("ping-pong": while one warpgroup gates and
 // stores, the other keeps the tensor cores busy).  384 threads:
 //   * warps 8-11 (producer warpgroup, one TMA lane): per 64-row tile 4 A chunks (tap -d, tap +d, conditioning, centre tap)
-//     through one 6-deep ring of 16 KB stages, the two warpgroups' tiles alternating; the conditioning stage holds a
+//     through one 4-deep ring of 16 KB stages, the two warpgroups' tiles alternating; the conditioning stage holds a
 //     16-column box of the band table and the 16-frame P window of the tile (32-byte swizzle).  W1 (three tap chunks) and
 //     W2 stay resident (128 KB);
 //   * warps 0-7 (two consumer warpgroups, one 64-row tile each): GEMM1 (wgmma, accumulator in registers, one commit group
 //     in flight), the gate in registers, z as the register A operand of GEMM2 - z never touches shared memory.  The residual
 //     add `+ x` is folded in by starting GEMM2's accumulator at [0 | x], read from the centre-tap chunk while it is in
-//     shared memory; that stage then holds y for one TMA store of the tile, and the skip sum is red.add-ed from the
-//     fragments (its rows were prefetched into L2 by the producer).  An ordering barrier alternates the warpgroups' GEMM1s.
+//     shared memory; every stage goes back to the producer during GEMM1.  An ordering barrier alternates the warpgroups'
+//     GEMM1s, so their epilogues alternate too and share one 32 KB staging area: y (split planes) and the fp32 skip tile,
+//     written by one TMA store and one TMA reduce-add.
 #include <stdlib.h>
 #include <string.h>
 
@@ -36,13 +37,15 @@ constexpr int kQTile = 64 * kSwizzleBytes;                   // 8 KB: one plane 
 constexpr int kConsumerThreads = 256;
 constexpr int kThreads = kConsumerThreads + 128;
 constexpr int kFcG1Chunks = 4;                               // tap -d, tap +d, conditioning, centre tap
-constexpr int kFcStages = 6;
+constexpr int kFcStages = 4;
 constexpr int kFcStageBytes = 2 * kQTile;                    // A hi, A lo
 constexpr int kFcUBytes = 2 * 64 * 32;                       // 4 KB: hi | lo of 16 band-table columns x 64 rows
 constexpr int kFcPBytes = 2 * 128 * 32;                      // 8 KB: hi | lo of 16 P frames x 128 output channels
 constexpr int kFcW1Bytes = 3 * 2 * kATile;                   // 96 KB: three tap chunks x 128 output channels
 constexpr int kFcW2Bytes = 2 * kATile;                       // 32 KB: 128 outputs (skip | out) x 64
-constexpr int kFcSmem = kFcW1Bytes + kFcW2Bytes + kFcStages * kFcStageBytes + 1024 + 256;
+constexpr int kFcYBytes = 2 * kQTile;                        // 16 KB: y staging, hi | lo planes of 64 rows
+constexpr int kFcSkipBytes = 64 * 64 * 4;                    // 16 KB: skip staging, 64 rows x 64 fp32 channels
+constexpr int kFcSmem = kFcW1Bytes + kFcW2Bytes + kFcStages * kFcStageBytes + kFcYBytes + kFcSkipBytes + 1024 + 256;
 static_assert(kFcUBytes + kFcPBytes <= kFcStageBytes, "the conditioning operands share one ring stage");
 static_assert(kFcSmem <= 227 * 1024, "shared memory budget");
 
@@ -103,16 +106,21 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
                     const __grid_constant__ CUtensorMap tm_p,          // 4-D maps: both planes of a tile in one TMA box
                     const __grid_constant__ CUtensorMap tm_w1_hi, const __grid_constant__ CUtensorMap tm_w1_lo,
                     const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
-                    const __grid_constant__ CUtensorMap tm_y, const FcLayerArgs p) {
+                    const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_skip,
+                    const FcLayerArgs p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t w1 = smem;                                    // [tap chunk][hi | lo] 128-row tiles, resident
   const uint32_t w2 = w1 + kFcW1Bytes;                         // [hi | lo]
   const uint32_t ring = w2 + kFcW2Bytes;                       // [stages] 64-row chunks [hi | lo]
-  const uint32_t bars = ring + kFcStages * kFcStageBytes;
+  // epilogue staging, used by the two consumer warpgroups in turn
+  const uint32_t ystage = ring + kFcStages * kFcStageBytes;    // y: [hi | lo] 64 rows, the layout of x in a ring stage
+  const uint32_t sstage = ystage + kFcYBytes;                  // skip: 64 rows x 2 lines of 32 fp32, 128B-swizzled
+  const uint32_t bars = sstage + kFcSkipBytes;
   const uint32_t full_bar = bars;                              // [stages]
   const uint32_t empty_bar = full_bar + 8 * kFcStages;         // [stages]
   const uint32_t w_bar = empty_bar + 8 * kFcStages;
+  const uint32_t free_bar = w_bar + 8;                         // [warpgroup]: the staging area is free for it
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -120,10 +128,11 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
   if (threadIdx.x == kConsumerThreads) {
     tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_u); tma_prefetch_desc(&tm_p);
     tma_prefetch_desc(&tm_w1_hi); tma_prefetch_desc(&tm_w1_lo); tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    tma_prefetch_desc(&tm_y);
+    tma_prefetch_desc(&tm_y); tma_prefetch_desc(&tm_skip);
     // a stage is read by one consumer warpgroup: one arrival per warp
     for (int s = 0; s < kFcStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, 4); }
     mbar_init_a(w_bar, 1);
+    mbar_init_a(free_bar, 1); mbar_init_a(free_bar + 8, 1);    // arrived on by the other warpgroup's store lane
     fence_barrier_init();
   }
   __syncthreads();
@@ -156,10 +165,6 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
         // 8 frames (16 B) - TMA faults on an unaligned innermost coordinate
         const int j0 = (m0 / p.hop - 2) & ~7;
         for (int wg = 0; wg < 2; ++wg) {                       // the 64-row tiles of consumer warpgroups 0 and 1
-          // the tile's rows of the skip sum go to L2 now, so that the red.add of its epilogue does not wait for HBM
-          const int rows = min(64, p.t - (mh + 64 * wg));
-          if (!p.skip_init && rows > 0)
-            bulk_prefetch_l2(p.skip + (static_cast<long long>(b) * p.t + mh + 64 * wg) * 64, rows * 64 * 4);
           for (int j = 0; j < kFcG1Chunks; ++j, ++it) {
             const int s = it % kFcStages;
             mbar_wait_a(empty_bar + 8 * s, ((it / kFcStages) & 1) ^ 1);
@@ -195,6 +200,11 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
     int b, m0, half;
     bool more = ti.next(b, m0, half);
     bool first = true;
+    // Both warpgroups take one 64-row tile of every half tile, and their epilogues alternate (0, 1, 0, 1, ...): warpgroup 1's
+    // k-th epilogue waits for the k-th release by warpgroup 0, warpgroup 0's k-th for the (k - 1)-th release by warpgroup 1
+    // (its first passes on the fresh barrier's parity).  A warpgroup cannot get two releases ahead of the other's waits, so a
+    // parity bit per warpgroup is enough.
+    uint32_t free_phase = wg ^ 1;
     while (more) {
       const int mh = m0 + 128 * half;
       float acc1[64], acc2[64];
@@ -252,9 +262,9 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
       }
       wgmma_wait<0>();
       reg_fence(acc1);
-      // the centre-tap stage stays with this warpgroup: it becomes the staging tile of y (same rows, same layout as x)
-      const int cs = (it + kFcG1Chunks - 1) % kFcStages;
-      const uint32_t ystage = ring + cs * kFcStageBytes;
+      // the centre-tap stage has been read by its wgmmas and for [0 | x]: back to the producer
+      __syncwarp();
+      if (lane == 0) mbar_arrive_a(empty_bar + 8 * ((it + kFcG1Chunks - 1) % kFcStages));
       it += 2 * kFcG1Chunks;                                   // the other warpgroup's tile sits in between
       // hand GEMM1 to the other warpgroup (warpgroup 1 skips this after its last tile: warpgroup 0 waits for no more turns)
       int nb, nm0, nhalf;
@@ -292,9 +302,11 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
       wgmma_commit();
       wgmma_wait<0>();
       reg_fence(acc2);
-      // stores: out half -> (out + b_out) * sqrt(1/2) as split planes into the staging tile, then one TMA store of the 64 rows
-      // (rows past t lie outside the tensor map: not written); skip half -> fp32 skip sum (write or red.add) from the
-      // fragments while the TMA engine reads the staging tile
+      // stores: out half -> (out + b_out) * sqrt(1/2) as split planes into the y staging tile, skip half -> the fp32 skip
+      // staging tile; then one TMA store of y and one TMA reduce-add (store at skip_init) of the skip tile.  Rows past t lie
+      // outside both tensor maps and are not written; rows in [len, t) get a zero y and their skip contribution.
+      mbar_wait_a(free_bar + 8 * wg, free_phase);
+      free_phase ^= 1;
       const int len = p.lens ? min(__ldg(p.lens + b), p.t) : p.t;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
@@ -310,34 +322,22 @@ pwg_layer_fc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
           const uint32_t off = r * kSwizzleBytes + (((c >> 3) ^ (r & 7)) << 4) + (cq & 7) * 2;   // where x was read
           sts_u32(ystage + off, oh);
           sts_u32(ystage + kQTile + off, ol);
+          // skip row r = 128-byte lines 2 r (channels 0..31) and 2 r + 1; the 16-byte chunk XOR (line & 7) keeps each
+          // half warp's 8-byte writes on 32 distinct banks
+          const int line = 2 * r + (c >> 5);
+          sts_f2(sstage + line * 128 + ((((c & 31) >> 2) ^ (line & 7)) << 4) + (c & 3) * 4, acc2[4 * jj + 2 * hh],
+                 acc2[4 * jj + 2 * hh + 1]);
         }
       }
-      // (shared memory only: a fence over all of the thread's writes would also wait for the previous tile's skip red.adds)
       fence_proxy_async_shared();
       named_bar_sync(3 + wg, 128);
-      const bool store_lane = (threadIdx.x & 127) == 0;
-      if (store_lane) {
+      if ((threadIdx.x & 127) == 0) {
         tma_store_4d_a(&tm_y, ystage, 0, mh + wg * 64, b, 0);
+        if (p.skip_init) tma_store_3d_a(&tm_skip, sstage, 0, 2 * (mh + wg * 64), b);
+        else tma_reduce_add_3d_a(&tm_skip, sstage, 0, 2 * (mh + wg * 64), b);
         bulk_commit();
-      }
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int trow = mh + wg * 64 + rl + 8 * hh;
-        if (trow < p.t) {
-          const long long row_off = (static_cast<long long>(b) * p.t + trow) * 64;
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            float* d2 = p.skip + row_off + 8 * jj + cq;
-            const float s0 = acc2[4 * jj + 2 * hh], s1 = acc2[4 * jj + 2 * hh + 1];
-            if (p.skip_init) *reinterpret_cast<float2*>(d2) = make_float2(s0, s1);
-            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(d2), "f"(s0), "f"(s1) : "memory");
-          }
-        }
-      }
-      if (store_lane) {
-        bulk_wait_read<0>();                                   // the stage has been read: back to the producer
-#pragma unroll
-        for (int w = 0; w < 4; ++w) mbar_arrive_a(empty_bar + 8 * cs);   // the arrivals of the warpgroup's 4 warps
+        bulk_wait_read<0>();                                   // the staging tiles have been read
+        mbar_arrive_a(free_bar + 8 * (wg ^ 1));
       }
       b = nb; m0 = nm0; half = nhalf; more = next;
     }
@@ -359,11 +359,13 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
                a->u_rows >= a->u_end_base + 384 * a->batch, "bad compact band table layout");
   PK_CHECK_ARG(a->p_rows > 0 && a->p_row0 >= 0 && a->p_row0 + 128 <= a->p_rows && (a->p_ld % 8) == 0 && a->p_ld >= 64 && a->p_frames > 0 &&
                a->p_frames <= a->p_ld, "bad P plane geometry");
-  CUtensorMap tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty;
+  CUtensorMap tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty, ts;
   int rc;
   const uint64_t T = a->t, B = a->batch;
   if ((rc = encode_tmap_bf16_planes(&tx, a->x_hi, a->x_lo, kPwgR, T, B, kPwgR, T * kPwgR, 64))) return rc;
   if ((rc = encode_tmap_bf16_planes(&ty, a->y_hi, a->y_lo, kPwgR, T, B, kPwgR, T * kPwgR, 64))) return rc;
+  // skip sum (B, T, 64) fp32: each 256-byte row is two 128-byte lines, a 64-row tile one box of 128 lines
+  if ((rc = encode_tmap_f32_3d(&ts, a->skip, 2 * T, B, 0, 128))) return rc;
   // compact band table planes (u_rows, 64): the K window sits in columns 0..15, a 16-column box of 64 rows
   if ((rc = encode_tmap_bf16_planes(&tu, a->u_hi, a->u_lo, 64, a->u_rows, 1, 64, 0, 64, 16))) return rc;
   // P planes (batch, p_rows, p_ld): frames are the K axis; columns >= p_frames (and < 0) read as zero
@@ -396,7 +398,7 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int tiles = ((a->t + 255) / 256) * 2 * a->batch;
   const int grid = std::min(tiles, sm_count());
-  pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty, p);
+  pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty, ts, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

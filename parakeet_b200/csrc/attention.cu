@@ -43,20 +43,6 @@ struct Args {
   __nv_bfloat16* ctx_lo;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float ra = a - __uint_as_float(hi << 16);
-  const float rb = b - __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
 template <int DK>
 __device__ __forceinline__ void wgmma_rs_o(float (&d)[DK / 2], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   if constexpr (DK == 64) wgmma_rs_n64(d, a, b, acc);
@@ -262,24 +248,20 @@ extern "C" int pk_fused_attention_ex(const PkAttentionArgs* a, pk_stream_t strea
   if ((rc = encode_tmap_bf16_planes(&tv, a->vt_hi, a->vt_lo, a->tp, dk, static_cast<uint64_t>(a->batch) * a->heads, a->tp,
                                     static_cast<uint64_t>(dk) * a->tp, dk)))
     return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    PK_CHECK_CUDA(cudaFuncSetAttribute(fused_attention_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
+  const int dkc = dk / 64;
+  static decltype(&fused_attention_kernel<1>) const kernels[kMaxDkc] = {fused_attention_kernel<1>, fused_attention_kernel<2>,
+                                                                        fused_attention_kernel<3>};
+  const auto kernel = kernels[dkc - 1];
+  if ((rc = prepare_kernel(kernel, kThreads, kSmem))) return rc;
   Args p;
-  p.batch = a->batch; p.t_q = a->t_q; p.t_k = a->t_k; p.heads = a->heads; p.dkc = dk / 64; p.a_dim = a_dim;
+  p.batch = a->batch; p.t_q = a->t_q; p.t_k = a->t_k; p.heads = a->heads; p.dkc = dkc; p.a_dim = a_dim;
   p.q_col0 = a->q_col0; p.k_col0 = a->k_col0; p.causal = a->causal ? 1 : 0;
   p.key_lens = a->key_lens; p.row_lens = a->row_lens;
   p.scale_log2e = a->scale * 1.4426950408889634f;
   p.ctx_hi = static_cast<__nv_bfloat16*>(a->ctx_hi); p.ctx_lo = static_cast<__nv_bfloat16*>(a->ctx_lo);
   dim3 grid((a->t_q + 127) / 128, a->heads, a->batch);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (p.dkc == 1) fused_attention_kernel<1><<<grid, kThreads, kSmem, st>>>(tq, tk, tv, p);
-  else if (p.dkc == 2) fused_attention_kernel<2><<<grid, kThreads, kSmem, st>>>(tq, tk, tv, p);
-  else fused_attention_kernel<3><<<grid, kThreads, kSmem, st>>>(tq, tk, tv, p);
+  kernel<<<grid, kThreads, kSmem, st>>>(tq, tk, tv, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

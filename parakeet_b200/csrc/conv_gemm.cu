@@ -527,11 +527,8 @@ static int launch(const pk_conv_gemm_args* a, cudaStream_t stream, const pk_gemm
     ta_lo = ta_hi;
     tb_lo = tb_hi;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
+  int resident = 0;
+  if ((rc = prepare_kernel(conv_gemm_kernel<BLOCK_N>, kGemmThreads, Cfg::kSmemBytes, &resident))) return rc;
   GemmKernelArgs p = to_kernel_args(a);
   if (e != nullptr) {
     p.epi = e->mode; p.epi_c = e->channels; p.e_res = e->residual; p.e_res_bs = e->residual_batch_stride; p.e_res_ld = e->residual_ld;
@@ -543,7 +540,7 @@ static int launch(const pk_conv_gemm_args* a, cudaStream_t stream, const pk_gemm
   const long long total = static_cast<long long>(p.tiles_m) * ((a->n + BLOCK_N - 1) / BLOCK_N) * a->batch * a->heads;
   PK_CHECK_ARG(total < (1LL << 31), "too many output tiles");
   p.total_tiles = static_cast<int>(total);
-  const int grid = static_cast<int>(std::min<long long>(total, sm_count()));   // persistent: one CTA per SM
+  const int grid = static_cast<int>(std::min<long long>(total, resident));   // persistent: every CTA resident (one per SM)
   conv_gemm_kernel<BLOCK_N><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();

@@ -19,11 +19,6 @@ static inline int nblk(long long n, int threads) { return static_cast<int>(std::
 #define PK_GRID_STRIDE(i, n) \
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); i += static_cast<long long>(gridDim.x) * blockDim.x)
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 // block-wide sum -> one atomicAdd per block (double accumulator: the sums feed loss values and gradient norms)
 __device__ __forceinline__ void block_accumulate(float v, double* out) {
   __shared__ float red[32];

@@ -17,7 +17,6 @@
 #include <stdint.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "pk_host.h"
 #include "pk_sm90.cuh"
@@ -30,14 +29,6 @@ constexpr int kRows = 64;       // rows per tile (the wgmma M)
 constexpr int kThreads = 128;   // one warpgroup
 constexpr int kGroupChunks = 4; // K-chunks of 64 of the backward's dgates tile staged at a time
 
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_inc(unsigned* p) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
-}
 __device__ __forceinline__ void wait_count(const unsigned* flag, unsigned target) {
   const long long t0 = clock64();
   while (ld_acquire_gpu(flag) < target) {
@@ -47,7 +38,6 @@ __device__ __forceinline__ void wait_count(const unsigned* flag, unsigned target
     if (clock64() - t0 > (1ll << 33)) __trap();
   }
 }
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
 __device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
@@ -479,35 +469,18 @@ int schedule(int rows, int slices, int max_ctas, int* groups) {
   return *groups >= 1 ? *groups * slices : 0;
 }
 
-template <class K>
-int max_resident(K kernel, int smem, int* out) {
-  PK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  int n = 0;
-  PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kThreads, smem));
-  *out = n * sm_count();
-  return PK_OK;
-}
-
 template <int H>
 int fwd_launch(const float* g_in, const float* b_hh, const void* w_hi, const void* w_lo, int rows, int T, float* h_all, void* h_hi,
                void* h_lo, float* c, int64_t c_step, float* gates, uint32_t* counters, int64_t counters_len, cudaStream_t st) {
   using G = Geo<H>;
-  static std::mutex mu;
-  static int max_ctas = -1;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (max_ctas < 0) {
-      int rc = max_resident(lstm_fwd_kernel<H>, G::kFwdSmem, &max_ctas);
-      if (rc) { max_ctas = -1; return rc; }
-    }
-  }
+  int max_ctas = 0, rc;
+  if ((rc = prepare_kernel(lstm_fwd_kernel<H>, kThreads, G::kFwdSmem, &max_ctas))) return rc;
   int groups = 0;
   const int grid = schedule(rows, G::kSlices, max_ctas, &groups);
   if (grid == 0) return fail(PK_ERR_UNSUPPORTED, "pk_lstm_fwd: %d slices cannot be co-resident (%d CTAs fit)", G::kSlices, max_ctas);
   const long long n_counters = static_cast<long long>(T) * ((rows + kRows - 1) / kRows);
   PK_CHECK_ARG(counters_len >= n_counters, "counters must hold t * ceil(rows / %d) = %lld entries", kRows, n_counters);
   FwdArgs<H> p;
-  int rc;
   if ((rc = encode_tmap_bf16_planes(&p.tm_w, w_hi, w_lo, H, 4 * H, 1, H, 0, 4 * kSlice))) return rc;
   if ((rc = encode_tmap_bf16_planes(&p.tm_h, h_hi, h_lo, H, rows, T + 1, H, static_cast<uint64_t>(rows) * H, kRows))) return rc;
   p.g_in = g_in; p.b_hh = b_hh; p.h_all = h_all; p.c = c; p.c_step = c_step; p.gates = gates;
@@ -526,22 +499,14 @@ int bwd_launch(const void* wt_hi, const void* wt_lo, const float* gates, const f
                int rows, int T, float* dc, float* dgates, void* dg_hi, void* dg_lo, uint32_t* counters, int64_t counters_len,
                cudaStream_t st) {
   using G = Geo<H>;
-  static std::mutex mu;
-  static int max_ctas = -1;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (max_ctas < 0) {
-      int rc = max_resident(lstm_bwd_kernel<H>, G::kBwdSmem, &max_ctas);
-      if (rc) { max_ctas = -1; return rc; }
-    }
-  }
+  int max_ctas = 0, rc;
+  if ((rc = prepare_kernel(lstm_bwd_kernel<H>, kThreads, G::kBwdSmem, &max_ctas))) return rc;
   int groups = 0;
   const int grid = schedule(rows, G::kSlices, max_ctas, &groups);
   if (grid == 0) return fail(PK_ERR_UNSUPPORTED, "pk_lstm_bwd: %d slices cannot be co-resident (%d CTAs fit)", G::kSlices, max_ctas);
   const long long n_counters = static_cast<long long>(T) * ((rows + kRows - 1) / kRows);
   PK_CHECK_ARG(counters_len >= n_counters, "counters must hold t * ceil(rows / %d) = %lld entries", kRows, n_counters);
   BwdArgs<H> p;
-  int rc;
   if ((rc = encode_tmap_bf16_planes(&p.tm_w, wt_hi, wt_lo, 4 * H, H, 1, 4 * H, 0, kSlice))) return rc;
   if ((rc = encode_tmap_bf16_planes(&p.tm_d, dg_hi, dg_lo, 4 * H, rows, T, 4 * H, static_cast<uint64_t>(rows) * 4 * H, kRows))) return rc;
   p.gates = gates; p.c_all = c_all; p.dh_in = dh_in; p.dh_last = dh_last; p.dc = dc; p.dgates = dgates;
@@ -560,8 +525,6 @@ int bwd_launch(const void* wt_hi, const void* wt_lo, const float* gates, const f
 
 using namespace pk;
 using namespace pk::lstm;
-
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 extern "C" int pk_lstm_fwd(const float* g_in, const float* b_hh, const void* w_hi, const void* w_lo, int32_t rows, int32_t t,
                            int32_t hidden, float* h_all, void* h_hi, void* h_lo, float* c, int64_t c_step, float* gates,

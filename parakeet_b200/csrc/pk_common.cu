@@ -1,9 +1,12 @@
-// Library-wide host plumbing: version, thread-local error string, launch counter, TMA descriptor encoding.
+// Library-wide host plumbing: version, thread-local error string, launch counter, launch setup, TMA descriptor encoding.
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
+#include <mutex>
+#include <vector>
 
 #include "pk_host.h"
 
@@ -40,6 +43,43 @@ int sm_count() {
     cache[dev].store(n, std::memory_order_relaxed);
   }
   return n;
+}
+
+int prepare_kernel(const void* kernel, int threads, size_t smem, int* resident_ctas) {
+  // cudaFuncSetAttribute applies to the current device only, so everything is remembered per device
+  struct Prepared {
+    const void* kernel;
+    int dev, threads;
+    size_t smem;
+    int resident;   // 0: not queried yet
+  };
+  static std::mutex mu;
+  static std::vector<Prepared> prepared;
+  int dev = 0;
+  PK_CHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  Prepared* e = nullptr;
+  size_t limit = 0;   // the kernel's raised limit on this device: never lowered, a larger launch prepared earlier relies on it
+  for (Prepared& x : prepared) {
+    if (x.kernel != kernel || x.dev != dev) continue;
+    limit = std::max(limit, x.smem);
+    if (x.threads == threads && x.smem == smem) e = &x;
+  }
+  if (e == nullptr) {
+    if (smem > limit)
+      PK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    prepared.push_back({kernel, dev, threads, smem, 0});
+    e = &prepared.back();
+  }
+  if (resident_ctas != nullptr) {
+    if (e->resident == 0) {
+      int per_sm = 0;
+      PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+      e->resident = per_sm * sm_count();
+    }
+    *resident_ctas = e->resident;
+  }
+  return PK_OK;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

@@ -5,26 +5,13 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "pk_sm90.cuh"
+
 namespace pk {
 namespace pdec {
 
 constexpr int kThreads = 512;
 constexpr int kWarps = kThreads / 32;
-
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_inc(unsigned* p) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;

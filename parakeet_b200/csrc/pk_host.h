@@ -1,4 +1,4 @@
-// Host-side helpers shared by the C-ABI translation units: error reporting, TMA descriptor encoding.
+// Host-side helpers shared by the C-ABI translation units: error reporting, TMA descriptor encoding, launch setup.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -42,5 +42,31 @@ int encode_tmap_f32_3d(CUtensorMap* out, const void* base, uint64_t rows, uint64
 
 int sm_count();
 void count_launch(int n = 1);
+
+// Readies a kernel for a launch with `threads` threads and `smem` bytes of dynamic shared memory on the current device: raises
+// its dynamic shared-memory limit to cover smem (a CUDA call only the first time the kernel needs more on that device).  With
+// resident_ctas, also returns how many such CTAs the device holds at once (occupancy x SMs, queried once per kernel, device and
+// smem).  Thread-safe; a failed call is not remembered, so the next one tries again.
+int prepare_kernel(const void* kernel, int threads, size_t smem, int* resident_ctas = nullptr);
+template <class... Args>
+int prepare_kernel(void (*kernel)(Args...), int threads, size_t smem, int* resident_ctas = nullptr) {
+  return prepare_kernel(reinterpret_cast<const void*>(kernel), threads, smem, resident_ctas);
+}
+
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// The PWG / WaveFlow gated activation tanh(a + b_a) * sigmoid(g + b_g) runs on ex2: tanh from exp2(kGateKa * a + gate_c[i]),
+// sigmoid from exp2(kGateKg * g + gate_c[64 + i]).  fold_gate_bias fills gate_c from the gate biases bias1 (per 64-channel
+// block: 64 a biases, then 64 g biases) for `channels` residual channels.
+constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kGateKa = -2.f * kLog2e, kGateKg = -kLog2e;
+inline void fold_gate_bias(float* gate_c, const float* bias1, int channels) {
+  for (int blk = 0; blk < channels / 64; ++blk) {
+    for (int i = 0; i < 64; ++i) {
+      gate_c[128 * blk + i] = -2.f * kLog2e * bias1[128 * blk + i];
+      gate_c[128 * blk + 64 + i] = -kLog2e * bias1[128 * blk + 64 + i];
+    }
+  }
+}
 
 }  // namespace pk

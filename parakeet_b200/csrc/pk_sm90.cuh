@@ -1,5 +1,6 @@
 // Device primitives for sm_90a (Hopper): mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with operands in
-// shared memory or, for A, in registers) and its shared-memory descriptors.  Inline PTX only - no CUTLASS dependency.
+// shared memory or, for A, in registers) and its shared-memory descriptors, and the small math, warp-reduction and gpu-scope
+// hand-off helpers the kernel files share.  Inline PTX only - no CUTLASS dependency.
 //
 // Conventions used by every kernel in this library:
 //   * GEMM operands are "split-bf16": a 32-bit value v is stored as two bf16 planes hi = bf16(v), lo = bf16(v - hi)
@@ -167,6 +168,43 @@ __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
   for (int i = 0; i < 8; ++i) split_bf16(v[i], h[i], l[i]);
   hi = make_uint4(pack_bf16x2(h[0], h[1]), pack_bf16x2(h[2], h[3]), pack_bf16x2(h[4], h[5]), pack_bf16x2(h[6], h[7]));
   lo = make_uint4(pack_bf16x2(l[0], l[1]), pack_bf16x2(l[2], l[3]), pack_bf16x2(l[4], l[5]), pack_bf16x2(l[6], l[7]));
+}
+// split two fp32 values into packed bf16x2 hi / lo words (cvt.rn.bf16x2.f32: one instruction per pair)
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  const float ra = a - __uint_as_float(hi << 16);
+  const float rb = b - __uint_as_float(hi & 0xffff0000u);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// ----------------------------------------------------------------------------------------------------------------
+// math, warp reductions, gpu-scope hand-offs
+// ----------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float ex2_approx(float x) {   // MUFU.EX2, 2 ulp; inf for x > 128, 0 for x < -150
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float rcp_approx(float x) {   // MUFU.RCP, 1 ulp; rcp(inf) = 0
+  float y;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_inc(unsigned* p) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(p) : "memory");
 }
 
 

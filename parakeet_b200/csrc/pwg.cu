@@ -67,27 +67,6 @@ struct PwgTileIter {
   }
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {   // MUFU.EX2, 2 ulp; inf for x > 128, 0 for x < -150
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float rcp_approx(float x) {   // MUFU.RCP, 1 ulp; rcp(inf) = 0
-  float y;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// split two fp32 values into packed bf16x2 hi / lo words (cvt.rn.bf16x2.f32: one instruction per pair)
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float ra = a - __uint_as_float(hi << 16);
-  const float rb = b - __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
 __global__ void __launch_bounds__(kPwgThreads, 1)
 pwg_layer_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
                  const __grid_constant__ CUtensorMap tm_c_hi, const __grid_constant__ CUtensorMap tm_c_lo,
@@ -549,26 +528,19 @@ extern "C" int pk_pwg_residual_layer(const pk_pwg_layer_args* a, pk_stream_t str
   if ((rc = encode_tmap_bf16_3d(&tw1_lo, a->w1_lo, k1_valid, kPwgG, 1, k1, k1 * kPwgG, w_box_rows))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, 128, 1, 64, 0, w_box_rows))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, w_box_rows))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPwgSmem));
-    attr_set = true;
-  }
+  int resident = 0;
+  if ((rc = prepare_kernel(pwg_layer_kernel, kPwgThreads, kPwgSmem, &resident))) return rc;
   PwgLayerArgs p;
   p.batch = a->batch; p.t = a->t; p.dil = a->dilation; p.aux_ch = a->aux_channels;
   p.tiles_per_b = (a->t + 127) / 128;
   p.total_tiles = p.tiles_per_b * a->batch;
   p.lens = a->lens; p.skip = a->skip; p.skip_init = a->skip_init;
-  constexpr float kLog2e = 1.4426950408889634f;
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
-  for (int i = 0; i < 64; ++i) {       // host pointers: the biases travel in the kernel's parameter block
-    p.gate_c[i] = -2.f * kLog2e * a->bias1[i];
-    p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
-    p.out_b[i] = a->bias2[64 + i];
-  }
+  p.k_a = kGateKa; p.k_g = kGateKg;
+  fold_gate_bias(p.gate_c, a->bias1, 64);   // host pointers: the biases travel in the kernel's parameter block
+  for (int i = 0; i < 64; ++i) p.out_b[i] = a->bias2[64 + i];
   p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int grid = std::min(p.total_tiles, sm_count());
+  const int grid = std::min(p.total_tiles, resident);
   pwg_layer_kernel<<<grid, kPwgThreads, kPwgSmem, st>>>(tx_hi, tx_lo, tc_hi, tc_lo, tw1_hi, tw1_lo, tw2_hi, tw2_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -604,11 +576,7 @@ extern "C" int pk_pwg_upsample(const float* mel, const float* conv_in_w, const f
     const int kin = 2 * window + 1;
     const size_t cin_smem = (static_cast<size_t>(aux) * kin * (aux + 1) + static_cast<size_t>(aux) * (kCinFrames + kin - 1)) * sizeof(float);
     PK_CHECK_ARG(cin_smem <= 220 * 1024, "conv_in weight does not fit shared memory (%zu bytes)", cin_smem);
-    static size_t cin_attr = 0;
-    if (cin_smem > cin_attr) {
-      PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_conv_in_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cin_smem)));
-      cin_attr = cin_smem;
-    }
+    if (int rc = prepare_kernel(pwg_conv_in_kernel, 320, cin_smem)) return rc;
     dim3 cgrid((frames + kCinFrames - 1) / kCinFrames, batch);
     pwg_conv_in_kernel<<<cgrid, 320, cin_smem, st>>>(mel, conv_in_w, aux, frames, window, conv_in_ws);
     PK_CHECK_CUDA(cudaGetLastError());
@@ -625,11 +593,7 @@ extern "C" int pk_pwg_upsample(const float* mel, const float* conv_in_w, const f
   }
   const size_t smem = floats * sizeof(float);
   PK_CHECK_ARG(smem <= 200 * 1024, "upsample tile does not fit shared memory (%zu bytes)", smem);
-  static size_t attr_smem = 0;
-  if (smem > attr_smem) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_upsample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_smem = smem;
-  }
+  if (int rc = prepare_kernel(pwg_upsample_kernel, 256, smem)) return rc;
   dim3 grid(frames, batch);
   pwg_upsample_kernel<<<grid, 256, smem, st>>>(conv_in_ws, frame_lens, a, c_f32, static_cast<__nv_bfloat16*>(c_hi),
                                                static_cast<__nv_bfloat16*>(c_lo));

@@ -61,25 +61,6 @@ struct FcLayerArgs {
   int skip_init;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float rcp_approx(float x) {
-  float y;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float ra = a - __uint_as_float(hi << 16);
-  const float rb = b - __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
 struct FcTileIter {   // 128-sample tiles = halves of the 256-sample windows; live windows only
   int idx, step, tiles_per_b, total, t;
   const int32_t* lens;
@@ -378,26 +359,19 @@ extern "C" int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* a, pk_stream
   if ((rc = encode_tmap_bf16_3d(&tw1_lo, a->w1_lo, 3 * kChunkK, kPwgG, 1, k1, k1 * kPwgG, 128))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, 128, 1, 64, 0, 128))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, 128, 1, 64, 0, 128))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(pwg_layer_fc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFcSmem));
-    attr_set = true;
-  }
+  int resident = 0;
+  if ((rc = prepare_kernel(pwg_layer_fc_kernel, kThreads, kFcSmem, &resident))) return rc;
   FcLayerArgs p;
   p.batch = a->batch; p.t = a->t; p.dil = a->dilation; p.hop = a->hop;
   p.u_period = a->u_period; p.u_start_row = a->u_start_row; p.u_end_base = a->u_end_base;
   p.p_row0 = a->p_row0;
   p.lens = a->lens; p.skip = a->skip; p.skip_init = a->skip_init;
-  constexpr float kLog2e = 1.4426950408889634f;
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
-  for (int i = 0; i < 64; ++i) {
-    p.gate_c[i] = -2.f * kLog2e * a->bias1[i];
-    p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
-    p.out_b[i] = a->bias2[64 + i];
-  }
+  p.k_a = kGateKa; p.k_g = kGateKg;
+  fold_gate_bias(p.gate_c, a->bias1, 64);
+  for (int i = 0; i < 64; ++i) p.out_b[i] = a->bias2[64 + i];
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int tiles = ((a->t + 255) / 256) * 2 * a->batch;
-  const int grid = std::min(tiles, sm_count());
+  const int grid = std::min(tiles, resident);
   pwg_layer_fc_kernel<<<grid, kThreads, kFcSmem, static_cast<cudaStream_t>(stream)>>>(tx, tu, tp, tw1_hi, tw1_lo, tw2_hi, tw2_lo, ty, ts, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();

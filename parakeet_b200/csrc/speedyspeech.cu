@@ -241,12 +241,11 @@ ss_residual_block_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __gr
   }
 }
 
-static bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
-
 }  // namespace ss
 }  // namespace pk
 
 extern "C" int pk_ss_residual_block(const pk_ss_residual_block_args* a, pk_stream_t stream) {
+  using namespace pk;
   using namespace pk::ss;
   PK_CHECK_ARG(a != nullptr, "args is NULL");
   if (a->channels != kC)
@@ -277,11 +276,7 @@ extern "C" int pk_ss_residual_block(const pk_ss_residual_block_args* a, pk_strea
     tw2_hi = tw1_hi;
     tw2_lo = tw1_lo;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(ss_residual_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    attr_set = true;
-  }
+  if ((rc = prepare_kernel(ss_residual_block_kernel, kThreads, kSmemBytes))) return rc;
   Args p;
   p.t = a->t;
   p.n_convs = a->n_convs;

@@ -128,11 +128,7 @@ extern "C" int pk_stft(const float* x, int32_t batch, int32_t t, const float* wi
   a.mel_w = mel_w; a.n_mels = n_mels; a.mel = mel; a.mel_log10 = mel_log10; a.mel_clip = mel_clip;
   a.energy = energy; a.energy_clip = energy_clip;
   const size_t smem = sizeof(float2) * (n_fft + n_fft / 2) + sizeof(float) * a.bins;
-  static size_t attr = 0;
-  if (smem > attr) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr = smem;
-  }
+  if (int rc = prepare_kernel(stft_kernel, 256, smem)) return rc;
   dim3 grid(a.frames, batch);
   stft_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(a);
   PK_CHECK_CUDA(cudaGetLastError());

@@ -19,8 +19,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <mutex>
-
 #include "pk_host.h"
 #include "pk_decode.cuh"
 #include "pk_sm90.cuh"
@@ -329,21 +327,8 @@ size_t smem_bytes(int bc, int d_enc, int dmr, int loc_k) {
 
 template <int BC>
 int decode_launch(Params& p, cudaStream_t st) {
-  static std::mutex mu;
-  static int max_ctas = -1;
-  static size_t sized_for = 0;
   const size_t smem = smem_bytes(BC, p.d_enc, p.dmr, p.loc_k);
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (max_ctas < 0 || smem > sized_for) {
-      PK_CHECK_CUDA(cudaFuncSetAttribute(taco2_decode_kernel<BC>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-      int n = 0;
-      PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, taco2_decode_kernel<BC>, kThreads, smem));
-      max_ctas = n * sm_count();
-      sized_for = smem;
-    }
-    p.grid = max_ctas;
-  }
+  if (int rc = prepare_kernel(taco2_decode_kernel<BC>, kThreads, smem, &p.grid)) return rc;
   if (p.prof && p.grid > 1024) return fail(PK_ERR_UNSUPPORTED, "pk_taco2_decode: phase timers hold 1024 CTAs (grid %d)", p.grid);
   if (p.grid < kMinGrid)
     return fail(PK_ERR_UNSUPPORTED, "pk_taco2_decode: only %d CTAs can be co-resident (needs %d)", p.grid, kMinGrid);
@@ -464,8 +449,6 @@ loss_kernel(const float* __restrict__ mel, const float* __restrict__ post, const
 
 using namespace pk;
 using namespace pk::taco2;
-
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 extern "C" int64_t pk_taco2_workspace(int32_t batch, int32_t t_enc, int32_t d_enc) { return ws_layout(batch, t_enc, d_enc).total; }
 

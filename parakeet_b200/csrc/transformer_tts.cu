@@ -22,8 +22,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include <mutex>
-
 #include "pk_decode.cuh"
 #include "pk_host.h"
 #include "pk_sm90.cuh"
@@ -389,8 +387,6 @@ size_t smem_bytes(int kmax, int steps, int t_enc, int dk) {
 using namespace pk;
 using namespace pk::tts;
 
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 extern "C" int64_t pk_tts_layer_floats(int32_t adim, int32_t units) { return layer_off(adim, units).total; }
 
 extern "C" int64_t pk_tts_workspace(int32_t adim, int32_t units, int32_t prenet_units, int32_t layers, int32_t steps) {
@@ -437,18 +433,7 @@ extern "C" int pk_tts_decode(const PkTtsDecodeArgs* a, pk_stream_t stream) {
   if (smem > 200 * 1024)
     return fail(PK_ERR_UNSUPPORTED, "pk_tts_decode: max(steps, t_enc) = %d does not fit the attention scores in shared memory",
                 p.steps > p.t_enc ? p.steps : p.t_enc);
-  static std::mutex mu;
-  static int per_sm = -1;
-  static size_t sized_for = 0;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (per_sm < 0 || smem > sized_for) {
-      PK_CHECK_CUDA(cudaFuncSetAttribute(tts_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-      PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tts_decode_kernel, kThreads, smem));
-      sized_for = smem;
-    }
-    p.grid = per_sm * sm_count();
-  }
+  if (int rc = prepare_kernel(tts_decode_kernel, kThreads, smem, &p.grid)) return rc;
   if (p.grid < H)
     return fail(PK_ERR_UNSUPPORTED, "pk_tts_decode: only %d CTAs can be co-resident (needs one per head, %d)", p.grid, H);
   auto st = static_cast<cudaStream_t>(stream);

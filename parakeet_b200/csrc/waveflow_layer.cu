@@ -50,24 +50,6 @@ struct Geo {
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float rcp_approx(float x) {
-  float y;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float ra = a - __uint_as_float(hi << 16);
-  const float rb = b - __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 __device__ __forceinline__ uint32_t ld_cg_u32(const void* ptr) {
   uint32_t v;
   asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
@@ -335,14 +317,6 @@ struct FlowTile {
   }
 };
 
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* ptr) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_gpu_inc(unsigned* ptr) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ptr) : "memory");
-}
 __device__ __forceinline__ void wait_tile_done(const unsigned* flag) {
   const long long t0 = clock64();
   while (ld_acquire_gpu(flag) < kTileDone) {
@@ -654,28 +628,21 @@ extern "C" int pk_waveflow_layer(const pk_waveflow_layer_args* a, pk_stream_t st
   if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, kW1Cols, kG, 1, kW1Cols, 0, kG))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, kG, 1, 64, 0, kG))) return rc;
   if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, kG, 1, 64, 0, kG))) return rc;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem));
-    attr_set = true;
-  }
+  int resident = 0;
+  if ((rc = prepare_kernel(waveflow_layer_kernel, kThreads, G::kSmem, &resident))) return rc;
   LayerArgs p;
   p.batch = a->batch; p.w = a->width; p.dil = a->dilation; p.slot = a->slot;
   p.cond_ksteps_last = (a->n_mels - 64 + kWgmmaK - 1) / kWgmmaK;
   p.tiles_per_b = (a->width + 127) / 128;
   p.total_tiles = p.tiles_per_b * a->batch;
-  constexpr float kLog2e = 1.4426950408889634f;
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
-  for (int i = 0; i < 64; ++i) {
-    p.gate_c[i] = -2.f * kLog2e * a->bias1[i];
-    p.gate_c[64 + i] = -kLog2e * a->bias1[64 + i];
-  }
+  p.k_a = kGateKa; p.k_g = kGateKg;
+  fold_gate_bias(p.gate_c, a->bias1, kC);
   for (int i = 0; i < 128; ++i) p.out_b[i] = a->bias2[i];
   p.skip = a->skip; p.skip_init = a->skip_init;
   p.x_hi = static_cast<const __nv_bfloat16*>(a->buf_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->buf_lo);
   p.y_hi = static_cast<__nv_bfloat16*>(a->next_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->next_lo);
   p.y_ld = 3 * kC; p.y_col0 = a->slot * kC;
-  const int grid = std::min(p.total_tiles, sm_count());
+  const int grid = std::min(p.total_tiles, resident);
   waveflow_layer_kernel<<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tx, tc, tw1, tw2_hi, tw2_lo, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -687,23 +654,14 @@ static int flow_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
   using namespace pk;
   using namespace pk::wf;
   using G = Geo<C>;
+  // every CTA must be resident at once (tiles wait for tiles of other CTAs): ask the driver how many fit
+  int max_ctas = 0, rc;
+  if ((rc = prepare_kernel(waveflow_flow_kernel<C>, kThreads, G::kSmem, &max_ctas))) return rc;
+  PK_CHECK_ARG(max_ctas >= 1, "no resident CTA available for pk_waveflow_flow");
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
-  static int max_ctas = 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PK_CHECK_CUDA(cudaFuncSetAttribute(waveflow_flow_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem));
-    // every CTA must be resident at once (tiles wait for tiles of other CTAs): ask the driver how many fit
-    int n = 0;
-    PK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, waveflow_flow_kernel<C>, kThreads, G::kSmem));
-    PK_CHECK_ARG(n >= 1, "no resident CTA available for pk_waveflow_flow");
-    max_ctas = n * sm_count();
-    attr_set = true;
-  }
   static FlowArgs<C> p;    // up to 22 KB of kernel parameters, built in place under `mu`; the launch copies them
   const uint64_t W = a->width, B = a->batch;
-  int rc;
-  constexpr float kLog2e = 1.4426950408889634f;
   for (int l = 0; l < a->n_layers; ++l) {
     PK_CHECK_ARG(a->ring_hi[l] && a->ring_lo[l] && a->w2_hi[l] && a->w2_lo[l] && a->bias1[l] && a->bias2[l], "NULL entry for layer %d", l);
     if ((rc = encode_tmap_bf16_planes(&p.tm_x[l], a->ring_hi[l], a->ring_lo[l], 3 * C, W, B, 3 * C, W * 3 * C, 128))) return rc;
@@ -714,12 +672,7 @@ static int flow_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
         return rc;
     }
     if ((rc = encode_tmap_bf16_planes(&p.tm_w2[l], a->w2_hi[l], a->w2_lo[l], C, 2 * C, 1, C, 0, 2 * C))) return rc;
-    for (int blk = 0; blk < C / 64; ++blk) {
-      for (int i = 0; i < 64; ++i) {
-        p.gate_c[l][128 * blk + i] = -2.f * kLog2e * a->bias1[l][128 * blk + i];
-        p.gate_c[l][128 * blk + 64 + i] = -kLog2e * a->bias1[l][128 * blk + 64 + i];
-      }
-    }
+    fold_gate_bias(p.gate_c[l], a->bias1[l], C);
     for (int i = 0; i < 2 * C; ++i) p.out_b[l][i] = a->bias2[l][i];
     p.ring_hi[l] = static_cast<__nv_bfloat16*>(a->ring_hi[l]);
     p.ring_lo[l] = static_cast<__nv_bfloat16*>(a->ring_lo[l]);
@@ -739,7 +692,7 @@ static int flow_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {
   }
   for (int i = 0; i < C; ++i) { p.in_w[i] = a->in_w[i]; p.in_b[i] = a->in_b[i]; p.po_w[i] = a->out_w[i]; p.po_w[C + i] = a->out_w[C + i]; }
   p.po_b[0] = a->out_b[0]; p.po_b[1] = a->out_b[1];
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
+  p.k_a = kGateKa; p.k_g = kGateKg;
   p.skip = a->skip; p.z = a->z; p.x = a->x; p.flags = a->flags;
   const int grid = std::max(1, std::min(max_ctas, p.total_tiles));
   waveflow_flow_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(p);
@@ -769,15 +722,10 @@ static int forward_layer_launch(const pk_waveflow_forward_layer_args* a, pk_stre
   using namespace pk;
   using namespace pk::wf;
   using G = Geo<C>;
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(waveflow_forward_layer_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem);
-  });
-  PK_CHECK_CUDA(attr_err);
+  int resident = 0, rc;
+  if ((rc = prepare_kernel(waveflow_forward_layer_kernel<C>, kThreads, G::kSmem, &resident))) return rc;
   const uint64_t W = a->width, B = a->batch, NG = a->n_group;
   CUtensorMap tx, tc, tw1, tw2;
-  int rc;
   if ((rc = encode_tmap_bf16_planes(&tx, a->x_hi, a->x_lo, C, W, B * (NG + 1), C, W * C, 128))) return rc;
   if ((rc = encode_tmap_bf16_planes(&tc, a->cond_hi, a->cond_lo, a->n_mels, W, B * NG, a->n_mels, W * a->n_mels, 128))) return rc;
   if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, G::kG1Chunks * kChunkK, 2 * C, 1, G::kG1Chunks * kChunkK, 0, 2 * C)))
@@ -794,19 +742,13 @@ static int forward_layer_launch(const pk_waveflow_forward_layer_args* a, pk_stre
     PK_CHECK_ARG(a->cond_rows[i] >= 0 && a->cond_rows[i] < a->n_group, "cond_rows[%d] out of range", i);
     p.cmap[i] = a->cond_rows[i];
   }
-  constexpr float kLog2e = 1.4426950408889634f;
-  p.k_a = -2.f * kLog2e; p.k_g = -kLog2e;
-  for (int blk = 0; blk < C / 64; ++blk) {
-    for (int i = 0; i < 64; ++i) {
-      p.gate_c[128 * blk + i] = -2.f * kLog2e * a->bias1[128 * blk + i];
-      p.gate_c[128 * blk + 64 + i] = -kLog2e * a->bias1[128 * blk + 64 + i];
-    }
-  }
+  p.k_a = kGateKa; p.k_g = kGateKg;
+  fold_gate_bias(p.gate_c, a->bias1, C);
   for (int i = 0; i < 2 * C; ++i) p.out_b[i] = a->bias2[i];
   p.skip = a->skip;
   p.x_hi = static_cast<const __nv_bfloat16*>(a->x_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->x_lo);
   p.y_hi = static_cast<__nv_bfloat16*>(a->y_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->y_lo);
-  const int grid = std::min(p.total_tiles, sm_count());
+  const int grid = std::min(p.total_tiles, resident);
   waveflow_forward_layer_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tx, tc, tw1, tw2, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();

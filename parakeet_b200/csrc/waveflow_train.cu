@@ -14,7 +14,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "pk_host.h"
 #include "pk_sm90.cuh"
@@ -26,11 +25,6 @@ static inline int nblk(long long n, int threads) { return static_cast<int>(std::
 #define WFT_GRID_STRIDE(i, n) \
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); i += static_cast<long long>(gridDim.x) * blockDim.x)
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 __device__ __forceinline__ void store_split(float v, __nv_bfloat16* hi, __nv_bfloat16* lo, long long i) {
   __nv_bfloat16 h, l;
   split_bf16(v, h, l);
@@ -455,14 +449,6 @@ __device__ __forceinline__ void mma_rs(float (&d)[C / 2], const uint32_t (&a)[4]
   if constexpr (C == 64) wgmma_rs_n64(d, a, b, acc);
   else wgmma_rs_n128(d, a, b, acc);
 }
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  const float ra = a - __uint_as_float(hi << 16);
-  const float rb = b - __uint_as_float(hi & 0xffff0000u);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(ra, rb);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 
 struct BwdArgs {
   int w, n_group, dil, tiles_per_row, total_tiles, has_gemm1, has_gemm2, dh_ld;
@@ -673,18 +659,13 @@ static int backward_layer_launch(const pk_waveflow_backward_layer_args* a, pk_st
   using namespace pk;
   using namespace pk::wfb;
   using G = Geo<C>;
-  static std::once_flag attr_once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once, [] {
-    attr_err = cudaFuncSetAttribute(waveflow_backward_layer_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::kSmem);
-  });
-  PK_CHECK_CUDA(attr_err);
+  int resident = 0, rc;
+  if ((rc = prepare_kernel(waveflow_backward_layer_kernel<C>, kThreads, G::kSmem, &resident))) return rc;
   const uint64_t W = a->width, Q = static_cast<uint64_t>(a->batch) * (a->n_group + 1);
   CUtensorMap tdh, tw1, tw2;                                   // a map the launch does not use stays zero and is never read
   memset(&tdh, 0, sizeof(tdh));
   memset(&tw1, 0, sizeof(tw1));
   memset(&tw2, 0, sizeof(tw2));
-  int rc;
   if (a->has_gemm1) {
     if ((rc = encode_tmap_bf16_planes(&tdh, a->dh_in_hi, a->dh_in_lo, 2 * C, W, Q + 2, a->dh_ld, W * a->dh_ld, 128))) return rc;
     if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, 18 * C, C, 1, 18 * C, 0, C))) return rc;
@@ -703,7 +684,7 @@ static int backward_layer_launch(const pk_waveflow_backward_layer_args* a, pk_st
   p.a2_hi = static_cast<__nv_bfloat16*>(a->a2_hi); p.a2_lo = static_cast<__nv_bfloat16*>(a->a2_lo);
   p.h = a->h;
   p.dh_hi = static_cast<__nv_bfloat16*>(a->dh_out_hi); p.dh_lo = static_cast<__nv_bfloat16*>(a->dh_out_lo);
-  const int grid = static_cast<int>(std::min<long long>(p.total_tiles, sm_count()));
+  const int grid = std::min(p.total_tiles, resident);
   waveflow_backward_layer_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tdh, tw1, tw2, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();

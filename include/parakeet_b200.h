@@ -9,7 +9,9 @@
  *   - the caller owns every buffer (inputs, outputs, workspaces); the library owns nothing but its code;
  *   - every function returns 0 (PK_OK) or a negative error code, never throws, never aborts, never falls back to
  *     a CPU path; pk_last_error() returns a thread-local message for the last failing call;
- *   - all work is enqueued on the caller's stream; no internal synchronisation unless documented.
+ *   - all work is enqueued on the caller's stream; no internal synchronisation unless documented;
+ *   - parakeet_b200/_lib.py builds its ctypes binding from this file: argument structs are `typedef struct ... { } NAME;`,
+ *     constants `#define PK_* n` or `enum { PK_* = n }`, and every type is one of those its type map lists.
  *
  * Number format of GEMM operands ("split-bf16"): an fp32 tensor v is carried as two bf16 planes
  * hi = bf16(v), lo = bf16(v - hi).  Producers in this library write both planes; pk_split_f32 converts.
@@ -335,14 +337,6 @@ int pk_waveflow_upsample(const float* x, const float* w, const float* bias, int3
 int pk_waveflow_input_proj(const float* x_row, int64_t x_batch_stride, const float* w, const float* bias, int32_t batch,
                            int32_t width, int32_t c, float* state, void* buf_hi, void* buf_lo, int32_t ld, int32_t col0,
                            pk_stream_t stream);
-/* tanh(h[:, :c]) * sigmoid(h[:, c:]) (waveflow.py:280-281, also parallel_wavegan.py:310-311): h fp32 (rows, 2c) ->
- * split planes (rows, c). */
-int pk_gated_activation(const float* h, int64_t rows, int32_t c, void* z_hi, void* z_lo, pk_stream_t stream);
-/* res / skip update of ResidualBlock.add_input (:283-286) + ResidualNet.add_input (:385-392): o fp32 (rows, 2c);
- * state += o[:, :c]; skip = skip_init ? o[:, c:] : skip + o[:, c:]; optional split copy of the new state into the next
- * layer's ring buffer (columns [col0, col0 + c) of a (rows, ld) plane). */
-int pk_waveflow_layer_update(const float* o, int64_t rows, int32_t c, float* state, float* skip, int32_t skip_init, void* buf_hi,
-                             void* buf_lo, int32_t ld, int32_t col0, pk_stream_t stream);
 /* Flow._predict_row_parameters tail + _inverse_transform_row (:496-510): (logs, b) = output_proj(skip) (C -> 2, w [2][C]);
  * x_next[b,w] = (z_row[b,w] - b) * exp(-logs). */
 int pk_waveflow_row_out(const float* skip, const float* w, const float* bias, const float* z_row, int64_t z_batch_stride,

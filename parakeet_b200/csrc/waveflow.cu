@@ -1,6 +1,6 @@
 // WaveFlow inference helpers (reference parakeet/models/waveflow.py): transposed-conv upsampler, and the small
 // row-wise kernels around the per-row residual net whose GEMMs run through pk_conv_gemm:
-//   input_proj (1 -> C), gated activation, residual / skip update, output_proj (C -> 2) + affine inverse of the row;
+//   input_proj (1 -> C), output_proj (C -> 2) + affine inverse of the row;
 // and of the density direction: the tail of Flow.forward (output_proj, transform, log-det, permutation, next input_proj)
 // and WaveFlowLoss.
 #include <algorithm>
@@ -52,41 +52,6 @@ __global__ void wf_input_proj_kernel(const float* __restrict__ x_row, long long 
   split_bf16(v, h, l);
   buf_hi[row * ld + col0 + ch] = h;
   buf_lo[row * ld + col0 + ch] = l;
-}
-
-// z = tanh(h[:, :c]) * sigmoid(h[:, c:])  (rows, 2c) fp32 -> split planes (rows, c)
-__global__ void gate_kernel(const float* __restrict__ h, int c, long long n, __nv_bfloat16* __restrict__ z_hi,
-                            __nv_bfloat16* __restrict__ z_lo) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const int ch = i % c;
-  const long long row = i / c;
-  const float a = h[row * 2 * c + ch], g = h[row * 2 * c + c + ch];
-  const float v = tanhf(a) * (1.f / (1.f + expf(-g)));
-  __nv_bfloat16 hh, ll;
-  split_bf16(v, hh, ll);
-  z_hi[i] = hh;
-  z_lo[i] = ll;
-}
-
-// o (rows, 2c): state += o[:, :c]; skip (+)= o[:, c:]; optional split copy of the new state into the next layer's buffer
-__global__ void wf_layer_update_kernel(const float* __restrict__ o, int c, long long n, float* __restrict__ state,
-                                       float* __restrict__ skip, int skip_init, __nv_bfloat16* __restrict__ buf_hi,
-                                       __nv_bfloat16* __restrict__ buf_lo, int ld, int col0) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const int ch = i % c;
-  const long long row = i / c;
-  const float v = state[i] + o[row * 2 * c + ch];
-  state[i] = v;
-  const float s = o[row * 2 * c + c + ch];
-  skip[i] = skip_init ? s : skip[i] + s;
-  if (buf_hi) {
-    __nv_bfloat16 h, l;
-    split_bf16(v, h, l);
-    buf_hi[row * ld + col0 + ch] = h;
-    buf_lo[row * ld + col0 + ch] = l;
-  }
 }
 
 // (logs, b) = output_proj(skip) (C -> 2); x_next = (z_row - b) * exp(-logs); one warp per (b, w)
@@ -277,28 +242,6 @@ extern "C" int pk_waveflow_input_proj(const float* x_row, int64_t x_batch_stride
   const long long n = static_cast<long long>(batch) * width * c;
   wf_input_proj_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x_row, x_batch_stride, w, bias, width, c, n, state, static_cast<__nv_bfloat16*>(buf_hi), static_cast<__nv_bfloat16*>(buf_lo), ld, col0);
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
-
-extern "C" int pk_gated_activation(const float* h, int64_t rows, int32_t c, void* z_hi, void* z_lo, pk_stream_t stream) {
-  PK_CHECK_ARG(h && z_hi && z_lo && rows > 0 && c > 0, "bad arguments");
-  const long long n = rows * c;
-  gate_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(h, c, n, static_cast<__nv_bfloat16*>(z_hi),
-                                                                              static_cast<__nv_bfloat16*>(z_lo));
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
-
-extern "C" int pk_waveflow_layer_update(const float* o, int64_t rows, int32_t c, float* state, float* skip, int32_t skip_init,
-                                        void* buf_hi, void* buf_lo, int32_t ld, int32_t col0, pk_stream_t stream) {
-  PK_CHECK_ARG(o && state && skip && rows > 0 && c > 0, "bad arguments");
-  PK_CHECK_ARG((buf_hi == nullptr) == (buf_lo == nullptr), "buf_hi and buf_lo must both be set or both NULL");
-  const long long n = rows * c;
-  wf_layer_update_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      o, c, n, state, skip, skip_init, static_cast<__nv_bfloat16*>(buf_hi), static_cast<__nv_bfloat16*>(buf_lo), ld, col0);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

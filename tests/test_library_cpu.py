@@ -1,6 +1,9 @@
 """CPU tests: the C-ABI library loads and exports everything the header declares; host-side logic."""
 import ctypes
 import os
+import re
+import shutil
+import subprocess
 
 import numpy as np
 import pytest
@@ -97,17 +100,33 @@ def test_polyphase_table_equals_stretch_then_fir():
         assert np.allclose(out, ref, atol=1e-5)
 
 
-def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
-    """include/parakeet_b200.h must compile as C (it is what a cgo / ctypes / cffi binding consumes) and the ctypes mirrors in
-    parakeet_b200/_lib.py must have the C compiler's field offsets and sizes."""
-    import shutil
-    import subprocess
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _gcc():
     gcc = shutil.which("gcc")
     if gcc is None:
         pytest.skip("no C compiler")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    mirrors = {"pk_operand": _lib.Operand, "pk_conv_gemm_args": _lib.ConvGemmArgs, "pk_pwg_layer_args": _lib.PwgLayerArgs,
-               "pk_gemm_epilogue": _lib.GemmEpilogue, "pk_pwg_layer_fc_args": _lib.PwgLayerFcArgs}
+    return gcc
+
+
+def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
+    """include/parakeet_b200.h must compile as C (it is what a cgo / ctypes / cffi binding consumes) and every struct it declares
+    must be bound by parakeet_b200/_lib.py, under its mechanical class name, with the C compiler's field offsets and sizes."""
+    gcc = _gcc()
+    mirrors = _lib.STRUCTS
+    # the parse misses no struct: count the `struct` keywords of the header with its comments stripped by the compiler
+    bare = subprocess.run([gcc, "-fpreprocessed", "-dD", "-E", "-P", os.path.join(ROOT, "include", "parakeet_b200.h")],
+                          check=True, capture_output=True, text=True).stdout
+    assert len(re.findall(r"\bstruct\b", bare)) == len(mirrors)
+    names = {"pk_operand": "Operand", "pk_conv_gemm_args": "ConvGemmArgs", "pk_gemm_epilogue": "GemmEpilogue",
+             "pk_pwg_layer_args": "PwgLayerArgs", "pk_pwg_layer_fc_args": "PwgLayerFcArgs", "PkAttentionArgs": "AttentionArgs",
+             "pk_waveflow_layer_args": "WaveflowLayerArgs", "pk_waveflow_flow_args": "WaveflowFlowArgs",
+             "pk_waveflow_forward_layer_args": "WaveflowForwardLayerArgs", "pk_waveflow_forward_tail_args": "WaveflowForwardTailArgs",
+             "pk_ss_residual_block_args": "SsResidualBlockArgs", "pk_waveflow_backward_layer_args": "WaveflowBackwardLayerArgs",
+             "PkTaco2DecodeArgs": "Taco2DecodeArgs", "PkTtsDecodeArgs": "TtsDecodeArgs"}
+    for cname, pyname in names.items():
+        assert mirrors[cname] is getattr(_lib, pyname), (cname, pyname)
     lines = ['#include <stddef.h>', '#include <stdio.h>', '#include "parakeet_b200.h"', "int main(void) {"]
     for cname, cls in mirrors.items():
         lines.append(f'  printf("{cname} size %zu\\n", sizeof({cname}));')
@@ -117,7 +136,7 @@ def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
     src = tmp_path / "layout.c"
     src.write_text("\n".join(lines))
     exe = tmp_path / "layout"
-    subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(root, "include"), str(src), "-o", str(exe)], check=True)
+    subprocess.run([gcc, "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout
     seen = 0
     for line in out.splitlines():
@@ -127,3 +146,43 @@ def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
         assert int(value) == expect, (cname, field, value, expect)
         seen += 1
     assert seen == sum(len(c._fields_) + 1 for c in mirrors.values())
+
+
+_C_NAMES = {ctypes.c_int32: "int32_t", ctypes.c_int64: "int64_t", ctypes.c_uint32: "uint32_t", ctypes.c_uint64: "uint64_t",
+            ctypes.c_float: "float", ctypes.c_char_p: "const char*"}
+
+
+def test_bound_signatures_match_the_header(tmp_path):
+    """Every entry point's restype and argtypes, as lib() binds them, are rebuilt as a C function pointer type to which the
+    header's function must be assignable under -Werror: a missing, extra or differently typed parameter or return fails to
+    compile.  ctypes binds every pointer as a pointer, so a bound pointer is rebuilt with the header's spelling at its
+    position when the header has a pointer there, and as void* (which no scalar accepts) when it has not."""
+    gcc = _gcc()
+    L = _lib.lib()
+    lines = ['#include "parakeet_b200.h"']
+    for name, proto in _lib.PROTOTYPES.items():
+        fn = getattr(L, name)
+        spelled = [re.sub(r"\s*\w+$", "", p) for p in proto.params]        # the header's types without parameter names
+        params = []
+        for i, t in enumerate(fn.argtypes or []):
+            if t is ctypes.c_void_p or issubclass(t, ctypes._Pointer):
+                is_ptr = i < len(spelled) and ("*" in spelled[i] or spelled[i] == "pk_stream_t")
+                params.append(spelled[i] if is_ptr else "void*")
+            else:
+                params.append(_C_NAMES[t])
+        lines.append(f"{_C_NAMES[fn.restype]} (*fp_{name})({', '.join(params) or 'void'}) = {name};")
+    src = tmp_path / "signatures.c"
+    src.write_text("\n".join(lines) + "\n")
+    r = subprocess.run([gcc, "-std=c99", "-Werror", "-Wincompatible-pointer-types", "-I", os.path.join(ROOT, "include"), "-c",
+                        str(src), "-o", str(tmp_path / "signatures.o")], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    assert len(_lib.PROTOTYPES) == len(_lib.exported_symbols()) >= 100
+
+
+def test_header_parse_refuses_unknown_types():
+    with pytest.raises(_lib.PkError, match="pk_x"):
+        _lib.parse_header("typedef void* pk_stream_t;\nint pk_x(size_t n, pk_stream_t stream);\n")
+    with pytest.raises(_lib.PkError, match="pk_y_args"):
+        _lib.parse_header("typedef struct pk_y_args { int32_t n; double scale; } pk_y_args;\n")
+    with pytest.raises(_lib.PkError, match="pk_z"):
+        _lib.parse_header("size_t pk_z(void);\n")

@@ -202,7 +202,17 @@ int pk_pwg_residual_layer(const pk_pwg_layer_args* args, pk_stream_t stream);
  *   p_hi / p_lo: P as split planes (batch, p_rows, p_ld), one allocation, frames along the last axis (p_frames valid
  *                columns, zeros up to p_ld >= 64); this layer's 128 output channels are rows [p_row0, p_row0 + 128).
  * x / y planes: one allocation each (lo after hi) so that a tile of both planes is ONE 4-D TMA box.
- * w1 / w2 / bias1 / bias2 / skip / lens as in pk_pwg_layer_args (the aux columns of w1 are not read).  hop >= 256. */
+ * w1 / w2 / bias1 / bias2 / skip / lens as in pk_pwg_layer_args (the aux columns of w1 are not read).  hop >= 256.
+ *
+ * The ends of the stack (at most one of noise / out is set; both NULL: a middle layer):
+ *   FIRST LAYER (noise != NULL): x = first_conv(noise) = first_w * noise[b, t] + first_b is computed in place, never read
+ *     from memory (x_hi / x_lo must be NULL) - its rows t >= lens[b] are zero as in pk_pwg_first_conv.  first_u / first_v
+ *     [3][128] hold W1_tap . first_w and W1_tap . first_b per tap (the conv of x collapses to rank one per tap).
+ *   LAST LAYER (out != NULL, skip_init == 0): instead of accumulating into skip, the epilogue applies pk_pwg_tail to
+ *     skip + this layer's skip branch and writes out (batch, t) fp32; skip is read, not written.  y is written as usual.
+ *     Rows t >= lens[b] of live tiles get 0; the tiles wholly past lens[b] do not write out at all.
+ *     tail_w1_hi / lo: last_conv_layers.1 [64 out][64 in] split planes (16-byte aligned); tail_b1 [64], tail_w2 [64],
+ *     tail_b2 [1], skip_bias [64] (the sum of all layers' conv1x1_skip biases) are HOST arrays; tail_scale = sqrt(1/layers). */
 typedef struct pk_pwg_layer_fc_args {
   int32_t batch, t, dilation, hop;
   const int32_t* lens;
@@ -224,6 +234,19 @@ typedef struct pk_pwg_layer_fc_args {
   const float* bias2;
   float* skip;
   int32_t skip_init;
+  const float* noise;      /* first layer: device fp32 (batch, t), or NULL */
+  const float* first_w;    /* HOST [64] */
+  const float* first_b;    /* HOST [64] */
+  const float* first_u;    /* HOST [3][128] */
+  const float* first_v;    /* HOST [3][128] */
+  float* out;              /* last layer: device fp32 (batch, t), or NULL */
+  const void* tail_w1_hi;
+  const void* tail_w1_lo;
+  const float* tail_b1;    /* HOST [64] */
+  const float* tail_w2;    /* HOST [64] */
+  const float* tail_b2;    /* HOST [1] */
+  const float* skip_bias;  /* HOST [64] */
+  float tail_scale;
 } pk_pwg_layer_fc_args;
 int pk_pwg_residual_layer_fc(const pk_pwg_layer_fc_args* args, pk_stream_t stream);
 

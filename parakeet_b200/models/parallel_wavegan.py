@@ -181,6 +181,17 @@ class PWGGenerator(Layer):
         pk["tail_b1"] = p["last_conv_layers.1.bias"].contiguous().to(dev)
         pk["tail_w2"] = p["last_conv_layers.3.weight"].reshape(-1).contiguous().to(dev)
         pk["tail_b2"] = p["last_conv_layers.3.bias"].contiguous().to(dev)
+        # the ends of the frame-rate stack (pk_pwg_layer_fc_args): layer 0 computes first_conv itself, from HOST vectors of
+        # first_conv and of W1_tap . w, W1_tap . b per tap (float64 here); the last layer runs the tail, on the split planes
+        # of last_conv_layers.1 and HOST copies of the tail vectors
+        fw, fb = p["first_conv.weight"].reshape(-1).double(), p["first_conv.bias"].double()
+        w0 = p["conv_layers.0.conv.weight"].double()                                   # [128, 64, 3]
+        host = lambda t: np.ascontiguousarray(t.numpy(), dtype=np.float32)  # noqa: E731
+        pk["first_host"] = dict(w=host(fw), b=host(fb), u=host(torch.einsum("oik,i->ko", w0, fw)),
+                                v=host(torch.einsum("oik,i->ko", w0, fb)))
+        pk["tail_host"] = dict(w1=_split_host(pk["tail_w1"].cpu(), dev), b1=host(pk["tail_b1"].cpu()),
+                               w2=host(pk["tail_w2"].cpu()), b2=host(pk["tail_b2"].cpu()),
+                               skip_bias=host(pk["skip_bias_sum"].cpu()))
         self._packed = pk
         return pk
 
@@ -268,14 +279,17 @@ class PWGGenerator(Layer):
                                      self.aux_channels, frames, self.aux_context_window, _ptr(frame_lens), _ptr(ws["conv_in"]),
                                      None, _ptr(ws["c"].hi) if not fcond else None, _ptr(ws["c"].lo) if not fcond else None, st),
                    "pk_pwg_upsample")
-        _lib.check(L.pk_pwg_first_conv(_ptr(x), _ptr(pk["first_w"]), _ptr(pk["first_b"]), lens_p, B, T, _ptr(ws["xa"].hi),
-                                       _ptr(ws["xa"].lo), st), "pk_pwg_first_conv")
         if lens is not None:
             ws["xb"].hi.zero_()
             ws["xb"].lo.zero_()
         src, dst = ws["xa"], ws["xb"]
         if fcond:
-            return self._forward_frame_cond(pk, ws, src, dst, B, T, frames, lens, frame_lens, st, lens_key)
+            if lens is not None:   # the layers skip tiles wholly past an utterance's end: their rows stay zero in both planes
+                ws["xa"].hi.zero_()
+                ws["xa"].lo.zero_()
+            return self._forward_frame_cond(pk, ws, x, src, dst, B, T, frames, lens, frame_lens, st, lens_key)
+        _lib.check(L.pk_pwg_first_conv(_ptr(x), _ptr(pk["first_w"]), _ptr(pk["first_b"]), lens_p, B, T, _ptr(ws["xa"].hi),
+                                       _ptr(ws["xa"].lo), st), "pk_pwg_first_conv")
         args = PwgLayerArgs()
         args.batch, args.t, args.aux_channels = B, T, self.aux_channels
         args.lens = lens.data_ptr() if lens is not None else None
@@ -305,10 +319,12 @@ class PWGGenerator(Layer):
         self._last_x = src  # layer-30 residual stream (tests)
         return out
 
-    def _forward_frame_cond(self, pk, ws, src, dst, B, T, frames, lens, frame_lens, st, lens_key=None):
+    def _forward_frame_cond(self, pk, ws, x, src, dst, B, T, frames, lens, frame_lens, st, lens_key=None):
         """Residual stack with frame-rate conditioning (DESIGN.md 5, csrc/pwg_fc.cu): conv1x1_aux of all 30 layers is applied
         to conv_in(mel) at frame rate by ONE GEMM per forward (P), and each layer multiplies the band table of the (linear,
-        per-channel) upsampling operator with the 16-frame window of P its tile touches - no sample-rate conditioning tensor."""
+        per-channel) upsampling operator with the 16-frame window of P its tile touches - no sample-rate conditioning tensor.
+        Layer 0 computes first_conv(x) itself and the last layer runs the tail into `out`, so neither x0 nor the final skip
+        sum goes through memory (a one-layer stack keeps pk_pwg_tail)."""
         from . import _pwg_frame_cond as fc
         L = _lib.lib()
         hop, A, NL = self.upsample_factor, self.aux_channels, self.layers
@@ -357,25 +373,35 @@ class PWGGenerator(Layer):
         args.u_period, args.u_start_row, args.u_end_base = lay["period"], lay["start_row"], lay["end_base"]
         args.p_hi, args.p_lo, args.p_rows, args.p_ld, args.p_frames = P.hi.data_ptr(), P.lo.data_ptr(), NL * 128, Fp, frames
         args.skip = ws["skip"].data_ptr()
+        out = torch.empty(B, 1, T, dtype=torch.float32, device=self.device)
+        fh, th = pk["first_host"], pk["tail_host"]
+        args.first_w, args.first_b, args.first_u, args.first_v = fh["w"].ctypes.data, fh["b"].ctypes.data, fh["u"].ctypes.data, fh["v"].ctypes.data
+        args.tail_w1_hi, args.tail_w1_lo = th["w1"].hi.data_ptr(), th["w1"].lo.data_ptr()
+        args.tail_b1, args.tail_w2, args.tail_b2 = th["b1"].ctypes.data, th["w2"].ctypes.data, th["b2"].ctypes.data
+        args.skip_bias, args.tail_scale = th["skip_bias"].ctypes.data, math.sqrt(1.0 / NL)
         ev = getattr(self, "_layer_events", None)
         if ev is not None:   # bench.py: CUDA events around the 30 residual-layer launches, on the launching stream
             ev_a, ev_b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             ev_a.record()
         for i, lay_ in enumerate(pk["layers"]):
+            first, last = i == 0, i == NL - 1 and i > 0
             args.dilation, args.p_row0 = lay_["dil"], i * 128
-            args.x_hi, args.x_lo, args.y_hi, args.y_lo = src.hi.data_ptr(), src.lo.data_ptr(), dst.hi.data_ptr(), dst.lo.data_ptr()
+            args.noise = x.data_ptr() if first else None
+            args.out = out.data_ptr() if last else None
+            args.x_hi, args.x_lo = (None, None) if first else (src.hi.data_ptr(), src.lo.data_ptr())
+            args.y_hi, args.y_lo = dst.hi.data_ptr(), dst.lo.data_ptr()
             args.w1_hi, args.w1_lo = lay_["w1"].hi.data_ptr(), lay_["w1"].lo.data_ptr()
             args.w2_hi, args.w2_lo = lay_["w2"].hi.data_ptr(), lay_["w2"].lo.data_ptr()
             args.bias1, args.bias2 = lay_["b1"].ctypes.data, lay_["b2"].ctypes.data
-            args.skip_init = 1 if i == 0 else 0
+            args.skip_init = 1 if first else 0
             _lib.check(L.pk_pwg_residual_layer_fc(C.byref(args), st), "pk_pwg_residual_layer_fc")
             src, dst = dst, src
         if ev is not None:
             ev_b.record()
             ev.append((ev_a, ev_b))
-        out = torch.empty(B, 1, T, dtype=torch.float32, device=self.device)
-        _lib.check(L.pk_pwg_tail(_ptr(ws["skip"]), _ptr(pk["skip_bias_sum"]), _ptr(pk["tail_w1"]), _ptr(pk["tail_b1"]), _ptr(pk["tail_w2"]),
-                                 _ptr(pk["tail_b2"]), math.sqrt(1.0 / self.layers), B * T, _ptr(out), st), "pk_pwg_tail")
+        if NL == 1:
+            _lib.check(L.pk_pwg_tail(_ptr(ws["skip"]), _ptr(pk["skip_bias_sum"]), _ptr(pk["tail_w1"]), _ptr(pk["tail_b1"]),
+                                     _ptr(pk["tail_w2"]), _ptr(pk["tail_b2"]), 1.0, B * T, _ptr(out), st), "pk_pwg_tail")
         if lens is not None:
             ops.mask_rows_(out.reshape(B, T, 1), lens)       # samples past an utterance's end: zero, not tail(bias)
         self._last_x = src

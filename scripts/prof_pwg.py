@@ -15,6 +15,8 @@ samples per step) goes, and A/B runs of bench.py across source trees.
 Shares: HBM = 1 024 B/sample per layer (x read 256, y write 256, skip read-modify-write 512) over the layer time, against
 3.35 TB/s; tensor = 208 896 executed FLOP/sample per layer over the layer time (51 wgmma m64n128k16 per 64 rows: GEMM1 3 taps x 4 K-steps + 1 conditioning K-step, GEMM2 4 K-steps,
 split-bf16, 3 passes each), against 989 TFLOP/s (data-sheet dense bf16 at 700 W; a card with a lower power limit clocks lower).
+Both are a middle layer's: the layer time is the mean over the 30 launches, and the first layer (no x read, a skip store: 512 B/sample,
+15 wgmma per 64 rows) and the last (no skip write, the tail on top: 768 B/sample) move less, so the shares slightly understate a middle layer's.
 """
 import argparse
 import json

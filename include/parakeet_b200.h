@@ -189,10 +189,10 @@ typedef struct pk_pwg_layer_args {
 } pk_pwg_layer_args;
 int pk_pwg_residual_layer(const pk_pwg_layer_args* args, pk_stream_t stream);
 
-/* ResidualBlock with FRAME-RATE CONDITIONING (the default residual-stack path of the Python model; PK_PWG_FRAME_COND=0
- * selects pk_pwg_residual_layer).  The upsampling network is linear and per channel, so conv1x1_aux(upsample(m'))[t, n] =
- * sum_j U[t, j] * P[j, n] with P = conv1x1_aux applied to m' = conv_in(mel) at FRAME rate.  Instead of the sample-rate
- * conditioning planes (1.2 GB at cfg 2) the kernel takes
+/* ResidualBlock with FRAME-RATE CONDITIONING (the residual-stack path of the Python model wherever the compact band tables
+ * are exact; other upsample scales run pk_pwg_residual_layer).  The upsampling network is linear and per channel, so
+ * conv1x1_aux(upsample(m'))[t, n] = sum_j U[t, j] * P[j, n] with P = conv1x1_aux applied to m' = conv_in(mel) at FRAME
+ * rate.  Instead of the sample-rate conditioning planes (1.2 GB at cfg 2) the kernel takes
  *   u_hi / u_lo: the COMPACT band table of U as split planes (u_rows, 64) from ONE allocation (lo after hi): a row holds
  *                U[t, j0 + k] in column k < 16 (zeros after), j0 = floor8(((t / 256) * 256) / hop - 2) (the K window of
  *                the 256-sample pair tile of t).  Rows [0, u_period): interior rows by t mod u_period; rows
@@ -345,10 +345,11 @@ int pk_stft(const float* x, int32_t batch, int32_t t, const float* window, const
 int pk_spectral_loss_sums(const float* x_mag, const float* y_mag, int64_t n, float eps, float* out3, pk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * WaveFlow inference (reference: parakeet/models/waveflow.py).  The per-row residual net of Flow.inverse (:515-556,
- * ResidualBlock.add_input :248-294) runs its three GEMMs per layer through pk_conv_gemm on a channels-last row
- * (batch, W, C): the 3-row causal buffer is a (batch, W, 3C) split-bf16 ring (slot = row mod 3) convolved along W with
- * 3 dilated taps and K = 3C; the kernels below are the row-wise glue.
+ * WaveFlow inference (reference: parakeet/models/waveflow.py).  For configs outside the range of pk_waveflow_flow (below),
+ * the per-row residual net of Flow.inverse (:515-556, ResidualBlock.add_input :248-294) runs its GEMMs per layer through
+ * pk_conv_gemm_ex on a channels-last row (batch, W, C): the 3-row causal buffer is a (batch, W, 3C) split-bf16 ring
+ * (slot = row mod 3) convolved along W with 3 dilated taps and K = 3C; the kernels below are that path's row-wise glue
+ * (pk_waveflow_input_proj also writes row 0 for pk_waveflow_flow).
  * ------------------------------------------------------------------------------------------------------------ */
 /* One layer of waveflow.UpsampleNet.forward (:103-132): Conv2DTranspose(1,1,(3,2f),stride (1,f),padding (1,f/2)) over
  * (mel, time), trim of the last f columns if trim != 0, leaky_relu(slope).  x (batch, c, t_in) -> y (batch, c,
@@ -365,48 +366,24 @@ int pk_waveflow_input_proj(const float* x_row, int64_t x_batch_stride, const flo
 int pk_waveflow_row_out(const float* skip, const float* w, const float* bias, const float* z_row, int64_t z_batch_stride,
                         int32_t batch, int32_t width, int32_t c, float* x_next, int64_t x_batch_stride, pk_stream_t stream);
 
-/* One whole ResidualBlock.add_input (:248-285) as ONE kernel (channels == 64; the default layer path of
- * ConditionalWaveFlow.inverse, PK_WF_FUSED=0 selects the pk_conv_gemm_ex pair above):
+/* All row steps i = 1 .. n_group-1 of one Flow.inverse (:515-556) in ONE persistent dataflow launch (ConditionalWaveFlow.inverse
+ * for 64 and 128 channels, 64 < n_mels <= 128 and at most 8 layers per flow).  Per row step, n_layers times
+ * ResidualBlock.add_input (:248-285):
  *   a | g = conv2d(3-row ring, dilation (1, 2^l)) + condition_proj(condition row) + bias1;  z = tanh(a) sigmoid(g);
- *   skip | res = out_proj(z) + bias2;  skip accumulator (=|+=) skip;  ring slot `slot` of the NEXT layer <- row + res.
- * buf planes (batch, width, 192) hold this layer's ring (slot s in columns [64 s, 64 s + 64)); `slot` is the newest row's slot
- * (the residual input).  cond planes: the condition row (batch, width, n_mels), batch stride cond_batch_stride elements.
- * Every pair of planes comes from ONE allocation (lo after hi).
- * w1 planes (128, 704): row n = gate channel (a: 0..63, g: 64..127); columns [192 tap + 64 s + c] = conv.weight[n, c, kh(s), tap]
- * for the ring slot s holding kernel row kh(s) at this row step, columns [576 + m] = condition_proj.weight[n, m] (zeros from
- * n_mels to 128).  w2 planes (128, 64): out_proj.weight with rows reordered to skip (0..63) | res (64..127).
- * bias1 / bias2: HOST pointers [128] (conv.bias + condition_proj.bias; out_proj.bias as skip | res), copied into the kernel
- * parameter block.  next_hi / next_lo: the next layer's ring planes, or NULL (last layer).  skip fp32 (batch, width, 64). */
-typedef struct pk_waveflow_layer_args {
-  int32_t batch, width, channels, n_mels, dilation, slot;
-  const void* buf_hi;
-  const void* buf_lo;
-  const void* cond_hi;
-  const void* cond_lo;
-  int64_t cond_batch_stride;
-  const void* w1_hi;
-  const void* w1_lo;
-  const void* w2_hi;
-  const void* w2_lo;
-  const float* bias1;
-  const float* bias2;
-  void* next_hi;
-  void* next_lo;
-  float* skip;
-  int32_t skip_init;
-} pk_waveflow_layer_args;
-int pk_waveflow_layer(const pk_waveflow_layer_args* args, pk_stream_t stream);
-
-/* All row steps i = 1 .. n_group-1 of one Flow.inverse (:515-556) in ONE persistent dataflow launch (the default path of
- * ConditionalWaveFlow.inverse for 64 and 128 channels; PK_WF_FUSED=layer selects one pk_waveflow_layer launch per layer and row).
- * Per row step: the n_layers ResidualBlock.add_input of pk_waveflow_layer, then on the completed skip sum
- * (logs, b) = output_proj(skip), x[:, i] = (z[:, i] - b) exp(-logs) (:496-510) and input_proj(x[:, i]) (:437-442) into the
- * first layer's ring slot i mod 3.  The caller provides row 0: x[:, 0] = z[:, 0], input_proj(x[:, 0]) in slot 0 of ring 0
- * (pk_waveflow_input_proj), all other ring contents zero, and `flags` (one uint32 per tile: (n_group - 1) * n_layers *
- * batch * ceil(width / 256)) zeroed.  z / x: fp32 (batch, n_group, width).  cond planes (batch, n_group, width, n_mels);
- * cond_rows[i] (HOST) = the condition row used at row step i.  ring / w1 / w2 / bias1 / bias2: HOST arrays indexed by layer
- * (w1: 3 * layer + variant, variant = i mod 3) of the per-layer pointers of pk_waveflow_layer_args (biases: HOST floats).
- * in_w / in_b [channels], out_w [2][channels], out_b [2]: HOST floats.
+ *   skip | res = out_proj(z) + bias2;  skip accumulator (=|+=) skip;  the next layer's ring slot (i - 1) mod 3 <- row + res,
+ * with the newest row (i - 1) as the residual input; then on the completed skip sum (logs, b) = output_proj(skip),
+ * x[:, i] = (z[:, i] - b) exp(-logs) (:496-510) and input_proj(x[:, i]) (:437-442) into the first layer's ring slot i mod 3.
+ * The caller provides row 0: x[:, 0] = z[:, 0], input_proj(x[:, 0]) in slot 0 of ring 0 (pk_waveflow_input_proj), all other
+ * ring contents zero, and `flags` (one uint32 per tile: (n_group - 1) * n_layers * batch * ceil(width / 256)) zeroed.
+ * z / x: fp32 (batch, n_group, width).  cond planes (batch, n_group, width, n_mels); cond_rows[i] (HOST) = the condition row
+ * used at row step i.  ring / w1 / w2: HOST arrays indexed by layer (w1: 3 * layer + variant, variant = i mod 3) of device
+ * split planes, each pair of planes from ONE allocation (lo after hi); bias1 / bias2: HOST arrays indexed by layer of HOST
+ * float vectors, copied into the kernel parameter block.  in_w / in_b [channels], out_w [2][channels], out_b [2]: HOST floats.
+ * channels == 64: ring planes (batch, width, 192) with slot s in columns [64 s, 64 s + 64); w1 planes (128, 704): row n = gate
+ * channel (a: 0..63, g: 64..127); columns [192 tap + 64 s + c] = conv.weight[n, c, kh(s), tap] for the ring slot s holding
+ * kernel row kh(s) at this row step, columns [576 + m] = condition_proj.weight[n, m] (zeros from n_mels to 128); w2 planes
+ * (128, 64): out_proj.weight with rows reordered to skip (0..63) | res (64..127); bias1 [128] = conv.bias + condition_proj.bias,
+ * bias2 [128] = out_proj.bias as skip | res; skip fp32 (batch, width, 64).
  * channels == 128 (examples/waveflow/config.py) runs the same dataflow with the channels as two blocks of 64: ring planes
  * (batch, width, 384) with slot s in columns [128 s, 128 s + 128); w1 planes (256, 1280): rows a0 | g0 | a1 | g1 (64 each: gate
  * channel a_k = conv output 64 k + c, g_k = 128 + 64 k + c), columns [128 (3 tap + s) + c] conv, [1152 + m] condition_proj;

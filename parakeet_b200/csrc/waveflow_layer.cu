@@ -1,21 +1,21 @@
-// pk_waveflow_layer: one ResidualBlock.add_input of the WaveFlow inverse (reference parakeet/models/waveflow.py:248-285) as
-// ONE kernel - the row-by-row autoregressive path spends its time here (8 flows x 15 rows x 8 layers launches).
+// The fused WaveFlow residual blocks (reference parakeet/models/waveflow.py) for 64 or 128 residual channels:
+// pk_waveflow_flow runs all row steps x layers of one Flow.inverse in one persistent launch, pk_waveflow_forward_layer one
+// ResidualBlock.forward of Flow.forward over all net rows.  Both compute, per 128-position tile, in consume_tile:
 //
-//   a | g   = conv2d(ring of the last 3 rows, dilation 2^l along the width) + condition_proj(condition row) + biases
+//   a | g   = conv2d(3 rows, dilation 2^l along the width) + condition_proj(condition row) + biases
 //   z       = tanh(a) * sigmoid(g)
-//   res|skip= out_proj(z);   new row = row + res  -> next layer's ring slot (split planes);   skip (=|+=) skip
+//   res|skip= out_proj(z);   new row = row + res  -> the next layer's input (split planes);   skip (=|+=) skip
 //
-// It replaces, per layer, two pk_conv_gemm_ex launches (gate epilogue, wf_update epilogue), one fp32 read of the hoisted
-// condition projections (2C floats per position) and the fp32 state read-modify-write.  Structure (shared with
-// pk_waveflow_flow below and with pwg.cu):
+// Structure:
 //   * persistent CTAs over 128-position tiles, 384 threads: a producer warpgroup (one TMA lane) and two consumer warpgroups
 //     of 64 positions each;
-//   * GEMM1 has 11 K-chunks: 3 width taps x 3 ring slots of 64 channels + the 80 condition channels (64 + 16); every stage
-//     of a 2-deep ring carries the A chunk (32 KB: hi | lo) and the weight chunk for all 128 gate channels (32 KB), and
-//     out_proj follows as one more weight-only chunk;
+//   * GEMM1 has 9 C/64 + 2 K-chunks: 3 width taps x 3 rows x C/64 channel blocks + the n_mels condition channels (64 + 64);
+//     every stage of a 2-deep ring carries the A chunk (32 KB: hi | lo) and the weight chunk for all 2C gate channels, and
+//     out_proj follows as C/64 weight-only chunks;
 //   * the accumulators live in registers (wgmma), the gate runs on them in place and z is GEMM2's register A operand;
-//   * the residual add reads the newest row (hi + lo, 16 mantissa bits, re-split after every layer) from its ring slot;
-//   * out_proj's rows are ordered [skip | res] so that the accumulator halves line up with the two kinds of stores.
+//   * the residual add reads the input row (hi + lo, 16 mantissa bits, re-split after every layer);
+//   * out_proj's rows are ordered [skip | res] per 64-channel block so that the accumulator halves line up with the two
+//     kinds of stores.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -29,11 +29,7 @@
 namespace pk {
 namespace wf {
 
-constexpr int kC = 64;                                       // residual channels of pk_waveflow_layer
-constexpr int kG = 128;                                      // gate channels (a | g) == out_proj outputs (skip | res)
 constexpr int kATile = 128 * kSwizzleBytes;                  // 16 KB: 128 positions x one 64-channel chunk of one plane
-constexpr int kChunks = 11;                                  // 9 conv chunks + 2 condition chunks
-constexpr int kW1Cols = kChunks * kChunkK;                   // 704: row length of the packed GEMM1 weight
 constexpr int kConsumerThreads = 256;
 constexpr int kThreads = kConsumerThreads + 128;
 constexpr int kStages = 2;
@@ -157,112 +153,6 @@ __device__ __forceinline__ void consume_tile(uint32_t smem, uint32_t full_bar, u
   }
   it += G::kG2Chunks;
 }
-
-struct LayerArgs {
-  int batch, w, dil, slot;
-  int cond_ksteps_last;         // K-steps of the second condition chunk ((n_mels - 64 + 15) / 16)
-  int tiles_per_b, total_tiles;
-  float gate_c[128];            // pre-scaled biases of the gate (see the host code)
-  float out_b[128];             // out_proj bias in accumulator order: skip | res
-  float k_a, k_g;
-  float* skip;
-  int skip_init;
-  const __nv_bfloat16* x_hi;    // this layer's ring planes (batch, w, 3C): the residual reads the newest slot
-  const __nv_bfloat16* x_lo;
-  __nv_bfloat16* y_hi;          // next layer's ring planes (batch, w, y_ld), written at column y_col0; NULL on the last layer
-  __nv_bfloat16* y_lo;
-  int y_ld, y_col0;
-};
-
-__global__ void __launch_bounds__(kThreads, 1)
-waveflow_layer_kernel(const __grid_constant__ CUtensorMap tm_x,    // ring planes (batch, w, 3C): 4-D, both planes in one box
-                      const __grid_constant__ CUtensorMap tm_c,    // condition row planes (batch, w, n_mels)
-                      const __grid_constant__ CUtensorMap tm_w1,   // packed GEMM1 weight planes (128, 704), box = 128 rows
-                      const __grid_constant__ CUtensorMap tm_w2_hi, const __grid_constant__ CUtensorMap tm_w2_lo,
-                      const LayerArgs p) {
-  using G = Geo<kC>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t full_bar = smem + kStages * G::kStageBytes;   // [stages]
-  const uint32_t empty_bar = full_bar + 8 * kStages;           // [stages]
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == kConsumerThreads) {
-    tma_prefetch_desc(&tm_x); tma_prefetch_desc(&tm_c); tma_prefetch_desc(&tm_w1);
-    tma_prefetch_desc(&tm_w2_hi); tma_prefetch_desc(&tm_w2_lo);
-    for (int s = 0; s < kStages; ++s) { mbar_init_a(full_bar + 8 * s, 1); mbar_init_a(empty_bar + 8 * s, kConsumerThreads / 32); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= kConsumerThreads / 32) {
-    setmaxnreg_dec<40>();
-    if (warp == kConsumerThreads / 32 && lane == 0) {
-      // ------------------------------ TMA producer ------------------------------
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int b = tile / p.tiles_per_b, row0 = (tile % p.tiles_per_b) * 128;
-        for (int j = 0; j < G::kG1Chunks + G::kG2Chunks; ++j, ++it) {
-          const int s = it % kStages;
-          mbar_wait_a(empty_bar + 8 * s, ((it / kStages) & 1) ^ 1);
-          const uint32_t st = smem + s * G::kStageBytes;
-          const uint32_t fb = full_bar + 8 * s;
-          if (j < kChunks) {
-            mbar_arrive_expect_tx_a(fb, G::kStageBytes);
-            if (j < 9) {
-              const int tap = j / 3, slot = j - 3 * tap;
-              tma_load_4d_a(st, &tm_x, fb, slot * kC, row0 + (tap - 1) * p.dil, b, 0);   // rows outside [0, w) read as zero
-            } else {
-              tma_load_4d_a(st, &tm_c, fb, (j - 9) * kChunkK, row0, b, 0);               // columns >= n_mels read as zero
-            }
-            tma_load_4d_a(st + 2 * kATile, &tm_w1, fb, j * kChunkK, 0, 0, 0);
-          } else {
-            mbar_arrive_expect_tx_a(fb, G::kWBytes);                                       // out_proj: weights only
-            tma_load_3d_a(st + 2 * kATile, &tm_w2_hi, fb, 0, 0, 0);
-            tma_load_3d_a(st + 2 * kATile + kG * kSwizzleBytes, &tm_w2_lo, fb, 0, 0, 0);
-          }
-        }
-      }
-    }
-  } else {
-    // ------------------------------ consumers ------------------------------
-    setmaxnreg_inc<232>();
-    const int wg = warp >> 2;
-    const int rl = wg * 64 + 16 * (warp & 3) + (lane >> 2);
-    const int cq = 2 * (lane & 3);
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int b = tile / p.tiles_per_b, row0 = (tile % p.tiles_per_b) * 128;
-      consume_tile<kC>(smem, full_bar, empty_bar, it, wg, lane, p.gate_c, p.k_a, p.k_g, p.cond_ksteps_last,
-                       [&](int, const float (&acc2)[64]) {
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int row = row0 + rl + 8 * hh;
-          if (row >= p.w) continue;                            // positions past the end of the row: nothing to store
-          const long long pos = static_cast<long long>(b) * p.w + row;
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const int c = 8 * jj + cq;
-            float* dst = p.skip + pos * kC + c;
-            const float o0 = acc2[4 * jj + 2 * hh] + p.out_b[c], o1 = acc2[4 * jj + 2 * hh + 1] + p.out_b[c + 1];
-            if (p.skip_init) *reinterpret_cast<float2*>(dst) = make_float2(o0, o1);
-            else asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(o0), "f"(o1) : "memory");
-            if (p.y_hi != nullptr) {
-              const float2 x = ld_split2(p.x_hi, p.x_lo, pos * (3 * kC) + p.slot * kC + c);
-              uint32_t oh, ol;
-              split2(acc2[4 * (8 + jj) + 2 * hh] + p.out_b[64 + c] + x.x, acc2[4 * (8 + jj) + 2 * hh + 1] + p.out_b[64 + c + 1] + x.y, oh, ol);
-              const long long off = pos * p.y_ld + p.y_col0 + c;
-              *reinterpret_cast<uint32_t*>(p.y_hi + off) = oh;
-              *reinterpret_cast<uint32_t*>(p.y_lo + off) = ol;
-            }
-          }
-        }
-      });
-    }
-  }
-}
-
 
 // ------------------------------------------------------------------------------------------------------------------------
 // pk_waveflow_flow: ALL row steps x layers of one Flow.inverse (:515-556) in ONE persistent launch, for 64 or 128 residual
@@ -604,50 +494,6 @@ waveflow_forward_layer_kernel(const __grid_constant__ CUtensorMap tm_x,    // in
 
 }  // namespace wf
 }  // namespace pk
-
-extern "C" int pk_waveflow_layer(const pk_waveflow_layer_args* a, pk_stream_t stream) {
-  using namespace pk;
-  using namespace pk::wf;
-  PK_CHECK_ARG(a != nullptr, "args is NULL");
-  PK_CHECK_ARG(a->batch > 0 && a->width > 0 && a->dilation >= 1, "bad batch/width/dilation");
-  PK_CHECK_ARG(a->channels == kC, "the fused WaveFlow layer is built for 64 residual channels (got %d)", a->channels);
-  PK_CHECK_ARG(a->n_mels > 64 && a->n_mels <= 128 && (a->n_mels % 8) == 0, "n_mels must be in (64, 128], a multiple of 8");
-  PK_CHECK_ARG(a->slot >= 0 && a->slot < 3, "slot must be 0..2");
-  PK_CHECK_ARG(a->buf_hi && a->buf_lo && a->cond_hi && a->cond_lo && a->w1_hi && a->w1_lo && a->w2_hi && a->w2_lo && a->bias1 &&
-               a->bias2 && a->skip, "NULL pointer in pk_waveflow_layer_args");
-  PK_CHECK_ARG((a->next_hi == nullptr) == (a->next_lo == nullptr), "next_hi / next_lo: both or neither");
-  PK_CHECK_ARG(a->next_hi != a->buf_hi, "the next layer's ring must not alias this layer's");
-  PK_CHECK_ARG(a->cond_batch_stride >= static_cast<int64_t>(a->width) * a->n_mels && (a->cond_batch_stride % 8) == 0,
-               "bad condition batch stride");
-  using G = Geo<kC>;
-  CUtensorMap tx, tc, tw1, tw2_hi, tw2_lo;
-  int rc;
-  const uint64_t W = a->width, B = a->batch;
-  if ((rc = encode_tmap_bf16_planes(&tx, a->buf_hi, a->buf_lo, 3 * kC, W, B, 3 * kC, W * 3 * kC, 128))) return rc;
-  if ((rc = encode_tmap_bf16_planes(&tc, a->cond_hi, a->cond_lo, a->n_mels, W, B, a->n_mels, a->cond_batch_stride, 128))) return rc;
-  if ((rc = encode_tmap_bf16_planes(&tw1, a->w1_hi, a->w1_lo, kW1Cols, kG, 1, kW1Cols, 0, kG))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_hi, a->w2_hi, 64, kG, 1, 64, 0, kG))) return rc;
-  if ((rc = encode_tmap_bf16_3d(&tw2_lo, a->w2_lo, 64, kG, 1, 64, 0, kG))) return rc;
-  int resident = 0;
-  if ((rc = prepare_kernel(waveflow_layer_kernel, kThreads, G::kSmem, &resident))) return rc;
-  LayerArgs p;
-  p.batch = a->batch; p.w = a->width; p.dil = a->dilation; p.slot = a->slot;
-  p.cond_ksteps_last = (a->n_mels - 64 + kWgmmaK - 1) / kWgmmaK;
-  p.tiles_per_b = (a->width + 127) / 128;
-  p.total_tiles = p.tiles_per_b * a->batch;
-  p.k_a = kGateKa; p.k_g = kGateKg;
-  fold_gate_bias(p.gate_c, a->bias1, kC);
-  for (int i = 0; i < 128; ++i) p.out_b[i] = a->bias2[i];
-  p.skip = a->skip; p.skip_init = a->skip_init;
-  p.x_hi = static_cast<const __nv_bfloat16*>(a->buf_hi); p.x_lo = static_cast<const __nv_bfloat16*>(a->buf_lo);
-  p.y_hi = static_cast<__nv_bfloat16*>(a->next_hi); p.y_lo = static_cast<__nv_bfloat16*>(a->next_lo);
-  p.y_ld = 3 * kC; p.y_col0 = a->slot * kC;
-  const int grid = std::min(p.total_tiles, resident);
-  waveflow_layer_kernel<<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tx, tc, tw1, tw2_hi, tw2_lo, p);
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
 
 template <int C>
 static int flow_launch(const pk_waveflow_flow_args* a, pk_stream_t stream) {

@@ -1,4 +1,4 @@
-"""Frame-rate conditioning for the Parallel WaveGAN residual stack (experimental, PK_PWG_FRAME_COND=1; DESIGN.md 7.2).
+"""Frame-rate conditioning for the Parallel WaveGAN residual stack (every config frame_rate_exact accepts; DESIGN.md 7.2).
 
 The upsampling network of ConvInUpsampleNet (parallel_wavegan.py:119-138,201-216) is linear and acts on every channel
 alike, so the 1x1 aux convolution of a residual block (:300-303) commutes with it:

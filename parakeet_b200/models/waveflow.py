@@ -12,7 +12,6 @@ held-out negative log-likelihood with WaveFlowLoss) runs for 64 or 128 channels 
 parakeet_b200.training.WaveFlowTrainStep.
 """
 import ctypes as C_
-import os
 
 import numpy as np
 import torch
@@ -101,22 +100,16 @@ class ConditionalWaveFlow(Layer):
         dev, C = self.device, self.channels
         pk = {"enc": [(p[f"encoder.{i}.weight"].reshape(3, -1).contiguous().to(dev), p[f"encoder.{i}.bias"].to(dev))
                       for i in range(len(self.upsample_factors))], "flows": []}
+        fused = self._eligible()
         for fl in range(self.n_flows):
             pre = f"decoder.{fl}."
             layers = []
             for l in range(self.n_layers):
                 q = f"{pre}resnet.{l}."
                 w = p[q + "conv.weight"]                                  # [2C, C, kh, kw]
-                variants = []
-                for v in range(3):                                        # row step i with i % 3 == v: slot s holds kh = (s - i) % 3
-                    wk = torch.zeros(2 * C, 3 * C, 3)
-                    for s in range(3):
-                        wk[:, s * C:(s + 1) * C, :] = w[:, :, (s - v) % 3, :]
-                    variants.append(ops.pack_weight(wk, dev))
-                fused = None
-                if self._eligible():
-                    # operands of pk_waveflow_flow / pk_waveflow_layer (include/parakeet_b200.h): channels in blocks of 64; gate rows
-                    # a_blk | g_blk per block, out_proj rows skip_blk | res_blk; GEMM1 columns [tap][slot][c] | condition_proj
+                if fused:
+                    # operands of pk_waveflow_flow / pk_waveflow_forward_layer (include/parakeet_b200.h): channels in blocks of 64;
+                    # gate rows a_blk | g_blk per block, out_proj rows skip_blk | res_blk; GEMM1 columns [tap][slot][c] | condition_proj
                     nb = C // 64
                     g_rows = torch.cat([torch.cat([torch.arange(64 * k, 64 * k + 64), torch.arange(C + 64 * k, C + 64 * k + 64)])
                                         for k in range(nb)])
@@ -132,40 +125,40 @@ class ConditionalWaveFlow(Layer):
                         m[:, 9 * C:9 * C + self.n_mels] = cw
                         w1.append(_planes(m[g_rows], dev))
                     ow, ob = p[q + "out_proj.weight"][:, :, 0, 0], p[q + "out_proj.bias"]
-                    fused = dict(w1=w1, w2=_planes(ow[o_rows], dev),
-                                 b1=(p[q + "conv.bias"] + p[q + "condition_proj.bias"])[g_rows].numpy().astype("float32").copy(),
-                                 b2=ob[o_rows].numpy().astype("float32").copy())
-                layers.append(dict(fused=fused, conv=variants, conv_b=p[q + "conv.bias"].to(dev),
-                                   cond=ops.pack_weight(p[q + "condition_proj.weight"][:, :, 0, 0], dev),
-                                   cond_b=p[q + "condition_proj.bias"].to(dev),
-                                   out=ops.pack_weight(p[q + "out_proj.weight"][:, :, 0, 0], dev), out_b=p[q + "out_proj.bias"].to(dev)))
-            # the condition projections of all layers of a flow in one GEMM per row step (they do not depend on the recurrence)
-            cond_w = torch.cat([p[f"{pre}resnet.{l}.condition_proj.weight"][:, :, 0, 0] for l in range(self.n_layers)], dim=0)
-            cond_b = torch.cat([p[f"{pre}resnet.{l}.condition_proj.bias"] for l in range(self.n_layers)])
+                    b1 = (p[q + "conv.bias"] + p[q + "condition_proj.bias"])[g_rows].numpy().astype("float32").copy()
+                    layers.append(dict(fused=dict(w1=w1, w2=_planes(ow[o_rows], dev), b1=b1, b2=ob[o_rows].numpy().astype("float32").copy())))
+                else:
+                    # operands of the two-GEMM row loop (pk_conv_gemm_ex)
+                    variants = []
+                    for v in range(3):                                    # row step i with i % 3 == v: slot s holds kh = (s - i) % 3
+                        wk = torch.zeros(2 * C, 3 * C, 3)
+                        for s in range(3):
+                            wk[:, s * C:(s + 1) * C, :] = w[:, :, (s - v) % 3, :]
+                        variants.append(ops.pack_weight(wk, dev))
+                    layers.append(dict(conv=variants, conv_b=p[q + "conv.bias"].to(dev),
+                                       out=ops.pack_weight(p[q + "out_proj.weight"][:, :, 0, 0], dev), out_b=p[q + "out_proj.bias"].to(dev)))
             f32 = lambda t: t.detach().float().contiguous().numpy().astype("float32").copy()
             host = dict(in_w=f32(p[pre + "input_proj.weight"].reshape(-1)), in_b=f32(p[pre + "input_proj.bias"]),
                         out_w=f32(p[pre + "output_proj.weight"].reshape(2, C)), out_b=f32(p[pre + "output_proj.bias"]))
-            pk["flows"].append(dict(host=host, in_w=p[pre + "input_proj.weight"].reshape(-1).contiguous().to(dev),
-                                    in_b=p[pre + "input_proj.bias"].to(dev), layers=layers,
-                                    cond_all=ops.pack_weight(cond_w, dev), cond_all_b=cond_b.contiguous().to(dev),
-                                    out_w=p[pre + "output_proj.weight"].reshape(2, C).contiguous().to(dev),
-                                    out_b=p[pre + "output_proj.bias"].to(dev)))
+            flow = dict(host=host, in_w=p[pre + "input_proj.weight"].reshape(-1).contiguous().to(dev),
+                        in_b=p[pre + "input_proj.bias"].to(dev), layers=layers)
+            if not fused:
+                # the condition projections of all layers of a flow in one GEMM per row step (they do not depend on the recurrence)
+                cond_w = torch.cat([p[f"{pre}resnet.{l}.condition_proj.weight"][:, :, 0, 0] for l in range(self.n_layers)], dim=0)
+                cond_b = torch.cat([p[f"{pre}resnet.{l}.condition_proj.bias"] for l in range(self.n_layers)])
+                flow.update(cond_all=ops.pack_weight(cond_w, dev), cond_all_b=cond_b.contiguous().to(dev),
+                            out_w=p[pre + "output_proj.weight"].reshape(2, C).contiguous().to(dev),
+                            out_b=p[pre + "output_proj.bias"].to(dev))
+            pk["flows"].append(flow)
         pk["perms"] = [torch.tensor(pm, dtype=torch.int64, device=dev) for pm in self.perms]   # device-side gather indices
         self._packed = pk
         return pk
 
-    def _fusable(self):
-        """The fused kernels cover 64 < n_mels <= 128 and up to 8 layers per flow: pk_waveflow_flow (one persistent launch per
-        flow) for 64 or 128 residual channels, pk_waveflow_layer (one launch per ResidualBlock.add_input, PK_WF_FUSED=layer)
-        for 64.  PK_WF_FUSED=0 selects the two-GEMM path (A/B runs; also what other channel counts use)."""
-        mode = os.environ.get("PK_WF_FUSED", "1")
-        return self._eligible() and mode != "0" and (mode != "layer" or self.channels == 64)
-
     def _eligible(self):
+        """Whether the fused kernels cover this config: 64 or 128 residual channels, 64 < n_mels <= 128 (a multiple of 8) and up
+        to 8 layers per flow.  Then inverse runs pk_waveflow_flow (one persistent launch per flow); any other config runs it as
+        the two-GEMM row loop (pk_conv_gemm_ex) and has no density direction."""
         return self.channels in (64, 128) and 64 < self.n_mels <= 128 and self.n_mels % 8 == 0 and self.n_layers <= 8
-
-    def _flow_mode(self):
-        return self._fusable() and os.environ.get("PK_WF_FUSED", "1") != "layer"
 
     def _run_flow(self, fw, z, x, cond_s, cmap, bufs, skip, flags, st):
         """Rows 1 .. G-1 of one flow in one launch (row 0 and the ring contents are prepared by the caller)."""
@@ -222,9 +215,8 @@ class ConditionalWaveFlow(Layer):
         zt = Split.empty((B, W, C), dev)
         bufs = [Split.zeros((B, W, 3 * C), dev) for _ in range(NL)]
         st = _stream()
-        fused = self._fusable()
-        flow_mode = self._flow_mode()
-        flags = torch.empty((G - 1) * NL * B * ((W + 255) // 256), dtype=torch.int32, device=dev) if flow_mode else None
+        fused = self._eligible()
+        flags = torch.empty((G - 1) * NL * B * ((W + 255) // 256), dtype=torch.int32, device=dev) if fused else None
         for fi in reversed(range(self.n_flows)):
             perm = self.perms[fi]
             z = z.index_select(1, pk["perms"][fi])                                        # geo.shuffle_dim(z, 2, perm)
@@ -235,7 +227,7 @@ class ConditionalWaveFlow(Layer):
             for b_ in bufs:
                 b_.hi.zero_()
                 b_.lo.zero_()
-            if flow_mode:
+            if fused:
                 z = z.contiguous()
                 _lib.check(L.pk_waveflow_input_proj(_ptr(x[:, 0]), G * W, _ptr(fw["in_w"]), _ptr(fw["in_b"]), B, W, C,
                                                     _ptr(state), _ptr(bufs[0].hi), _ptr(bufs[0].lo), 3 * C, 0, st),
@@ -250,23 +242,6 @@ class ConditionalWaveFlow(Layer):
                                                     _ptr(state), _ptr(bufs[0].hi), _ptr(bufs[0].lo), 3 * C, slot * C, st),
                            "pk_waveflow_input_proj")
                 c_row = Split(cond_s.hi[:, cmap[i]], cond_s.lo[:, cmap[i]])              # (B, W, n_mels) views, batch stride G*W*n_mels
-                if fused:
-                    for l, lay in enumerate(fw["layers"]):
-                        f = lay["fused"]
-                        a = _lib.WaveflowLayerArgs()
-                        a.batch, a.width, a.channels, a.n_mels, a.dilation, a.slot = B, W, C, self.n_mels, 2 ** l, slot
-                        a.buf_hi, a.buf_lo = _ptr(bufs[l].hi), _ptr(bufs[l].lo)
-                        a.cond_hi, a.cond_lo, a.cond_batch_stride = _ptr(c_row.hi), _ptr(c_row.lo), G * W * self.n_mels
-                        w1 = f["w1"][i % 3]
-                        a.w1_hi, a.w1_lo, a.w2_hi, a.w2_lo = _ptr(w1[0]), _ptr(w1[1]), _ptr(f["w2"][0]), _ptr(f["w2"][1])
-                        a.bias1, a.bias2 = f["b1"].ctypes.data, f["b2"].ctypes.data
-                        if l + 1 < NL:
-                            a.next_hi, a.next_lo = _ptr(bufs[l + 1].hi), _ptr(bufs[l + 1].lo)
-                        a.skip, a.skip_init = _ptr(skip), 1 if l == 0 else 0
-                        _lib.check(L.pk_waveflow_layer(C_.byref(a), st), "pk_waveflow_layer")
-                    _lib.check(L.pk_waveflow_row_out(_ptr(skip), _ptr(fw["out_w"]), _ptr(fw["out_b"]), _ptr(z[:, i]), G * W, B, W, C,
-                                                     _ptr(x[:, i]), G * W, st), "pk_waveflow_row_out")
-                    continue
                 ops.conv_gemm(c_row, fw["cond_all"], n=NL * 2 * C, k=self.n_mels, bias=fw["cond_all_b"], y_f32=h_all)
                 for l, lay in enumerate(fw["layers"]):
                     # dilated conv over the 3-row ring + condition slice -> tanh * sigmoid, fused in the GEMM epilogue

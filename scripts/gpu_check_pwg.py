@@ -28,8 +28,6 @@ with torch.no_grad():
     y_ref, inter = opwg.generator_forward(folded, x, c, return_intermediates=True)
 y = gen(x.to(dev), c.to(dev))
 torch.cuda.synchronize()
-if gen._ws[(2, 12000)]["c"] is not None:      # sample-rate conditioning planes exist only on the legacy path (PK_PWG_FRAME_COND=0)
-    print("c planes err:", err(gen._ws[(2, 12000)]["c"].float().transpose(1, 2), c_ref))
 print("x30 err:", err(gen._last_x.float().transpose(1, 2), inter["x_layers"][-1]))
 print("skip err (incl. deferred bias):", err((gen._ws[(2, 12000)]["skip"] + gen._pack()["skip_bias_sum"]).transpose(1, 2) * math.sqrt(1 / 30), inter["skips"]))
 e = err(y, y_ref)

@@ -1,5 +1,4 @@
-"""ConditionalWaveFlow.infer at cfg4 shapes: CUDA-event time of a graph replay (third call of the same shape).
-PK_WF_FUSED=0 selects the two-GEMM layer path."""
+"""ConditionalWaveFlow.infer at cfg4 shapes: CUDA-event time of a graph replay (third call of the same shape)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -20,5 +19,5 @@ for _ in range(3):
     y = wf.infer(mel, z=z)
 e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / 3
-print(f"waveflow {CH} ch b16 x 400 frames (PK_WF_FUSED={os.environ.get('PK_WF_FUSED', '1')}): {ms:.1f} ms/call, "
+print(f"waveflow {CH} ch b16 x 400 frames: {ms:.1f} ms/call, "
       f"{y.numel() / ms * 1e3 / 1e6:.2f} M samples/s, replays {wf._graphs.replays}, finite {bool(torch.isfinite(y).all())}", flush=True)

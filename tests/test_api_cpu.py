@@ -1,6 +1,8 @@
 """Host-side API pieces of SURVEY.md 8b that need no GPU: spectrogram normalisers (audio/spec_normalizer.py), token-averaged
 energy (data/get_feats.py:205-220), checkpoint writer round trip, ConditionalWaveFlow.from_pretrained (models/waveflow.py:827-852)
 and the known-answer checks that pin the Slaney mel filterbank to librosa's documented output."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -114,7 +116,7 @@ def test_mel_filterbank_known_answers():
 
 @pytest.mark.parametrize("channels", [64, 128])
 def test_waveflow_fused_operand_layout(channels):
-    """The packed operands of pk_waveflow_flow / pk_waveflow_layer (include/parakeet_b200.h) restated on the CPU: one
+    """The packed operands of pk_waveflow_flow / pk_waveflow_forward_layer (include/parakeet_b200.h) restated on the CPU: one
     ResidualBlock.add_input evaluated as the kernel does it - GEMM1 over [tap][ring slot][channel] | condition columns with the
     row-step variant's weight, gate per 64-channel block, GEMM2 with the reordered out_proj - against conv2d on the 3-row buffer
     (reference parakeet/models/waveflow.py:248-285).  Host logic only: no CUDA."""
@@ -158,3 +160,31 @@ def test_waveflow_fused_operand_layout(channels):
         zk = torch.cat([torch.tanh(acc1[128 * k:128 * k + 64]) * torch.sigmoid(acc1[128 * k + 64:128 * k + 128]) for k in range(nb)])
         acc2 = w2 @ zk + torch.from_numpy(fused["b2"]).double()[:, None]
         assert torch.allclose(acc2, o[o_rows], rtol=0, atol=2e-4 * o.abs().max().item())
+
+
+def test_vocoder_layer_path_follows_the_model_config(monkeypatch):
+    """Which layer kernel Parallel WaveGAN runs follows from its upsample scales alone: with every PK_* environment variable
+    reading "0", [4, 5, 3, 5] (hop 300) still runs the frame-rate kernel and [2, 16, 8] (whose band tables are not exact) the
+    sample-rate kernel."""
+    from parakeet_b200.models import PWGGenerator
+
+    class PkOff(dict):
+        def get(self, key, default=None):
+            return "0" if key.startswith("PK_") else super().get(key, default)
+    monkeypatch.setattr(os, "environ", PkOff(os.environ))
+    assert PWGGenerator(upsample_scales=[4, 5, 3, 5], device="cpu")._uses_frame_cond()
+    assert not PWGGenerator(upsample_scales=[2, 16, 8], device="cpu")._uses_frame_cond()
+
+
+def test_waveflow_packs_only_the_operands_of_its_layer_path():
+    """An eligible ConditionalWaveFlow packs the fused kernels' operands and none of the two-GEMM row loop's; an n_mels = 64
+    model (outside the fused kernels' range) the reverse."""
+    from parakeet_b200.models import ConditionalWaveFlow
+    for n_mels, eligible in ((80, True), (64, False)):
+        m = ConditionalWaveFlow([16, 16], 2, 3, 16, 64, n_mels, (3, 3), device="cpu", seed=9)
+        assert m._eligible() == eligible
+        for fw in m._pack()["flows"]:
+            flow_keys = {"host", "in_w", "in_b", "layers"} | (set() if eligible else {"cond_all", "cond_all_b", "out_w", "out_b"})
+            assert set(fw) == flow_keys
+            for lay in fw["layers"]:
+                assert set(lay) == ({"fused"} if eligible else {"conv", "conv_b", "out", "out_b"})

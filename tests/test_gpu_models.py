@@ -75,31 +75,6 @@ def test_pwg_ragged_batch_equals_single_utterances(cuda, pwg):
         assert rel_err(y[i, :, :f * hop], refs[i]) < TOL
 
 
-def test_pwg_sample_rate_conditioning_path_vs_oracle(cuda, pwg, monkeypatch):
-    """PK_PWG_FRAME_COND=0 selects pk_pwg_residual_layer (sample-rate conditioning planes): whole batch and a ragged batch
-    against the oracle, like the default frame-rate path."""
-    from oracle import pwg as opwg
-    gen, folded = pwg
-    monkeypatch.setenv("PK_PWG_FRAME_COND", "0")
-    x, c = opwg.synth_inputs(6, batch=2, mel_frames=40)
-    with torch.no_grad():
-        y_ref = opwg.generator_forward(folded, x, c)
-    assert rel_err(gen(x.to(cuda), c.to(cuda)), y_ref) < TOL
-    frames, hop = [40, 25, 33], 300
-    xs = torch.zeros(3, 1, max(frames) * hop)
-    cs = torch.zeros(3, 80, max(frames) + 4)
-    refs = []
-    for i, f in enumerate(frames):
-        xi, ci = opwg.synth_inputs(20 + i, batch=1, mel_frames=f)
-        xs[i, :, :f * hop], cs[i, :, :f + 4] = xi[0], ci[0]
-        with torch.no_grad():
-            refs.append(opwg.generator_forward(folded, xi, ci)[0])
-    lens = torch.tensor([f * hop for f in frames], dtype=torch.int32, device=cuda)
-    y = gen(xs.to(cuda), cs.to(cuda), lens=lens)
-    for i, f in enumerate(frames):
-        assert rel_err(y[i, :, :f * hop], refs[i]) < TOL
-
-
 def test_pwg_ragged_batch_graph_replay_and_empty_utterance(cuda, pwg):
     """A ragged batch holding an EMPTY utterance, run three times (eager, CUDA-graph capture, replay): every call reproduces the
     single-utterance oracle results, the empty row stays zero, and a different set of lengths of the same padded shape (another
@@ -265,34 +240,30 @@ def test_waveflow_wide_rows_vs_oracle(cuda):
     assert list(out.shape) == list(ref.shape) and rel_err(out, ref) < TOL
 
 
-@pytest.mark.parametrize("mode", ["layer", "0"])
-def test_waveflow_layer_paths_agree(cuda, monkeypatch, mode):
-    """The per-layer fused kernel (PK_WF_FUSED=layer) and the two-GEMM path (PK_WF_FUSED=0) stay parity-green: they are the
-    A/B baselines of the persistent flow kernel (default) and the fallback for channel counts it does not cover."""
+@pytest.mark.parametrize("channels", [64, 128])
+def test_waveflow_two_gemm_path_vs_oracle(cuda, channels):
+    """n_mels = 64 is outside the fused kernels' range, so inverse runs the two-GEMM row loop (pk_conv_gemm_ex with the gate and
+    wf_update epilogues, N = 2C gate channels, K = 3C per tap); W = 431 columns so that every width dilation reaches live
+    columns; odd batch."""
     from oracle import waveflow as owf
     from parakeet_b200.models import ConditionalWaveFlow
-    params = owf.synth_params(4)
+    params = owf.synth_params(6, channels=channels, n_mels=64)
     folded = owf.fold_weight_norm(params)
+    m = ConditionalWaveFlow([16, 16], 8, 8, 16, channels, 64, (3, 3), device=cuda)
+    m.set_state_dict(params)
+    assert not m._eligible()
     g = torch.Generator().manual_seed(43)
-    mel = torch.randn(2, 80, 20, generator=g) * 0.5 - 3
-    z = torch.randn(2, 256 * 20 - 272, generator=g)
+    mel = torch.randn(3, 64, 28, generator=g) * 0.5 - 3
+    z = torch.randn(3, 256 * 28 - 272, generator=g)
     with torch.no_grad():
         ref = owf.infer(folded, mel, z)
-    monkeypatch.setenv("PK_WF_FUSED", mode)
-    m = ConditionalWaveFlow([16, 16], 8, 8, 16, 64, 80, (3, 3), device=cuda)
-    m.set_state_dict(params)
     out = m.infer(mel.to(cuda), z=z.to(cuda))
-    assert rel_err(out, ref) < TOL
-    monkeypatch.setenv("PK_WF_FUSED", "1")
-    m2 = ConditionalWaveFlow([16, 16], 8, 8, 16, 64, 80, (3, 3), device=cuda)
-    m2.set_state_dict(params)
-    assert rel_err(m2.infer(mel.to(cuda), z=z.to(cuda)), out) < 1e-4
+    assert list(out.shape) == list(ref.shape) and rel_err(out, ref) < TOL
 
 
-def test_waveflow_shipped_config_128_channels(cuda, monkeypatch):
+def test_waveflow_shipped_config_128_channels(cuda):
     """examples/waveflow/config.py ships channels = 128 (BASELINE cfg 4 is the 64-channel variant): the flow kernel runs the
-    channels as two blocks of 64 (N = 256 MMAs); W = 431 columns so that every width dilation reaches live columns; the
-    two-GEMM path (PK_WF_FUSED=0: N = 256 gate channels, K = 3 x 384 per tap through pk_conv_gemm_ex) must agree."""
+    channels as two blocks of 64 (N = 256 MMAs); W = 431 columns so that every width dilation reaches live columns."""
     from oracle import waveflow as owf
     from parakeet_b200.models import ConditionalWaveFlow
     params = owf.synth_params(5, channels=128)
@@ -302,16 +273,11 @@ def test_waveflow_shipped_config_128_channels(cuda, monkeypatch):
     z = torch.randn(3, 256 * 28 - 272, generator=g)
     with torch.no_grad():
         ref = owf.infer(folded, mel, z)
-    outs = []
-    for mode in ("1", "0"):
-        monkeypatch.setenv("PK_WF_FUSED", mode)
-        m = ConditionalWaveFlow([16, 16], 8, 8, 16, 128, 80, (3, 3), device=cuda)
-        m.set_state_dict(params)
-        assert m._flow_mode() == (mode == "1")
-        out = m.infer(mel.to(cuda), z=z.to(cuda))
-        assert list(out.shape) == list(ref.shape) and rel_err(out, ref) < TOL, mode
-        outs.append(out)
-    assert rel_err(outs[0], outs[1]) < 1e-4
+    m = ConditionalWaveFlow([16, 16], 8, 8, 16, 128, 80, (3, 3), device=cuda)
+    m.set_state_dict(params)
+    assert m._eligible()
+    out = m.infer(mel.to(cuda), z=z.to(cuda))
+    assert list(out.shape) == list(ref.shape) and rel_err(out, ref) < TOL
 
 
 @pytest.mark.parametrize("channels", [64, 128])
@@ -324,7 +290,7 @@ def test_waveflow_flow_kernel_single_utterance_and_edges(cuda, channels):
     folded = owf.fold_weight_norm(params)
     m = ConditionalWaveFlow([16, 16], 8, 8, 16, channels, 80, (3, 3), device=cuda)
     m.set_state_dict(params)
-    assert m._flow_mode()
+    assert m._eligible()
     for batch, frames, seed in ((1, 9, 51), (1, 18, 52), (2, 18, 53)):     # W = 127, 271, 271
         g = torch.Generator().manual_seed(seed)
         mel = torch.randn(batch, 80, frames, generator=g) * 0.5 - 3

@@ -121,7 +121,7 @@ def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
     assert len(re.findall(r"\bstruct\b", bare)) == len(mirrors)
     names = {"pk_operand": "Operand", "pk_conv_gemm_args": "ConvGemmArgs", "pk_gemm_epilogue": "GemmEpilogue",
              "pk_pwg_layer_args": "PwgLayerArgs", "pk_pwg_layer_fc_args": "PwgLayerFcArgs", "PkAttentionArgs": "AttentionArgs",
-             "pk_waveflow_layer_args": "WaveflowLayerArgs", "pk_waveflow_flow_args": "WaveflowFlowArgs",
+             "pk_waveflow_flow_args": "WaveflowFlowArgs",
              "pk_waveflow_forward_layer_args": "WaveflowForwardLayerArgs", "pk_waveflow_forward_tail_args": "WaveflowForwardTailArgs",
              "pk_ss_residual_block_args": "SsResidualBlockArgs", "pk_waveflow_backward_layer_args": "WaveflowBackwardLayerArgs",
              "PkTaco2DecodeArgs": "Taco2DecodeArgs", "PkTtsDecodeArgs": "TtsDecodeArgs"}

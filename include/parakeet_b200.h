@@ -901,6 +901,41 @@ int pk_tts_shift_frames(const float* ys, int32_t batch, int32_t l, int32_t odim,
 int pk_tts_prenet_dropout(float* x, int32_t batch, int32_t l, int32_t units, float p, uint64_t seed, int32_t site, pk_stream_t stream);
 int pk_tts_stop_labels(const int32_t* olens, int32_t batch, int32_t width, float* out, pk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * TransformerTTS training step (reference: TransformerTTSUpdater.update_core, models/transformer_tts/
+ * transformer_tts_updater.py:73-170).  The attention runs on the materialised path of the FastSpeech2 step (pk_conv_gemm,
+ * softmax, pk_dropout); these add the causal mask, the guided source-attention loss and TransformerTTSLoss.  No atomics.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* pk_masked_softmax with an optional causal mask: s (batch * heads, rows, ld) -> p split planes; query row i of utterance b
+ * attends keys j < key_lens[b] (key_lens NULL: all `keys`) and, when causal != 0, j <= i.  Rows with no key left are zeros. */
+int pk_masked_softmax_ex(const float* s, const int32_t* key_lens, int32_t batch, int32_t heads, int32_t rows, int32_t keys, int32_t ld,
+                         int32_t causal, void* p_hi, void* p_lo, pk_stream_t stream);
+/* pk_softmax_bwd with GuidedMultiHeadAttentionLoss (transformer_tts.py:874-1075) fused in.  p, dp, ds: (batch * heads, rows, ld).
+ * For heads h < guided_heads, rows i < olens[b], keys j < ilens[b]: dp[i, j] + coef G[i, j] enters the backward, with
+ * G = 1 - exp(-(j / ilens[b] - i / olens[b])^2 / (2 sigma^2)) and coef = lambda / (guided_heads * guided_layers *
+ * sum_b ilens[b] olens[b]); partials[(b * guided_heads + h) * rows + i] = sum_j G P (0 for i >= olens[b]).  dp is the gradient
+ * w.r.t. the pre-dropout probabilities and is not written; ds = scale * p * (dp' - sum_k p dp'), 0 in columns >= keys.
+ * guided_heads 0 is pk_softmax_bwd (ilens, olens and partials may then be NULL). */
+int pk_softmax_bwd_guided(const void* p_hi, const void* p_lo, const float* dp, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
+                          int32_t ld, float scale, int32_t guided_heads, int32_t guided_layers, const int32_t* ilens, const int32_t* olens,
+                          float sigma, float lambda, float* partials, void* ds_hi, void* ds_lo, pk_stream_t stream);
+/* The guided loss from the n partials of pk_softmax_bwd_guided (every guided layer's): lambda * sum / (heads_layers *
+ * sum_b min(ilens[b], keys) min(olens[b], rows)) -> losses[4], and added to losses[0]. */
+int pk_tts_guided_loss(const float* partials, int64_t n, const int32_t* ilens, const int32_t* olens, int32_t batch, int32_t rows,
+                       int32_t keys, int32_t heads_layers, float lambda, float* losses, pk_stream_t stream);
+/* TransformerTTSLoss (transformer_tts.py:770-872, use_masking=True) over the frames t < olens[b] of before / after / ys
+ * (batch, l_max, odim) and logits / labels (batch, l_max): losses[0..3] = {loss, l1, l2, bce}; l1 = mean|after - ys| +
+ * mean|before - ys|, l2 the same with squares, bce = BCEWithLogitsLoss(pos_weight) on the logits, loss = l1 + bce (loss_type 0),
+ * l2 + bce (1) or l1 + l2 + bce (2).  workspace: pk_tts_loss_workspace(batch, l_max) floats. */
+int64_t pk_tts_loss_workspace(int32_t batch, int32_t l_max);
+int pk_tts_loss(const float* before, const float* after, const float* ys, const float* logits, const float* labels, const int32_t* olens,
+                int32_t batch, int32_t l_max, int32_t odim, float pos_weight, int32_t loss_type, float* workspace, float* losses,
+                pk_stream_t stream);
+/* gradients of losses[0] of pk_tts_loss w.r.t. before, after and logits (0 on the padded frames) */
+int pk_tts_loss_bwd(const float* before, const float* after, const float* ys, const float* logits, const float* labels,
+                    const int32_t* olens, int32_t batch, int32_t l_max, int32_t odim, float pos_weight, int32_t loss_type, float* g_before,
+                    float* g_after, float* g_logits, pk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

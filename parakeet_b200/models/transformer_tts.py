@@ -13,8 +13,12 @@ The eval-mode `forward` and `inference(use_teacher_forcing=True)` run the teache
 `pk_layer_norm`, and `pk_fused_attention_ex` for the causal self-attention and the source attention; the source-attention weights
 are computed (`batched_matmul_nt` + `pk_masked_softmax`) only where they are returned.
 
-Not implemented, and refused before any launch: the training step (`train()` raises), GST, speaker embeddings, the encoder
-prenet, concat_after, post-LN and non-conv1d position-wise layers.
+The training step of the ljspeech recipe is `training.TransformerTTSTrainStep` (update_core: the train-mode forward with dropout,
+TransformerTTSLoss, the guided source-attention loss, backward and Adam); `train()` keeps raising, as the step is the training entry
+point.
+
+Not implemented, and refused before any launch: GST, speaker embeddings, the encoder prenet, concat_after, post-LN and non-conv1d
+position-wise layers.
 """
 import math
 
@@ -80,6 +84,16 @@ class TransformerTTS(Layer):
         self.num_heads_applied_guided_attn = aheads if num_heads_applied_guided_attn == -1 else num_heads_applied_guided_attn
         self.num_layers_applied_guided_attn = elayers if num_layers_applied_guided_attn == -1 else num_layers_applied_guided_attn
         self.use_scaled_pos_enc = use_scaled_pos_enc
+        # the train-mode rates, read by training/transformer_tts_step.py (the decoder prenet's p = 0.5 is not among them: its
+        # F.dropout ignores dprenet_dropout_rate)
+        self.dropout_rates = dict(transformer_enc_dropout_rate=transformer_enc_dropout_rate,
+                                  transformer_enc_positional_dropout_rate=transformer_enc_positional_dropout_rate,
+                                  transformer_enc_attn_dropout_rate=transformer_enc_attn_dropout_rate,
+                                  transformer_dec_dropout_rate=transformer_dec_dropout_rate,
+                                  transformer_dec_positional_dropout_rate=transformer_dec_positional_dropout_rate,
+                                  transformer_dec_attn_dropout_rate=transformer_dec_attn_dropout_rate,
+                                  transformer_enc_dec_attn_dropout_rate=transformer_enc_dec_attn_dropout_rate,
+                                  postnet_dropout_rate=postnet_dropout_rate)
         self.training = False
         g = torch.Generator().manual_seed(0)
         A, k = adim, positionwise_conv_kernel_size

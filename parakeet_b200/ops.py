@@ -820,3 +820,55 @@ def tts_stop_labels(olens, width):
     out = torch.empty(B, width, dtype=torch.float32, device=olens.device)
     _lib.check(_lib.lib().pk_tts_stop_labels(_ptr(olens), B, width, _ptr(out), _stream()), "pk_tts_stop_labels")
     return out
+
+
+def masked_softmax_ex(s, key_lens, batch, heads, rows, keys, causal=False):
+    """pk_masked_softmax_ex: s fp32 (batch*heads, rows, ld) -> split planes of the same shape; causal adds the j <= i mask."""
+    ld = s.shape[-1]
+    p = Split.empty(tuple(s.shape), s.device)
+    _lib.check(_lib.lib().pk_masked_softmax_ex(_ptr(s), _ptr(key_lens), batch, heads, rows, keys, ld, 1 if causal else 0, _ptr(p.hi),
+                                               _ptr(p.lo), _stream()), "pk_masked_softmax_ex")
+    return p
+
+
+def softmax_bwd_guided(p, dp, batch, heads, rows, keys, scale, guided_heads, guided_layers, ilens, olens, sigma, lam, partials):
+    """pk_softmax_bwd_guided -> dS split planes (batch*heads, rows, ld); writes the guided loss's row partials (batch, guided_heads,
+    rows) into `partials` (a contiguous fp32 view)."""
+    ld = dp.shape[-1]
+    ds = Split.empty(tuple(dp.shape), dp.device)
+    _lib.check(_lib.lib().pk_softmax_bwd_guided(_ptr(p.hi), _ptr(p.lo), _ptr(dp), batch, heads, rows, keys, ld, float(scale), guided_heads,
+                                                guided_layers, _ptr(ilens), _ptr(olens), float(sigma), float(lam), _ptr(partials),
+                                                _ptr(ds.hi), _ptr(ds.lo), _stream()), "pk_softmax_bwd_guided")
+    return ds
+
+
+def tts_guided_loss(partials, ilens, olens, rows, keys, heads_layers, lam, losses):
+    """pk_tts_guided_loss: losses[4] = the guided attention loss from every guided layer's partials, added to losses[0]."""
+    _lib.check(_lib.lib().pk_tts_guided_loss(_ptr(partials), partials.numel(), _ptr(ilens), _ptr(olens), ilens.numel(), rows, keys,
+                                             heads_layers, float(lam), _ptr(losses), _stream()), "pk_tts_guided_loss")
+
+
+TTS_LOSS_TYPES = {"L1": 0, "L2": 1, "L1+L2": 2}
+
+
+def tts_loss(before, after, ys, logits, labels, olens, pos_weight=5.0, loss_type="L1", losses=None):
+    """pk_tts_loss: -> losses fp32 (5,) = loss, l1, l2, bce and a slot for the guided loss (left as it was); before / after / ys
+    (B, L, odim), logits / labels (B, L), olens int32 (B,), all contiguous on the device."""
+    B, L, odim = before.shape
+    lib = _lib.lib()
+    ws = torch.empty(int(lib.pk_tts_loss_workspace(B, L)), dtype=torch.float32, device=before.device)
+    if losses is None:
+        losses = torch.zeros(5, dtype=torch.float32, device=before.device)
+    _lib.check(lib.pk_tts_loss(_ptr(before), _ptr(after), _ptr(ys), _ptr(logits), _ptr(labels), _ptr(olens), B, L, odim, float(pos_weight),
+                               TTS_LOSS_TYPES[loss_type], _ptr(ws), _ptr(losses), _stream()), "pk_tts_loss")
+    return losses
+
+
+def tts_loss_bwd(before, after, ys, logits, labels, olens, pos_weight=5.0, loss_type="L1"):
+    """pk_tts_loss_bwd -> (d loss / d before, d loss / d after, d loss / d logits)."""
+    B, L, odim = before.shape
+    gb, ga, gl = torch.empty_like(before), torch.empty_like(after), torch.empty_like(logits)
+    _lib.check(_lib.lib().pk_tts_loss_bwd(_ptr(before), _ptr(after), _ptr(ys), _ptr(logits), _ptr(labels), _ptr(olens), B, L, odim,
+                                          float(pos_weight), TTS_LOSS_TYPES[loss_type], _ptr(gb), _ptr(ga), _ptr(gl), _stream()),
+               "pk_tts_loss_bwd")
+    return gb, ga, gl

@@ -15,7 +15,6 @@ row-wise kernels of train.cu.
 torch is used for buffers, views, permutes / copies (layout plumbing) and torch.distributed.
 """
 import ctypes as C
-import math
 import os
 
 import torch
@@ -23,13 +22,19 @@ import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.fastspeech2 import FastSpeech2, _i32
-from ..ops import Split, _ptr, _stream, ceil_to
+from ..ops import Split, _ptr, _stream
 from . import wgrad
 from .conv import ConvOps
 from .flat import BUFFERS, FlatAdam, broadcast_from_rank0, load_updater_state, step_graphs, updater_state
+from .transformer import TransformerTrainOps
 
 
-class FastSpeech2TrainStep:
+class FastSpeech2TrainStep(TransformerTrainOps):
+    """Dropout sites (TransformerTrainOps.site; oracle/fastspeech2.py: dropout_site restates this numbering): stack 0 encoder,
+    1 decoder, 2 pitch, 3 energy, 4 duration predictor, 5 postnet; kind 0 positional encoding, 1 attention probabilities,
+    2 attention sub-layer output, 3 feed-forward hidden, 4 feed-forward sub-layer output, 5 predictor layer, 6 postnet layer;
+    (6, 0, 7) / (6, 0, 8): pitch / energy embedding."""
+
     def __init__(self, model: FastSpeech2, learning_rate=1e-3, beta1=0.9, beta2=0.999, epsilon=1e-8,
                  stop_gradient_from_pitch_predictor=None, stop_gradient_from_energy_predictor=None, process_group=None,
                  dropout=True, seed=0, use_graphs=None):
@@ -85,210 +90,6 @@ class FastSpeech2TrainStep:
     # GEMM-shaped forward / backward pieces
     # ------------------------------------------------------------------------------------------------------------
     step_count = property(lambda self: self.opt.steps)
-
-    def P(self, name):
-        return self.m._params[name]
-
-    @staticmethod
-    def site(stack, layer, kind):
-        """stack: 0 encoder, 1 decoder, 2 pitch, 3 energy, 4 duration predictor, 5 postnet; kind: 0 positional encoding,
-        1 attention probabilities, 2 attention sub-layer output, 3 feed-forward hidden, 4 feed-forward sub-layer output,
-        5 predictor layer, 6 postnet layer; (6, 0, 7) / (6, 0, 8): pitch / energy embedding
-        (oracle/fastspeech2.py: dropout_site restates this numbering)."""
-        return stack * 1000 + layer * 10 + kind
-
-    def drop(self, x, p, site, **kw):
-        """Forward AND backward: the mask depends only on (seed, step, site, element index)."""
-        return ops.dropout(x, p, self.seed, site, 1, step_dev=self.step_dev, **kw)      # step = 1 + completed steps (device counter)
-
-    def layer_fwd(self, x, wname, bname, kind, **kw):
-        return self.conv.fwd(x, wname, self.P(wname), linear=kind == "lin", bias=self.P(bname) if bname else None, **kw)
-
-    def layer_bwd(self, dy, x_saved, wname, bname, kind, need_dx=True):
-        """dy fp32 (B,T,cout), x_saved split (B,T,cin): writes the grads of weight / bias, returns dx fp32 (B,T,cin)."""
-        w, linear = self.P(wname), kind == "lin"
-        dys = ops.split_pad8(dy)
-
-        def param_grads():
-            if bname:      # from the split copy: dy itself may be the residual-stream gradient, which LayerNorm backward updates in place
-                ops.colsum_split_(dys, dy.shape[-1], self.grads[bname])
-            self.conv.wgrad(x_saved, dys, w, linear=linear, out=self.grads[wname])
-
-        # the parameter gradients are leaves of the backward graph: they run beside the dx chain (the critical path)
-        self.on_side(param_grads, dys, x_saved)
-        return self.conv.dgrad(dys, wname, w, linear=linear) if need_dx else None
-
-    def on_side(self, fn, *keep):
-        """Run fn() on the side stream, after everything issued so far on the current stream (fork); join_side() is the join.
-        The small-batch step is launch / latency bound (~750 kernels of 5-30 us on a few SMs each): the weight-gradient
-        transposes, split-K GEMMs and bias sums overlap the activation-gradient chain - in the captured graph they become
-        parallel branches.  `keep`: tensors fn reads that were allocated on the current stream - held until the join so that the
-        caching allocator (also at capture time) cannot hand their memory to a later tensor while the side branch still reads it."""
-        if not self.overlap:
-            fn()
-            return
-        cur = torch.cuda.current_stream()
-        if self._side is None:
-            self._side = torch.cuda.Stream(device=self.dev)
-        self._side.wait_stream(cur)
-        self._keep.extend(keep)
-        with torch.cuda.stream(self._side):
-            fn()
-        self._side_used = True
-
-    def join_side(self):
-        if self._side_used:
-            torch.cuda.current_stream().wait_stream(self._side)
-            self._side_used = False
-        self._keep.clear()
-
-    def zbuf(self, role, shape):
-        """Persistent zero-initialised operand planes of the current batch shape (training/wgrad.py: ZeroPlanes)."""
-        return self._zp.get(role, shape, self.dev)
-
-    def wqkv(self, q):
-        """The fused Q | K | V projection of layer prefix `q` as one Paddle Linear weight [A, 3A]."""
-        return torch.cat([self.P(q + "self_attn.linear_q.weight"), self.P(q + "self_attn.linear_k.weight"),
-                          self.P(q + "self_attn.linear_v.weight")], dim=1)
-
-    # ------------------------------------------------------------------------------------------------------------
-    # FFT-block stack (Encoder.forward after the embedding) with saved context
-    # ------------------------------------------------------------------------------------------------------------
-    def stack_fwd(self, x, pre, n_layers, key_lens):
-        m = self.m
-        sid = 0 if pre == "encoder." else 1
-        tag = "enc" if sid == 0 else "dec"
-        r_layer, r_attn = self.rates[f"transformer_{tag}_dropout_rate"], self.rates[f"transformer_{tag}_attn_dropout_rate"]
-        B, T, A = x.shape
-        H, dk = m.aheads, A // m.aheads
-        Tp = ceil_to(T, 64)
-        ctxs = []
-        kind = "lin" if m._linear_ffn else "conv"
-        for i in range(n_layers):
-            q = f"{pre}encoders.{i}."
-            c = dict(x0=x)
-            _, c["h1"] = ops.layer_norm(x, self.P(q + "norm1.weight"), self.P(q + "norm1.bias"))
-            bqkv = torch.cat([self.P(q + "self_attn.linear_q.bias"), self.P(q + "self_attn.linear_k.bias"), self.P(q + "self_attn.linear_v.bias")])
-            _, qkv = self.conv.fwd(c["h1"], q + "qkv", self.wqkv(q), linear=True, bias=bqkv, out_f32=False, out_split=True)
-            c["qkv"] = qkv
-            ld = 3 * A
-            s_buf = torch.empty(B * H, T, Tp, dtype=torch.float32, device=x.device)
-            q_spec = dict(rows=T, cols=ld, ld=ld, batch_stride=T * ld, batches=B, bmul=1, hmul=0, col0=0, colh=dk)
-            k_spec = dict(rows=T, cols=ld, ld=ld, batch_stride=T * ld, batches=B, bmul=1, hmul=0, col0=A, colh=dk)
-            ops.batched_matmul_nt(qkv, qkv, batch=B, heads=H, m=T, n=T, k=dk, a_spec=q_spec, b_spec=k_spec, scale=1.0 / math.sqrt(dk),
-                                  y_f32=s_buf, y_batch_stride=H * T * Tp, y_head_stride=T * Tp, y_ld=Tp)
-            c["p"] = ops.masked_softmax(s_buf, key_lens, B, H, T, T)
-            c["pd"] = self.drop(c["p"], r_attn, self.site(sid, i, 1), out_f32=False, out_split=True)[1] if r_attn > 0 else c["p"]
-            vt = ops.transpose_heads(qkv, col0=2 * A, dk=dk, heads=H, ld_dst=Tp)
-            ctx = Split.empty((B, T, A), x.device)
-            p_spec = dict(rows=T, cols=Tp, ld=Tp, batch_stride=T * Tp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)
-            v_spec = dict(rows=dk, cols=Tp, ld=Tp, batch_stride=dk * Tp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)
-            ops.batched_matmul_nt(c["pd"], vt, batch=B, heads=H, m=T, n=dk, k=Tp, a_spec=p_spec, b_spec=v_spec, y_split=ctx,
-                                  y_batch_stride=T * A, y_head_stride=dk, y_ld=A)
-            c["ctx"] = ctx
-            if r_layer > 0:      # x1 = x + dropout(attention): the residual add cannot ride in the GEMM epilogue any more
-                a_out, _ = self.layer_fwd(ctx, q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin")
-                self.drop(a_out, r_layer, self.site(sid, i, 2), inplace=True)
-                ops.axpy_(1.0, x, a_out)
-                x1 = a_out
-            else:
-                x1, _ = self.layer_fwd(ctx, q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin", residual=x)
-            c["x1"] = x1
-            _, c["h2"] = ops.layer_norm(x1, self.P(q + "norm2.weight"), self.P(q + "norm2.bias"))
-            _, c["u"] = self.layer_fwd(c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind, act="relu", out_f32=False, out_split=True)
-            c["ud"] = self.drop(c["u"], r_layer, self.site(sid, i, 3), out_f32=False, out_split=True)[1] if r_layer > 0 else c["u"]
-            if r_layer > 0:
-                f_out, _ = self.layer_fwd(c["ud"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", kind)
-                self.drop(f_out, r_layer, self.site(sid, i, 4), inplace=True)
-                ops.axpy_(1.0, x1, f_out)
-                x = f_out
-            else:
-                x, _ = self.layer_fwd(c["u"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", kind, residual=x1)
-            ctxs.append(c)
-        y, ys = ops.layer_norm(x, self.P(pre + "after_norm.weight"), self.P(pre + "after_norm.bias"), want_f32=True, want_split=True)
-        return y, ys, dict(layers=ctxs, x_last=x, pre=pre, n=n_layers, sid=sid, r_layer=r_layer, r_attn=r_attn)
-
-    def stack_bwd(self, dy, S):
-        """dy: gradient w.r.t. the after_norm output (fp32).  Returns the gradient w.r.t. the stack input."""
-        m = self.m
-        pre = S["pre"]
-        B, T, A = dy.shape
-        H, dk = m.aheads, A // m.aheads
-        Tp = ceil_to(T, 64)
-        dev = dy.device
-        kind = "lin" if m._linear_ffn else "conv"
-        dx = torch.empty_like(dy)
-        ops.layer_norm_bwd(S["x_last"], self.P(pre + "after_norm.weight"), dy, dx, False, self.grads[pre + "after_norm.weight"],
-                           self.grads[pre + "after_norm.bias"])
-        sid, r_layer, r_attn = S["sid"], S["r_layer"], S["r_attn"]
-        for i in reversed(range(S["n"])):
-            q = f"{pre}encoders.{i}."
-            c = S["layers"][i]
-            # x2 = x1 + drop(conv2(drop(relu(conv1(LN2(x1))))))
-            dsub = self.drop(dx, r_layer, self.site(sid, i, 4))[0] if r_layer > 0 else dx
-            du = self.layer_bwd(dsub, c["ud"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", kind)
-            if r_layer > 0:
-                self.drop(du, r_layer, self.site(sid, i, 3), inplace=True)
-            du_f, _ = ops.relu_bwd(du, c["u"], want_f32=True)
-            dh2 = self.layer_bwd(du_f, c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind)
-            ops.layer_norm_bwd(c["x1"], self.P(q + "norm2.weight"), dh2, dx, True, self.grads[q + "norm2.weight"], self.grads[q + "norm2.bias"])
-            # x1 = x0 + drop(out_proj(attention(LN1(x0))))
-            dsub = self.drop(dx, r_layer, self.site(sid, i, 2))[0] if r_layer > 0 else dx
-            dctx = self.layer_bwd(dsub, c["ctx"], q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin")
-            dctx_s = Split.from_f32(dctx)
-            qkv, p = c["qkv"], c["p"]
-            ld = 3 * A
-            dqkv = torch.zeros(B, T, ld, dtype=torch.float32, device=dev)
-            o_spec = dict(rows=T, cols=A, ld=A, batch_stride=T * A, batches=B, bmul=1, hmul=0, col0=0, colh=dk)
-            v_spec = dict(rows=T, cols=ld, ld=ld, batch_stride=T * ld, batches=B, bmul=1, hmul=0, col0=2 * A, colh=dk)
-            dp = torch.zeros(B * H, T, Tp, dtype=torch.float32, device=dev)
-            ops.batched_matmul_nt(dctx_s, qkv, batch=B, heads=H, m=T, n=T, k=dk, a_spec=o_spec, b_spec=v_spec, y_f32=dp,
-                                  y_batch_stride=H * T * Tp, y_head_stride=T * Tp, y_ld=Tp)                       # d(drop(P)) = dO V^T
-            if r_attn > 0:
-                self.drop(dp, r_attn, self.site(sid, i, 1), inplace=True)                                         # -> dP
-            ds = ops.softmax_bwd(p, dp, T, 1.0 / math.sqrt(dk))                                                  # includes the 1/sqrt(dk)
-            z_spec = dict(rows=T, cols=Tp, ld=Tp, batch_stride=T * Tp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)
-            d_spec = dict(rows=dk, cols=Tp, ld=Tp, batch_stride=dk * Tp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)
-
-            def t_sq(src):       # (B*H, T, Tp) -> transposed (B*H, T, Tp)
-                dst = self.zbuf("tsq", (B * H, T, Tp))
-                ops.transpose_planes(src, z=B * H, rows=T, src_zstride=T * Tp, ld_src=Tp, c0=0, cols=T, shift=0, r_out=T, dst=dst,
-                                     dst_zstride=T * Tp, ld_dst=Tp)
-                return dst
-
-            def t_heads(src, ld_src, col0):   # (B, T, ld_src)[.., col0 + h*dk + d] -> (B*H, dk, Tp)
-                dst = self.zbuf(("th", T), (B, H, dk, Tp))
-                for h in range(H):
-                    ops.transpose_planes(src, z=B, rows=T, src_zstride=T * ld_src, ld_src=ld_src, c0=col0 + h * dk, cols=dk, shift=0,
-                                         r_out=T, dst=Split(dst.hi[:, h], dst.lo[:, h]), dst_zstride=H * dk * Tp, ld_dst=Tp)
-                return dst
-
-            pt, dot = t_sq(c["pd"]), t_heads(dctx_s, A, 0)                                                        # dV uses the dropped P
-            ops.batched_matmul_nt(pt, dot, batch=B, heads=H, m=T, n=dk, k=Tp, a_spec=z_spec, b_spec=d_spec, y_f32=dqkv[:, :, 2 * A:],
-                                  y_batch_stride=T * ld, y_head_stride=dk, y_ld=ld)                               # dV = P^T dO
-            kt = t_heads(qkv, ld, A)
-            ops.batched_matmul_nt(ds, kt, batch=B, heads=H, m=T, n=dk, k=Tp, a_spec=z_spec, b_spec=d_spec, y_f32=dqkv,
-                                  y_batch_stride=T * ld, y_head_stride=dk, y_ld=ld)                               # dQ = dS K
-            dst_, qt = t_sq(ds), t_heads(qkv, ld, 0)
-            ops.batched_matmul_nt(dst_, qt, batch=B, heads=H, m=T, n=dk, k=Tp, a_spec=z_spec, b_spec=d_spec, y_f32=dqkv[:, :, A:],
-                                  y_batch_stride=T * ld, y_head_stride=dk, y_ld=ld)                               # dK = dS^T Q
-            # fused QKV projection: h1 [A] -> [3A]
-            dqs = Split.from_f32(dqkv)
-            wqkv = self.wqkv(q)
-
-            def qkv_param_grads(q=q, dqkv=dqkv, dqs=dqs, h1=c["h1"], wqkv=wqkv):
-                bsum = torch.zeros(ld, dtype=torch.float32, device=dev)
-                ops.colsum_(dqkv.reshape(B * T, ld), bsum)
-                for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
-                    self.grads[q + "self_attn." + nm + ".bias"].copy_(bsum[j * A:(j + 1) * A])
-                gw = self.conv.wgrad(h1, dqs, wqkv, linear=True)
-                for j, nm in enumerate(("linear_q", "linear_k", "linear_v")):
-                    self.grads[q + "self_attn." + nm + ".weight"].copy_(gw[:, j * A:(j + 1) * A])
-
-            self.on_side(qkv_param_grads, dqkv, dqs, c["h1"])
-            dh1 = self.conv.dgrad(dqs, q + "qkv", wqkv, linear=True)
-            ops.layer_norm_bwd(c["x0"], self.P(q + "norm1.weight"), dh1, dx, True, self.grads[q + "norm1.weight"], self.grads[q + "norm1.bias"])
-        return dx
 
     # ------------------------------------------------------------------------------------------------------------
     # predictors
@@ -389,7 +190,9 @@ class FastSpeech2TrainStep:
         x = ops.embed_pe(text, self.P("encoder.embed.0.weight"), None, self.P("encoder.embed.1.alpha"), None, m.padding_idx)
         if R["transformer_enc_positional_dropout_rate"] > 0:
             self.drop(x, R["transformer_enc_positional_dropout_rate"], self.site(0, 0, 0), inplace=True)
-        hs, hs_split, S_enc = self.stack_fwd(x, "encoder.", m.elayers, ilens)
+        ffn = "lin" if m._linear_ffn else "conv"
+        hs, hs_split, S_enc = self.stack_fwd(x, "encoder.", m.elayers, ilens, heads=m.aheads, ffn=ffn, sid=0,
+                                             r_layer=R["transformer_enc_dropout_rate"], r_attn=R["transformer_enc_attn_dropout_rate"])
         if self.spk:
             hs, hs_split, S_spk = self.spk_fwd(hs, hs_split, spk_id)
         p_raw, S_p = self.pred_fwd("pitch_predictor.", m.cfg["pitch"][0], hs_split)
@@ -422,7 +225,8 @@ class FastSpeech2TrainStep:
         xd = ops.embed_pe(None, None, hs_lr, self.P("decoder.embed.0.alpha"), None)
         if R["transformer_dec_positional_dropout_rate"] > 0:
             self.drop(xd, R["transformer_dec_positional_dropout_rate"], self.site(1, 0, 0), inplace=True)
-        zs, zs_split, S_dec = self.stack_fwd(xd, "decoder.", m.dlayers, olens)
+        zs, zs_split, S_dec = self.stack_fwd(xd, "decoder.", m.dlayers, olens, heads=m.aheads, ffn=ffn, sid=1,
+                                             r_layer=R["transformer_dec_dropout_rate"], r_attn=R["transformer_dec_attn_dropout_rate"])
         before, before_split = self.layer_fwd(zs_split, "feat_out.weight", "feat_out.bias", "lin", out_split=True)
         post, h = [], before_split
         rows = B * t_dec

@@ -17,6 +17,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
     python scripts/make_golden_ref.py ge2e               # only tests/golden/ref_executed_ge2e.npz
     python scripts/make_golden_ref.py tacotron2          # only tests/golden/ref_executed_tacotron2.npz
     python scripts/make_golden_ref.py transformer_tts    # only tests/golden/ref_executed_transformer_tts.npz
+    python scripts/make_golden_ref.py transformer_tts_train    # only tests/golden/ref_executed_transformer_tts_train.npz
 """
 import importlib.util
 import os
@@ -649,6 +650,62 @@ def transformer_tts(out):
             del paddle_standin.Tensor.shape
 
 
+def transformer_tts_train(out):
+    """The training losses and gradients: torch autograd through the reference's own TransformerTTS in train() mode, its own
+    TransformerTTSLoss and GuidedMultiHeadAttentionLoss, composed as TransformerTTSUpdater.update_core does
+    (transformer_tts_updater.py:73-170; the updater class itself needs the Trainer runtime and is not imported), at
+    oracle.transformer_tts_train.TRAIN_SMALL and one ragged batch.  Transformer and postnet dropout rates are 0; the decoder prenet's
+    always-on F.dropout is supplied with the training step's Philox masks (oracle.transformer_tts_train.train_prenet_masks, step 1).
+    Stored: the batch, the losses, every parameter gradient (tensors of up to 1024 elements in full, larger ones as every
+    stride-th element, stride = numel // 1024, plus their L2 norm)."""
+    import types
+    from oracle import transformer_tts_train as ot
+    from parakeet.models.transformer_tts.transformer_tts import (GuidedMultiHeadAttentionLoss, TransformerTTS,
+                                                                 TransformerTTSLoss)
+    from parakeet.modules.tacotron2 import decoder as prenet_mod
+    cfg, seed = ot.TRAIN_SMALL, 13
+    kw = {k: v for k, v in cfg.items() if k not in ("idim", "odim")}
+    ref = TransformerTTS(cfg["idim"], cfg["odim"], **kw)
+    params = ot.synth_params(seed, cfg)
+    check_keys(ref, params, "TransformerTTS(train)")
+    ref.set_state_dict(params)
+    ref.train()
+    text, tl, sp, sl = ot.golden_batch(cfg, seed + 300, lens=(9, 4, 6), frames=(14, 9, 11))
+    for k, v in (("text", text), ("text_lengths", tl), ("speech", sp), ("speech_lengths", sl)):
+        out[f"batch/{k}"] = v.numpy()
+    keep = ot.train_prenet_masks(ot.TRAIN_SEED, 1, sp.shape[0], sp.shape[1], cfg["dprenet_units"], cfg["dprenet_layers"])
+    calls = [0]
+
+    def dropout(x, p=0.5, training=True, **k):
+        assert p == ot.P_PRENET and training and x.dim() == 3
+        i = calls[0] % cfg["dprenet_layers"]
+        calls[0] += 1
+        return T(x * keep[i] * (1.0 / (1.0 - p)))
+
+    saved = prenet_mod.F
+    prenet_mod.F = types.SimpleNamespace(dropout=dropout)
+    try:
+        after, before, logits, ys, labels, olens, ilens, need = ref(T(text), T(tl), T(sp), T(sl))
+        l1, l2, bce = TransformerTTSLoss(use_masking=True, bce_pos_weight=5.0)(after, before, logits, ys, labels, olens)
+        loss = l1 + bce
+        att = []
+        for idx, layer_idx in enumerate(reversed(range(len(need["decoder"].decoders)))):
+            att += [need["decoder"].decoders[layer_idx].src_attn.attn[:, :need["num_heads_applied_guided_attn"]]]
+            if idx + 1 == need["num_layers_applied_guided_attn"]:
+                break
+        g = GuidedMultiHeadAttentionLoss(sigma=0.4, alpha=ot.TRAIN_LAMBDA)(torch.cat(att, 1), ilens, olens)
+        loss = loss + g
+        loss.backward()
+    finally:
+        prenet_mod.F = saved
+    for k, v in dict(loss=loss, l1_loss=l1, l2_loss=l2, bce_loss=bce, enc_dec_attn_loss=g).items():
+        out[k] = np.asarray(float(v.detach().reshape(-1)[0]))
+    for k, v in ref.named_parameters():
+        gk = (v.grad if v.grad is not None else torch.zeros_like(v)).detach().reshape(-1)
+        out[f"grad/{k}"] = gk[::max(1, gk.numel() // 1024)].numpy().astype(np.float32)
+        out[f"gradnorm/{k}"] = np.asarray(float(gk.double().norm()))
+
+
 def wrappers_and_stft(out):
     """FastSpeech2Inference / PWGInference (normaliser wrappers, PWG's replicate padding and transposes) and modules/audio.STFT."""
     import paddle
@@ -721,7 +778,7 @@ def sampled(models):
 def main():
     single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
               "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e,
-              "tacotron2": tacotron2, "transformer_tts": transformer_tts}
+              "tacotron2": tacotron2, "transformer_tts": transformer_tts, "transformer_tts_train": transformer_tts_train}
     if len(sys.argv) == 2 and sys.argv[1] in single:
         uninstall = loader.install(paddle_standin.build())
         try:

@@ -160,6 +160,7 @@ def build():
     P.full = lambda shape, v, dtype=None: T(torch.full(tuple(shape), v, dtype=_dt(dtype) or torch.float32))
     P.ones_like = lambda x, dtype=None: T(torch.ones_like(x, dtype=_dt(dtype)))
     P.zeros_like = lambda x, dtype=None: T(torch.zeros_like(x, dtype=_dt(dtype)))
+    P.meshgrid = lambda *xs: [T(t) for t in torch.meshgrid(*xs, indexing="ij")]       # paddle.meshgrid: 'ij' indexing
     P.arange = lambda start, end=None, step=1, dtype=None: T(torch.arange(start, end, step, dtype=_dt(dtype)) if end is not None else torch.arange(start, dtype=_dt(dtype)))
     P.reshape = lambda x, shape: T(x.reshape(tuple(shape)))
     P.transpose = lambda x, perm: T(x.permute(*perm))
@@ -573,7 +574,8 @@ def build():
     nn.MSELoss = lambda reduction="mean": (lambda a, b: T(TF.mse_loss(a, b, reduction=reduction)))
     nn.L1Loss = lambda reduction="mean": (lambda a, b: T(TF.l1_loss(a, b, reduction=reduction)))
     nn.BCEWithLogitsLoss = lambda weight=None, reduction="mean", pos_weight=None: \
-        (lambda a, b: T(TF.binary_cross_entropy_with_logits(a, b.to(a.dtype), reduction=reduction)))
+        (lambda a, b: T(TF.binary_cross_entropy_with_logits(a, b.to(a.dtype), reduction=reduction, weight=weight,
+                                                            pos_weight=None if pos_weight is None else torch.as_tensor(pos_weight).to(a.dtype))))
 
     init = types.ModuleType("paddle.nn.initializer")
     for name in ("XavierUniform", "XavierNormal", "KaimingUniform", "KaimingNormal", "Uniform", "Normal"):

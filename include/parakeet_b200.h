@@ -367,7 +367,7 @@ int pk_waveflow_row_out(const float* skip, const float* w, const float* bias, co
                         int32_t batch, int32_t width, int32_t c, float* x_next, int64_t x_batch_stride, pk_stream_t stream);
 
 /* All row steps i = 1 .. n_group-1 of one Flow.inverse (:515-556) in ONE persistent dataflow launch (ConditionalWaveFlow.inverse
- * for 64 and 128 channels, 64 < n_mels <= 128 and at most 8 layers per flow).  Per row step, n_layers times
+ * for 64 and 128 channels, 64 < n_mels <= 128 and 2 to 8 layers per flow).  Per row step, n_layers times
  * ResidualBlock.add_input (:248-285):
  *   a | g = conv2d(3-row ring, dilation (1, 2^l)) + condition_proj(condition row) + bias1;  z = tanh(a) sigmoid(g);
  *   skip | res = out_proj(z) + bias2;  skip accumulator (=|+=) skip;  the next layer's ring slot (i - 1) mod 3 <- row + res,

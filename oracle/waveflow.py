@@ -70,7 +70,7 @@ def flow_inverse(p, pre, z, condition, n_layers, n_group, kernel_size=(3, 3)):
             rh = 1 + (kernel_size[0] - 1) * dil[0]
             rw = 1 + (kernel_size[1] - 1) * dil[1]
             if bufs[l] is None:
-                bufs[l] = torch.zeros(B, C, rh, W)
+                bufs[l] = torch.zeros(B, C, rh, W, dtype=z.dtype)
             bufs[l] = torch.cat([bufs[l][:, :, 1:], h], dim=2)
             xin = h
             y = F.conv2d(F.pad(bufs[l], (rw // 2, (rw - 1) // 2, 0, 0)), p[q + "conv.weight"], p[q + "conv.bias"], dilation=dil)

@@ -555,8 +555,12 @@ extern "C" int pk_waveflow_flow(const pk_waveflow_flow_args* a, pk_stream_t stre
   PK_CHECK_ARG(a->channels == 64 || a->channels == 128, "the fused WaveFlow flow is built for 64 or 128 residual channels (got %d)",
                a->channels);
   PK_CHECK_ARG(a->n_mels > 64 && a->n_mels <= 128 && (a->n_mels % 8) == 0, "n_mels must be in (64, 128], a multiple of 8");
-  PK_CHECK_ARG(a->n_layers >= 1 && a->n_layers <= kMaxLayers && a->n_group >= 2 && a->n_group <= kMaxGroup,
-               "n_layers must be 1..8 (width dilation 2^l <= 128) and n_group 2..16");
+  // One layer is refused: the last layer's epilogue writes the next row's input_proj into layer 0's ring slot (r + 1) % 3, which
+  // layer 0 of the same layer-step still reads through its +-1 width taps in the neighbouring tiles, and nothing orders them.
+  PK_CHECK_ARG(a->n_layers >= 2, "n_layers must be at least 2: with one layer the next row's input_proj overwrites layer 0's "
+               "ring slot in the same layer-step whose neighbouring tiles still read it (got %d)", a->n_layers);
+  PK_CHECK_ARG(a->n_layers <= kMaxLayers && a->n_group >= 2 && a->n_group <= kMaxGroup,
+               "n_layers must be 2..8 (width dilation 2^l <= 128) and n_group 2..16");
   PK_CHECK_ARG(a->cond_rows && a->ring_hi && a->ring_lo && a->cond_hi && a->cond_lo && a->w1_hi && a->w1_lo && a->w2_hi && a->w2_lo &&
                a->bias1 && a->bias2 && a->in_w && a->in_b && a->out_w && a->out_b && a->z && a->x && a->skip && a->flags,
                "NULL pointer in pk_waveflow_flow_args");

@@ -6,10 +6,11 @@ state-dict keys (`encoder.{i}.{weight_g,weight_v,bias}`, `decoder.{f}.input_proj
 `predict(mel)`, `forward(audio, mel)` and WaveFlowLoss.  All arithmetic is in libparakeet_b200.so; fold / permute / row
 slicing are torch views and gathers.
 
-Supported this round: kernel_size (3, 3) and n_group in {8, 16} (height dilation 1 -> a 3-row causal buffer), which
-covers the shipped config (examples/waveflow/config.py).  The density direction (`forward`: audio -> z, log-det, the
-held-out negative log-likelihood with WaveFlowLoss) runs for 64 or 128 channels and n_mels in (64, 128]; its training step is
-parakeet_b200.training.WaveFlowTrainStep.
+Accepted configs: kernel_size (3, 3), n_group 8 or 16 (height dilation 1 -> a 3-row causal buffer), even n_flows, 64 or 128
+residual channels and n_mels a multiple of 8; this covers the shipped config (examples/waveflow/config.py).  Within that range
+the fused kernels run every config with 64 < n_mels <= 128 and 2 to 8 layers per flow (`_eligible`); `inverse` runs every
+other accepted config on the two-GEMM row loop.  The density direction (`forward`: audio -> z, log-det, the held-out negative
+log-likelihood with WaveFlowLoss) and its training step (parakeet_b200.training.WaveFlowTrainStep) need the fused kernels.
 """
 import ctypes as C_
 
@@ -52,8 +53,12 @@ class ConditionalWaveFlow(Layer):
             raise NotImplementedError("this round supports kernel_size (3,3) and n_group 8 / 16 (height dilation 1)")
         if n_group % 2 or n_flows % 2:
             raise ValueError("number of flows and number of group must be even")
-        if channels % 64:
-            raise NotImplementedError("channels must be a multiple of 64")
+        if channels not in (64, 128):
+            # the two-GEMM row loop's gate and update epilogues hold at most 2C = 256 output channels
+            raise NotImplementedError(f"channels must be 64 or 128 (got {channels})")
+        if n_mels % 8:
+            # condition rows are GEMM / TMA operands whose row stride (n_mels bf16 elements) must be a multiple of 16 bytes
+            raise NotImplementedError(f"n_mels must be a multiple of 8 (got {n_mels})")
         self.upsample_factors = list(upsample_factors)
         self.n_flows, self.n_layers, self.n_group, self.channels, self.n_mels = n_flows, n_layers, n_group, channels, n_mels
         g = torch.Generator().manual_seed(seed)
@@ -155,10 +160,12 @@ class ConditionalWaveFlow(Layer):
         return pk
 
     def _eligible(self):
-        """Whether the fused kernels cover this config: 64 or 128 residual channels, 64 < n_mels <= 128 (a multiple of 8) and up
+        """Whether the fused kernels cover this config: 64 or 128 residual channels, 64 < n_mels <= 128 (a multiple of 8) and 2
         to 8 layers per flow.  Then inverse runs pk_waveflow_flow (one persistent launch per flow); any other config runs it as
-        the two-GEMM row loop (pk_conv_gemm_ex) and has no density direction."""
-        return self.channels in (64, 128) and 64 < self.n_mels <= 128 and self.n_mels % 8 == 0 and self.n_layers <= 8
+        the two-GEMM row loop (pk_conv_gemm_ex) and has no density direction.  One layer is excluded because pk_waveflow_flow's
+        dataflow needs the last layer's write of the next row into layer 0's ring to be a later layer-step than layer 0's reads
+        of that ring slot."""
+        return self.channels in (64, 128) and 64 < self.n_mels <= 128 and self.n_mels % 8 == 0 and 2 <= self.n_layers <= 8
 
     def _run_flow(self, fw, z, x, cond_s, cmap, bufs, skip, flags, st):
         """Rows 1 .. G-1 of one flow in one launch (row 0 and the ring contents are prepared by the caller)."""
@@ -260,7 +267,7 @@ class ConditionalWaveFlow(Layer):
     def _check_forward(self, audio_len, cond_len):
         if not self._eligible():
             raise NotImplementedError("ConditionalWaveFlow.forward needs 64 or 128 channels, 64 < n_mels <= 128 (a multiple of 8) "
-                                      "and at most 8 layers per flow")
+                                      "and 2 to 8 layers per flow")
         if audio_len > cond_len:
             raise ValueError(f"audio ({audio_len} samples) is longer than its condition ({cond_len} samples)")
 

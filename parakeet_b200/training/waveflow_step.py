@@ -30,7 +30,7 @@ class WaveFlowTrainStep(PdCheckpoint):
     def __init__(self, model, learning_rate=2e-4, sigma=1.0, beta1=0.9, beta2=0.999, epsilon=1e-8, process_group=None):
         if not model._eligible():
             raise NotImplementedError("the WaveFlow training step needs 64 or 128 channels, 64 < n_mels <= 128 (a multiple of 8) "
-                                      "and at most 8 layers per flow")
+                                      "and 2 to 8 layers per flow")
         if model.device.type != "cuda":
             raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
         if not sigma > 0:

@@ -10,6 +10,7 @@ REFERENCE code computes.  tests/test_oracle_cpu.py then holds the oracle to thes
 
     python scripts/make_golden_ref.py        # needs /root/reference; writes tests/golden/ref_executed*.npz
     python scripts/make_golden_ref.py waveflow_forward   # only tests/golden/ref_executed_waveflow_forward.npz
+    python scripts/make_golden_ref.py waveflow_configs   # only tests/golden/ref_executed_waveflow_configs.npz
     python scripts/make_golden_ref.py speedyspeech       # only tests/golden/ref_executed_speedyspeech.npz
     python scripts/make_golden_ref.py waveflow_train     # only tests/golden/ref_executed_waveflow_train.npz
     python scripts/make_golden_ref.py fs2ms_train        # only tests/golden/ref_executed_fs2ms_train.npz
@@ -337,6 +338,37 @@ def waveflow_forward(out):
             out[f"{tag}_z"], out[f"{tag}_log_det"] = z.numpy(), log_det.numpy().reshape(1)
             for sigma in (1.0, 0.7):
                 out[f"{tag}_loss_sigma{sigma}"] = np.asarray(WaveFlowLoss(sigma)(z, log_det).numpy(), dtype=np.float32).reshape(1)
+
+
+WAVEFLOW_CONFIGS = dict(upsample_factors=[8, 32], n_flows=4, n_layers=8, n_group=8, channels=128, n_mels=128)
+
+
+def waveflow_configs(out):
+    """A config away from the shipped one in every dimension the CUDA kernels branch on: n_group 8 (7 row steps), 128 mel
+    bands (4 condition K-steps in the last chunk), 4 flows (the permutations split at 2), upsample factors 8 x 32, 128
+    channels and 8 layers (the only count the reference's ResidualNet takes).  Seed-7 parameters, B = 2, 10 mel frames:
+    the reference's inverse from a given z (W = 284 > 2 x 128) and its forward (audio of 10 * 256 - 5 samples, W = 319) with
+    WaveFlowLoss at two sigmas."""
+    from oracle import waveflow as owf
+    from parakeet.models.waveflow import ConditionalWaveFlow, WaveFlowLoss
+    cfg = WAVEFLOW_CONFIGS
+    ref = ConditionalWaveFlow(kernel_size=[3, 3], **cfg)
+    ref.eval()
+    params = owf.synth_params(7, **cfg)
+    check_keys(ref, params, "ConditionalWaveFlow(waveflow_configs)")
+    ref.set_state_dict(params)
+    g = torch.Generator().manual_seed(48)
+    mel = torch.randn(2, cfg["n_mels"], 10, generator=g) * 0.5 - 3
+    audio = (torch.rand(2, 10 * 256 - 5, generator=g) * 2 - 1) * 0.5
+    with torch.no_grad():
+        cond = ref.encoder(T(mel), trim_conv_artifact=True)
+        z = torch.randn(2, cond.shape[-1], generator=g)
+        out["mel"], out["z"], out["audio"] = mel.numpy(), z.numpy(), audio.numpy()
+        out["x"] = ref.decoder.inverse(T(z), cond).numpy()
+        fz, log_det = ref(T(audio), T(mel))
+        out["fwd_z"], out["fwd_log_det"] = fz.numpy(), log_det.numpy().reshape(1)
+        for sigma in (1.0, 0.7):
+            out[f"loss_sigma{sigma}"] = np.asarray(WaveFlowLoss(sigma)(fz, log_det).numpy(), dtype=np.float32).reshape(1)
 
 
 def waveflow_train(out):
@@ -776,7 +808,7 @@ def sampled(models):
 
 
 def main():
-    single = {"waveflow_forward": waveflow_forward, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
+    single = {"waveflow_forward": waveflow_forward, "waveflow_configs": waveflow_configs, "speedyspeech": speedyspeech, "waveflow_train": waveflow_train,
               "fs2ms_train": fastspeech2_multispeaker_training, "speedyspeech_train": speedyspeech_train, "ge2e": ge2e,
               "tacotron2": tacotron2, "transformer_tts": transformer_tts, "transformer_tts_train": transformer_tts_train}
     if len(sys.argv) == 2 and sys.argv[1] in single:

@@ -178,10 +178,10 @@ def test_vocoder_layer_path_follows_the_model_config(monkeypatch):
 
 def test_waveflow_packs_only_the_operands_of_its_layer_path():
     """An eligible ConditionalWaveFlow packs the fused kernels' operands and none of the two-GEMM row loop's; an n_mels = 64
-    model (outside the fused kernels' range) the reverse."""
+    model (outside the fused kernels' range) and a one-layer model (which pk_waveflow_flow refuses) the reverse."""
     from parakeet_b200.models import ConditionalWaveFlow
-    for n_mels, eligible in ((80, True), (64, False)):
-        m = ConditionalWaveFlow([16, 16], 2, 3, 16, 64, n_mels, (3, 3), device="cpu", seed=9)
+    for n_mels, n_layers, eligible in ((80, 3, True), (64, 3, False), (80, 1, False)):
+        m = ConditionalWaveFlow([16, 16], 2, n_layers, 16, 64, n_mels, (3, 3), device="cpu", seed=9)
         assert m._eligible() == eligible
         for fw in m._pack()["flows"]:
             flow_keys = {"host", "in_w", "in_b", "layers"} | (set() if eligible else {"cond_all", "cond_all_b", "out_w", "out_b"})

@@ -164,7 +164,7 @@ def test_cpu_model_raises_pkerror():
         WaveFlowTrainStep(_model())
 
 
-@pytest.mark.parametrize("kw", [dict(channels=192), dict(n_mels=64), dict(n_mels=136), dict(n_layers=9)])
+@pytest.mark.parametrize("kw", [dict(channels=192), dict(n_mels=64), dict(n_mels=136), dict(n_layers=1), dict(n_layers=9)])
 def test_ineligible_configs_raise_not_implemented(kw):
     from parakeet_b200.training.waveflow_step import WaveFlowTrainStep
     with pytest.raises(NotImplementedError):

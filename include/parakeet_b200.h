@@ -273,10 +273,12 @@ int pk_embed_pe(const int64_t* ids, const float* table, int32_t vocab, int32_t p
  * Outputs: y fp32 and/or split planes (either may be NULL). */
 int pk_layer_norm(const float* x, const float* gamma, const float* beta, float eps, const int32_t* lens, int32_t batch,
                   int32_t t, int32_t d, float* y, void* y_hi, void* y_lo, pk_stream_t stream);
-/* masked_fill(min) -> softmax -> masked_fill(0) of attention.py:107-119 over keys: s fp32 (batch*heads, rows, ld),
- * keys >= key_lens[b] and the padding columns [keys, ld) get probability 0; output split planes, same layout. */
+/* masked_fill(min) -> softmax -> masked_fill(0) of attention.py:107-119 over keys: s fp32 (batch*heads, rows, ld) -> p split
+ * planes, same layout.  Query row i of utterance b attends keys j < key_lens[b] (key_lens NULL: all `keys`) and, when
+ * causal != 0, j <= i (the TransformerTTS decoder's self-attention mask); the other keys and the padding columns [keys, ld)
+ * get probability 0, and a row with no key left is zeros. */
 int pk_masked_softmax(const float* s, const int32_t* key_lens, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
-                      int32_t ld, void* p_hi, void* p_lo, pk_stream_t stream);
+                      int32_t ld, int32_t causal, void* p_hi, void* p_lo, pk_stream_t stream);
 /* paddle.nn.functional.normalize(x, p=2, axis=1, epsilon) on x viewed as (outer, n, inner), norm over the middle axis: the
  * speaker / tone embedding normalisation of FastSpeech2 (fastspeech2.py:577,581,606,611; axis 1 of a (B, T, D) tone tensor is
  * TIME in the reference's batched forward).  x, y fp32 contiguous; in place allowed. */
@@ -501,9 +503,15 @@ int pk_transpose_planes(const void* src_hi, const void* src_lo, int32_t z, int32
 /* LayerNorm backward: dx (+)= d/dx, dgamma += sum dy*xhat, dbeta += sum dy (fp32 [d], accumulated atomically). */
 int pk_layer_norm_bwd(const float* x, const float* gamma, const float* dy, float eps, int64_t rows, int32_t d, float* dx,
                       int32_t accumulate, float* dgamma, float* dbeta, pk_stream_t stream);
-/* softmax backward: ds = scale * p * (dp - sum_k p dp) over the first `keys` columns of rows of pitch ld (rest -> 0). */
-int pk_softmax_bwd(const void* p_hi, const void* p_lo, const float* dp, int64_t rows, int32_t keys, int32_t ld, float scale,
-                   void* ds_hi, void* ds_lo, pk_stream_t stream);
+/* softmax backward: ds = scale * p * (dp' - sum_k p dp') over the first `keys` columns of p, dp, ds (batch * heads, rows, ld),
+ * 0 in columns >= keys; dp is not written.  dp' = dp, except that for heads h < guided_heads GuidedMultiHeadAttentionLoss
+ * (transformer_tts.py:874-1075) is fused in: for rows i < olens[b] and keys j < ilens[b], dp'[i, j] = dp[i, j] + coef G[i, j]
+ * with G = 1 - exp(-(j / ilens[b] - i / olens[b])^2 / (2 sigma^2)) and coef = lambda / (guided_heads * guided_layers *
+ * sum_b ilens[b] olens[b]), and partials[(b * guided_heads + h) * rows + i] = sum_j G P (0 for i >= olens[b]).
+ * With guided_heads 0, ilens, olens and partials may be NULL. */
+int pk_softmax_bwd(const void* p_hi, const void* p_lo, const float* dp, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
+                   int32_t ld, float scale, int32_t guided_heads, int32_t guided_layers, const int32_t* ilens, const int32_t* olens,
+                   float sigma, float lambda, float* partials, void* ds_hi, void* ds_lo, pk_stream_t stream);
 /* out[c] += sum_rows x[row, c] (bias gradients). */
 int pk_colsum(const float* x, int64_t rows, int32_t c, float* out, pk_stream_t stream);
 /* pk_colsum on split planes (rows, ld): out[c] += sum_rows (x_hi + x_lo)[row, c] for c < cols (bias gradients from the split
@@ -539,8 +547,6 @@ int pk_length_regulate_bwd(const float* dy, const int64_t* dur, int32_t batch, i
 /* weight / bias gradients of pitch_embed / energy_embed (Conv1D(1 -> c, k) on a scalar track): dw [c][k], db [c] accumulated */
 int pk_scalar_conv_wgrad(const float* dhs, const float* track, int32_t batch, int32_t t, int32_t c, int32_t k, float* dw, float* db,
                          pk_stream_t stream);
-/* paddle.optimizer.Adam step on a flat buffer (training/optimizer.py:17-46): g * grad_scale (1/world for DataParallel),
- * lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), p -= lr_t * m / (sqrt(v) + eps * sqrt(1 - beta2^t)). */
 /* nn.Dropout in training mode (upscale_in_train): y[i] = keep(i) ? x[i] / (1 - p) : 0, keep(i) = word (i & 3) of
  * Philox4x32-10(counter {i >> 2 low, high, site, step}, key {seed low, high}) >= p * 2^32.  Input fp32 x or split planes
  * (x_hi + x_lo), outputs fp32 and/or split planes; in place allowed.  The backward pass applies the same call to the gradient
@@ -550,8 +556,12 @@ int pk_scalar_conv_wgrad(const float* dhs, const float* track, int32_t batch, in
 int pk_dropout(const float* x, const void* x_hi, const void* x_lo, int64_t n, float p, uint64_t seed, uint32_t site, uint32_t step,
                const uint32_t* step_dev /* device uint32 added to `step` (NULL: none) - lets a CUDA graph replay draw fresh masks */,
                float* y, void* y_hi, void* y_lo, pk_stream_t stream);
+/* paddle.optimizer.Adam step on a flat buffer (training/optimizer.py:17-46) with ClipGradByGlobalNorm folded in: the gradient
+ * g * grad_scale * clip_norm / max(sqrt(*sqnorm), clip_norm) (grad_scale 1/world for DataParallel; sqnorm from pk_sq_sum; sqnorm
+ * NULL or clip_norm <= 0: no clipping), lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), p -= lr_t * m / (sqrt(v) + eps *
+ * sqrt(1 - beta2^t)). */
 int pk_adam(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
-            int32_t step, float grad_scale, pk_stream_t stream);
+            int32_t step, float grad_scale, const double* sqnorm, float clip_norm, pk_stream_t stream);
 /* Speaker conditioning of the multi-speaker training step (fastspeech2.py:148-152 spk_embedding_table = nn.Embedding(num_speakers,
  * D, padding_idx=0); :395-401 and _integrate_with_spk_embed :560-590: F.normalize(p=2, axis=1, epsilon) then the "concat" / "add"
  * projection, whose GEMMs run through pk_conv_gemm).  Speaker ids are int64 on the device and never read on the host; ids equal
@@ -591,11 +601,8 @@ int pk_weight_norm_fwd(const float* v, const float* g, int32_t rows, int32_t inn
 int pk_weight_norm_bwd(const float* v, const float* g, const float* dw, int32_t rows, int32_t inner, float* dg, float* dv, pk_stream_t stream);
 /* MSELoss against a constant over x[i * ld + col], i < n: acc[0] += sum (x - target)^2 (device double); dx (or NULL) = coef * (x - target). */
 int pk_mse_const(const float* x, int64_t n, int32_t ld, int32_t col, float target, double* acc, float* dx, float coef, pk_stream_t stream);
-/* acc[0] += sum x^2 (device double): the global gradient norm of ClipGradByGlobalNorm. */
+/* acc[0] += sum x^2 (device double): the global gradient norm of ClipGradByGlobalNorm (pk_adam's sqnorm). */
 int pk_sq_sum(const float* x, int64_t n, double* acc, pk_stream_t stream);
-/* pk_adam with ClipGradByGlobalNorm folded in: g <- g * clip / max(sqrt(*sqnorm), clip) (sqnorm NULL or clip <= 0: no clipping). */
-int pk_adam_clip(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
-                 int32_t step, const double* sqnorm, float clip_norm, pk_stream_t stream);
 /* generator residual / skip update (:311-315, :466-468): so (rows, 128) = [skip | out]; skips (=|+=) skip; xo = (out + x) * sqrt(1/2)
  * as fp32 and split planes; and its backward: dso = [dskips | dxo * sqrt(1/2)], dx_res = dxo * sqrt(1/2). */
 int pk_pwg_res_update(const float* so, const float* x, int64_t rows, float* skips, int32_t init, float* xo, void* xo_hi, void* xo_lo,
@@ -904,22 +911,10 @@ int pk_tts_stop_labels(const int32_t* olens, int32_t batch, int32_t width, float
 /* ------------------------------------------------------------------------------------------------------------
  * TransformerTTS training step (reference: TransformerTTSUpdater.update_core, models/transformer_tts/
  * transformer_tts_updater.py:73-170).  The attention runs on the materialised path of the FastSpeech2 step (pk_conv_gemm,
- * softmax, pk_dropout); these add the causal mask, the guided source-attention loss and TransformerTTSLoss.  No atomics.
+ * pk_masked_softmax with its causal mask, pk_dropout, pk_softmax_bwd with the guided source-attention loss fused in); these
+ * add the guided loss's value and TransformerTTSLoss.  No atomics.
  * ------------------------------------------------------------------------------------------------------------ */
-/* pk_masked_softmax with an optional causal mask: s (batch * heads, rows, ld) -> p split planes; query row i of utterance b
- * attends keys j < key_lens[b] (key_lens NULL: all `keys`) and, when causal != 0, j <= i.  Rows with no key left are zeros. */
-int pk_masked_softmax_ex(const float* s, const int32_t* key_lens, int32_t batch, int32_t heads, int32_t rows, int32_t keys, int32_t ld,
-                         int32_t causal, void* p_hi, void* p_lo, pk_stream_t stream);
-/* pk_softmax_bwd with GuidedMultiHeadAttentionLoss (transformer_tts.py:874-1075) fused in.  p, dp, ds: (batch * heads, rows, ld).
- * For heads h < guided_heads, rows i < olens[b], keys j < ilens[b]: dp[i, j] + coef G[i, j] enters the backward, with
- * G = 1 - exp(-(j / ilens[b] - i / olens[b])^2 / (2 sigma^2)) and coef = lambda / (guided_heads * guided_layers *
- * sum_b ilens[b] olens[b]); partials[(b * guided_heads + h) * rows + i] = sum_j G P (0 for i >= olens[b]).  dp is the gradient
- * w.r.t. the pre-dropout probabilities and is not written; ds = scale * p * (dp' - sum_k p dp'), 0 in columns >= keys.
- * guided_heads 0 is pk_softmax_bwd (ilens, olens and partials may then be NULL). */
-int pk_softmax_bwd_guided(const void* p_hi, const void* p_lo, const float* dp, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
-                          int32_t ld, float scale, int32_t guided_heads, int32_t guided_layers, const int32_t* ilens, const int32_t* olens,
-                          float sigma, float lambda, float* partials, void* ds_hi, void* ds_lo, pk_stream_t stream);
-/* The guided loss from the n partials of pk_softmax_bwd_guided (every guided layer's): lambda * sum / (heads_layers *
+/* The guided loss from the n partials of pk_softmax_bwd (every guided layer's): lambda * sum / (heads_layers *
  * sum_b min(ilens[b], keys) min(olens[b], rows)) -> losses[4], and added to losses[0]. */
 int pk_tts_guided_loss(const float* partials, int64_t n, const int32_t* ilens, const int32_t* olens, int32_t batch, int32_t rows,
                        int32_t keys, int32_t heads_layers, float lambda, float* losses, pk_stream_t stream);

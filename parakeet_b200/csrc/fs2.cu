@@ -10,12 +10,6 @@
 
 namespace pk {
 
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // x[b,t,:] = (ids ? W[ids[b,t]] (zeros for id == padding_idx) : x_in[b,t,:]) + alpha * PE[t,:]
 // PE[t, 2i] = sin(t * exp(2i * -ln(1e4)/d)), PE[t, 2i+1] = cos(...)   (embedding.py:46-62, fp32 arithmetic)
@@ -97,18 +91,20 @@ layer_norm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Masked softmax over keys: s (z, rows, ld) fp32 -> p split planes (z, rows, ld); keys >= klen[b] (and the padding
-// columns up to ld) get probability 0; a fully masked row yields zeros (attention.py:107-119).  One warp per row.
+// Masked softmax over keys, optionally causal: s (batch * heads, rows, ld) fp32 -> p split planes of the same shape.  Query row
+// i of utterance b attends keys j < key_lens[b] (all `keys` when key_lens is NULL) and, when causal, j <= i: attention.py:107-119
+// and the TransformerTTS decoder's non_pad(olens) & tril mask (transformer_tts.py:692 _target_mask).  Masked and padding
+// columns get 0; a row with no key left is all zeros (masked_fill(min) -> softmax -> masked_fill(0)).  One warp per row.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-softmax_kernel(const float* __restrict__ s, const int32_t* __restrict__ klens, int heads, int rows_per_z, int keys, int ld,
-               long long rows, __nv_bfloat16* __restrict__ p_hi, __nv_bfloat16* __restrict__ p_lo) {
+masked_softmax_kernel(const float* __restrict__ s, const int32_t* __restrict__ klens, int heads, int rows_per_z, int keys, int ld,
+                      int causal, long long rows, __nv_bfloat16* __restrict__ p_hi, __nv_bfloat16* __restrict__ p_lo) {
   const long long row = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const int z = row / rows_per_z;
-  const int b = z / heads;
-  const int klen = klens ? min(__ldg(klens + b), keys) : keys;
+  const int z = static_cast<int>(row / rows_per_z), i = static_cast<int>(row % rows_per_z);
+  int klen = klens ? min(__ldg(klens + z / heads), keys) : keys;
+  if (causal) klen = min(klen, i + 1);
   const float* sr = s + row * ld;
   float m = -CUDART_INF_F;
   for (int c = lane; c < klen; c += 32) m = fmaxf(m, sr[c]);
@@ -221,8 +217,6 @@ __global__ void zscore_kernel(const float* __restrict__ x, const float* __restri
   y[i] = mode == 0 ? (x[i] - __ldg(mu + ch)) / __ldg(sigma + ch) : fmaf(x[i], __ldg(sigma + ch), __ldg(mu + ch));
 }
 
-static inline int blocks_for(long long n, int threads) { return static_cast<int>((n + threads - 1) / threads); }
-
 }  // namespace pk
 
 using namespace pk;
@@ -234,8 +228,8 @@ extern "C" int pk_embed_pe(const int64_t* ids, const float* table, int32_t vocab
   PK_CHECK_ARG(ids == nullptr || table != nullptr, "table is NULL");
   PK_CHECK_ARG(alpha && y && batch > 0 && t > 0 && d > 0, "bad arguments");
   const long long rows = static_cast<long long>(batch) * t;
-  embed_pe_kernel<<<blocks_for(rows * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ids, table, vocab, padding_idx, x_in,
-                                                                                            alpha, lens, t, rows, d, y);
+  embed_pe_kernel<<<nblk(rows * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ids, table, vocab, padding_idx, x_in,
+                                                                                       alpha, lens, t, rows, d, y);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -248,7 +242,7 @@ extern "C" int pk_layer_norm(const float* x, const float* gamma, const float* be
   PK_CHECK_ARG((y_hi == nullptr) == (y_lo == nullptr), "y_hi and y_lo must both be set or both NULL");
   PK_CHECK_ARG(d <= 2048, "layer_norm supports d <= 2048 (got %d)", d);
   const long long rows = static_cast<long long>(batch) * t;
-  const int blocks = blocks_for(rows * 32, 256);
+  const int blocks = nblk(rows * 32, 256);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   auto* hi = static_cast<__nv_bfloat16*>(y_hi);
   auto* lo = static_cast<__nv_bfloat16*>(y_lo);
@@ -261,14 +255,12 @@ extern "C" int pk_layer_norm(const float* x, const float* gamma, const float* be
 }
 
 extern "C" int pk_masked_softmax(const float* s, const int32_t* key_lens, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
-                                 int32_t ld, void* p_hi, void* p_lo, pk_stream_t stream) {
-  PK_CHECK_ARG(s && p_hi && p_lo && batch > 0 && heads > 0 && rows > 0 && keys > 0 && ld >= keys, "bad arguments");
+                                 int32_t ld, int32_t causal, void* p_hi, void* p_lo, pk_stream_t stream) {
+  PK_CHECK_ARG(s && p_hi && p_lo && batch > 0 && heads > 0 && rows > 0 && keys > 0 && ld >= keys, "bad arguments to pk_masked_softmax");
   const long long total = static_cast<long long>(batch) * heads * rows;
-  softmax_kernel<<<blocks_for(total * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      s, key_lens, heads, rows, keys, ld, total, static_cast<__nv_bfloat16*>(p_hi), static_cast<__nv_bfloat16*>(p_lo));
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
+  masked_softmax_kernel<<<nblk(total * 32, 256), 256, 0, PK_STREAM>>>(s, key_lens, heads, rows, keys, ld, causal ? 1 : 0, total,
+                                                                       static_cast<__nv_bfloat16*>(p_hi), static_cast<__nv_bfloat16*>(p_lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_transpose_heads(const void* src_hi, const void* src_lo, int32_t batch, int32_t t, int32_t ld_src, int32_t col0,
@@ -287,7 +279,7 @@ extern "C" int pk_duration_post(const float* x, const int32_t* lens, int32_t bat
                                 int64_t* d_i64, pk_stream_t stream) {
   PK_CHECK_ARG(x && (d_f32 || d_i64) && batch > 0 && t > 0, "bad arguments");
   const long long n = static_cast<long long>(batch) * t;
-  duration_post_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, lens, t, n, offset, d_f32, d_i64);
+  duration_post_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, lens, t, n, offset, d_f32, d_i64);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -295,7 +287,7 @@ extern "C" int pk_duration_post(const float* x, const int32_t* lens, int32_t bat
 
 extern "C" int pk_duration_scale(const int64_t* d, float alpha, int64_t n, int64_t* out, pk_stream_t stream) {
   PK_CHECK_ARG(d && out && n > 0 && alpha > 0.f, "bad arguments");
-  duration_scale_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(d, alpha, n, out);
+  duration_scale_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(d, alpha, n, out);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -304,7 +296,7 @@ extern "C" int pk_duration_scale(const int64_t* d, float alpha, int64_t n, int64
 extern "C" int pk_mask_rows(float* x, const int32_t* lens, int32_t batch, int32_t t, int32_t inner, pk_stream_t stream) {
   PK_CHECK_ARG(x && lens && batch > 0 && t > 0 && inner > 0, "bad arguments");
   const long long n = static_cast<long long>(batch) * t * inner;
-  mask_rows_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, lens, t, inner, n);
+  mask_rows_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, lens, t, inner, n);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -316,8 +308,8 @@ extern "C" int pk_variance_embed_add(const float* hs, const float* pitch, const 
   PK_CHECK_ARG(hs && pitch && energy && wp && bp && we && be && y, "NULL pointer");
   PK_CHECK_ARG(batch > 0 && t > 0 && c > 0 && kp >= 1 && ke >= 1 && (kp & 1) && (ke & 1), "bad sizes (odd kernel sizes only)");
   const long long n = static_cast<long long>(batch) * t * c;
-  variance_embed_add_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(hs, pitch, energy, wp, bp, kp, we, be,
-                                                                                              ke, lens, t, c, n, y);
+  variance_embed_add_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(hs, pitch, energy, wp, bp, kp, we, be,
+                                                                                         ke, lens, t, c, n, y);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -326,7 +318,7 @@ extern "C" int pk_variance_embed_add(const float* hs, const float* pitch, const 
 extern "C" int pk_zscore(const float* x, const float* mu, const float* sigma, int32_t c, int64_t n, int32_t inverse, float* y,
                          pk_stream_t stream) {
   PK_CHECK_ARG(x && mu && sigma && y && c > 0 && n > 0, "bad arguments");
-  zscore_kernel<<<blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, mu, sigma, c, n, inverse ? 1 : 0, y);
+  zscore_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, mu, sigma, c, n, inverse ? 1 : 0, y);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

@@ -119,7 +119,6 @@ spk_table_grad_kernel(const float* __restrict__ de, const int64_t* __restrict__ 
 }  // namespace pk
 
 using namespace pk;
-#define PK_STREAM static_cast<cudaStream_t>(stream)
 
 extern "C" int pk_spk_embed_fwd(const float* table, int32_t num_speakers, int32_t d, const int64_t* ids, int32_t batch,
                                 int32_t padding_idx, float eps, float* e, float* norms, pk_stream_t stream) {

@@ -6,7 +6,8 @@
 //   weight norm w = g v / ||v|| forward / backward (nn.utils.weight_norm, dim 0), MSE against a constant (criterion_mse),
 //   the generator's residual / skip update, the upsampling stages (Stretch2D + FIR Conv2D, :48-63,119-138) one stage at a time
 //   with their backward, the multi-resolution STFT loss gradient (modules/stft_loss.py:163-219) and the framing adjoint
-//   (overlap-add through the reflect padding), the global gradient norm (ClipGradByGlobalNorm) and Adam with the clip folded in.
+//   (overlap-add through the reflect padding), the global gradient norm (ClipGradByGlobalNorm) that
+//   pk_adam (train.cu) clips with.
 #include <math.h>
 
 #include "pk_host.h"
@@ -14,10 +15,6 @@
 
 namespace pk {
 namespace gan {
-
-static inline int nblk(long long n, int threads) { return static_cast<int>(std::min<long long>((n + threads - 1) / threads, 1 << 20)); }
-#define PK_GRID_STRIDE(i, n) \
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); i += static_cast<long long>(gridDim.x) * blockDim.x)
 
 // block-wide sum -> one atomicAdd per block (double accumulator: the sums feed loss values and gradient norms)
 __device__ __forceinline__ void block_accumulate(float v, double* out) {
@@ -131,23 +128,6 @@ __global__ void sq_sum_kernel(const float* __restrict__ x, long long n, double* 
   PK_GRID_STRIDE(i, n) s = fmaf(x[i], x[i], s);
   block_accumulate(s, acc);
 }
-// paddle.optimizer.Adam + ClipGradByGlobalNorm: g <- g * clip / max(||g||, clip) with the global norm read from device memory
-__global__ void adam_clip_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n,
-                                 float lr_t, float b1, float b2, float eps_t, const double* __restrict__ sqnorm, float clip) {
-  float sc = 1.f;
-  if (sqnorm != nullptr && clip > 0.f) {
-    const float gn = sqrtf(static_cast<float>(*sqnorm));
-    sc = clip / fmaxf(gn, clip);
-  }
-  PK_GRID_STRIDE(i, n) {
-    const float gi = g[i] * sc;
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi; v[i] = vi;
-    p[i] -= lr_t * mi / (sqrtf(vi) + eps_t);
-  }
-}
-
 // ---------------------------------------------------------------- generator residual / skip update (parallel_wavegan.py:311-315, :466-468)
 // so (rows, 128) = [skip | out] of conv1x1_skip / conv1x1_out (bias included); skips (=|+=) skip; x' = (out + x) * sqrt(1/2)
 __global__ void pwg_res_update_kernel(const float* __restrict__ so, const float* __restrict__ x, long long rows, float* __restrict__ skips, int init,
@@ -272,100 +252,86 @@ __global__ void frames_overlap_add_kernel(const float* __restrict__ fg, const fl
 }  // namespace gan
 }  // namespace pk
 
-#define PK_ST static_cast<cudaStream_t>(stream)
-#define PK_DONE()                      \
-  PK_CHECK_CUDA(cudaGetLastError());   \
-  pk::count_launch();                  \
-  return PK_OK;
-
 extern "C" int pk_gate_fwd(const float* h, int64_t rows, int32_t c, float* z, void* z_hi, void* z_lo, pk_stream_t stream) {
   PK_CHECK_ARG(h && rows > 0 && c > 0 && (z || z_hi) && (z_hi == nullptr) == (z_lo == nullptr), "bad arguments");
-  pk::gan::gate_fwd_kernel<<<pk::gan::nblk(rows * c, 256), 256, 0, PK_ST>>>(h, rows, c, z, static_cast<__nv_bfloat16*>(z_hi), static_cast<__nv_bfloat16*>(z_lo));
-  PK_DONE()
+  pk::gan::gate_fwd_kernel<<<pk::grid_stride_blocks(rows * c, 256), 256, 0, PK_STREAM>>>(h, rows, c, z, static_cast<__nv_bfloat16*>(z_hi), static_cast<__nv_bfloat16*>(z_lo));
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_gate_bwd(const float* h, const float* dz, int64_t rows, int32_t c, float* dh, pk_stream_t stream) {
   PK_CHECK_ARG(h && dz && dh && rows > 0 && c > 0, "bad arguments");
-  pk::gan::gate_bwd_kernel<<<pk::gan::nblk(rows * c, 256), 256, 0, PK_ST>>>(h, dz, rows, c, dh);
-  PK_DONE()
+  pk::gan::gate_bwd_kernel<<<pk::grid_stride_blocks(rows * c, 256), 256, 0, PK_STREAM>>>(h, dz, rows, c, dh);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_leaky_relu(const float* x, int64_t n, float slope, float* y, void* y_hi, void* y_lo, pk_stream_t stream) {
   PK_CHECK_ARG(x && n > 0 && (y || y_hi) && (y_hi == nullptr) == (y_lo == nullptr), "bad arguments");
-  pk::gan::leaky_fwd_kernel<<<pk::gan::nblk(n, 256), 256, 0, PK_ST>>>(x, n, slope, y, static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo));
-  PK_DONE()
+  pk::gan::leaky_fwd_kernel<<<pk::grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(x, n, slope, y, static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo));
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_leaky_relu_bwd(const float* x, const float* dy, int64_t n, float slope, float* dx, pk_stream_t stream) {
   PK_CHECK_ARG(x && dy && dx && n > 0, "bad arguments");
-  pk::gan::leaky_bwd_kernel<<<pk::gan::nblk(n, 256), 256, 0, PK_ST>>>(x, dy, n, slope, dx);
-  PK_DONE()
+  pk::gan::leaky_bwd_kernel<<<pk::grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(x, dy, n, slope, dx);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_weight_norm_fwd(const float* v, const float* g, int32_t rows, int32_t inner, float* w, float* norm, pk_stream_t stream) {
   PK_CHECK_ARG(v && g && w && rows > 0 && inner > 0, "bad arguments");
-  pk::gan::weight_norm_fwd_kernel<<<rows, 128, 0, PK_ST>>>(v, g, inner, w, norm);
-  PK_DONE()
+  pk::gan::weight_norm_fwd_kernel<<<rows, 128, 0, PK_STREAM>>>(v, g, inner, w, norm);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_weight_norm_bwd(const float* v, const float* g, const float* dw, int32_t rows, int32_t inner, float* dg, float* dv,
                                   pk_stream_t stream) {
   PK_CHECK_ARG(v && g && dw && dg && dv && rows > 0 && inner > 0, "bad arguments");
-  pk::gan::weight_norm_bwd_kernel<<<rows, 128, 0, PK_ST>>>(v, g, dw, inner, dg, dv);
-  PK_DONE()
+  pk::gan::weight_norm_bwd_kernel<<<rows, 128, 0, PK_STREAM>>>(v, g, dw, inner, dg, dv);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_mse_const(const float* x, int64_t n, int32_t ld, int32_t col, float target, double* acc, float* dx, float coef,
                             pk_stream_t stream) {
   PK_CHECK_ARG(x && acc && n > 0 && ld > 0 && col >= 0 && col < ld, "bad arguments");
-  pk::gan::mse_const_kernel<<<pk::gan::nblk(n, 256), 256, 0, PK_ST>>>(x, n, ld, col, target, acc, dx, coef);
-  PK_DONE()
+  pk::gan::mse_const_kernel<<<pk::grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(x, n, ld, col, target, acc, dx, coef);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_sq_sum(const float* x, int64_t n, double* acc, pk_stream_t stream) {
   PK_CHECK_ARG(x && acc && n > 0, "bad arguments");
-  pk::gan::sq_sum_kernel<<<std::min(pk::gan::nblk(n, 256), 2048), 256, 0, PK_ST>>>(x, n, acc);
-  PK_DONE()
-}
-extern "C" int pk_adam_clip(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
-                            int32_t step, const double* sqnorm, float clip_norm, pk_stream_t stream) {
-  PK_CHECK_ARG(params && grads && m && v && n > 0 && step >= 1, "bad arguments");
-  const double c1 = 1.0 - pow(static_cast<double>(beta1), step), c2 = sqrt(1.0 - pow(static_cast<double>(beta2), step));
-  pk::gan::adam_clip_kernel<<<pk::gan::nblk(n, 256), 256, 0, PK_ST>>>(params, grads, m, v, n, static_cast<float>(lr * c2 / c1), beta1, beta2,
-                                                                     static_cast<float>(eps * c2), sqnorm, clip_norm);
-  PK_DONE()
+  pk::gan::sq_sum_kernel<<<std::min(pk::grid_stride_blocks(n, 256), 2048), 256, 0, PK_STREAM>>>(x, n, acc);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_pwg_res_update(const float* so, const float* x, int64_t rows, float* skips, int32_t init, float* xo, void* xo_hi, void* xo_lo,
                                  pk_stream_t stream) {
   PK_CHECK_ARG(so && x && skips && xo && xo_hi && xo_lo && rows > 0, "bad arguments");
-  pk::gan::pwg_res_update_kernel<<<pk::gan::nblk(rows * 64, 256), 256, 0, PK_ST>>>(so, x, rows, skips, init, xo, static_cast<__nv_bfloat16*>(xo_hi),
-                                                                                  static_cast<__nv_bfloat16*>(xo_lo));
-  PK_DONE()
+  pk::gan::pwg_res_update_kernel<<<pk::grid_stride_blocks(rows * 64, 256), 256, 0, PK_STREAM>>>(so, x, rows, skips, init, xo, static_cast<__nv_bfloat16*>(xo_hi),
+                                                                                                static_cast<__nv_bfloat16*>(xo_lo));
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_pwg_res_update_bwd(const float* dskips, const float* dxo, int64_t rows, float* dso, float* dx_res, pk_stream_t stream) {
   PK_CHECK_ARG(dskips && dxo && dso && dx_res && rows > 0, "bad arguments");
-  pk::gan::pwg_res_update_bwd_kernel<<<pk::gan::nblk(rows * 64, 256), 256, 0, PK_ST>>>(dskips, dxo, rows, dso, dx_res);
-  PK_DONE()
+  pk::gan::pwg_res_update_bwd_kernel<<<pk::grid_stride_blocks(rows * 64, 256), 256, 0, PK_STREAM>>>(dskips, dxo, rows, dso, dx_res);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_up_stage_fwd(const float* x, const float* fir, int64_t rows, int32_t tin, int32_t s, float* y, pk_stream_t stream) {
   PK_CHECK_ARG(x && fir && y && rows > 0 && tin > 0 && s >= 1, "bad arguments");
-  pk::gan::up_stage_fwd_kernel<<<pk::gan::nblk(rows * tin * s, 256), 256, 0, PK_ST>>>(x, fir, rows, tin, s, y);
-  PK_DONE()
+  pk::gan::up_stage_fwd_kernel<<<pk::grid_stride_blocks(rows * tin * s, 256), 256, 0, PK_STREAM>>>(x, fir, rows, tin, s, y);
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_up_stage_bwd(const float* x, const float* dy, const float* fir, int64_t rows, int32_t tin, int32_t s, float* dx, double* dfir,
                                pk_stream_t stream) {
   PK_CHECK_ARG(x && dy && fir && rows > 0 && tin > 0 && s >= 1 && (dx || dfir), "bad arguments");
-  if (dx) pk::gan::up_stage_bwd_data_kernel<<<pk::gan::nblk(rows * tin, 256), 256, 0, PK_ST>>>(dy, fir, rows, tin, s, dx);
+  if (dx) pk::gan::up_stage_bwd_data_kernel<<<pk::grid_stride_blocks(rows * tin, 256), 256, 0, PK_STREAM>>>(dy, fir, rows, tin, s, dx);
   if (dfir) {
-    dim3 grid(std::min(pk::gan::nblk(rows * tin * s, 256), 512), 2 * s + 1);
-    pk::gan::up_stage_bwd_fir_kernel<<<grid, 256, 0, PK_ST>>>(x, dy, rows, tin, s, dfir);
+    dim3 grid(std::min(pk::grid_stride_blocks(rows * tin * s, 256), 512), 2 * s + 1);
+    pk::gan::up_stage_bwd_fir_kernel<<<grid, 256, 0, PK_STREAM>>>(x, dy, rows, tin, s, dfir);
   }
-  PK_DONE()
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_stft_loss_grad(const float* xre, const float* xim, const float* yre, const float* yim, int32_t batch, int32_t bins,
                                  int32_t frames, int32_t bins_p, const float* sums, float weight, float* g, pk_stream_t stream) {
   PK_CHECK_ARG(xre && xim && yre && yim && sums && g && batch > 0 && bins > 0 && frames > 0 && bins_p >= bins, "bad arguments");
-  pk::gan::stft_loss_grad_kernel<<<pk::gan::nblk(static_cast<long long>(batch) * bins * frames, 256), 256, 0, PK_ST>>>(
+  pk::gan::stft_loss_grad_kernel<<<pk::grid_stride_blocks(static_cast<long long>(batch) * bins * frames, 256), 256, 0, PK_STREAM>>>(
       xre, xim, yre, yim, batch, bins, frames, bins_p, sums, weight, g);
-  PK_DONE()
+  PK_LAUNCH_DONE(1);
 }
 extern "C" int pk_frames_overlap_add(const float* frames_grad, const float* window, int32_t batch, int32_t frames, int32_t n_fft, int32_t hop,
                                      int32_t t, float* dx, pk_stream_t stream) {
   PK_CHECK_ARG(frames_grad && window && dx && batch > 0 && frames > 0 && n_fft > 0 && hop > 0 && t > n_fft / 2, "bad arguments");
-  pk::gan::frames_overlap_add_kernel<<<pk::gan::nblk(static_cast<long long>(batch) * frames * n_fft, 256), 256, 0, PK_ST>>>(
+  pk::gan::frames_overlap_add_kernel<<<pk::grid_stride_blocks(static_cast<long long>(batch) * frames * n_fft, 256), 256, 0, PK_STREAM>>>(
       frames_grad, window, batch, frames, n_fft, hop, t, dx);
-  PK_DONE()
+  PK_LAUNCH_DONE(1);
 }

@@ -292,19 +292,6 @@ __global__ void __launch_bounds__(kThreads, 1) lstm_bwd_kernel(const __grid_cons
 // GE2E softmax loss on embeds (n, m, c), one block in double (lstm_speaker_encoder.py similarity_matrix / loss; phases below).
 constexpr int kLossThreads = 512;
 
-__device__ double block_sum(double v, double* red) {
-  // fixed-order tree over the block (deterministic); red holds kLossThreads doubles
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = kLossThreads / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-    __syncthreads();
-  }
-  const double r = red[0];
-  __syncthreads();
-  return r;
-}
-
 __global__ void __launch_bounds__(kLossThreads, 1)
 ge2e_loss_kernel(const float* __restrict__ e, int N, int M, int C, const float* __restrict__ wp, const float* __restrict__ bp,
                  double* ws, float* loss, float* sim, float* de, float* dw, float* db) {
@@ -369,12 +356,12 @@ ge2e_loss_kernel(const float* __restrict__ e, int N, int M, int C, const float* 
   __syncthreads();
   double part = 0.0;
   for (int r = tid; r < NM; r += kLossThreads) part += lrow[r];
-  const double total = block_sum(part, red);
+  const double total = block_sum_tree<kLossThreads>(part, red);
   if (tid == 0) loss[0] = static_cast<float>(total * inv);
   if (!de) return;
   double pw = 0.0, pb = 0.0;
   for (int i = tid; i < NM * N; i += kLossThreads) { pw += dsm[i] * p[i]; pb += dsm[i]; }
-  const double gw = block_sum(pw, red), gb = block_sum(pb, red);
+  const double gw = block_sum_tree<kLossThreads>(pw, red), gb = block_sum_tree<kLossThreads>(pb, red);
   if (tid == 0) { dw[0] = static_cast<float>(0.01 * gw); db[0] = static_cast<float>(0.01 * gb); }   // do_gradient_ops
   for (int i = tid; i < NM * C; i += kLossThreads) {
     const int r = i / C, cc = i - r * C, j = r / M;

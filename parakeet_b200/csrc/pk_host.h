@@ -43,6 +43,21 @@ int encode_tmap_f32_3d(CUtensorMap* out, const void* base, uint64_t rows, uint64
 int sm_count();
 void count_launch(int n = 1);
 
+// Grid size for n items, one thread per item: ceil(n / threads) blocks.
+inline int nblk(long long n, int threads) { return static_cast<int>((n + threads - 1) / threads); }
+// The same capped at 2^20 blocks.  Only for grid-stride kernels (PK_GRID_STRIDE), which cover any n with a capped grid.
+inline int grid_stride_blocks(long long n, int threads) {
+  const long long b = (n + threads - 1) / threads;
+  return static_cast<int>(b < (1 << 20) ? b : (1 << 20));
+}
+
+// The stream argument of a C entry point, and its tail after the last of `n` launches.
+#define PK_STREAM static_cast<cudaStream_t>(stream)
+#define PK_LAUNCH_DONE(n)            \
+  PK_CHECK_CUDA(cudaGetLastError()); \
+  ::pk::count_launch(n);             \
+  return PK_OK
+
 // Readies a kernel for a launch with `threads` threads and `smem` bytes of dynamic shared memory on the current device: raises
 // its dynamic shared-memory limit to cover smem (a CUDA call only the first time the kernel needs more on that device).  With
 // resident_ctas, also returns how many such CTAs the device holds at once (occupancy x SMs, queried once per kernel, device and

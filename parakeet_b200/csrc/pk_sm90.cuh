@@ -154,6 +154,10 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
+// element i of a split-bf16 tensor as fp32
+__device__ __forceinline__ float ld_split(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long long i) {
+  return __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
+}
 __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
   hi = __float2bfloat16_rn(v);
   lo = __float2bfloat16_rn(v - __bfloat162float(hi));
@@ -198,6 +202,28 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+// Sum of v over a block of kThreads threads (a power of two) as a fixed-order tree in double; red holds kThreads doubles.
+// Every thread returns the sum, and red may be reused right away.
+template <int kThreads>
+__device__ __forceinline__ double block_sum_tree(double v, double* red) {
+  red[threadIdx.x] = v;
+  __syncthreads();
+  for (int s = kThreads / 2; s > 0; s >>= 1) {
+    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+    __syncthreads();
+  }
+  const double r = red[0];
+  __syncthreads();
+  return r;
+}
+// for (i = global thread index; i < n; i += all threads of the grid): launch with grid_stride_blocks (pk_host.h)
+#define PK_GRID_STRIDE(i, n) \
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); i += static_cast<long long>(gridDim.x) * blockDim.x)
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");

@@ -174,17 +174,6 @@ __device__ __forceinline__ void gaussian_window(float* w) {
   }
 }
 
-// fixed-order block sum of a double (blockDim.x = 256); the result is valid in thread 0
-__device__ double block_sum256(double v, double* red) {
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-    __syncthreads();
-  }
-  return red[0];
-}
-
 // ssim map and its derivatives with respect to the three filtered maps that depend on the prediction (mu_x, E[x^2], E[xy]),
 // scaled by gscale = d loss / d ssim_map = -1 / (batch * l * odim); per-block partial sums of the ssim map and of |d - y| * mask
 __global__ void __launch_bounds__(256)
@@ -246,9 +235,8 @@ ss_ssim_fwd_kernel(const float* __restrict__ dec, const float* __restrict__ feat
     }
     if (t < nf) s_l1 += fabs(static_cast<double>(dec[o]) - static_cast<double>(feats[o]));
   }
-  const double t_ssim = block_sum256(s_ssim, red);
-  __syncthreads();
-  const double t_l1 = block_sum256(s_l1, red);
+  const double t_ssim = block_sum_tree<256>(s_ssim, red);
+  const double t_l1 = block_sum_tree<256>(s_l1, red);
   if (threadIdx.x == 0) {
     const long long blk = static_cast<long long>(b) * gridDim.x + blockIdx.x;
     part[2 * blk] = static_cast<float>(t_ssim);
@@ -322,10 +310,8 @@ ss_loss_finalize_kernel(const float* __restrict__ part, int nblk, const int32_t*
   __shared__ double s_tok;
   double s_ssim = 0.0, s_l1 = 0.0;
   for (int i = threadIdx.x; i < nblk; i += 256) { s_ssim += part[2 * i]; s_l1 += part[2 * i + 1]; }
-  const double t_ssim = block_sum256(s_ssim, red);
-  __syncthreads();
-  const double t_l1 = block_sum256(s_l1, red);
-  __syncthreads();
+  const double t_ssim = block_sum_tree<256>(s_ssim, red);
+  const double t_l1 = block_sum_tree<256>(s_l1, red);
   if (threadIdx.x == 0) {
     long long toks = 0;
     for (int b = 0; b < batch; ++b) toks += max(min(num_phones[b], t_max), 0);
@@ -345,7 +331,7 @@ ss_loss_finalize_kernel(const float* __restrict__ part, int nblk, const int32_t*
     }
     if (g_dur) g_dur[i] = g * static_cast<float>(inv_tok);
   }
-  const double t_h = block_sum256(s_h, red);
+  const double t_h = block_sum_tree<256>(s_h, red);
   if (threadIdx.x == 0) {
     long long frames = 0;
     for (int b = 0; b < batch; ++b) frames += max(min(num_frames[b], l), 0);
@@ -363,7 +349,6 @@ ss_loss_finalize_kernel(const float* __restrict__ part, int nblk, const int32_t*
 }  // namespace pk
 
 using namespace pk;
-#define PK_STREAM static_cast<cudaStream_t>(stream)
 
 extern "C" int pk_ss_bn_train_fwd(const float* r, int64_t rows, int32_t c, const float* gamma, const float* beta, float eps, float momentum,
                                   float* run_mean, float* run_var, const float* residual, float* scratch, float* y, void* y_hi, void* y_lo,

@@ -162,8 +162,7 @@ __device__ int attention_phase(const Params& p, int b, int t, const float* h_att
   // softmax over T (fixed-order block reductions)
   float m = -INFINITY;
   for (int i = threadIdx.x; i < T; i += kThreads) m = fmaxf(m, __ldcg(e + i));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   if (lane == 0) s.red[warp] = m;
   __syncthreads();
   m = s.red[0];
@@ -387,18 +386,6 @@ __global__ void bilstm_merge_kernel(const float* __restrict__ hf, const float* _
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kLossThreads = 1024;
 
-__device__ double block_sum(double v, double* red) {
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = kLossThreads / 2; s > 0; s >>= 1) {
-    if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-    __syncthreads();
-  }
-  const double r = red[0];
-  __syncthreads();
-  return r;
-}
-
 __global__ void __launch_bounds__(kLossThreads, 1)
 loss_kernel(const float* __restrict__ mel, const float* __restrict__ post, const float* __restrict__ tgt, int B, int T, int C,
             const float* __restrict__ align, int t_enc, const int32_t* __restrict__ slens, const int32_t* __restrict__ plens, double sigma,
@@ -411,7 +398,7 @@ loss_kernel(const float* __restrict__ mel, const float* __restrict__ post, const
     a += d1 * d1;
     c += d2 * d2;
   }
-  const double mel_loss = block_sum(a, red) / n, post_loss = block_sum(c, red) / n;
+  const double mel_loss = block_sum_tree<kLossThreads>(a, red) / n, post_loss = block_sum_tree<kLossThreads>(c, red) / n;
   double total = mel_loss + post_loss, gal = 0.0, st = 0.0;
   if (align) {
     for (int b = 0; b < B; ++b) {
@@ -423,7 +410,7 @@ loss_kernel(const float* __restrict__ mel, const float* __restrict__ post, const
         const double d = static_cast<double>(nn) / dl - static_cast<double>(tt) / el;
         s += (1.0 - exp(-d * d / (2.0 * sigma * sigma))) * align[static_cast<long long>(b) * T * t_enc + i];
       }
-      gal += block_sum(s, red) / (static_cast<double>(dl) * el);
+      gal += block_sum_tree<kLossThreads>(s, red) / (static_cast<double>(dl) * el);
     }
     gal /= B;
     total += gal;
@@ -435,7 +422,7 @@ loss_kernel(const float* __restrict__ mel, const float* __restrict__ post, const
       const double x = stop[i], y = nn == slens[b] - 1 ? 1.0 : 0.0;
       s += fmax(x, 0.0) - x * y + log1p(exp(-fabs(x)));
     }
-    st = block_sum(s, red) / (static_cast<double>(B) * T);
+    st = block_sum_tree<kLossThreads>(s, red) / (static_cast<double>(B) * T);
     total += st;
   }
   if (threadIdx.x == 0) {

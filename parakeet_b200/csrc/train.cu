@@ -9,16 +9,6 @@
 
 namespace pk {
 
-static inline int nblk(long long n, int threads) { return static_cast<int>((n + threads - 1) / threads); }
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float ld_split(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long long i) {
-  return __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // dst[z*dst_zstride + c*ld_dst + r] = src[z, r + shift, c0 + c]  (0 where r + shift is outside [0, rows)), split planes.
 // 32x32 tiles through shared memory.  grid = (ceil(r_out/32), ceil(cols/32), Z)
@@ -80,7 +70,7 @@ layer_norm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gam
       v[i] = c < d ? xr[c] : 0.f;
       s += v[i];
     }
-    const float mean = wsum(s) / d;
+    const float mean = warp_sum(s) / d;
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < MAX_PER_LANE; ++i) {
@@ -88,7 +78,7 @@ layer_norm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gam
       const float dv = c < d ? v[i] - mean : 0.f;
       q += dv * dv;
     }
-    const float rstd = rsqrtf(wsum(q) / d + eps);
+    const float rstd = rsqrtf(warp_sum(q) / d + eps);
     float sg1 = 0.f, sg2 = 0.f;
 #pragma unroll
     for (int i = 0; i < MAX_PER_LANE; ++i) {
@@ -106,7 +96,7 @@ layer_norm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gam
         g[i] = 0.f;
       }
     }
-    const float m1 = wsum(sg1) / d, m2 = wsum(sg2) / d;
+    const float m1 = warp_sum(sg1) / d, m2 = warp_sum(sg2) / d;
 #pragma unroll
     for (int i = 0; i < MAX_PER_LANE; ++i) {
       const int c = lane + 32 * i;
@@ -123,23 +113,73 @@ layer_norm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gam
   }
 }
 
-// softmax backward: ds = scale * p * (dp - sum_k p*dp) over the first `keys` columns; padding columns -> 0. warp per row.
+// ---------------------------------------------------------------------------------------------------------------
+// Softmax backward of the attention probabilities P (batch * heads, rows, ld):
+//   dS = scale * P * (dP - sum_k P dP) over the first `keys` columns, 0 in the padding columns.  One warp per row.
+// The TransformerTTS guided attention loss (GuidedMultiHeadAttentionLoss, transformer_tts.py:874-1075) is folded into dP of the
+// heads h < guided_heads (none for guided_heads = 0): for query row i < olen_b and key j < ilen_b,
+//   dP[i, j] += coef * G[i, j],  G = 1 - exp(-(j / ilen_b - i / olen_b)^2 / (2 sigma^2)),
+// coef = lambda / (guided_heads * guided_layers * sum_b ilen_b olen_b) (the mean over the selected elements of every guided
+// layer), and partials[(b * guided_heads + h) * rows + i] = sum_j G[i, j] P[i, j] (0 for rows i >= olen_b).
+// kGuided = false (guided_heads = 0) compiles the guided terms away: the plain backward keeps its unrolled, load-bound loops.
+// ---------------------------------------------------------------------------------------------------------------
+template <bool kGuided>
 __global__ void __launch_bounds__(256)
 softmax_bwd_kernel(const __nv_bfloat16* __restrict__ p_hi, const __nv_bfloat16* __restrict__ p_lo, const float* __restrict__ dp,
-                   long long rows, int keys, int ld, float scale, __nv_bfloat16* __restrict__ ds_hi, __nv_bfloat16* __restrict__ ds_lo) {
+                   int batch, int heads, int rows_per_z, int keys, int ld, float scale, int guided_heads, int guided_layers,
+                   const int32_t* __restrict__ ilens, const int32_t* __restrict__ olens, float inv_two_sigma2, float lambda,
+                   float* __restrict__ partials, __nv_bfloat16* __restrict__ ds_hi, __nv_bfloat16* __restrict__ ds_lo) {
+  const long long rows = static_cast<long long>(batch) * heads * rows_per_z;
   const long long row = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  float dot = 0.f;
-  for (int c = lane; c < keys; c += 32) dot += ld_split(p_hi, p_lo, row * ld + c) * dp[row * ld + c];
-  dot = wsum(dot);
+  const int z = static_cast<int>(row / rows_per_z), i = static_cast<int>(row % rows_per_z);
+  const int b = z / heads, h = z % heads;
+  const bool guided_head = kGuided && h < guided_heads;
+  int il = 0, ol = 0;
+  float coef = 0.f;
+  if (guided_head) {
+    long long n = 0;
+    for (int q = 0; q < batch; ++q) n += static_cast<long long>(min(__ldg(ilens + q), keys)) * min(__ldg(olens + q), rows_per_z);
+    coef = n > 0 ? lambda / (static_cast<float>(guided_heads) * guided_layers * static_cast<float>(n)) : 0.f;
+    il = min(__ldg(ilens + b), keys);
+    ol = min(__ldg(olens + b), rows_per_z);
+  }
+  const bool live = guided_head && i < ol && il > 0;
+  const float fi = live ? static_cast<float>(i) / static_cast<float>(ol) : 0.f;
+  const float inv_il = live ? 1.f / static_cast<float>(il) : 0.f;
+  const float* dr = dp + row * ld;
+  float dot = 0.f, gp = 0.f;
+  for (int c = lane; c < keys; c += 32) {
+    const float pv = ld_split(p_hi, p_lo, row * ld + c);
+    float d = dr[c];
+    if (live && c < il) {
+      const float x = static_cast<float>(c) * inv_il - fi;
+      const float g = 1.f - expf(-(x * x) * inv_two_sigma2);
+      d = fmaf(coef, g, d);
+      gp = fmaf(g, pv, gp);
+    }
+    dot = fmaf(pv, d, dot);
+  }
+  dot = warp_sum(dot);
+  if (guided_head) {
+    gp = warp_sum(gp);
+    if (lane == 0) partials[(static_cast<long long>(b) * guided_heads + h) * rows_per_z + i] = gp;
+  }
   for (int c = lane; c < ld; c += 32) {
     float v = 0.f;
-    if (c < keys) v = scale * ld_split(p_hi, p_lo, row * ld + c) * (dp[row * ld + c] - dot);
-    __nv_bfloat16 h, l;
-    split_bf16(v, h, l);
-    ds_hi[row * ld + c] = h;
-    ds_lo[row * ld + c] = l;
+    if (c < keys) {
+      float d = dr[c];
+      if (live && c < il) {
+        const float x = static_cast<float>(c) * inv_il - fi;
+        d = fmaf(coef, 1.f - expf(-(x * x) * inv_two_sigma2), d);
+      }
+      v = scale * ld_split(p_hi, p_lo, row * ld + c) * (d - dot);
+    }
+    __nv_bfloat16 hh, ll;
+    split_bf16(v, hh, ll);
+    ds_hi[row * ld + c] = hh;
+    ds_lo[row * ld + c] = ll;
   }
 }
 
@@ -368,7 +408,7 @@ embed_pe_bwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ d
       acc += g * ((c & 1) ? cosf(ang) : sinf(ang));
     }
   }
-  acc = wsum(acc);
+  acc = warp_sum(acc);
   __shared__ float red[8];
   if (lane == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
@@ -424,28 +464,29 @@ scalar_conv_wgrad_kernel(const float* __restrict__ dhs, const float* __restrict_
   }
 }
 
-// Adam (paddle.optimizer.Adam semantics): m = b1 m + (1-b1) g; v = b2 v + (1-b2) g^2;
-//   lr_t = lr * sqrt(1 - b2^t) / (1 - b1^t);  p -= lr_t * m / (sqrt(v) + eps * sqrt(1 - b2^t));  g is pre-scaled by grad_scale
+// Adam (paddle.optimizer.Adam semantics) with ClipGradByGlobalNorm folded in:
+//   g' = g * grad_scale * sc, sc = clip / max(sqrt(*sqnorm), clip) (1 without sqnorm or for clip <= 0);
+//   m = b1 m + (1-b1) g'; v = b2 v + (1-b2) g'^2; lr_t = lr * sqrt(1 - b2^t) / (1 - b1^t);
+//   p -= lr_t * m / (sqrt(v) + eps * sqrt(1 - b2^t)).
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                            long long n, float lr_t, float beta1, float beta2, float eps_t, float grad_scale) {
-  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const float gi = g[i] * grad_scale;
-  const float mi = beta1 * m[i] + (1.f - beta1) * gi;
-  const float vi = beta2 * v[i] + (1.f - beta2) * gi * gi;
-  m[i] = mi;
-  v[i] = vi;
-  p[i] -= lr_t * mi / (sqrtf(vi) + eps_t);
+                            long long n, float lr_t, float beta1, float beta2, float eps_t, float grad_scale,
+                            const double* __restrict__ sqnorm, float clip) {
+  float sc = 1.f;
+  if (sqnorm != nullptr && clip > 0.f) sc = clip / fmaxf(sqrtf(static_cast<float>(*sqnorm)), clip);
+#pragma unroll 1  // each thread takes one element at the steps' flat sizes; the unrolled loop is slower there
+  PK_GRID_STRIDE(i, n) {
+    const float gi = g[i] * grad_scale * sc;
+    const float mi = beta1 * m[i] + (1.f - beta1) * gi;
+    const float vi = beta2 * v[i] + (1.f - beta2) * gi * gi;
+    m[i] = mi;
+    v[i] = vi;
+    p[i] -= lr_t * mi / (sqrtf(vi) + eps_t);
+  }
 }
 
 }  // namespace pk
 
 using namespace pk;
-#define PK_STREAM static_cast<cudaStream_t>(stream)
-#define PK_LAUNCH_DONE()             \
-  PK_CHECK_CUDA(cudaGetLastError()); \
-  count_launch();                    \
-  return PK_OK;
 
 extern "C" int pk_transpose_planes(const void* src_hi, const void* src_lo, int32_t z, int32_t rows, int64_t src_zstride, int32_t ld_src,
                                    int32_t c0, int32_t cols, int32_t shift, int32_t r_out, void* dst_hi, void* dst_lo,
@@ -455,7 +496,7 @@ extern "C" int pk_transpose_planes(const void* src_hi, const void* src_lo, int32
   transpose_planes_kernel<<<grid, 256, 0, PK_STREAM>>>(static_cast<const __nv_bfloat16*>(src_hi), static_cast<const __nv_bfloat16*>(src_lo),
                                                        rows, src_zstride, ld_src, c0, cols, shift, r_out, static_cast<__nv_bfloat16*>(dst_hi),
                                                        static_cast<__nv_bfloat16*>(dst_lo), dst_zstride, ld_dst);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_layer_norm_bwd(const float* x, const float* gamma, const float* dy, float eps, int64_t rows, int32_t d, float* dx,
@@ -465,23 +506,30 @@ extern "C" int pk_layer_norm_bwd(const float* x, const float* gamma, const float
   const size_t smem = 2 * d * sizeof(float);
   if (d <= 256) layer_norm_bwd_kernel<8><<<blocks, 256, smem, PK_STREAM>>>(x, gamma, dy, eps, rows, d, dx, accumulate, dgamma, dbeta);
   else layer_norm_bwd_kernel<16><<<blocks, 256, smem, PK_STREAM>>>(x, gamma, dy, eps, rows, d, dx, accumulate, dgamma, dbeta);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
-extern "C" int pk_softmax_bwd(const void* p_hi, const void* p_lo, const float* dp, int64_t rows, int32_t keys, int32_t ld, float scale,
-                              void* ds_hi, void* ds_lo, pk_stream_t stream) {
-  PK_CHECK_ARG(p_hi && p_lo && dp && ds_hi && ds_lo && rows > 0 && keys > 0 && ld >= keys, "bad arguments");
-  softmax_bwd_kernel<<<nblk(rows * 32, 256), 256, 0, PK_STREAM>>>(static_cast<const __nv_bfloat16*>(p_hi),
-                                                                  static_cast<const __nv_bfloat16*>(p_lo), dp, rows, keys, ld, scale,
-                                                                  static_cast<__nv_bfloat16*>(ds_hi), static_cast<__nv_bfloat16*>(ds_lo));
-  PK_LAUNCH_DONE()
+extern "C" int pk_softmax_bwd(const void* p_hi, const void* p_lo, const float* dp, int32_t batch, int32_t heads, int32_t rows,
+                              int32_t keys, int32_t ld, float scale, int32_t guided_heads, int32_t guided_layers,
+                              const int32_t* ilens, const int32_t* olens, float sigma, float lambda, float* partials, void* ds_hi,
+                              void* ds_lo, pk_stream_t stream) {
+  PK_CHECK_ARG(p_hi && p_lo && dp && ds_hi && ds_lo && batch > 0 && heads > 0 && rows > 0 && keys > 0 && ld >= keys,
+               "bad arguments to pk_softmax_bwd");
+  PK_CHECK_ARG(guided_heads >= 0 && guided_heads <= heads && guided_layers >= 1 && sigma > 0.f, "bad guided-loss arguments");
+  PK_CHECK_ARG(guided_heads == 0 || (ilens && olens && partials), "the guided heads need ilens, olens and partials");
+  const long long total = static_cast<long long>(batch) * heads * rows;
+  const float inv_two_sigma2 = static_cast<float>(1.0 / (2.0 * static_cast<double>(sigma) * sigma));
+  (guided_heads > 0 ? softmax_bwd_kernel<true> : softmax_bwd_kernel<false>)<<<nblk(total * 32, 256), 256, 0, PK_STREAM>>>(
+      static_cast<const __nv_bfloat16*>(p_hi), static_cast<const __nv_bfloat16*>(p_lo), dp, batch, heads, rows, keys, ld, scale, guided_heads,
+      guided_layers, ilens, olens, inv_two_sigma2, lambda, partials, static_cast<__nv_bfloat16*>(ds_hi), static_cast<__nv_bfloat16*>(ds_lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_colsum(const float* x, int64_t rows, int32_t c, float* out, pk_stream_t stream) {
   PK_CHECK_ARG(x && out && rows > 0 && c > 0, "bad arguments");
   dim3 grid(static_cast<unsigned>((rows + 63) / 64), (c + 63) / 64);
   colsum_kernel<<<grid, 256, 0, PK_STREAM>>>(x, rows, c, out);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_colsum_split(const void* x_hi, const void* x_lo, int64_t rows, int32_t cols, int32_t ld, float* out, pk_stream_t stream) {
@@ -489,14 +537,14 @@ extern "C" int pk_colsum_split(const void* x_hi, const void* x_lo, int64_t rows,
   dim3 grid(static_cast<unsigned>((rows + 63) / 64), (cols + 63) / 64);
   colsum_split_kernel<<<grid, 256, 0, PK_STREAM>>>(static_cast<const __nv_bfloat16*>(x_hi), static_cast<const __nv_bfloat16*>(x_lo), rows, cols,
                                                    ld, out);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_sum_slices(const float* part, int32_t slices, int64_t n, float* out, pk_stream_t stream) {
   PK_CHECK_ARG(part && out && slices > 0 && n > 0, "bad arguments");
   const int vec = (n & 3) == 0 && (reinterpret_cast<uintptr_t>(part) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
   sum_slices_kernel<<<nblk((n + 3) / 4, 256), 256, 0, PK_STREAM>>>(part, slices, n, out, vec);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_batch_norm_train(const float* x, int64_t rows, int32_t c, const float* gamma, const float* beta, float eps,
@@ -511,9 +559,7 @@ extern "C" int pk_batch_norm_train(const float* x, int64_t rows, int32_t c, cons
   bn_train_fwd_kernel<<<nblk(rows * c, 256), 256, 0, PK_STREAM>>>(x, sums2c, gamma, beta, eps, act, rows, c, momentum, run_mean, run_var, y,
                                                                   static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo),
                                                                   save_mean, save_rstd);
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch(3);
-  return PK_OK;
+  PK_LAUNCH_DONE(3);
 }
 
 extern "C" int pk_batch_norm_bwd(const float* x, const float* dy, const float* y_act, const float* mean, const float* rstd,
@@ -524,22 +570,20 @@ extern "C" int pk_batch_norm_bwd(const float* x, const float* dy, const float* y
   dim3 grid(static_cast<unsigned>((rows + 63) / 64), (c + 63) / 64);
   bn_bwd_stats_kernel<<<grid, 256, 0, PK_STREAM>>>(x, dy, y_act, mean, rstd, act, rows, c, sums2c);
   bn_bwd_apply_kernel<<<nblk(rows * c, 256), 256, 0, PK_STREAM>>>(x, dy, y_act, mean, rstd, gamma, sums2c, act, rows, c, dx);
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch(2);
-  return PK_OK;
+  PK_LAUNCH_DONE(2);
 }
 
 extern "C" int pk_relu_bwd(const float* dy, const void* y_hi, int64_t n, float* dx, void* dx_hi, void* dx_lo, pk_stream_t stream) {
   PK_CHECK_ARG(dy && y_hi && n > 0 && (dx || dx_hi), "bad arguments");
   relu_bwd_kernel<<<nblk(n, 256), 256, 0, PK_STREAM>>>(dy, static_cast<const __nv_bfloat16*>(y_hi), n, dx,
                                                        static_cast<__nv_bfloat16*>(dx_hi), static_cast<__nv_bfloat16*>(dx_lo));
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_axpy(float a, const float* x, int64_t n, float* y, pk_stream_t stream) {
   PK_CHECK_ARG(x && y && n > 0, "bad arguments");
   axpy_kernel<<<nblk(n, 256), 256, 0, PK_STREAM>>>(a, x, n, y);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_fs2_loss_bwd(const float* before, const float* after, const float* ys, const int32_t* olens, int32_t l_max,
@@ -551,7 +595,7 @@ extern "C" int pk_fs2_loss_bwd(const float* before, const float* after, const fl
   const long long n = std::max(static_cast<long long>(batch) * l_max * odim, static_cast<long long>(batch) * t_max);
   fs2_loss_bwd_kernel<<<nblk(n, 256), 256, 0, PK_STREAM>>>(before, after, ys, olens, l_max, odim, d_outs, ds, p_outs, ps, e_outs, es, ilens,
                                                           t_max, batch, g_before, g_after, g_d, g_p, g_e);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_embed_pe_bwd(const int64_t* ids, const float* dx, int32_t vocab, int32_t padding_idx, int32_t batch, int32_t t,
@@ -559,7 +603,7 @@ extern "C" int pk_embed_pe_bwd(const int64_t* ids, const float* dx, int32_t voca
   PK_CHECK_ARG(dx && dalpha && batch > 0 && t > 0 && d > 0 && (ids == nullptr || dtable != nullptr), "bad arguments");
   const long long rows = static_cast<long long>(batch) * t;
   embed_pe_bwd_kernel<<<nblk(rows * 32, 256), 256, 0, PK_STREAM>>>(ids, dx, vocab, padding_idx, t, rows, d, dtable, dalpha);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_length_regulate_bwd(const float* dy, const int64_t* dur, int32_t batch, int32_t t_in, int32_t c, int32_t t_out,
@@ -567,7 +611,7 @@ extern "C" int pk_length_regulate_bwd(const float* dy, const int64_t* dur, int32
   PK_CHECK_ARG(dy && dur && dx && batch > 0 && t_in > 0 && c > 0 && t_out > 0, "bad arguments");
   dim3 grid(t_in, batch);
   lr_bwd_kernel<<<grid, 128, 0, PK_STREAM>>>(dy, dur, t_in, c, t_out, dx);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_scalar_conv_wgrad(const float* dhs, const float* track, int32_t batch, int32_t t, int32_t c, int32_t k, float* dw,
@@ -575,16 +619,16 @@ extern "C" int pk_scalar_conv_wgrad(const float* dhs, const float* track, int32_
   PK_CHECK_ARG(dhs && track && dw && db && batch > 0 && t > 0 && c > 0 && k >= 1 && k <= 16, "bad arguments (k <= 16)");
   const long long rows = static_cast<long long>(batch) * t;
   scalar_conv_wgrad_kernel<<<nblk(rows, 64), 256, 0, PK_STREAM>>>(dhs, track, t, c, k, rows, dw, db);
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_adam(float* params, const float* grads, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
-                       int32_t step, float grad_scale, pk_stream_t stream) {
+                       int32_t step, float grad_scale, const double* sqnorm, float clip_norm, pk_stream_t stream) {
   PK_CHECK_ARG(params && grads && m && v && n > 0 && step >= 1, "bad arguments");
   const double c1 = 1.0 - pow(static_cast<double>(beta1), step), c2 = sqrt(1.0 - pow(static_cast<double>(beta2), step));
-  adam_kernel<<<nblk(n, 256), 256, 0, PK_STREAM>>>(params, grads, m, v, n, static_cast<float>(lr * c2 / c1), beta1, beta2,
-                                                   static_cast<float>(eps * c2), grad_scale);
-  PK_LAUNCH_DONE()
+  adam_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(params, grads, m, v, n, static_cast<float>(lr * c2 / c1), beta1, beta2,
+                                                                 static_cast<float>(eps * c2), grad_scale, sqnorm, clip_norm);
+  PK_LAUNCH_DONE(1);
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -635,5 +679,5 @@ extern "C" int pk_dropout(const float* x, const void* x_hi, const void* x_lo, in
   dropout_kernel<<<nblk(blocks4, 256), 256, 0, PK_STREAM>>>(x, static_cast<const __nv_bfloat16*>(x_hi), static_cast<const __nv_bfloat16*>(x_lo), n,
                                                             thresh, 1.f / (1.f - p), static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32),
                                                             site, step, step_dev, y, static_cast<__nv_bfloat16*>(y_hi), static_cast<__nv_bfloat16*>(y_lo));
-  PK_LAUNCH_DONE()
+  PK_LAUNCH_DONE(1);
 }

@@ -155,8 +155,7 @@ __device__ __forceinline__ void attend(const Params& p, const float* q, const fl
   __syncthreads();
   float m = -INFINITY;
   for (int i = threadIdx.x; i < n; i += kThreads) m = fmaxf(m, s.sc[i]);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   if (lane == 0) s.red[warp] = m;
   __syncthreads();
   m = s.red[0];
@@ -448,14 +447,12 @@ extern "C" int pk_tts_decode(const PkTtsDecodeArgs* a, pk_stream_t stream) {
   return PK_OK;
 }
 
-static unsigned blocks_for(long long n) { return static_cast<unsigned>((n + 255) / 256); }
-
 extern "C" int pk_tts_text_eos(const int64_t* text, const int32_t* lens, int32_t batch, int32_t t, int64_t eos, int64_t* xs, int32_t* ilens,
                                pk_stream_t stream) {
   // text may be NULL when t == 0 (an empty tensor has no storage): every row is then [eos] and text is never read
   PK_CHECK_ARG((text || t == 0) && lens && xs && ilens && batch > 0 && t >= 0, "bad arguments to pk_tts_text_eos");
-  text_eos_kernel<<<blocks_for(static_cast<long long>(batch) * (t + 1)), 256, 0, static_cast<cudaStream_t>(stream)>>>(text, lens, batch, t,
-                                                                                                                       eos, xs, ilens);
+  text_eos_kernel<<<nblk(static_cast<long long>(batch) * (t + 1), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(text, lens, batch, t,
+                                                                                                                     eos, xs, ilens);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -463,8 +460,8 @@ extern "C" int pk_tts_text_eos(const int64_t* text, const int32_t* lens, int32_t
 
 extern "C" int pk_tts_shift_frames(const float* ys, int32_t batch, int32_t l, int32_t odim, int32_t r, float* out, pk_stream_t stream) {
   PK_CHECK_ARG(ys && out && batch > 0 && l >= r && odim > 0 && r >= 1, "bad arguments to pk_tts_shift_frames");
-  shift_frames_kernel<<<blocks_for(static_cast<long long>(batch) * (l / r) * odim), 256, 0, static_cast<cudaStream_t>(stream)>>>(ys, batch, l,
-                                                                                                                                 odim, r, out);
+  shift_frames_kernel<<<nblk(static_cast<long long>(batch) * (l / r) * odim, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(ys, batch, l,
+                                                                                                                                odim, r, out);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -475,7 +472,7 @@ extern "C" int pk_tts_prenet_dropout(float* x, int32_t batch, int32_t l, int32_t
   PK_CHECK_ARG(x && batch > 0 && l > 0 && units > 0 && p >= 0.f && p < 1.f && site >= 0, "bad arguments to pk_tts_prenet_dropout");
   const double th = static_cast<double>(p) * 4294967296.0;
   const uint32_t thresh = th >= 4294967295.0 ? 0xFFFFFFFFu : static_cast<uint32_t>(th);
-  prenet_dropout_kernel<<<blocks_for(static_cast<long long>(batch) * l * units), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  prenet_dropout_kernel<<<nblk(static_cast<long long>(batch) * l * units, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, batch, l, units, thresh, p > 0.f ? 1.f / (1.f - p) : 1.f, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32),
       static_cast<uint32_t>(site));
   PK_CHECK_CUDA(cudaGetLastError());
@@ -485,7 +482,7 @@ extern "C" int pk_tts_prenet_dropout(float* x, int32_t batch, int32_t l, int32_t
 
 extern "C" int pk_tts_stop_labels(const int32_t* olens, int32_t batch, int32_t width, float* out, pk_stream_t stream) {
   PK_CHECK_ARG(olens && out && batch > 0 && width > 0, "bad arguments to pk_tts_stop_labels");
-  stop_labels_kernel<<<blocks_for(static_cast<long long>(batch) * width), 256, 0, static_cast<cudaStream_t>(stream)>>>(olens, batch, width, out);
+  stop_labels_kernel<<<nblk(static_cast<long long>(batch) * width, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(olens, batch, width, out);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

@@ -1,26 +1,13 @@
-// Kernels of the TransformerTTS training step (reference: TransformerTTSUpdater.update_core, parakeet/models/transformer_tts/
-// transformer_tts_updater.py:73-170): the causal masked softmax of the decoder self-attention, the softmax backward with the
-// guided source-attention loss (GuidedMultiHeadAttentionLoss, transformer_tts.py:874-1075) fused in, and TransformerTTSLoss
-// (transformer_tts.py:770-872) with its gradients.  No atomics: every reduction runs in a fixed order.
-#include <math_constants.h>
-
+// Losses of the TransformerTTS training step (reference: TransformerTTSUpdater.update_core, parakeet/models/transformer_tts/
+// transformer_tts_updater.py:73-170): the guided source-attention loss (GuidedMultiHeadAttentionLoss, transformer_tts.py:874-1075)
+// from the row partials that pk_softmax_bwd (train.cu) writes while it folds the loss's gradient into the softmax backward, and
+// TransformerTTSLoss (transformer_tts.py:770-872) with its gradients.  The causal self-attention mask is pk_masked_softmax's
+// (fs2.cu).  No atomics: every reduction runs in a fixed order.
 #include "pk_host.h"
 #include "pk_sm90.cuh"
 
 namespace pk {
 namespace {
-
-inline int nblk(long long n, int threads) { return static_cast<int>((n + threads - 1) / threads); }
-
-__device__ __forceinline__ float warp_max_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-__device__ __forceinline__ float ld_split(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long long i) {
-  return __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
-}
 
 // Sum of v over a 256-thread block in a fixed order (warp trees, then the 8 warp sums in order); every thread gets the result.
 __device__ float block_sum_256(float v, float* red) {
@@ -32,104 +19,6 @@ __device__ float block_sum_256(float v, float* red) {
 #pragma unroll
   for (int w = 0; w < 8; ++w) s += red[w];
   return s;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Masked softmax over keys, optionally causal: s (batch * heads, rows, ld) fp32 -> p split planes of the same shape.  Query row
-// i of utterance b attends keys j < key_lens[b] (all `keys` when key_lens is NULL) and, when causal, j <= i: the reference's
-// non_pad(olens) & tril mask (transformer_tts.py:692 _target_mask).  Masked and padding columns get 0; a row with no key left
-// is all zeros (masked_fill(min) -> softmax -> masked_fill(0)).  One warp per row.
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-softmax_causal_kernel(const float* __restrict__ s, const int32_t* __restrict__ klens, int heads, int rows_per_z, int keys, int ld,
-                      int causal, long long rows, __nv_bfloat16* __restrict__ p_hi, __nv_bfloat16* __restrict__ p_lo) {
-  const long long row = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const int z = static_cast<int>(row / rows_per_z), i = static_cast<int>(row % rows_per_z);
-  int klen = klens ? min(__ldg(klens + z / heads), keys) : keys;
-  if (causal) klen = min(klen, i + 1);
-  const float* sr = s + row * ld;
-  float m = -CUDART_INF_F;
-  for (int c = lane; c < klen; c += 32) m = fmaxf(m, sr[c]);
-  m = warp_max_f(m);
-  float sum = 0.f;
-  for (int c = lane; c < klen; c += 32) sum += expf(sr[c] - m);
-  sum = warp_sum(sum);
-  const float inv = klen > 0 ? 1.f / sum : 0.f;
-  for (int c = lane; c < ld; c += 32) {
-    const float pv = c < klen ? expf(sr[c] - m) * inv : 0.f;
-    __nv_bfloat16 h, l;
-    split_bf16(pv, h, l);
-    p_hi[row * ld + c] = h;
-    p_lo[row * ld + c] = l;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Softmax backward with the guided attention loss folded into dP.  For head h < guided_heads, query row i < olen_b and key
-// j < ilen_b:  dP[i, j] += coef * G[i, j],  G = 1 - exp(-(j / ilen_b - i / olen_b)^2 / (2 sigma^2)),
-// coef = lambda / (guided_heads * guided_layers * sum_b ilen_b olen_b) (the mean over the selected elements of every guided
-// layer), and partials[(b * guided_heads + h) * rows + i] = sum_j G[i, j] P[i, j] (0 for rows i >= olen_b).  Then
-// dS = scale * P * (dP - sum_k P dP) over the first `keys` columns, 0 in the padding columns.  One warp per row.
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-softmax_bwd_guided_kernel(const __nv_bfloat16* __restrict__ p_hi, const __nv_bfloat16* __restrict__ p_lo, const float* __restrict__ dp,
-                          int batch, int heads, int rows_per_z, int keys, int ld, float scale, int guided_heads, int guided_layers,
-                          const int32_t* __restrict__ ilens, const int32_t* __restrict__ olens, float inv_two_sigma2, float lambda,
-                          float* __restrict__ partials, __nv_bfloat16* __restrict__ ds_hi, __nv_bfloat16* __restrict__ ds_lo) {
-  const long long rows = static_cast<long long>(batch) * heads * rows_per_z;
-  const long long row = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (row >= rows) return;
-  const int z = static_cast<int>(row / rows_per_z), i = static_cast<int>(row % rows_per_z);
-  const int b = z / heads, h = z % heads;
-  const bool guided_head = h < guided_heads;
-  int il = 0, ol = 0;
-  float coef = 0.f;
-  if (guided_head) {
-    long long n = 0;
-    for (int q = 0; q < batch; ++q) n += static_cast<long long>(min(__ldg(ilens + q), keys)) * min(__ldg(olens + q), rows_per_z);
-    coef = n > 0 ? lambda / (static_cast<float>(guided_heads) * guided_layers * static_cast<float>(n)) : 0.f;
-    il = min(__ldg(ilens + b), keys);
-    ol = min(__ldg(olens + b), rows_per_z);
-  }
-  const bool live = guided_head && i < ol && il > 0;
-  const float fi = live ? static_cast<float>(i) / static_cast<float>(ol) : 0.f;
-  const float inv_il = live ? 1.f / static_cast<float>(il) : 0.f;
-  const float* dr = dp + row * ld;
-  float dot = 0.f, gp = 0.f;
-  for (int c = lane; c < keys; c += 32) {
-    const float pv = ld_split(p_hi, p_lo, row * ld + c);
-    float d = dr[c];
-    if (live && c < il) {
-      const float x = static_cast<float>(c) * inv_il - fi;
-      const float g = 1.f - expf(-(x * x) * inv_two_sigma2);
-      d = fmaf(coef, g, d);
-      gp = fmaf(g, pv, gp);
-    }
-    dot = fmaf(pv, d, dot);
-  }
-  dot = warp_sum(dot);
-  if (guided_head) {
-    gp = warp_sum(gp);
-    if (lane == 0) partials[(static_cast<long long>(b) * guided_heads + h) * rows_per_z + i] = gp;
-  }
-  for (int c = lane; c < ld; c += 32) {
-    float v = 0.f;
-    if (c < keys) {
-      float d = dr[c];
-      if (live && c < il) {
-        const float x = static_cast<float>(c) * inv_il - fi;
-        d = fmaf(coef, 1.f - expf(-(x * x) * inv_two_sigma2), d);
-      }
-      v = scale * ld_split(p_hi, p_lo, row * ld + c) * (d - dot);
-    }
-    __nv_bfloat16 hh, ll;
-    split_bf16(v, hh, ll);
-    ds_hi[row * ld + c] = hh;
-    ds_lo[row * ld + c] = ll;
-  }
 }
 
 // guided loss = lambda * sum(partials) / (heads_layers * sum_b ilen_b olen_b) -> losses[4], added to losses[0].  One block.
@@ -259,36 +148,6 @@ tts_loss_bwd_kernel(const float* __restrict__ before, const float* __restrict__ 
 }  // namespace pk
 
 using namespace pk;
-#define PK_STREAM static_cast<cudaStream_t>(stream)
-
-extern "C" int pk_masked_softmax_ex(const float* s, const int32_t* key_lens, int32_t batch, int32_t heads, int32_t rows, int32_t keys,
-                                    int32_t ld, int32_t causal, void* p_hi, void* p_lo, pk_stream_t stream) {
-  PK_CHECK_ARG(s && p_hi && p_lo && batch > 0 && heads > 0 && rows > 0 && keys > 0 && ld >= keys, "bad arguments to pk_masked_softmax_ex");
-  const long long total = static_cast<long long>(batch) * heads * rows;
-  softmax_causal_kernel<<<nblk(total * 32, 256), 256, 0, PK_STREAM>>>(s, key_lens, heads, rows, keys, ld, causal ? 1 : 0, total,
-                                                                       static_cast<__nv_bfloat16*>(p_hi), static_cast<__nv_bfloat16*>(p_lo));
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
-
-extern "C" int pk_softmax_bwd_guided(const void* p_hi, const void* p_lo, const float* dp, int32_t batch, int32_t heads, int32_t rows,
-                                     int32_t keys, int32_t ld, float scale, int32_t guided_heads, int32_t guided_layers,
-                                     const int32_t* ilens, const int32_t* olens, float sigma, float lambda, float* partials, void* ds_hi,
-                                     void* ds_lo, pk_stream_t stream) {
-  PK_CHECK_ARG(p_hi && p_lo && dp && ds_hi && ds_lo && batch > 0 && heads > 0 && rows > 0 && keys > 0 && ld >= keys,
-               "bad arguments to pk_softmax_bwd_guided");
-  PK_CHECK_ARG(guided_heads >= 0 && guided_heads <= heads && guided_layers >= 1 && sigma > 0.f, "bad guided-loss arguments");
-  PK_CHECK_ARG(guided_heads == 0 || (ilens && olens && partials), "the guided heads need ilens, olens and partials");
-  const long long total = static_cast<long long>(batch) * heads * rows;
-  const float inv_two_sigma2 = static_cast<float>(1.0 / (2.0 * static_cast<double>(sigma) * sigma));
-  softmax_bwd_guided_kernel<<<nblk(total * 32, 256), 256, 0, PK_STREAM>>>(
-      static_cast<const __nv_bfloat16*>(p_hi), static_cast<const __nv_bfloat16*>(p_lo), dp, batch, heads, rows, keys, ld, scale, guided_heads,
-      guided_layers, ilens, olens, inv_two_sigma2, lambda, partials, static_cast<__nv_bfloat16*>(ds_hi), static_cast<__nv_bfloat16*>(ds_lo));
-  PK_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PK_OK;
-}
 
 extern "C" int pk_tts_guided_loss(const float* partials, int64_t n, const int32_t* ilens, const int32_t* olens, int32_t batch, int32_t rows,
                                   int32_t keys, int32_t heads_layers, float lambda, float* losses, pk_stream_t stream) {

@@ -81,8 +81,6 @@ wf_row_out_kernel(const float* __restrict__ skip, const float* __restrict__ wo /
   }
 }
 
-static inline int nblocks(long long n, int threads) { return static_cast<int>((n + threads - 1) / threads); }
-
 // ---------------------------------------------------------------- density direction (Flow.forward tail, WaveFlowLoss)
 constexpr int kFwdMaxGroup = 16;
 constexpr int kFwdTailThreads = 256;
@@ -229,7 +227,7 @@ extern "C" int pk_waveflow_upsample(const float* x, const float* w, const float*
   const int t_out = t_in * factor - (trim ? factor : 0);
   PK_CHECK_ARG(t_out > 0, "empty output");
   const long long n = static_cast<long long>(batch) * c * t_out;
-  wf_upsample_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, w, bias, c, t_in, factor, t_out, slope, n, y);
+  wf_upsample_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, w, bias, c, t_in, factor, t_out, slope, n, y);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;
@@ -240,7 +238,7 @@ extern "C" int pk_waveflow_input_proj(const float* x_row, int64_t x_batch_stride
                                       pk_stream_t stream) {
   PK_CHECK_ARG(x_row && w && bias && state && buf_hi && buf_lo && batch > 0 && width > 0 && c > 0 && ld >= col0 + c, "bad arguments");
   const long long n = static_cast<long long>(batch) * width * c;
-  wf_input_proj_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  wf_input_proj_kernel<<<nblk(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x_row, x_batch_stride, w, bias, width, c, n, state, static_cast<__nv_bfloat16*>(buf_hi), static_cast<__nv_bfloat16*>(buf_lo), ld, col0);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
@@ -251,7 +249,7 @@ extern "C" int pk_waveflow_row_out(const float* skip, const float* w, const floa
                                    int32_t batch, int32_t width, int32_t c, float* x_next, int64_t x_batch_stride, pk_stream_t stream) {
   PK_CHECK_ARG(skip && w && bias && z_row && x_next && batch > 0 && width > 0 && c > 0, "bad arguments");
   const long long rows = static_cast<long long>(batch) * width;
-  wf_row_out_kernel<<<nblocks(rows * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(skip, w, bias, z_row, z_batch_stride, width,
+  wf_row_out_kernel<<<nblk(rows * 32, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(skip, w, bias, z_row, z_batch_stride, width,
                                                                                            c, rows, x_next, x_batch_stride);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();

@@ -21,10 +21,6 @@
 namespace pk {
 namespace wft {
 
-static inline int nblk(long long n, int threads) { return static_cast<int>(std::min<long long>((n + threads - 1) / threads, 1 << 20)); }
-#define WFT_GRID_STRIDE(i, n) \
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < (n); i += static_cast<long long>(gridDim.x) * blockDim.x)
-
 __device__ __forceinline__ void store_split(float v, __nv_bfloat16* hi, __nv_bfloat16* lo, long long i) {
   __nv_bfloat16 h, l;
   split_bf16(v, h, l);
@@ -34,7 +30,7 @@ __device__ __forceinline__ void store_split(float v, __nv_bfloat16* hi, __nv_bfl
 
 __global__ void gather_split_kernel(const float* __restrict__ src, const int32_t* __restrict__ idx, long long n, __nv_bfloat16* hi,
                                     __nv_bfloat16* lo) {
-  WFT_GRID_STRIDE(i, n) {
+  PK_GRID_STRIDE(i, n) {
     const int32_t j = idx[i];
     store_split(j >= 0 ? src[j] : 0.f, hi, lo, i);
   }
@@ -43,7 +39,7 @@ __global__ void gather_split_kernel(const float* __restrict__ src, const int32_t
 // input_proj (1x1 Conv2D 1 -> C) of the flow input rows 0 .. G-2
 __global__ void input_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b, int G, int W, int C,
                                  long long n, float* __restrict__ h, __nv_bfloat16* x_hi, __nv_bfloat16* x_lo) {
-  WFT_GRID_STRIDE(i, n) {                                   // n = batch * (G + 1) * W * C, net layout
+  PK_GRID_STRIDE(i, n) {                                   // n = batch * (G + 1) * W * C, net layout
     const int c = static_cast<int>(i % C);
     const long long p = i / C;                              // position q * W + w
     const long long q = p / W;
@@ -61,7 +57,7 @@ __global__ void input_fwd_kernel(const float* __restrict__ x, const float* __res
 // h += res, skip (= or +=) skip_part; next layer input planes <- h
 __global__ void update_kernel(const float* __restrict__ out, int G, int W, int C, long long n, float* __restrict__ h, float* __restrict__ skip,
                               int skip_init, __nv_bfloat16* x_hi, __nv_bfloat16* x_lo) {
-  WFT_GRID_STRIDE(i, n) {
+  PK_GRID_STRIDE(i, n) {
     const int c = static_cast<int>(i % C);
     const long long p = i / C;
     const float res = out[p * 2 * C + c], sk = out[p * 2 * C + C + c];
@@ -188,12 +184,12 @@ __global__ void sum_partials_kernel(const float* __restrict__ partials, int npar
 
 // upsampler backward, leaky_relu part: dpre = dy * (y > 0 ? 1 : slope) (y the post-activation; slope > 0 keeps the sign)
 __global__ void leaky_bwd_post_kernel(const float* __restrict__ y, const float* __restrict__ dy, long long n, float slope, float* __restrict__ dpre) {
-  WFT_GRID_STRIDE(i, n) dpre[i] = y[i] > 0.f ? dy[i] : slope * dy[i];
+  PK_GRID_STRIDE(i, n) dpre[i] = y[i] > 0.f ? dy[i] : slope * dy[i];
 }
 // dx[b, ih, iw] = sum_{kh, kw} w[kh, kw] dpre[b, ih - 1 + kh, iw f - f/2 + kw]
 __global__ void upsample_dx_kernel(const float* __restrict__ dpre, const float* __restrict__ w, int M, int t_in, int f, int t_out, long long n,
                                    float* __restrict__ dx) {
-  WFT_GRID_STRIDE(i, n) {
+  PK_GRID_STRIDE(i, n) {
     const int iw = static_cast<int>(i % t_in);
     const long long bm = i / t_in;
     const int m = static_cast<int>(bm % M);
@@ -242,7 +238,7 @@ __global__ void upsample_dw_partial_kernel(const float* __restrict__ x, const fl
 // condition of one flow, gathered into the net layout: row (b, j) <- condition height rows[j + 1]; (batch, n_mels, t_cond) -> split planes
 __global__ void cond_gather_kernel(const float* __restrict__ cond, const int32_t* __restrict__ rows, int G, int W, int M, int t_cond, long long n,
                                    __nv_bfloat16* hi, __nv_bfloat16* lo) {
-  WFT_GRID_STRIDE(i, n) {
+  PK_GRID_STRIDE(i, n) {
     const int m = static_cast<int>(i % M);
     const long long p = i / M, q = p / W;
     const int w_ = static_cast<int>(p - q * W);
@@ -255,7 +251,7 @@ __global__ void cond_gather_kernel(const float* __restrict__ cond, const int32_t
 __global__ void cond_scatter_kernel(const float* __restrict__ dc, const int32_t* __restrict__ rows, int B, int G, int W, int M, int t_cond,
                                     float* __restrict__ dcond) {
   const long long n = static_cast<long long>(B) * (G - 1) * W * M;
-  WFT_GRID_STRIDE(i, n) {
+  PK_GRID_STRIDE(i, n) {
     const int m = static_cast<int>(i % M);
     const long long p = i / M;
     const int w_ = static_cast<int>(p % W);
@@ -292,34 +288,30 @@ __global__ void __launch_bounds__(1024) loss_kernel(const float* __restrict__ z,
 }  // namespace wft
 }  // namespace pk
 
+using namespace pk;
 using namespace pk::wft;
-#define WFT_ST static_cast<cudaStream_t>(stream)
-#define WFT_DONE()                   \
-  PK_CHECK_CUDA(cudaGetLastError()); \
-  ::pk::count_launch();              \
-  return PK_OK;
 #define BF(p) static_cast<__nv_bfloat16*>(p)
 
 extern "C" int pk_waveflow_train_gather_split(const float* src, const int32_t* idx, int64_t n, void* dst_hi, void* dst_lo, pk_stream_t stream) {
   PK_CHECK_ARG(src && idx && dst_hi && dst_lo && n > 0, "bad arguments");
-  gather_split_kernel<<<nblk(n, 256), 256, 0, WFT_ST>>>(src, idx, n, BF(dst_hi), BF(dst_lo));
-  WFT_DONE()
+  gather_split_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(src, idx, n, BF(dst_hi), BF(dst_lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_input_fwd(const float* x, const float* w, const float* bias, int32_t batch, int32_t n_group, int32_t width, int32_t c,
                                 float* h, void* x_hi, void* x_lo, pk_stream_t stream) {
   PK_CHECK_ARG(x && w && bias && h && x_hi && x_lo && batch > 0 && n_group >= 2 && width > 0 && c > 0, "bad arguments");
   const long long n = static_cast<long long>(batch) * (n_group + 1) * width * c;
-  input_fwd_kernel<<<nblk(n, 256), 256, 0, WFT_ST>>>(x, w, bias, n_group, width, c, n, h, BF(x_hi), BF(x_lo));
-  WFT_DONE()
+  input_fwd_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(x, w, bias, n_group, width, c, n, h, BF(x_hi), BF(x_lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_update(const float* out, int32_t batch, int32_t n_group, int32_t width, int32_t c, float* h, float* skip, int32_t skip_init,
                              void* x_hi, void* x_lo, pk_stream_t stream) {
   PK_CHECK_ARG(out && h && skip && batch > 0 && n_group >= 2 && width > 0 && c > 0 && (x_hi == nullptr) == (x_lo == nullptr), "bad arguments");
   const long long n = static_cast<long long>(batch) * (n_group + 1) * width * c;
-  update_kernel<<<nblk(n, 256), 256, 0, WFT_ST>>>(out, n_group, width, c, n, h, skip, skip_init, BF(x_hi), BF(x_lo));
-  WFT_DONE()
+  update_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(out, n_group, width, c, n, h, skip, skip_init, BF(x_hi), BF(x_lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_tail_fwd(const float* skip, const float* out_w, const float* out_b, const float* x, const int32_t* inv_perm, int32_t batch,
@@ -327,8 +319,8 @@ extern "C" int pk_waveflow_train_tail_fwd(const float* skip, const float* out_w,
   PK_CHECK_ARG(skip && out_w && out_b && x && inv_perm && x_next && logs && x != x_next && batch > 0 && n_group >= 2 && width > 0 && c > 0,
                "bad arguments");
   const long long warps = static_cast<long long>(batch) * n_group * width;
-  tail_fwd_kernel<<<nblk(warps * 32, 256), 256, 0, WFT_ST>>>(skip, out_w, out_b, x, inv_perm, batch, n_group, width, c, x_next, logs);
-  WFT_DONE()
+  tail_fwd_kernel<<<grid_stride_blocks(warps * 32, 256), 256, 0, PK_STREAM>>>(skip, out_w, out_b, x, inv_perm, batch, n_group, width, c, x_next, logs);
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_forward_tail_bwd(const float* skip, const float* out_w, const float* out_b, const float* x, const int32_t* inv_perm, const float* dy,
@@ -337,17 +329,17 @@ extern "C" int pk_waveflow_forward_tail_bwd(const float* skip, const float* out_
   PK_CHECK_ARG(skip && out_w && out_b && x && inv_perm && (dy || y) && dx && dparams && dskip && ds_hi && ds_lo && batch > 0 && n_group >= 2 &&
                width > 0 && c > 0 && ds_col0 + c <= ds_ld, "bad arguments");
   const long long warps = static_cast<long long>(batch) * n_group * width;
-  tail_bwd_kernel<<<nblk(warps * 32, 256), 256, 0, WFT_ST>>>(skip, out_w, out_b, x, inv_perm, dy, y, y_coef, dlogs, batch, n_group, width, c, dx,
-                                                             dparams, dskip, BF(ds_hi), BF(ds_lo), ds_ld, ds_col0);
-  WFT_DONE()
+  tail_bwd_kernel<<<grid_stride_blocks(warps * 32, 256), 256, 0, PK_STREAM>>>(skip, out_w, out_b, x, inv_perm, dy, y, y_coef, dlogs, batch, n_group, width, c, dx,
+                                                                              dparams, dskip, BF(ds_hi), BF(ds_lo), ds_ld, ds_col0);
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_input_bwd(const float* dh, const float* x, const float* w, int32_t batch, int32_t n_group, int32_t width, int32_t c, float* dx,
                                 float* xcol, pk_stream_t stream) {
   PK_CHECK_ARG(dh && x && w && dx && xcol && batch > 0 && n_group >= 2 && width > 0 && c > 0, "bad arguments");
   const long long warps = static_cast<long long>(batch) * (n_group - 1) * width;
-  input_bwd_kernel<<<nblk(warps * 32, 256), 256, 0, WFT_ST>>>(dh, x, w, batch, n_group, width, c, dx, xcol);
-  WFT_DONE()
+  input_bwd_kernel<<<grid_stride_blocks(warps * 32, 256), 256, 0, PK_STREAM>>>(dh, x, w, batch, n_group, width, c, dx, xcol);
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_outer_sum(const float* a, int32_t lda, int32_t ka, const float* b, int32_t ldb, int32_t kb, int64_t rows, float* scratch,
@@ -358,12 +350,10 @@ extern "C" int pk_waveflow_train_outer_sum(const float* a, int32_t lda, int32_t 
   PK_CHECK_ARG(nparts >= 1, "scratch too small");
   const long long chunk = (rows + nparts - 1) / nparts;
   const int used = static_cast<int>((rows + chunk - 1) / chunk);
-  outer_partial_kernel<<<used, 256, 0, WFT_ST>>>(a, lda, ka, b, ldb, kb, rows, chunk, scratch);
+  outer_partial_kernel<<<used, 256, 0, PK_STREAM>>>(a, lda, ka, b, ldb, kb, rows, chunk, scratch);
   PK_CHECK_CUDA(cudaGetLastError());
-  sum_partials_kernel<<<(ka * kb + 255) / 256, 256, 0, WFT_ST>>>(scratch, used, ka * kb, ka, kb, out, os_i, os_j, accumulate);
-  PK_CHECK_CUDA(cudaGetLastError());
-  ::pk::count_launch(2);
-  return PK_OK;
+  sum_partials_kernel<<<(ka * kb + 255) / 256, 256, 0, PK_STREAM>>>(scratch, used, ka * kb, ka, kb, out, os_i, os_j, accumulate);
+  PK_LAUNCH_DONE(2);
 }
 
 extern "C" int pk_waveflow_upsample_bwd(const float* x, const float* y, const float* dy, const float* w, int32_t batch, int32_t c, int32_t t_in,
@@ -377,36 +367,34 @@ extern "C" int pk_waveflow_upsample_bwd(const float* x, const float* y, const fl
   const int rows_per_block = static_cast<int>(std::max<long long>(std::max<long long>(1, (rows + 1023) / 1024), (rows * per + scratch_len - 1) / scratch_len));
   const int nparts = static_cast<int>((rows + rows_per_block - 1) / rows_per_block);
   PK_CHECK_ARG(static_cast<long long>(nparts) * per <= scratch_len, "scratch too small");
-  leaky_bwd_post_kernel<<<nblk(n_out, 256), 256, 0, WFT_ST>>>(y, dy, n_out, slope, dpre);
-  if (dx) upsample_dx_kernel<<<nblk(rows * t_in, 256), 256, 0, WFT_ST>>>(dpre, w, c, t_in, factor, t_out, rows * t_in, dx);
-  upsample_dw_partial_kernel<<<nparts, 128 * ((per + 127) / 128), 0, WFT_ST>>>(x, dpre, batch, c, t_in, factor, t_out, rows_per_block, scratch);
-  sum_partials_kernel<<<1, 256, 0, WFT_ST>>>(scratch, nparts, per, per - 1, 1, dw, 1, 0, 0);
-  sum_partials_kernel<<<1, 32, 0, WFT_ST>>>(scratch + (per - 1), nparts, per, 1, 1, db, 0, 0, 0);
-  PK_CHECK_CUDA(cudaGetLastError());
-  ::pk::count_launch(dx ? 5 : 4);
-  return PK_OK;
+  leaky_bwd_post_kernel<<<grid_stride_blocks(n_out, 256), 256, 0, PK_STREAM>>>(y, dy, n_out, slope, dpre);
+  if (dx) upsample_dx_kernel<<<grid_stride_blocks(rows * t_in, 256), 256, 0, PK_STREAM>>>(dpre, w, c, t_in, factor, t_out, rows * t_in, dx);
+  upsample_dw_partial_kernel<<<nparts, 128 * ((per + 127) / 128), 0, PK_STREAM>>>(x, dpre, batch, c, t_in, factor, t_out, rows_per_block, scratch);
+  sum_partials_kernel<<<1, 256, 0, PK_STREAM>>>(scratch, nparts, per, per - 1, 1, dw, 1, 0, 0);
+  sum_partials_kernel<<<1, 32, 0, PK_STREAM>>>(scratch + (per - 1), nparts, per, 1, 1, db, 0, 0, 0);
+  PK_LAUNCH_DONE(dx ? 5 : 4);
 }
 
 extern "C" int pk_waveflow_train_cond_gather(const float* cond, const int32_t* rows, int32_t batch, int32_t n_group, int32_t width, int32_t n_mels, int32_t t_cond,
                                   void* hi, void* lo, pk_stream_t stream) {
   PK_CHECK_ARG(cond && rows && hi && lo && batch > 0 && n_group >= 2 && width > 0 && n_mels > 0 && t_cond >= width * n_group, "bad arguments");
   const long long n = static_cast<long long>(batch) * (n_group + 1) * width * n_mels;
-  cond_gather_kernel<<<nblk(n, 256), 256, 0, WFT_ST>>>(cond, rows, n_group, width, n_mels, t_cond, n, BF(hi), BF(lo));
-  WFT_DONE()
+  cond_gather_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(cond, rows, n_group, width, n_mels, t_cond, n, BF(hi), BF(lo));
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_cond_scatter(const float* dc, const int32_t* rows, int32_t batch, int32_t n_group, int32_t width, int32_t n_mels, int32_t t_cond,
                                    float* dcond, pk_stream_t stream) {
   PK_CHECK_ARG(dc && rows && dcond && batch > 0 && n_group >= 2 && width > 0 && n_mels > 0 && t_cond >= width * n_group, "bad arguments");
   const long long n = static_cast<long long>(batch) * (n_group - 1) * width * n_mels;
-  cond_scatter_kernel<<<nblk(n, 256), 256, 0, WFT_ST>>>(dc, rows, batch, n_group, width, n_mels, t_cond, dcond);
-  WFT_DONE()
+  cond_scatter_kernel<<<grid_stride_blocks(n, 256), 256, 0, PK_STREAM>>>(dc, rows, batch, n_group, width, n_mels, t_cond, dcond);
+  PK_LAUNCH_DONE(1);
 }
 
 extern "C" int pk_waveflow_train_loss(const float* z, int64_t n, const float* logs, int64_t n_logs, float sigma, float* loss, pk_stream_t stream) {
   PK_CHECK_ARG(z && logs && loss && n > 0 && n_logs > 0 && sigma > 0.f, "bad arguments");
-  loss_kernel<<<1, 1024, 0, WFT_ST>>>(z, n, logs, n_logs, sigma, loss);
-  WFT_DONE()
+  loss_kernel<<<1, 1024, 0, PK_STREAM>>>(z, n, logs, n_logs, sigma, loss);
+  PK_LAUNCH_DONE(1);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
@@ -685,7 +673,7 @@ static int backward_layer_launch(const pk_waveflow_backward_layer_args* a, pk_st
   p.h = a->h;
   p.dh_hi = static_cast<__nv_bfloat16*>(a->dh_out_hi); p.dh_lo = static_cast<__nv_bfloat16*>(a->dh_out_lo);
   const int grid = std::min(p.total_tiles, resident);
-  waveflow_backward_layer_kernel<C><<<grid, kThreads, G::kSmem, static_cast<cudaStream_t>(stream)>>>(tdh, tw1, tw2, p);
+  waveflow_backward_layer_kernel<C><<<grid, kThreads, G::kSmem, PK_STREAM>>>(tdh, tw1, tw2, p);
   PK_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PK_OK;

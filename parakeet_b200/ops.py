@@ -279,12 +279,12 @@ def layer_norm(x, gamma, beta, lens=None, want_f32=False, want_split=True, eps=1
     return y, ys
 
 
-def masked_softmax(s, key_lens, batch, heads, rows, keys):
-    """s fp32 (batch*heads, rows, ld) -> split planes of the same shape."""
+def masked_softmax(s, key_lens, batch, heads, rows, keys, causal=False):
+    """s fp32 (batch*heads, rows, ld) -> split planes of the same shape; causal adds the j <= i mask."""
     ld = s.shape[-1]
     p = Split.empty(tuple(s.shape), s.device)
-    _lib.check(_lib.lib().pk_masked_softmax(_ptr(s), _ptr(key_lens), batch, heads, rows, keys, ld, _ptr(p.hi), _ptr(p.lo),
-                                            _stream()), "pk_masked_softmax")
+    _lib.check(_lib.lib().pk_masked_softmax(_ptr(s), _ptr(key_lens), batch, heads, rows, keys, ld, 1 if causal else 0, _ptr(p.hi),
+                                            _ptr(p.lo), _stream()), "pk_masked_softmax")
     return p
 
 
@@ -430,12 +430,21 @@ def layer_norm_bwd(x, gamma, dy, dx, accumulate, dgamma, dbeta, eps=1e-5):
                                             _ptr(dgamma), _ptr(dbeta), _stream()), "pk_layer_norm_bwd")
 
 
-def softmax_bwd(p, dp, keys, scale):
-    ld = dp.shape[-1]
-    rows = dp.numel() // ld
+def softmax_bwd(p, dp, keys, scale, guided=None):
+    """pk_softmax_bwd: p split planes, dp fp32 (..., rows, ld) -> dS split planes of the same shape.  guided: None, or
+    dict(heads, layers, ilens, olens, sigma, lam, partials) to fold the guided attention loss into heads h < guided["heads"] of
+    a (batch * heads, rows, ld) layout, batch = ilens.numel(); the loss's row partials (batch, guided["heads"], rows) go to
+    `partials` (a contiguous fp32 view)."""
+    rows, ld = (dp.shape[-2] if dp.dim() > 1 else 1), dp.shape[-1]
+    z = dp.numel() // (rows * ld)
     ds = Split.empty(tuple(dp.shape), dp.device)
-    _lib.check(_lib.lib().pk_softmax_bwd(_ptr(p.hi), _ptr(p.lo), _ptr(dp), rows, keys, ld, scale, _ptr(ds.hi), _ptr(ds.lo), _stream()),
-               "pk_softmax_bwd")
+    g = guided or dict(heads=0, layers=1, ilens=None, olens=None, sigma=1.0, lam=0.0, partials=None)
+    batch = g["ilens"].numel() if guided else z
+    if z % batch:
+        raise ValueError(f"softmax_bwd: {z} (batch * heads) rows of attention for {batch} utterances")
+    _lib.check(_lib.lib().pk_softmax_bwd(_ptr(p.hi), _ptr(p.lo), _ptr(dp), batch, z // batch, rows, keys, ld, float(scale), g["heads"],
+                                         g["layers"], _ptr(g["ilens"]), _ptr(g["olens"]), float(g["sigma"]), float(g["lam"]),
+                                         _ptr(g["partials"]), _ptr(ds.hi), _ptr(ds.lo), _stream()), "pk_softmax_bwd")
     return ds
 
 
@@ -820,26 +829,6 @@ def tts_stop_labels(olens, width):
     out = torch.empty(B, width, dtype=torch.float32, device=olens.device)
     _lib.check(_lib.lib().pk_tts_stop_labels(_ptr(olens), B, width, _ptr(out), _stream()), "pk_tts_stop_labels")
     return out
-
-
-def masked_softmax_ex(s, key_lens, batch, heads, rows, keys, causal=False):
-    """pk_masked_softmax_ex: s fp32 (batch*heads, rows, ld) -> split planes of the same shape; causal adds the j <= i mask."""
-    ld = s.shape[-1]
-    p = Split.empty(tuple(s.shape), s.device)
-    _lib.check(_lib.lib().pk_masked_softmax_ex(_ptr(s), _ptr(key_lens), batch, heads, rows, keys, ld, 1 if causal else 0, _ptr(p.hi),
-                                               _ptr(p.lo), _stream()), "pk_masked_softmax_ex")
-    return p
-
-
-def softmax_bwd_guided(p, dp, batch, heads, rows, keys, scale, guided_heads, guided_layers, ilens, olens, sigma, lam, partials):
-    """pk_softmax_bwd_guided -> dS split planes (batch*heads, rows, ld); writes the guided loss's row partials (batch, guided_heads,
-    rows) into `partials` (a contiguous fp32 view)."""
-    ld = dp.shape[-1]
-    ds = Split.empty(tuple(dp.shape), dp.device)
-    _lib.check(_lib.lib().pk_softmax_bwd_guided(_ptr(p.hi), _ptr(p.lo), _ptr(dp), batch, heads, rows, keys, ld, float(scale), guided_heads,
-                                                guided_layers, _ptr(ilens), _ptr(olens), float(sigma), float(lam), _ptr(partials),
-                                                _ptr(ds.hi), _ptr(ds.lo), _stream()), "pk_softmax_bwd_guided")
-    return ds
 
 
 def tts_guided_loss(partials, ilens, olens, rows, keys, heads_layers, lam, losses):

@@ -98,16 +98,15 @@ class FlatAdam:
         if world > 1:
             self.buffers.all_reduce_grads(group)
         self.steps += 1
-        if self.clip_norm is None:
-            _lib.check(L.pk_adam(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), n, lr, self.beta1, self.beta2, self.epsilon,
-                                 self.steps, 1.0 / world, _stream()), "pk_adam")
-            return
-        if world > 1:
-            self.gflat.mul_(1.0 / world)                 # the mean comes before the clip, like paddle
-        self.sq.zero_()
-        _lib.check(L.pk_sq_sum(_ptr(self.gflat), n, _ptr(self.sq), _stream()), "pk_sq_sum")
-        _lib.check(L.pk_adam_clip(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), n, lr, self.beta1, self.beta2, self.epsilon,
-                                  self.steps, _ptr(self.sq), float(self.clip_norm), _stream()), "pk_adam_clip")
+        grad_scale = 1.0 / world
+        if self.clip_norm is not None:
+            if world > 1:
+                self.gflat.mul_(1.0 / world)             # the mean comes before the clip, like paddle
+            grad_scale = 1.0
+            self.sq.zero_()
+            _lib.check(L.pk_sq_sum(_ptr(self.gflat), n, _ptr(self.sq), _stream()), "pk_sq_sum")
+        _lib.check(L.pk_adam(_ptr(self.flat), _ptr(self.gflat), _ptr(self.m), _ptr(self.v), n, lr, self.beta1, self.beta2, self.epsilon,
+                             self.steps, grad_scale, _ptr(self.sq), float(self.clip_norm or 0.0), _stream()), "pk_adam")
 
     def _views(self):
         b = self.buffers

@@ -5,7 +5,7 @@ call `mha_fwd` / `mha_bwd` for the causal self-attention and the source attentio
 
 Attention is materialised: S = Q K^T / sqrt(dk) into a (B*H, Tq, ceil64(Tk)) fp32 buffer, the masked softmax, dropout on the
 probabilities (pk_dropout, regenerated in the backward), ctx = P V; the backward forms dP = dO V^T, the softmax backward (with the
-guided attention loss folded in where requested: pk_softmax_bwd_guided), and dQ = dS K, dK = dS^T Q, dV = P^T dO as pk_conv_gemm NT
+guided attention loss folded in where requested: pk_softmax_bwd), and dQ = dS K, dK = dS^T Q, dV = P^T dO as pk_conv_gemm NT
 matmuls on transposed split planes (pk_transpose_planes).  Q comes from one tensor, K and V from another (column offsets and
 leading dimensions free), so the source attention reads the fused K | V memory of every decoder layer in place.
 
@@ -99,10 +99,7 @@ class TransformerTrainOps:
         k_spec = dict(rows=Tk, cols=kv_ld, ld=kv_ld, batch_stride=Tk * kv_ld, batches=B, bmul=1, hmul=0, col0=k_col0, colh=dk)
         ops.batched_matmul_nt(q, kv, batch=B, heads=heads, m=Tq, n=Tk, k=dk, a_spec=q_spec, b_spec=k_spec, scale=1.0 / math.sqrt(dk),
                               y_f32=s_buf, y_batch_stride=heads * Tq * Tp, y_head_stride=Tq * Tp, y_ld=Tp)
-        if causal:
-            p = ops.masked_softmax_ex(s_buf, key_lens, B, heads, Tq, Tk, causal=True)
-        else:
-            p = ops.masked_softmax(s_buf, key_lens, B, heads, Tq, Tk)
+        p = ops.masked_softmax(s_buf, key_lens, B, heads, Tq, Tk, causal=causal)
         pd = self.drop(p, rate, site, out_f32=False, out_split=True)[1] if rate > 0 else p
         vt = ops.transpose_heads(kv, col0=v_col0, dk=dk, heads=heads, ld_dst=Tp)
         ctx = Split.empty((B, Tq, A), q.hi.device)
@@ -115,7 +112,7 @@ class TransformerTrainOps:
     def mha_bwd(self, dctx_s, S, dq, dkv, guided=None):
         """dctx_s Split (B, Tq, A): gradient w.r.t. mha_fwd's ctx.  Writes dQ into dq (fp32 (B, Tq, >= q_col0 + A)) at mha_fwd's
         q_col0, dK and dV into dkv (fp32 (B, Tk, kv_ld)) at k_col0 / v_col0 (dq may be dkv: the fused Q | K | V).
-        guided: None, or dict(heads, layers, ilens, olens, sigma, lam, partials) for pk_softmax_bwd_guided."""
+        guided: None, or dict(heads, layers, ilens, olens, sigma, lam, partials): the guided loss of ops.softmax_bwd."""
         q, kv, p, H, dk = S["q"], S["kv"], S["p"], S["heads"], S["dk"]
         B, Tq, q_ld = q.hi.shape
         Tk, kv_ld = kv.hi.shape[1], kv.hi.shape[2]
@@ -130,11 +127,7 @@ class TransformerTrainOps:
                               y_batch_stride=H * Tq * Tkp, y_head_stride=Tq * Tkp, y_ld=Tkp)                  # d(drop(P)) = dO V^T
         if S["rate"] > 0:
             self.drop(dp, S["rate"], S["site"], inplace=True)                                               # -> dP
-        if guided is None:
-            ds = ops.softmax_bwd(p, dp, Tk, 1.0 / math.sqrt(dk))                                            # includes the 1/sqrt(dk)
-        else:
-            ds = ops.softmax_bwd_guided(p, dp, B, H, Tq, Tk, 1.0 / math.sqrt(dk), guided["heads"], guided["layers"], guided["ilens"],
-                                        guided["olens"], guided["sigma"], guided["lam"], guided["partials"])
+        ds = ops.softmax_bwd(p, dp, Tk, 1.0 / math.sqrt(dk), guided)                                            # includes the 1/sqrt(dk)
         # K-major operands: (B*H, Tk, Tqp) for dV / dK, (B*H, Tq, Tkp) for dQ
         z_spec = dict(rows=Tk, cols=Tqp, ld=Tqp, batch_stride=Tk * Tqp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)
         dq_spec = dict(rows=Tq, cols=Tkp, ld=Tkp, batch_stride=Tq * Tkp, batches=B * H, bmul=H, hmul=1, col0=0, colh=0)

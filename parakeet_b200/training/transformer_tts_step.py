@@ -10,7 +10,7 @@ examples/transformer_tts/ljspeech/conf/default.yaml).
 
 The encoder is the FFT-block stack of training/transformer.py; each decoder layer (pre-LN causal self-attention, source attention
 over the fused K | V memory of all layers, Linear feed-forward) calls its mha_fwd / mha_bwd.  The guided loss is folded into the
-softmax backward of the guided layers (pk_softmax_bwd_guided): dP of the selected heads gains lambda / N * G, and the loss's row
+softmax backward of the guided layers (pk_softmax_bwd): dP of the selected heads gains lambda / N * G, and the loss's row
 partials come out of the same pass.  The model's own `train()` keeps refusing; this class is the training entry point and
 neither reads nor changes `model.training`.
 
@@ -374,8 +374,8 @@ class TransformerTTSTrainStep(TransformerTrainOps):
             zero = torch.zeros(B * m.aheads, Lm, Tk, dtype=torch.float32, device=self.dev)
             for j in range(self.g_layers):          # the loss's partial sums from the guided softmax backward on dP = 0
                 p = Split.from_f32(att[:, m.dlayers - 1 - j].reshape(B * m.aheads, Lm, Tk))
-                ops.softmax_bwd_guided(p, zero, B, m.aheads, Lm, Tk, 1.0, self.g_heads, self.g_layers, ilens, olens, self.sigma, self.lam,
-                                       partials[j])
+                ops.softmax_bwd(p, zero, Tk, 1.0, dict(heads=self.g_heads, layers=self.g_layers, ilens=ilens, olens=olens, sigma=self.sigma,
+                                                       lam=self.lam, partials=partials[j]))
             ops.tts_guided_loss(partials, ilens, olens, Lm, Tk, self.g_heads * self.g_layers, self.lam, losses)
         return self._named(losses)
 

@@ -45,8 +45,13 @@ def test_no_process_wide_launch_caches(pattern):
     ("sigmoidf_", "pk_sm90.cuh"),
     ("ld_acquire_gpu", "pk_sm90.cuh"),
     ("red_release_gpu_inc", "pk_sm90.cuh"),
+    ("warp_max", "pk_sm90.cuh"),
+    ("ld_split", "pk_sm90.cuh"),
+    ("block_sum_tree", "pk_sm90.cuh"),
     ("aligned16", "pk_host.h"),
     ("fold_gate_bias", "pk_host.h"),
+    ("nblk", "pk_host.h"),
+    ("grid_stride_blocks", "pk_host.h"),
 ])
 def test_helper_defined_once(name, home):
     # a definition: return type, the name, its parameter list and an opening brace (calls end in ';' or sit inside expressions)
@@ -59,3 +64,24 @@ def test_helper_defined_once(name, home):
 def test_log2e_constant_defined_once():
     where = sorted(name for name, text in SOURCES.items() if re.search(r"constexpr float kLog2e\b", text))
     assert where == ["pk_host.h"], where
+
+
+def test_launch_macros_defined_once():
+    # the stream cast, the launch tail and the grid-stride loop live in pk_host.h / pk_sm90.cuh under one name each
+    stream_cast = re.compile(r"^[ \t]*#[ \t]*define[ \t]+\w+[^\n]*static_cast<cudaStream_t>", re.MULTILINE)
+    launch_tail = re.compile(r"^[ \t]*#[ \t]*define[ \t]+\w+(?:\([^)]*\))?[ \t]*\\?\s*PK_CHECK_CUDA\(cudaGetLastError\(\)\)", re.MULTILINE)
+    grid_stride = re.compile(r"^[ \t]*#[ \t]*define[ \t]+\w+\([^)]*\)[ \t]*\\?\s*for \(long long", re.MULTILINE)
+    for pattern, home in ((stream_cast, "pk_host.h"), (launch_tail, "pk_host.h"), (grid_stride, "pk_sm90.cuh")):
+        where = [(name, len(pattern.findall(text))) for name, text in SOURCES.items() if pattern.search(text)]
+        assert where == [(home, 1)], (pattern.pattern, where)
+
+
+def test_merged_entry_points_are_gone():
+    # the causal mask, the guided attention loss and the gradient clip are arguments of these three, not entry points of their own
+    with open(os.path.join(ROOT, "include", "parakeet_b200.h")) as f:
+        header = f.read()
+    for name, variant in (("pk_masked_softmax", "_ex"), ("pk_softmax_bwd", "_guided"), ("pk_adam", "_clip")):
+        assert re.search(rf"\b{name}\(", header), name
+        gone = name + variant
+        assert not re.search(rf"\b{gone}\b", header), gone
+        assert not [f for f, text in SOURCES.items() if re.search(rf"\b{gone}\b", text)], gone

@@ -34,7 +34,7 @@ def _leaf(params):
     return {k: v.clone().requires_grad_(True) for k, v in params.items()}
 
 
-def test_gan_kernels_unit(cuda):
+def test_gan_kernels_and_clipped_adam_unit(cuda):
     from oracle import pwg as opwg
     from oracle import stft as ostft
     from parakeet_b200 import _lib, ops
@@ -83,7 +83,7 @@ def test_gan_kernels_unit(cuda):
     pc, gc2, mc, vc2 = p0.clone().to(cuda), g0.to(cuda), torch.zeros(1000, device=cuda), torch.zeros(1000, device=cuda)
     sq = torch.zeros(1, dtype=torch.float64, device=cuda)
     _lib.check(L.pk_sq_sum(_ptr(gc2), 1000, _ptr(sq), _stream()), "sq")
-    _lib.check(L.pk_adam_clip(_ptr(pc), _ptr(gc2), _ptr(mc), _ptr(vc2), 1000, 1e-4, 0.9, 0.999, 1e-6, 1, _ptr(sq), clip, _stream()), "adam")
+    _lib.check(L.pk_adam(_ptr(pc), _ptr(gc2), _ptr(mc), _ptr(vc2), 1000, 1e-4, 0.9, 0.999, 1e-6, 1, 1.0, _ptr(sq), clip, _stream()), "adam")
     assert abs(float(sq) - float(g0.double().pow(2).sum())) < 1e-3 * float(sq) and torch.allclose(pc.cpu(), ref, atol=1e-8)
 
 

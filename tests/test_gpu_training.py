@@ -12,7 +12,7 @@ def _close(a, ref, rtol=2e-3, atol=2e-6):
     return (a - ref).abs().max().item() <= rtol * ref.abs().max().item() + atol
 
 
-def test_train_kernels_unit(cuda):
+def test_fs2_train_kernels_unit(cuda):
     """Row-wise backward kernels against torch autograd."""
     from parakeet_b200 import _lib, ops
     from parakeet_b200.ops import _ptr, _stream
@@ -81,13 +81,13 @@ def test_train_kernels_unit(cuda):
     ref2 = ofs.adam_step({"w": ref1}, {"w": g0 * 0.5}, st, lr=1e-3)["w"]
     pc, mc, vc = p0.clone().to(cuda), torch.zeros(1000, device=cuda), torch.zeros(1000, device=cuda)
     g0c, g1c = g0.to(cuda), (g0 * 0.5).to(cuda)
-    _lib.check(L.pk_adam(_ptr(pc), _ptr(g0c), _ptr(mc), _ptr(vc), 1000, 1e-3, 0.9, 0.999, 1e-8, 1, 1.0, _stream()), "adam")
+    _lib.check(L.pk_adam(_ptr(pc), _ptr(g0c), _ptr(mc), _ptr(vc), 1000, 1e-3, 0.9, 0.999, 1e-8, 1, 1.0, None, 0.0, _stream()), "adam")
     assert torch.allclose(pc.cpu(), ref1, atol=1e-7)
-    _lib.check(L.pk_adam(_ptr(pc), _ptr(g1c), _ptr(mc), _ptr(vc), 1000, 1e-3, 0.9, 0.999, 1e-8, 2, 1.0, _stream()), "adam")
+    _lib.check(L.pk_adam(_ptr(pc), _ptr(g1c), _ptr(mc), _ptr(vc), 1000, 1e-3, 0.9, 0.999, 1e-8, 2, 1.0, None, 0.0, _stream()), "adam")
     assert torch.allclose(pc.cpu(), ref2, atol=1e-7)
 
 
-def test_fs2_training_step_gradients_and_update(cuda):
+def test_fs2_training_step_gradients_and_adam_update(cuda):
     from oracle import fastspeech2 as ofs
     from parakeet_b200.models import FastSpeech2
     from parakeet_b200.training import FastSpeech2TrainStep
@@ -123,7 +123,7 @@ def test_fs2_training_step_gradients_and_update(cuda):
     from parakeet_b200 import _lib
     from parakeet_b200.ops import _ptr, _stream
     _lib.check(_lib.lib().pk_adam(_ptr(ts.flat), _ptr(ts.gflat), _ptr(ts.adam_m), _ptr(ts.adam_v), ts.flat.numel(), 1e-3, 0.9, 0.999, 1e-8, 1,
-                                  1.0, _stream()), "pk_adam")
+                                  1.0, None, 0.0, _stream()), "pk_adam")
     # Adam's first step moves every weight by ~lr * sign(g): compare where the gradient is not numerically zero (|g| > 1e-5;
     # elements whose true gradient is ~0, e.g. the key biases of the attention, take an arbitrary sign) and not kink-affected
     worst = 0.0

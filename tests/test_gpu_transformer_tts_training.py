@@ -26,8 +26,8 @@ def _rel(a, b):
 # kernels
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("tq", [1, 63, 64, 65, 800])
-def test_causal_softmax_and_guided_softmax_bwd(cuda, tq):
-    """pk_masked_softmax_ex (causal self-attention, Tq = Tk) and pk_softmax_bwd_guided (source attention, ragged ilens / olens,
+def test_causal_masked_softmax_and_guided_softmax_bwd(cuda, tq):
+    """pk_masked_softmax (causal self-attention, Tq = Tk) and pk_softmax_bwd (source attention, ragged ilens / olens,
     guided heads 0..1 of 3) against fp64 autograd of softmax -> <P, dP> + coef * sum G P."""
     from parakeet_b200 import ops
     g = torch.Generator().manual_seed(tq)
@@ -36,7 +36,7 @@ def test_causal_softmax_and_guided_softmax_bwd(cuda, tq):
     olens = torch.tensor([tq, max(1, tq - tq // 3)], dtype=torch.int32)
     ld = (tq + 63) // 64 * 64
     s = torch.randn(B * H, tq, ld, generator=g) * 2
-    p = ops.masked_softmax_ex(s.to(cuda), olens.to(cuda), B, H, tq, tq, causal=True).float().cpu()
+    p = ops.masked_softmax(s.to(cuda), olens.to(cuda), B, H, tq, tq, causal=True).float().cpu()
     keep = ofs.make_non_pad_mask(olens, tq).unsqueeze(1) & torch.tril(torch.ones(tq, tq, dtype=torch.bool))
     keep = keep.repeat_interleave(H, 0)
     ref = torch.softmax(s[..., :tq].double().masked_fill(~keep, -1e300), -1).masked_fill(~keep, 0.0)
@@ -61,8 +61,8 @@ def test_causal_softmax_and_guided_softmax_bwd(cuda, tq):
     Pp = torch.nn.functional.pad(P.detach().float(), (0, ldk - tk))
     dpp = torch.nn.functional.pad(dp.float(), (0, ldk - tk))
     partials = torch.full((B, Hg, tq), 7.0, device=cuda)
-    ds = ops.softmax_bwd_guided(ops.Split.from_f32(Pp.to(cuda)), dpp.to(cuda), B, H, tq, tk, scale, Hg, layers, ilens.to(cuda),
-                                olens.to(cuda), sigma, lam, partials).float().cpu()
+    guided = dict(heads=Hg, layers=layers, ilens=ilens.to(cuda), olens=olens.to(cuda), sigma=sigma, lam=lam, partials=partials)
+    ds = ops.softmax_bwd(ops.Split.from_f32(Pp.to(cuda)), dpp.to(cuda), tk, scale, guided).float().cpu()
     assert _rel(ds[..., :tk], z.grad * scale) < 3e-5 and (ldk == tk or ds[..., tk:].abs().max().item() == 0)
     pref = (G * P.detach()).sum(-1).reshape(B, H, tq)[:, :Hg]
     assert _rel(partials, pref) < 1e-5

@@ -14,7 +14,7 @@ from oracle import transformer_tts_train as ot
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_executed_transformer_tts_train.npz")
-ENTRY_POINTS = ("pk_masked_softmax_ex", "pk_softmax_bwd_guided", "pk_tts_guided_loss", "pk_tts_loss_workspace", "pk_tts_loss",
+ENTRY_POINTS = ("pk_masked_softmax", "pk_softmax_bwd", "pk_tts_guided_loss", "pk_tts_loss_workspace", "pk_tts_loss",
                 "pk_tts_loss_bwd")
 
 
@@ -84,15 +84,15 @@ def test_model_still_refuses_train_mode_and_speaker_embeddings():
         _cpu_model(spk_embed_dim=16)
 
 
-def test_entry_points_in_header_and_binding():
+def test_step_entry_points_in_header_and_binding():
     from parakeet_b200 import _lib
     with open(_lib.HEADER) as f:
         header = f.read()
     for name in ENTRY_POINTS:
         assert re.search(rf"\b{name}\s*\(", header), name
         assert name in _lib.exported_symbols(), name
-    assert len(_lib.PROTOTYPES["pk_softmax_bwd_guided"].argtypes) == 19
-    assert len(_lib.PROTOTYPES["pk_masked_softmax_ex"].argtypes) == 11
+    assert len(_lib.PROTOTYPES["pk_softmax_bwd"].argtypes) == 19
+    assert len(_lib.PROTOTYPES["pk_masked_softmax"].argtypes) == 11
 
 
 def _nvcc():
@@ -102,26 +102,27 @@ def _nvcc():
     return None
 
 
-def test_training_kernels_compile_for_sm90a_without_spills(tmp_path):
+def test_step_kernels_compile_for_sm90a_without_spills(tmp_path):
     nvcc = _nvcc()
     if nvcc is None:
         pytest.skip("nvcc not available")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "transformer_tts_train.cu"), "-o", str(tmp_path / "t.o")],
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    blocks, cur = {}, None
-    for ln in r.stderr.splitlines():
-        m = re.search(r"Compiling entry function '(\w+)'", ln)
-        if m:
-            cur = m.group(1)
-            blocks[cur] = []
-        elif cur:
-            blocks[cur].append(ln)
-    kernels = ("softmax_causal_kernel", "softmax_bwd_guided_kernel", "guided_loss_kernel", "tts_loss_partial_kernel",
-               "tts_loss_final_kernel", "tts_loss_bwd_kernel")
-    for k in kernels:
-        found = [v for name, v in blocks.items() if k in name]
-        assert found, f"ptxas reported no entry function {k}"
-        spills = [ln for ln in found[0] if "spill" in ln]
-        assert spills and all(re.search(r"\b0 bytes spill stores, 0 bytes spill loads", ln) for ln in spills), (k, spills)
+    kernels = {"fs2.cu": ("masked_softmax_kernel",), "train.cu": ("softmax_bwd_kernel",),
+               "transformer_tts_train.cu": ("guided_loss_kernel", "tts_loss_partial_kernel", "tts_loss_final_kernel", "tts_loss_bwd_kernel")}
+    for src, names in kernels.items():
+        r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
+                            os.path.join(ROOT, "parakeet_b200", "csrc", src), "-o", str(tmp_path / "t.o")],
+                           capture_output=True, text=True, timeout=600)
+        assert r.returncode == 0, r.stderr[-4000:]
+        blocks, cur = {}, None
+        for ln in r.stderr.splitlines():
+            m = re.search(r"Compiling entry function '(\w+)'", ln)
+            if m:
+                cur = m.group(1)
+                blocks[cur] = []
+            elif cur:
+                blocks[cur].append(ln)
+        for k in names:
+            found = [v for name, v in blocks.items() if k in name]
+            assert found, f"ptxas reported no entry function {k} in {src}"
+            spills = [ln for ln in found[0] if "spill" in ln]
+            assert spills and all(re.search(r"\b0 bytes spill stores, 0 bytes spill loads", ln) for ln in spills), (k, spills)

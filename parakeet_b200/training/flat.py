@@ -1,14 +1,17 @@
-"""Flat parameter / gradient buffers for the data-parallel training step.
+"""Flat parameter / gradient buffers for the data-parallel training step, and what every training step shares around them.
 
 The reference wraps the model in `paddle.DataParallel` (examples/fastspeech2/*/train.py:117-119), which all-reduces
 gradients bucket by bucket.  Here every trainable tensor is a view into ONE flat fp32 buffer (and its gradient into a second
 one), so the exchange step of the path is a single `all_reduce(SUM)` of the flat gradient and the optimiser (`FlatAdam`, the
 one every training step uses) is a single kernel over the flat buffers; it also applies the 1/world scale of the DataParallel
 mean.
-Device-agnostic on purpose: the CPU tests run the buffers over gloo (tests/test_dist_cpu.py) and the optimiser's checkpoint
-entries on the CPU (tests/test_flat_adam_cpu.py); only `FlatAdam.update` needs the library.
-The rest is what every training step shares around its buffers: rank 0's broadcast at construction, the snapshot container of
-`StandardUpdater` and the switch of the step's CUDA graphs.
+Device-agnostic on purpose: the CPU tests run the buffers over gloo (tests/test_dist_cpu.py), the optimiser's checkpoint
+entries (tests/test_flat_adam_cpu.py) and the graph / zero-plane owner `StepGraphs` (tests/test_graph_cpu.py) on the CPU; only
+`FlatAdam.update` needs the library.
+`TrainStep` is the base of the FastSpeech2, SpeedySpeech, TransformerTTS, WaveFlow and GE2E steps: set-up (FlatAdam, rank 0's
+broadcast), the CUDA graphs of the forward + backward with their zero planes, and the three entry points `forward_backward`,
+`forward_backward_graphed` and `step`.  `UpdaterSnapshot` (the `StandardUpdater` container) and `PdCheckpoint` (the old-style
+pair) are the two snapshot formats.
 """
 import os
 from collections import OrderedDict
@@ -19,15 +22,40 @@ import torch.distributed as dist
 from .. import _lib
 from ..graph import GraphRunner
 from ..ops import _ptr, _stream
+from .conv import ConvOps
+from .wgrad import ZeroPlanes
 
 BUFFERS = ("_mean", "_variance")      # BatchNorm running statistics: state-dict entries that are not trained
 
 
+def _train_graphs_on(use_graphs):
+    return os.environ.get("PK_TRAIN_GRAPH", "1") != "0" if use_graphs is None else bool(use_graphs)
+
+
 def step_graphs(max_graphs, use_graphs=None):
     """The GraphRunner that replays a training step's forward + backward: on when `use_graphs` says so, else unless
-    PK_TRAIN_GRAPH=0 (PK_CUDA_GRAPHS=0 turns every graph off)."""
-    on = os.environ.get("PK_TRAIN_GRAPH", "1") != "0" if use_graphs is None else bool(use_graphs)
-    return GraphRunner(max_graphs=max_graphs, enabled=on)
+    PK_TRAIN_GRAPH=0 (PK_CUDA_GRAPHS=0 turns every graph off).  PWGTrainStep's; the other steps own a StepGraphs."""
+    return GraphRunner(max_graphs=max_graphs, enabled=_train_graphs_on(use_graphs))
+
+
+class StepGraphs(GraphRunner):
+    """The CUDA graphs of a training step's forward + backward, one per batch shape, and the zero planes baked into them
+    (`planes`, wgrad.ZeroPlanes), filed under the same key.  `run` makes the key's planes current (most recently used) before it
+    runs the function eagerly or through its graph; evicting a key's planes beyond `max_graphs` drops the graph of that key,
+    whose kernels hold the planes' addresses.  Switched like step_graphs."""
+
+    def __init__(self, max_graphs, use_graphs=None):
+        super().__init__(max_graphs=max_graphs, enabled=_train_graphs_on(use_graphs))
+        self.planes = ZeroPlanes(max_geoms=max_graphs, on_evict=self.drop)
+
+    def run(self, key, fn, inputs, graph=True):
+        self.planes.begin(key)
+        return super().run(key, fn, inputs) if graph else fn(*inputs)
+
+
+def need_cuda(model):
+    if model.device.type != "cuda":
+        raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
 
 
 def broadcast_from_rank0(flat, params, group=None):
@@ -37,22 +65,6 @@ def broadcast_from_rank0(flat, params, group=None):
     for k, v in params.items():
         if k.endswith(BUFFERS):
             dist.broadcast(v, src=0, group=group)
-
-
-def updater_state(model, opt, lr, epoch=0):
-    """StandardUpdater.state_dict's container {"main_params", "main_optimizer", "epoch", "iteration"}: Adam moments per
-    parameter under Paddle's accumulator suffixes (FlatAdam.moments) plus the step count the bias correction needs."""
-    o = opt.moments()
-    o["step_count"] = opt.steps
-    o["LR_Scheduler"] = {"last_lr": lr}
-    return {"main_params": model.state_dict(), "main_optimizer": o, "epoch": int(epoch), "iteration": int(opt.steps)}
-
-
-def load_updater_state(model, opt, state):
-    model.set_state_dict(state["main_params"])                  # in place: the parameters stay views of the flat buffer
-    o = state.get("main_optimizer", {})
-    opt.load_moments(o)
-    opt.steps = int(o.get("step_count", state.get("iteration", opt.steps)))
 
 
 class FlatBuffers:
@@ -128,11 +140,8 @@ class FlatAdam:
 
 
 class PdCheckpoint:
-    """The old-style `step-N.pdparams` / `step-N.pdopt` pair of ExperimentBase (utils/checkpoint.py:61-138) for a training step
-    that holds its model as `self.m` and its optimiser as `self.opt` (a FlatAdam): the model's state dict, and the Adam state
-    under Paddle's accumulator suffixes (`<name>_moment1_0`, `<name>_moment2_0`, `<name>_beta1_pow_acc_0`, `<name>_beta2_pow_acc_0`)."""
-
-    step_count = property(lambda self: self.opt.steps)
+    """The old-style `step-N.pdparams` / `step-N.pdopt` pair of ExperimentBase (utils/checkpoint.py:61-138) for a TrainStep: the
+    model's state dict, and the Adam state under Paddle's accumulator suffixes (`<name>_moment1_0`, `<name>_moment2_0`, `<name>_beta1_pow_acc_0`, `<name>_beta2_pow_acc_0`)."""
 
     def state_dict(self):
         """(params, opt)."""
@@ -170,3 +179,99 @@ class PdCheckpoint:
         base = os.path.join(checkpoint_dir, f"step-{iteration}")
         self.set_state_dict(checkpoint.load(base + ".pdparams"), checkpoint.load(base + ".pdopt"))
         return int(iteration)
+
+
+class UpdaterSnapshot:
+    """StandardUpdater.state_dict's container {"main_params", "main_optimizer", "epoch", "iteration"} (training/updaters/
+    standard_updater.py; the Snapshot extension writes it with paddle.save as snapshot_iter_<n>.pdz) for a training step that
+    holds self.m, self.opt (a FlatAdam) and self.lr: the Adam moments per parameter under Paddle's accumulator suffixes
+    (FlatAdam.moments) plus the step count the bias correction needs.  train.py resumes by constructing the updater first and
+    loading afterwards, which is why Layer.set_state_dict copies IN PLACE into the flat buffer."""
+
+    def state_dict(self, epoch=0):
+        o = self.opt.moments()
+        o["step_count"] = self.opt.steps
+        o["LR_Scheduler"] = {"last_lr": self.lr}
+        return {"main_params": self.m.state_dict(), "main_optimizer": o, "epoch": int(epoch), "iteration": int(self.opt.steps)}
+
+    def set_state_dict(self, state):
+        self.m.set_state_dict(state["main_params"])
+        o = state.get("main_optimizer", {})
+        self.opt.load_moments(o)
+        self.opt.steps = int(o.get("step_count", state.get("iteration", self.opt.steps)))
+        if hasattr(self, "step_dev"):
+            self.step_dev.fill_(self.opt.steps)      # the dropout masks continue from the restored step
+
+    def save(self, path, epoch=0):
+        from .. import checkpoint
+        checkpoint.save(self.state_dict(epoch), path)
+
+    def load(self, path):
+        from .. import checkpoint
+        self.set_state_dict(checkpoint.load(path))
+
+
+class TrainStep:
+    """The base of a training step.  A subclass runs its own refusals, then this constructor, and provides
+    `_prepare(batch) -> (tensors, key)` (host-side checks and the device tensors of the batch; `key` names its shape) and
+    `_forward_backward(*tensors)` (losses on the device, every gradient in gflat; a step that runs ConvOps and accumulates into
+    gflat calls `_prologue()` first).
+
+    Construction refuses a non-CUDA model, turns the model's trainable tensors (every state-dict entry but the BatchNorm running
+    statistics) into views of FlatAdam's flat buffer and broadcasts rank 0's parameters under data parallelism.
+    `max_graphs`: the CUDA graphs kept (a graph pins every saved activation of its batch shape); `use_graphs`: None -> env
+    PK_TRAIN_GRAPH (default on).  A graph replays forward + backward as one launch per batch shape: eager the first time a shape
+    is seen, captured the second, replayed afterwards."""
+
+    def __init__(self, model, learning_rate, process_group, max_graphs, use_graphs=None, **adam):
+        need_cuda(model)
+        self.m, self.dev, self.lr, self.group = model, model.device, learning_rate, process_group
+        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
+        self.opt = FlatAdam(model._params, [k for k in model._params if not k.endswith(BUFFERS)], self.dev, **adam)
+        opt = self.opt
+        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
+        self._graphs = StepGraphs(max_graphs, use_graphs)
+        self._zp = self._graphs.planes
+        self.conv = ConvOps(self._zp)
+        model._packed = None
+        if self.world > 1:
+            broadcast_from_rank0(self.flat, model._params, process_group)
+
+    step_count = property(lambda self: self.opt.steps)
+
+    def _prologue(self):
+        """Every forward + backward packs the weights of its own step (inside a captured graph the pack kernels are part of the
+        graph) and accumulates into a zeroed gradient."""
+        self.conv.reset()
+        self.gflat.zero_()
+
+    def _named(self, out):
+        """The result of forward_backward and step, from the outputs of _forward_backward."""
+        return out
+
+    def _run(self, batch, graph):
+        tensors, key = self._prepare(batch)
+        return self._graphs.run(key, self._forward_backward, tensors, graph=graph)
+
+    def forward_backward(self, batch):
+        """Forward + backward, eager and without an update: the losses, and every gradient in self.grads."""
+        return self._named(self._run(batch, graph=False))
+
+    def forward_backward_graphed(self, batch):
+        """Forward + backward through the CUDA graph of the batch's shape, without an update: the outputs of _forward_backward,
+        the graph's own tensors (valid until its next replay)."""
+        return self._run(batch, graph=True)
+
+    def step(self, batch):
+        """One update: forward + backward through the graph of the batch's shape, the flat all-reduce when data-parallel, Adam.
+        Returns the losses as device tensors, the values before the update."""
+        out = self._run(batch, graph=True).clone()
+        self._update()
+        return self._named(out)
+
+    def _update(self):
+        """The update after a forward + backward: the one exchange step of the path, then Adam with the 1/world mean folded in."""
+        self.opt.update(self.lr, self.world, self.group)
+        if hasattr(self, "step_dev"):
+            self.step_dev += 1           # the next step's dropout masks
+        self.m._packed = None            # inference re-packs the updated weights and running statistics

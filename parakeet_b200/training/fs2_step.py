@@ -14,22 +14,18 @@ splitk_wgrad -, attention dQ/dK/dV/dP) reuse pk_conv_gemm on transposed split pl
 row-wise kernels of train.cu.
 torch is used for buffers, views, permutes / copies (layout plumbing) and torch.distributed.
 """
-import ctypes as C
-import os
-
 import torch
-import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.fastspeech2 import FastSpeech2, _i32
 from ..ops import Split, _ptr, _stream
-from . import wgrad
-from .conv import ConvOps
-from .flat import BUFFERS, FlatAdam, broadcast_from_rank0, load_updater_state, step_graphs, updater_state
+from .flat import UpdaterSnapshot, need_cuda
 from .transformer import TransformerTrainOps
 
+_KEYS = ("text", "text_lengths", "speech", "speech_lengths", "durations", "pitch", "energy")
 
-class FastSpeech2TrainStep(TransformerTrainOps):
+
+class FastSpeech2TrainStep(UpdaterSnapshot, TransformerTrainOps):
     """Dropout sites (TransformerTrainOps.site; oracle/fastspeech2.py: dropout_site restates this numbering): stack 0 encoder,
     1 decoder, 2 pitch, 3 energy, 4 duration predictor, 5 postnet; kind 0 positional encoding, 1 attention probabilities,
     2 attention sub-layer output, 3 feed-forward hidden, 4 feed-forward sub-layer output, 5 predictor layer, 6 postnet layer;
@@ -38,58 +34,38 @@ class FastSpeech2TrainStep(TransformerTrainOps):
     def __init__(self, model: FastSpeech2, learning_rate=1e-3, beta1=0.9, beta2=0.999, epsilon=1e-8,
                  stop_gradient_from_pitch_predictor=None, stop_gradient_from_energy_predictor=None, process_group=None,
                  dropout=True, seed=0, use_graphs=None):
-        """dropout: True -> the model's constructor rates (the reference trains in model.train() mode), a dict of the
-        reference's rate keywords to override them, or False / None -> every rate 0 (deterministic step, parity tests).
-        seed: base seed of the Philox masks; every rank should pass its own (paddle seeds each process's generator).
-        use_graphs: replay forward + backward as ONE CUDA graph per batch shape (eager the first time a shape is seen, captured
-        the second, replayed afterwards); None -> env PK_TRAIN_GRAPH (default on).  The step is host-bound otherwise (~700
-        launches of 10-40 us); bucketing samplers repeat shapes, so do synthetic benchmarks."""
-        if not model.device.type == "cuda":
-            raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
+        """dropout, seed: TransformerTrainOps.
+        use_graphs: replay forward + backward as ONE CUDA graph per batch shape (TrainStep); None -> env PK_TRAIN_GRAPH (default
+        on).  The step is host-bound otherwise (~700 launches of 10-40 us); bucketing samplers repeat shapes, so do synthetic
+        benchmarks."""
+        need_cuda(model)
         if model.tone_embed_dim is not None:
             raise NotImplementedError("the training step does not cover tone conditioning (tone_embed_dim): no recipe trains with tones")
         # multi-speaker recipes (aishell3, vctk): batch["spk_id"] -> spk_embedding_table -> F.normalize -> spk_projection
         self.spk = model.spk_embed_dim is not None
-        self._order = self._BATCH_ORDER + (("spk_id",) if self.spk else ())
-        self.m = model
-        self.lr = learning_rate
         self.sg_pitch = model.stop_gradient_from_pitch_predictor if stop_gradient_from_pitch_predictor is None else stop_gradient_from_pitch_predictor
         self.sg_energy = model.stop_gradient_from_energy_predictor if stop_gradient_from_energy_predictor is None else stop_gradient_from_energy_predictor
-        self.group = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
-        dev = model.device
-        self.dev = dev
-        self.overlap = os.environ.get("PK_TRAIN_OVERLAP", "1") != "0"      # parameter gradients on a side stream (on_side)
-        self._side, self._side_used, self._keep = None, False, []
-        names = [k for k in model._params if not k.endswith(BUFFERS)]
-        self.opt = opt = FlatAdam(model._params, names, dev, beta1, beta2, epsilon)   # the model's tensors become views of one flat buffer
-        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
-        model._packed = None
-        if dropout is True:
-            self.rates = dict(model.dropout_rates)
-        elif isinstance(dropout, dict):
-            self.rates = {**model.dropout_rates, **dropout}
-        else:
-            self.rates = {k: 0.0 for k in model.dropout_rates}
-        self.seed = int(seed)
-        # completed steps, on the device: the dropout kernels add it to their step argument, so a captured graph of forward +
-        # backward draws new masks on every replay
-        self.step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._fb_graphs = step_graphs(16, use_graphs)
-        self._zp = wgrad.ZeroPlanes(max_geoms=16, on_evict=self._fb_graphs.drop)     # planes and graph of a batch shape go together
-        self.conv = ConvOps(self._zp)
-        # workspace of the BatchNorm / LayerNorm reductions: 2 floats per channel (pk_batch_norm_train / _bwd)
-        widest = max([model.odim, model.adim] + [int(v.shape[0]) for k, v in model._params.items() if k.startswith("postnet.")])
-        self.sums = torch.zeros(max(4096, 2 * widest), dtype=torch.float32, device=dev)
-        if model.adim > 512:
-            raise NotImplementedError("pk_layer_norm_bwd supports rows of at most 512 channels (adim)")
-        if self.world > 1:
-            broadcast_from_rank0(self.flat, model._params, process_group)
+        super().__init__(model, dropout, seed, learning_rate=learning_rate, process_group=process_group, max_graphs=16,
+                         use_graphs=use_graphs, beta1=beta1, beta2=beta2, epsilon=epsilon)
 
-    # ------------------------------------------------------------------------------------------------------------
-    # GEMM-shaped forward / backward pieces
-    # ------------------------------------------------------------------------------------------------------------
-    step_count = property(lambda self: self.opt.steps)
+    _fb_graphs = property(lambda self: self._graphs)         # the name this step has always given its graphs
+
+    def _prepare(self, batch):
+        """The batch's tensors on the device in _forward_backward's order (+ spk_id for speaker models: a replay reads the ids of
+        the current batch), and their shapes as the graph key."""
+        if batch.get("spembs") is not None:
+            raise NotImplementedError("training with utterance-level speaker embeddings (spembs) is not supported: the recipes pass spk_id")
+        if self.spk and batch.get("spk_id") is None:
+            raise ValueError("this model has a speaker embedding table: the batch needs spk_id (int64, (B,))")
+        dev = self.dev
+        text = batch["text"].to(dev, torch.int64).contiguous()
+        B, T = text.shape
+        ts = [text, _i32(batch["text_lengths"].to(dev)), batch["speech"].to(dev, torch.float32).contiguous(), _i32(batch["speech_lengths"].to(dev)),
+              batch["durations"].to(dev, torch.int64).contiguous(), batch["pitch"].to(dev, torch.float32).reshape(B, T).contiguous(),
+              batch["energy"].to(dev, torch.float32).reshape(B, T).contiguous()]
+        if self.spk:
+            ts.append(batch["spk_id"].to(dev, torch.int64).reshape(B).contiguous())
+        return ts, tuple(tuple(t.shape) for t in ts)
 
     # ------------------------------------------------------------------------------------------------------------
     # predictors
@@ -161,29 +137,13 @@ class FastSpeech2TrainStep(TransformerTrainOps):
     # ------------------------------------------------------------------------------------------------------------
     # one training step
     # ------------------------------------------------------------------------------------------------------------
-    def forward_backward(self, batch):
+    def _forward_backward(self, text, ilens, ys, olens, ds, ps, es, spk_id=None):
         m = self.m
         L = _lib.lib()
         st = _stream()
-        dev = m.device
-        self.conv.reset()
-        self._zp.begin(self._batch_key(batch))
-        self.gflat.zero_()
-        text = batch["text"].to(dev, torch.int64).contiguous()
+        dev = self.dev
+        self._prologue()
         B, T = text.shape
-        ilens = _i32(batch["text_lengths"].to(dev))
-        olens = _i32(batch["speech_lengths"].to(dev))
-        ds = batch["durations"].to(dev, torch.int64).contiguous()
-        ps = batch["pitch"].to(dev, torch.float32).reshape(B, T).contiguous()
-        es = batch["energy"].to(dev, torch.float32).reshape(B, T).contiguous()
-        ys = batch["speech"].to(dev, torch.float32).contiguous()
-        if batch.get("spembs") is not None:
-            raise NotImplementedError("training with utterance-level speaker embeddings (spembs) is not supported: the recipes pass spk_id")
-        spk_id = None
-        if self.spk:
-            if batch.get("spk_id") is None:
-                raise ValueError("this model has a speaker embedding table: the batch needs spk_id (int64, (B,))")
-            spk_id = batch["spk_id"].to(dev, torch.int64).reshape(B).contiguous()
         A, odim = m.adim, m.odim
         # ---- forward (train mode) ----
         R = self.rates
@@ -228,29 +188,7 @@ class FastSpeech2TrainStep(TransformerTrainOps):
         zs, zs_split, S_dec = self.stack_fwd(xd, "decoder.", m.dlayers, olens, heads=m.aheads, ffn=ffn, sid=1,
                                              r_layer=R["transformer_dec_dropout_rate"], r_attn=R["transformer_dec_attn_dropout_rate"])
         before, before_split = self.layer_fwd(zs_split, "feat_out.weight", "feat_out.bias", "lin", out_split=True)
-        post, h = [], before_split
-        rows = B * t_dec
-        for i in range(m.postnet_layers):
-            last = i == m.postnet_layers - 1
-            cw = f"postnet.postnet.{i}.0.weight"
-            q = f"postnet.postnet.{i}.1."
-            conv_out, _ = self.layer_fwd(h, cw, None, "conv")
-            cdim = conv_out.shape[-1]
-            y = torch.empty_like(conv_out)
-            ysplit = Split.empty(tuple(conv_out.shape), dev) if not last else None
-            mean = torch.empty(cdim, device=dev)
-            rstd = torch.empty(cdim, device=dev)
-            _lib.check(L.pk_batch_norm_train(_ptr(conv_out), rows, cdim, _ptr(self.P(q + "weight")), _ptr(self.P(q + "bias")), 1e-5,
-                                             0 if last else 2, 0.9, _ptr(m._params[q + "_mean"]), _ptr(m._params[q + "_variance"]),
-                                             _ptr(self.sums), _ptr(y), _ptr(ysplit.hi) if ysplit else None,
-                                             _ptr(ysplit.lo) if ysplit else None, _ptr(mean), _ptr(rstd), st), "pk_batch_norm_train")
-            yd = y
-            if R["postnet_dropout_rate"] > 0:                # Dropout closes every postnet layer (tacotron2/decoder.py:144-180)
-                yd, ysplit = self.drop(y, R["postnet_dropout_rate"], self.site(5, i, 6), out_f32=True, out_split=not last)
-            post.append(dict(x=h, conv=conv_out, y=y, yd=yd, mean=mean, rstd=rstd))
-            h = ysplit
-        after = before.clone()
-        ops.axpy_(1.0, post[-1]["yd"], after)
+        after, post = self.postnet_fwd(before, before_split)
         # ---- loss and its gradient ----
         losses = torch.empty(4, dtype=torch.float32, device=dev)
         ws = torch.empty(12, dtype=torch.float32, device=dev)
@@ -262,22 +200,7 @@ class FastSpeech2TrainStep(TransformerTrainOps):
                                      _ptr(ps), _ptr(e_outs), _ptr(es), _ptr(ilens), T, B, _ptr(g_before), _ptr(g_after), _ptr(g_d), _ptr(g_p),
                                      _ptr(g_e), st), "pk_fs2_loss_bwd")
         # ---- backward ----
-        g = g_after                                            # after = before + postnet(before)
-        for i in reversed(range(m.postnet_layers)):
-            last = i == m.postnet_layers - 1
-            c = post[i]
-            q = f"postnet.postnet.{i}.1."
-            cdim = c["conv"].shape[-1]
-            dconv = torch.empty_like(c["conv"])
-            if R["postnet_dropout_rate"] > 0:
-                g = self.drop(g, R["postnet_dropout_rate"], self.site(5, i, 6))[0]
-            _lib.check(L.pk_batch_norm_bwd(_ptr(c["conv"]), _ptr(g), _ptr(c["y"]), _ptr(c["mean"]), _ptr(c["rstd"]), _ptr(self.P(q + "weight")),
-                                           0 if last else 2, rows, cdim, _ptr(self.sums), _ptr(dconv), st), "pk_batch_norm_bwd")
-            self.grads[q + "bias"].copy_(self.sums[:cdim])
-            self.grads[q + "weight"].copy_(self.sums[cdim:2 * cdim])
-            g = self.layer_bwd(dconv, c["x"], f"postnet.postnet.{i}.0.weight", None, "conv")
-        ops.axpy_(1.0, g_after, g)                             # residual path of `after`
-        ops.axpy_(1.0, g_before, g)                            # direct L1 on `before`
+        g = self.postnet_bwd(g_after, g_before, post)
         dzs = self.layer_bwd(g, zs_split, "feat_out.weight", "feat_out.bias", "lin")
         dxd = self.stack_bwd(dzs, S_dec)
         if R["transformer_dec_positional_dropout_rate"] > 0:
@@ -308,44 +231,4 @@ class FastSpeech2TrainStep(TransformerTrainOps):
         _lib.check(L.pk_embed_pe_bwd(_ptr(text), _ptr(dx), m.idim, m.padding_idx, B, T, A, _ptr(self.grads["encoder.embed.0.weight"]),
                                      _ptr(self.grads["encoder.embed.1.alpha"]), st), "pk_embed_pe_bwd")
         self.join_side()
-        return losses
-
-    _BATCH_ORDER = ("text", "text_lengths", "speech", "speech_lengths", "durations", "pitch", "energy")
-
-    def _batch_key(self, batch):
-        return tuple(tuple(batch[k].shape) for k in self._order)
-
-    def _forward_backward_graphed(self, batch):
-        dev = self.m.device
-        order = self._order            # + spk_id for speaker models: a replay reads the ids of the current batch
-        if self.spk and batch.get("spk_id") is None:
-            raise ValueError("this model has a speaker embedding table: the batch needs spk_id (int64, (B,))")
-        if batch.get("spembs") is not None:
-            raise NotImplementedError("training with utterance-level speaker embeddings (spembs) is not supported: the recipes pass spk_id")
-        dtypes = (torch.int64, torch.int64, torch.float32, torch.int64, torch.int64, torch.float32, torch.float32, torch.int64)
-        tensors = [batch[k].to(dev, dt).contiguous() for k, dt in zip(order, dtypes)]
-        key = tuple(tuple(t.shape) for t in tensors)
-        self._zp.touch(key)                      # a replay does not pass through forward_backward: keep the LRU order honest
-        fn = lambda *ts: self.forward_backward(dict(zip(order, ts)))
-        return self._fb_graphs.run(key, fn, tensors).clone()
-
-    # ------------------------------------------------------------------------------------------------------------
-    # snapshot / resume (reference: StandardUpdater.state_dict / set_state_dict, training/updaters/standard_updater.py;
-    # Snapshot extension writes it with paddle.save as snapshot_iter_<n>.pdz and train.py resumes by constructing the
-    # updater first and loading afterwards - which is why Layer.set_state_dict copies IN PLACE into the flat buffer)
-    # ------------------------------------------------------------------------------------------------------------
-    def state_dict(self, epoch=0):
-        return updater_state(self.m, self.opt, self.lr, epoch)
-
-    def set_state_dict(self, state):
-        load_updater_state(self.m, self.opt, state)
-        self.step_dev.fill_(self.step_count)
-        self.conv.reset()
-
-    def step(self, batch):
-        """One update: returns the four loss values (device tensor: l1, duration, pitch, energy)."""
-        losses = self._forward_backward_graphed(batch)
-        self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
-        self.step_dev += 1
-        self.m._packed = None
         return losses

@@ -13,55 +13,44 @@ flat buffers.
 """
 
 import torch
-import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.lstm_speaker_encoder import lstm_key, start_states
 from ..ops import Split
-from .conv import ConvOps
-from .flat import FlatAdam, PdCheckpoint, broadcast_from_rank0, step_graphs
-from .wgrad import ZeroPlanes
+from .flat import PdCheckpoint, TrainStep
 
 
-class GE2ETrainStep(PdCheckpoint):
+class GE2ETrainStep(PdCheckpoint, TrainStep):
     def __init__(self, model, learning_rate=1e-4, max_grad_norm=3.0, num_speakers=64, beta1=0.9, beta2=0.999, epsilon=1e-8,
                  process_group=None):
-        if model.device.type != "cuda":
-            raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
-        self.m, self.lr, self.num_speakers = model, learning_rate, num_speakers
-        self.group = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
-        self.opt = FlatAdam(model._params, list(model._params), model.device, beta1, beta2, epsilon, clip_norm=max_grad_norm)
-        self.flat, self.gflat, self.grads = self.opt.flat, self.opt.gflat, self.opt.grads
-        self._graphs = step_graphs(2)
-        self._zp = ZeroPlanes(max_geoms=2, on_evict=self._graphs.drop)
-        self.conv = ConvOps(self._zp)
+        super().__init__(model, learning_rate, process_group, max_graphs=2, beta1=beta1, beta2=beta2, epsilon=epsilon,
+                         clip_norm=max_grad_norm)
+        self.num_speakers = num_speakers
         self._perm = ops.lstm_gate_perm(model.hidden_size, model.device)
-        model._packed = None
-        if self.world > 1:
-            broadcast_from_rank0(self.flat, model._params, process_group)
 
-    def _n(self, specs):
+    def _groups(self, B):
+        """(N, M'): the speakers of the batch and the utterances per speaker."""
+        return self.num_speakers, self.m.grouping(B, self.m.output_size, self.num_speakers)
+
+    def _prepare(self, specs):
         m = self.m
         if not specs.is_cuda:
             raise _lib.PkError("GE2ETrainStep needs CUDA tensors (no CPU fallback)")
         if specs.dim() != 3 or specs.shape[2] != m.n_mels or specs.shape[1] < 1:
             raise ValueError(f"expected specs (B, T, {m.n_mels}), got {tuple(specs.shape)}")
-        n = self.num_speakers
-        if n is None:
+        if self.num_speakers is None:
             raise ValueError("num_speakers (the recipe's speakers_per_batch) is needed for the forward's reshape")
-        return n, m.grouping(specs.shape[0], m.output_size, n)
+        self._groups(specs.shape[0])                # raises for a batch the reference's reshape cannot group
+        return [specs.contiguous().float()], tuple(specs.shape)
 
-    def forward_backward(self, specs):
+    def _forward_backward(self, specs):
         """-> (loss (1,), similarity matrix (N*M', N)); the gradients (after do_gradient_ops) are left in self.grads."""
-        N, Mg = self._n(specs)
         m, P, G = self.m, self.m._params, self.grads
         B, T, _ = specs.shape
+        N, Mg = self._groups(B)
         H, dev = m.hidden_size, specs.device
-        self.conv.reset()
-        self._zp.begin((B, T))
-        self.gflat.zero_()
-        inp = specs.float().transpose(0, 1).contiguous().reshape(1, T * B, m.n_mels)          # time-major
+        self._prologue()
+        inp = specs.transpose(0, 1).contiguous().reshape(1, T * B, m.n_mels)          # time-major
         counters = ops.lstm_counters(B, T, dev)
         perm = self._perm
         saved = []
@@ -105,18 +94,13 @@ class GE2ETrainStep(PdCheckpoint):
                 dh_in = self.conv.dgrad(dgs, ("ih", l), w_ih).reshape(T, B, H)
         return loss, sim
 
-    def forward_backward_graphed(self, specs):
-        return self._graphs.run(tuple(specs.shape), lambda s: self.forward_backward(s), [specs])
-
     def step(self, specs, eer=False):
         """One train_batch: forward, GE2E loss, backward, do_gradient_ops, clipped Adam.  Returns the loss (device tensor (1,),
         the value before the update), and with eer=True also the batch's EER (one device -> host copy)."""
-        N, Mg = self._n(specs)
-        loss, sim = self.forward_backward_graphed(specs.contiguous().float())
+        loss, sim = self.forward_backward_graphed(specs)
         out_eer = None
         if eer:
             from ..models.lstm_speaker_encoder import equal_error_rate
-            out_eer = equal_error_rate(sim.cpu().numpy(), N, Mg)
-        self.opt.update(self.lr, self.world, self.group)
-        self.m._packed = None
+            out_eer = equal_error_rate(sim.cpu().numpy(), *self._groups(specs.shape[0]))
+        self._update()
         return (loss.clone(), out_eer) if eer else loss.clone()

@@ -17,19 +17,16 @@ block's residual gradient added in its epilogue) and the split-K weight gradient
 their gradients are pk_ss_loss; the embedding tables' dense gradients are pk_spk_table_grad over the B*T tokens.
 """
 import torch
-import torch.distributed as dist
 
 from .. import _lib, ops
 from ..models.speedyspeech import CHANNELS, SpeedySpeech, _i32, paddle_same_conv
 from ..ops import Split, _ptr, _stream
-from . import wgrad
-from .conv import ConvOps
-from .flat import BUFFERS, FlatAdam, broadcast_from_rank0, load_updater_state, step_graphs, updater_state
+from .flat import TrainStep, UpdaterSnapshot
 
 _KEYS = ("phones", "tones", "num_phones", "num_frames", "feats", "durations")
 
 
-class SpeedySpeechTrainStep:
+class SpeedySpeechTrainStep(UpdaterSnapshot, TrainStep):
     def __init__(self, model: SpeedySpeech, learning_rate=2e-3, max_grad_norm=1.0, beta1=0.9, beta2=0.999, epsilon=1e-8,
                  process_group=None, check_durations=True):
         """check_durations: compare the longest row sum of batch["durations"] with feats.shape[1] on every call and raise PkError
@@ -37,23 +34,11 @@ class SpeedySpeechTrainStep:
         is then cut at feats.shape[1] frames and a shorter one leaves zero rows, as pk_length_regulate defines)."""
         if not isinstance(model, SpeedySpeech):
             raise _lib.PkError("SpeedySpeechTrainStep needs a parakeet_b200.models.SpeedySpeech")
-        if model.device.type != "cuda":
-            raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
-        self.m, self.dev, self.group = model, model.device, process_group
-        self.lr = learning_rate
         self.check_durations = check_durations
-        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
-        names = [k for k in model._params if not k.endswith(BUFFERS)]
-        # the model's tensors become views of one flat buffer; a falsy max_grad_norm never clips
-        self.opt = opt = FlatAdam(model._params, names, self.dev, beta1, beta2, epsilon, clip_norm=max_grad_norm or 0.0)
-        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
+        # a falsy max_grad_norm never clips; a graph pins every saved activation of its batch shape
+        super().__init__(model, learning_rate, process_group, max_graphs=4, beta1=beta1, beta2=beta2, epsilon=epsilon,
+                         clip_norm=max_grad_norm or 0.0)
         self.one = torch.ones(1, device=self.dev)
-        model._packed = None
-        self._graphs = step_graphs(4)          # a graph pins every saved activation of its batch shape
-        self._zp = wgrad.ZeroPlanes(max_geoms=4, on_evict=self._graphs.drop)
-        self.conv = ConvOps(self._zp)
-        if self.world > 1:
-            broadcast_from_rank0(self.flat, model._params, process_group)
 
     # ------------------------------------------------------------------------------------------------------------
     # batch checks (host side; nothing here can fault on the device)
@@ -95,8 +80,6 @@ class SpeedySpeechTrainStep:
     # ------------------------------------------------------------------------------------------------------------
     # GEMM-shaped pieces
     # ------------------------------------------------------------------------------------------------------------
-    step_count = property(lambda self: self.opt.steps)
-
     def P(self, name):
         return self.m._params[name]
 
@@ -161,10 +144,8 @@ class SpeedySpeechTrainStep:
         B, T = phones.shape
         L = feats.shape[1]
         C = CHANNELS
-        self.conv.reset()
+        self._prologue()
         self._ws = sc = self.workspace(max(B * T, B * L), B, L)
-        self._zp.begin((B, T, L, tones is not None))
-        self.gflat.zero_()
         ek, dk = m.encoder_kernel_size, m.decoder_kernel_size
         # ---- encoder (:100-106) ----
         text_w = self.P("encoder.embedding.text_embedding.weight")
@@ -238,11 +219,6 @@ class SpeedySpeechTrainStep:
     def _named(losses):
         return dict(loss=losses[0], l1_loss=losses[1], duration_loss=losses[2], ssim_loss=losses[3])
 
-    def forward_backward(self, batch):
-        """Losses and the flat gradient (self.grads: name -> view), no update and no graph; the running statistics move."""
-        tensors, _ = self._prepare(batch)
-        return self._named(self._forward_backward(*tensors))
-
     def evaluate(self, batch):
         """SpeedySpeechEvaluator.evaluate_core (:110-157): the eval-mode forward (running statistics) and the same four numbers.
         Reads the current parameters; changes nothing, the model's `training` flag included."""
@@ -252,31 +228,3 @@ class SpeedySpeechTrainStep:
         sc = self.workspace(0, B, L)
         losses, _, _ = ops.ss_loss(decoded.contiguous(), feats, num_frames, pred.contiguous(), dur, num_phones, sc, want_grads=False)
         return self._named(losses)
-
-    def step(self, batch):
-        """One update.  Forward + backward replay as one CUDA graph per (B, T, L, tones?) (eager the first time a shape is seen,
-        captured the second); the gradient norm and the clipped Adam update follow as two launches, because Adam's bias
-        correction takes the step number from the host.  Returns the four losses as device scalars."""
-        tensors, key = self._prepare(batch)
-        self._zp.touch(key)
-        losses = self._graphs.run(key, self._forward_backward, tensors).clone()
-        self.opt.update(self.lr, self.world, self.group)
-        self.m._packed = None            # inference re-packs the updated weights and running statistics, and drops its graphs
-        return self._named(losses)
-
-    # ------------------------------------------------------------------------------------------------------------
-    # snapshot / resume: the container of StandardUpdater.state_dict, as FastSpeech2TrainStep writes it
-    # ------------------------------------------------------------------------------------------------------------
-    def state_dict(self, epoch=0):
-        return updater_state(self.m, self.opt, self.lr, epoch)
-
-    def set_state_dict(self, state):
-        load_updater_state(self.m, self.opt, state)
-
-    def save(self, path, epoch=0):
-        from .. import checkpoint
-        checkpoint.save(self.state_dict(epoch), path)
-
-    def load(self, path):
-        from .. import checkpoint
-        self.set_state_dict(checkpoint.load(path))

@@ -1,7 +1,8 @@
-"""The transformer pieces of the training steps: materialised multi-head attention forward / backward and the FFT-block stack
-(pre-LN self-attention + position-wise feed-forward, Encoder.forward after the embedding) with its saved context.  The FastSpeech2
-step runs its encoder and decoder through `stack_fwd` / `stack_bwd`; the TransformerTTS step its encoder, and its decoder layers
-call `mha_fwd` / `mha_bwd` for the causal self-attention and the source attention.
+"""What the FastSpeech2 and TransformerTTS training steps share: their set-up (dropout rates, Philox seed, device step counter,
+side stream, BatchNorm workspace), materialised multi-head attention forward / backward, the residual sub-layer, the pre-LN
+self-attention and feed-forward blocks, the FFT-block stack (Encoder.forward after the embedding) and the Tacotron2 postnet, each
+with its saved context.  The FastSpeech2 step runs its encoder and decoder through `stack_fwd` / `stack_bwd`; the TransformerTTS
+step its encoder, and its decoder layers are the stack's two blocks around a source attention.
 
 Attention is materialised: S = Q K^T / sqrt(dk) into a (B*H, Tq, ceil64(Tk)) fp32 buffer, the masked softmax, dropout on the
 probabilities (pk_dropout, regenerated in the backward), ctx = P V; the backward forms dP = dO V^T, the softmax backward (with the
@@ -9,18 +10,43 @@ guided attention loss folded in where requested: pk_softmax_bwd), and dQ = dS K,
 matmuls on transposed split planes (pk_transpose_planes).  Q comes from one tensor, K and V from another (column offsets and
 leading dimensions free), so the source attention reads the fused K | V memory of every decoder layer in place.
 
-A step class mixes TransformerTrainOps in and provides m (the model), grads (name -> gradient view), conv (ConvOps), seed,
-step_dev (device step counter), _zp (ZeroPlanes) and the side-stream state of on_side (_side, _side_used, _keep, overlap).
+The step classes derive from TransformerTrainOps, a TrainStep (training/flat.py).
 """
 import math
+import os
 
 import torch
 
-from .. import ops
-from ..ops import Split, ceil_to
+from .. import _lib, ops
+from ..ops import Split, _ptr, _stream, ceil_to
+from .flat import TrainStep
 
 
-class TransformerTrainOps:
+class TransformerTrainOps(TrainStep):
+    def __init__(self, model, dropout, seed, **base):
+        """dropout: True -> the model's constructor rates (the reference trains in model.train() mode), a dict of the reference's
+        rate keywords to override some, or False / None -> every rate 0 (deterministic step, parity tests).
+        seed: base seed of the Philox masks; every rank should pass its own (paddle seeds each process's generator).
+        base: TrainStep's arguments."""
+        if model.adim > 512:
+            raise NotImplementedError("pk_layer_norm_bwd supports rows of at most 512 channels (adim)")
+        super().__init__(model, **base)
+        self.overlap = os.environ.get("PK_TRAIN_OVERLAP", "1") != "0"      # parameter gradients on a side stream (on_side)
+        self._side, self._side_used, self._keep = None, False, []
+        if dropout is True:
+            self.rates = dict(model.dropout_rates)
+        elif isinstance(dropout, dict):
+            self.rates = {**model.dropout_rates, **dropout}
+        else:
+            self.rates = {k: 0.0 for k in model.dropout_rates}
+        self.seed = int(seed)
+        # completed steps, on the device: the dropout kernels add it to their step argument, so a captured graph of forward +
+        # backward draws new masks on every replay
+        self.step_dev = torch.zeros(1, dtype=torch.int32, device=self.dev)
+        # workspace of the BatchNorm / LayerNorm reductions: 2 floats per channel (pk_batch_norm_train / _bwd)
+        widest = max([model.odim, model.adim] + [int(v.shape[0]) for k, v in model._params.items() if k.startswith("postnet.")])
+        self.sums = torch.zeros(max(4096, 2 * widest), dtype=torch.float32, device=self.dev)
+
     def P(self, name):
         return self.m._params[name]
 
@@ -180,71 +206,142 @@ class TransformerTrainOps:
         return self.conv.dgrad(dqs, q + "qkv", wqkv, linear=True)
 
     # ------------------------------------------------------------------------------------------------------------
+    # pre-LN blocks (EncoderLayer / DecoderLayer.forward, concat_after=False) with saved context in `c`
+    # ------------------------------------------------------------------------------------------------------------
+    def sub_fwd(self, ctx, name, x, rate, site, kind="lin"):
+        """x + dropout(layer `name`(ctx)): the residual add rides in the GEMM epilogue when there is no dropout."""
+        if rate > 0:
+            y, _ = self.layer_fwd(ctx, name + ".weight", name + ".bias", kind)
+            self.drop(y, rate, site, inplace=True)
+            ops.axpy_(1.0, x, y)
+            return y
+        return self.layer_fwd(ctx, name + ".weight", name + ".bias", kind, residual=x)[0]
+
+    def sub_bwd(self, dx, ctx, name, rate, site, kind="lin"):
+        """The gradient at the ctx input of sub_fwd (its weight / bias gradients written)."""
+        dsub = self.drop(dx, rate, site)[0] if rate > 0 else dx
+        return self.layer_bwd(dsub, ctx, name + ".weight", name + ".bias", kind)
+
+    def attn_fwd(self, x, q, key_lens, c, *, heads, causal, r_attn, r_layer, sid, l):
+        """x + dropout(out_proj(self-attention(norm1(x)))) of layer prefix q; dropout sites (sid, l, 1) and (sid, l, 2)."""
+        A = x.shape[2]
+        c["x0"] = x
+        _, c["h1"] = ops.layer_norm(x, self.P(q + "norm1.weight"), self.P(q + "norm1.bias"))
+        bqkv = torch.cat([self.P(q + "self_attn.linear_q.bias"), self.P(q + "self_attn.linear_k.bias"), self.P(q + "self_attn.linear_v.bias")])
+        _, qkv = self.conv.fwd(c["h1"], q + "qkv", self.wqkv(q), linear=True, bias=bqkv, out_f32=False, out_split=True)
+        c["ctx1"], c["a1"] = self.mha_fwd(qkv, qkv, heads=heads, dk=A // heads, q_col0=0, k_col0=A, v_col0=2 * A, key_lens=key_lens,
+                                          causal=causal, rate=r_attn, site=self.site(sid, l, 1))
+        return self.sub_fwd(c["ctx1"], q + "self_attn.linear_out", x, r_layer, self.site(sid, l, 2))
+
+    def attn_bwd(self, dx, c, q, *, r_layer, sid, l):
+        """dx: gradient at attn_fwd's output, updated in place to the gradient at its input."""
+        B, T, A = dx.shape
+        dctx_s = Split.from_f32(self.sub_bwd(dx, c["ctx1"], q + "self_attn.linear_out", r_layer, self.site(sid, l, 2)))
+        dqkv = torch.zeros(B, T, 3 * A, dtype=torch.float32, device=dx.device)
+        self.mha_bwd(dctx_s, c["a1"], dqkv, dqkv)
+        dh1 = self.qkv_bwd(q, dqkv, c["h1"], dx.device)
+        ops.layer_norm_bwd(c["x0"], self.P(q + "norm1.weight"), dh1, dx, True, self.grads[q + "norm1.weight"], self.grads[q + "norm1.bias"])
+
+    def ffn_fwd(self, x, q, norm, c, *, kind, r_layer, sid, l):
+        """x + dropout(w_2(dropout(relu(w_1(norm(x)))))) of layer prefix q; kind: "lin" or "conv" (the position-wise layers);
+        dropout sites (sid, l, 3) and (sid, l, 4)."""
+        c["xf"] = x
+        _, c["hf"] = ops.layer_norm(x, self.P(q + norm + ".weight"), self.P(q + norm + ".bias"))
+        _, c["u"] = self.layer_fwd(c["hf"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind, act="relu", out_f32=False,
+                                   out_split=True)
+        c["ud"] = self.drop(c["u"], r_layer, self.site(sid, l, 3), out_f32=False, out_split=True)[1] if r_layer > 0 else c["u"]
+        return self.sub_fwd(c["ud"], q + "feed_forward.w_2", x, r_layer, self.site(sid, l, 4), kind)
+
+    def ffn_bwd(self, dx, c, q, norm, *, kind, r_layer, sid, l):
+        """dx: gradient at ffn_fwd's output, updated in place to the gradient at its input."""
+        du = self.sub_bwd(dx, c["ud"], q + "feed_forward.w_2", r_layer, self.site(sid, l, 4), kind)
+        if r_layer > 0:
+            self.drop(du, r_layer, self.site(sid, l, 3), inplace=True)
+        du_f, _ = ops.relu_bwd(du, c["u"], want_f32=True)
+        dh = self.layer_bwd(du_f, c["hf"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind)
+        ops.layer_norm_bwd(c["xf"], self.P(q + norm + ".weight"), dh, dx, True, self.grads[q + norm + ".weight"], self.grads[q + norm + ".bias"])
+
+    # ------------------------------------------------------------------------------------------------------------
     # FFT-block stack (Encoder.forward after the embedding) with saved context
     # ------------------------------------------------------------------------------------------------------------
     def stack_fwd(self, x, pre, n_layers, key_lens, *, heads, ffn, sid, r_layer, r_attn):
         """x fp32 (B, T, A) -> (after_norm output fp32, its split planes, saved context).  ffn: "lin" or "conv" (the position-wise
         layers' kind); sid: the stack's dropout-site number; r_layer / r_attn: the sub-layer and attention-probability rates."""
-        A = x.shape[2]
         ctxs = []
         for i in range(n_layers):
-            q = f"{pre}encoders.{i}."
-            c = dict(x0=x)
-            _, c["h1"] = ops.layer_norm(x, self.P(q + "norm1.weight"), self.P(q + "norm1.bias"))
-            bqkv = torch.cat([self.P(q + "self_attn.linear_q.bias"), self.P(q + "self_attn.linear_k.bias"), self.P(q + "self_attn.linear_v.bias")])
-            _, qkv = self.conv.fwd(c["h1"], q + "qkv", self.wqkv(q), linear=True, bias=bqkv, out_f32=False, out_split=True)
-            ctx, c["attn"] = self.mha_fwd(qkv, qkv, heads=heads, dk=A // heads, q_col0=0, k_col0=A, v_col0=2 * A, key_lens=key_lens,
-                                          rate=r_attn, site=self.site(sid, i, 1))
-            c["ctx"] = ctx
-            if r_layer > 0:      # x1 = x + dropout(attention): the residual add cannot ride in the GEMM epilogue any more
-                a_out, _ = self.layer_fwd(ctx, q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin")
-                self.drop(a_out, r_layer, self.site(sid, i, 2), inplace=True)
-                ops.axpy_(1.0, x, a_out)
-                x1 = a_out
-            else:
-                x1, _ = self.layer_fwd(ctx, q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin", residual=x)
-            c["x1"] = x1
-            _, c["h2"] = ops.layer_norm(x1, self.P(q + "norm2.weight"), self.P(q + "norm2.bias"))
-            _, c["u"] = self.layer_fwd(c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", ffn, act="relu", out_f32=False, out_split=True)
-            c["ud"] = self.drop(c["u"], r_layer, self.site(sid, i, 3), out_f32=False, out_split=True)[1] if r_layer > 0 else c["u"]
-            if r_layer > 0:
-                f_out, _ = self.layer_fwd(c["ud"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", ffn)
-                self.drop(f_out, r_layer, self.site(sid, i, 4), inplace=True)
-                ops.axpy_(1.0, x1, f_out)
-                x = f_out
-            else:
-                x, _ = self.layer_fwd(c["u"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", ffn, residual=x1)
+            q, c = f"{pre}encoders.{i}.", {}
+            x1 = self.attn_fwd(x, q, key_lens, c, heads=heads, causal=False, r_attn=r_attn, r_layer=r_layer, sid=sid, l=i)
+            x = self.ffn_fwd(x1, q, "norm2", c, kind=ffn, r_layer=r_layer, sid=sid, l=i)
             ctxs.append(c)
         y, ys = ops.layer_norm(x, self.P(pre + "after_norm.weight"), self.P(pre + "after_norm.bias"), want_f32=True, want_split=True)
         return y, ys, dict(layers=ctxs, x_last=x, pre=pre, n=n_layers, sid=sid, r_layer=r_layer, ffn=ffn)
 
     def stack_bwd(self, dy, S):
         """dy: gradient w.r.t. the after_norm output (fp32).  Returns the gradient w.r.t. the stack input."""
-        pre = S["pre"]
-        B, T, A = dy.shape
-        dev = dy.device
-        kind = S["ffn"]
+        pre, sid, r_layer = S["pre"], S["sid"], S["r_layer"]
         dx = torch.empty_like(dy)
         ops.layer_norm_bwd(S["x_last"], self.P(pre + "after_norm.weight"), dy, dx, False, self.grads[pre + "after_norm.weight"],
                            self.grads[pre + "after_norm.bias"])
-        sid, r_layer = S["sid"], S["r_layer"]
         for i in reversed(range(S["n"])):
-            q = f"{pre}encoders.{i}."
-            c = S["layers"][i]
-            # x2 = x1 + drop(conv2(drop(relu(conv1(LN2(x1))))))
-            dsub = self.drop(dx, r_layer, self.site(sid, i, 4))[0] if r_layer > 0 else dx
-            du = self.layer_bwd(dsub, c["ud"], q + "feed_forward.w_2.weight", q + "feed_forward.w_2.bias", kind)
-            if r_layer > 0:
-                self.drop(du, r_layer, self.site(sid, i, 3), inplace=True)
-            du_f, _ = ops.relu_bwd(du, c["u"], want_f32=True)
-            dh2 = self.layer_bwd(du_f, c["h2"], q + "feed_forward.w_1.weight", q + "feed_forward.w_1.bias", kind)
-            ops.layer_norm_bwd(c["x1"], self.P(q + "norm2.weight"), dh2, dx, True, self.grads[q + "norm2.weight"], self.grads[q + "norm2.bias"])
-            # x1 = x0 + drop(out_proj(attention(LN1(x0))))
-            dsub = self.drop(dx, r_layer, self.site(sid, i, 2))[0] if r_layer > 0 else dx
-            dctx = self.layer_bwd(dsub, c["ctx"], q + "self_attn.linear_out.weight", q + "self_attn.linear_out.bias", "lin")
-            dctx_s = Split.from_f32(dctx)
-            dqkv = torch.zeros(B, T, 3 * A, dtype=torch.float32, device=dev)
-            self.mha_bwd(dctx_s, c["attn"], dqkv, dqkv)
-            dh1 = self.qkv_bwd(q, dqkv, c["h1"], dev)
-            ops.layer_norm_bwd(c["x0"], self.P(q + "norm1.weight"), dh1, dx, True, self.grads[q + "norm1.weight"], self.grads[q + "norm1.bias"])
+            q, c = f"{pre}encoders.{i}.", S["layers"][i]
+            self.ffn_bwd(dx, c, q, "norm2", kind=S["ffn"], r_layer=r_layer, sid=sid, l=i)
+            self.attn_bwd(dx, c, q, r_layer=r_layer, sid=sid, l=i)
         return dx
+
+    # ------------------------------------------------------------------------------------------------------------
+    # Tacotron2 postnet (tacotron2/decoder.py:144-180): Conv1D -> train-mode BatchNorm1D over all B x T rows (-> tanh but on
+    # the last layer) -> Dropout at site (5, i, 6); after = before + postnet(before)
+    # ------------------------------------------------------------------------------------------------------------
+    def postnet_fwd(self, before, before_split):
+        """before fp32 / before_split Split (B, T, odim) -> (after fp32, saved context)."""
+        m, L, st, dev = self.m, _lib.lib(), _stream(), self.dev
+        rate = self.rates["postnet_dropout_rate"]
+        post, h, rows = [], before_split, before.shape[0] * before.shape[1]
+        for i in range(m.postnet_layers):
+            last = i == m.postnet_layers - 1
+            q = f"postnet.postnet.{i}.1."
+            conv_out, _ = self.layer_fwd(h, f"postnet.postnet.{i}.0.weight", None, "conv")
+            cdim = conv_out.shape[-1]
+            y = torch.empty_like(conv_out)
+            ysplit = Split.empty(tuple(conv_out.shape), dev) if not last else None
+            mean, rstd = torch.empty(cdim, device=dev), torch.empty(cdim, device=dev)
+            _lib.check(L.pk_batch_norm_train(_ptr(conv_out), rows, cdim, _ptr(self.P(q + "weight")), _ptr(self.P(q + "bias")), 1e-5,
+                                             0 if last else 2, 0.9, _ptr(m._params[q + "_mean"]), _ptr(m._params[q + "_variance"]),
+                                             _ptr(self.sums), _ptr(y), _ptr(ysplit.hi) if ysplit else None,
+                                             _ptr(ysplit.lo) if ysplit else None, _ptr(mean), _ptr(rstd), st), "pk_batch_norm_train")
+            yd = y
+            if rate > 0:
+                yd, ysplit = self.drop(y, rate, self.site(5, i, 6), out_f32=True, out_split=not last)
+            post.append(dict(x=h, conv=conv_out, y=y, yd=yd, mean=mean, rstd=rstd))
+            h = ysplit
+        after = before.clone()
+        if post:
+            ops.axpy_(1.0, post[-1]["yd"], after)
+        return after, post
+
+    def postnet_bwd(self, g_after, g_before, post):
+        """The gradients at `after` and `before` -> the gradient at postnet_fwd's `before` (the postnet's parameter gradients
+        written)."""
+        L, st = _lib.lib(), _stream()
+        rate = self.rates["postnet_dropout_rate"]
+        g = g_after
+        for i in reversed(range(len(post))):
+            last = i == len(post) - 1
+            c = post[i]
+            q = f"postnet.postnet.{i}.1."
+            rows, cdim = c["conv"].shape[0] * c["conv"].shape[1], c["conv"].shape[-1]
+            dconv = torch.empty_like(c["conv"])
+            if rate > 0:
+                g = self.drop(g, rate, self.site(5, i, 6))[0]
+            _lib.check(L.pk_batch_norm_bwd(_ptr(c["conv"]), _ptr(g), _ptr(c["y"]), _ptr(c["mean"]), _ptr(c["rstd"]), _ptr(self.P(q + "weight")),
+                                           0 if last else 2, rows, cdim, _ptr(self.sums), _ptr(dconv), st), "pk_batch_norm_bwd")
+            self.grads[q + "bias"].copy_(self.sums[:cdim])
+            self.grads[q + "weight"].copy_(self.sums[cdim:2 * cdim])
+            g = self.layer_bwd(dconv, c["x"], f"postnet.postnet.{i}.0.weight", None, "conv")
+        if post:
+            ops.axpy_(1.0, g_after, g)                         # the residual path of `after`
+            ops.axpy_(1.0, g_before, g)                        # the loss on `before` itself
+        else:
+            g = g_before.clone()
+            ops.axpy_(1.0, g_after, g)
+        return g

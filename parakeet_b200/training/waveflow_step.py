@@ -15,34 +15,28 @@ import ctypes as C_
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 from .. import _lib, ops
 from ..ops import Split, _ptr, _stream, ceil_to
 from . import wgrad
-from .flat import FlatAdam, PdCheckpoint, broadcast_from_rank0, step_graphs
+from .flat import PdCheckpoint, TrainStep, need_cuda
 
 SLOPE = 0.4            # UpsampleNet's leaky_relu (waveflow.py:130)
 _SCRATCH = 1024 * 256  # fp32 partials of pk_waveflow_train_outer_sum / pk_waveflow_upsample_bwd
 
 
-class WaveFlowTrainStep(PdCheckpoint):
+class WaveFlowTrainStep(PdCheckpoint, TrainStep):
     def __init__(self, model, learning_rate=2e-4, sigma=1.0, beta1=0.9, beta2=0.999, epsilon=1e-8, process_group=None):
         if not model._eligible():
             raise NotImplementedError("the WaveFlow training step needs 64 or 128 channels, 64 < n_mels <= 128 (a multiple of 8) "
                                       "and 2 to 8 layers per flow")
-        if model.device.type != "cuda":
-            raise _lib.PkError("training needs a CUDA device (no CPU fallback)")
+        need_cuda(model)
         if not sigma > 0:
             raise ValueError("sigma must be positive")
-        self.m = model
-        self.lr, self.sigma = learning_rate, float(sigma)
-        self.group = process_group
-        self.world = dist.get_world_size(process_group) if dist.is_initialized() else 1
-        dev = self.dev = model.device
-        names = list(model._params)
-        self.opt = opt = FlatAdam(model._params, names, dev, beta1, beta2, epsilon)      # the model's tensors become views of one flat buffer
-        self.buffers, self.flat, self.gflat, self.grads, self.adam_m, self.adam_v = opt.buffers, opt.flat, opt.gflat, opt.grads, opt.m, opt.v
+        self.sigma = float(sigma)
+        # a captured graph pins its own memory pool: ~20 GB at the recipe's batch and 128 channels, so only a few shapes are kept
+        super().__init__(model, learning_rate, process_group, max_graphs=2, beta1=beta1, beta2=beta2, epsilon=epsilon)
+        dev, names = self.dev, self.buffers.names
         self.off = dict(zip(names, self.buffers.offsets))
         self.weff = torch.zeros_like(self.flat)     # weights as the forward uses them: weight norm folded into the weight_v slots
         self.dweff = torch.zeros_like(self.flat)    # gradients with respect to weff
@@ -60,12 +54,7 @@ class WaveFlowTrainStep(PdCheckpoint):
         self.cmaps = [i32(c) for c in cmaps]                                   # condition height of each height, per flow
         self.inv_perms = [i32(np.argsort(pm).tolist()) for pm in self.perms]
         self._build_packs()
-        # a captured graph pins its own memory pool: ~20 GB at the recipe's batch and 128 channels, so only a few shapes are kept
-        self._graphs = step_graphs(2)
         self._lens = {}
-        model._packed = None
-        if self.world > 1:
-            broadcast_from_rank0(self.flat, model._params, process_group)
 
     # ------------------------------------------------------------------------------------------------------------
     # weights: offsets into the flat buffers and the packed GEMM operands
@@ -130,11 +119,12 @@ class WaveFlowTrainStep(PdCheckpoint):
     # ------------------------------------------------------------------------------------------------------------
     # forward + backward
     # ------------------------------------------------------------------------------------------------------------
-    def forward_backward(self, audio, mel, lens):
-        """audio (B, T) fp32, mel (B, n_mels, T') fp32, lens the int32 net-row mask (see _net_lens): loss (1,) on the device; the
-        gradient of every parameter in self.gflat."""
+    def _forward_backward(self, audio, mel):
+        """audio (B, T) fp32, mel (B, n_mels, T') fp32: loss (1,) on the device; the gradient of every parameter in self.gflat
+        (written whole, so there is no prologue)."""
         m, L, st, dev = self.m, _lib.lib(), _stream(), self.dev
         G, C, NL, NF, M = m.n_group, m.channels, m.n_layers, m.n_flows, m.n_mels
+        lens = self._net_lens(audio.shape[0], audio.shape[-1] // G)
         chk, p = _lib.check, self._p
         weff, dweff = self.weff, self.dweff
         # weights of this step: weight norm folded (weff), packed operands gathered from it
@@ -319,11 +309,13 @@ class WaveFlowTrainStep(PdCheckpoint):
         return self._lens[key]
 
     def forward_backward_graphed(self, audio, mel):
-        lens = self._net_lens(audio.shape[0], audio.shape[-1] // self.m.n_group)
-        key = (audio.shape[0], audio.shape[-1], mel.shape[-1])
-        return self._graphs.run(key, lambda a_, m_: self.forward_backward(a_, m_, lens), [audio, mel])
+        """Forward + backward of audio (B, T) and mel (B, n_mels, T') through the CUDA graph of their shape, without an update:
+        the loss, the graph's own tensor (valid until its next replay)."""
+        return self._run((mel, audio), graph=True)
 
-    def _check(self, audio, mel):
+    def _prepare(self, batch):
+        """batch = (mel, wav) as the reference's collate yields it."""
+        mel, audio = batch
         if not (audio.is_cuda and mel.is_cuda):
             raise _lib.PkError("WaveFlowTrainStep needs CUDA tensors (no CPU fallback)")
         m = self.m
@@ -335,14 +327,4 @@ class WaveFlowTrainStep(PdCheckpoint):
         m._check_forward(audio.shape[-1], t_cond)
         if audio.shape[-1] < m.n_group:
             raise ValueError(f"audio shorter than n_group ({m.n_group}) samples")
-
-    def step(self, batch):
-        """batch = (mel, wav) as the reference's collate yields it: one update; returns the loss (device tensor (1,), the
-        value before the update)."""
-        mel, wav = batch
-        self._check(wav, mel)
-        wav, mel = wav.contiguous().float(), mel.contiguous().float()
-        loss = self.forward_backward_graphed(wav, mel)
-        self.opt.update(self.lr, self.world, self.group)        # the one exchange step of the path, then Adam with the 1/world mean folded in
-        self.m._packed = None                                                        # inference weights are re-packed on demand
-        return loss.clone()
+        return [audio.contiguous().float(), mel.contiguous().float()], (audio.shape[0], audio.shape[-1], mel.shape[-1])

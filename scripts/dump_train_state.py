@@ -1,4 +1,4 @@
-"""Fingerprint the four training steps, to compare two builds of this repository bit for bit.
+"""Fingerprint the training steps, to compare two builds of this repository bit for bit.
 
 For each step class the small seeded model and batch of its GPU test run three `step` calls with CUDA graphs (eager, capture,
 replay) and three without (PK_TRAIN_GRAPH=0, PK_CUDA_GRAPHS=0).  Per class and mode the JSON holds the SHA-256 of the flat
@@ -27,9 +27,8 @@ def sha(t):
 
 
 def state(opt):
-    """opt: anything with flat / gflat and the moments as adam_m / adam_v (the steps) or m / v (FlatAdam)."""
-    m, v = (opt.adam_m, opt.adam_v) if hasattr(opt, "adam_m") else (opt.m, opt.v)
-    return dict(flat=sha(opt.flat), gflat=sha(opt.gflat), adam_m=sha(m), adam_v=sha(v))
+    """opt: a FlatAdam (its flat / gflat buffers and moments m / v)."""
+    return dict(flat=sha(opt.flat), gflat=sha(opt.gflat), adam_m=sha(opt.m), adam_v=sha(opt.v))
 
 
 def run(make, dev):
@@ -54,7 +53,7 @@ def fastspeech2(dev):
     m.set_state_dict(ofs.synth_params(1))
     batch = ofs.synth_train_batch(5, [9, 14, 11], dur_range=(1, 4))
     ts = FastSpeech2TrainStep(m, learning_rate=1e-3, dropout=True, seed=3)
-    return (lambda: [float(v) for v in ts.step(batch)]), (lambda: {"net": state(ts)})
+    return (lambda: [float(v) for v in ts.step(batch)]), (lambda: {"net": state(ts.opt)})
 
 
 def waveflow(dev):
@@ -67,7 +66,7 @@ def waveflow(dev):
     mel = (torch.randn(3, 80, 12, generator=g) * 0.5 - 3).to(dev)
     audio = ((torch.rand(3, 12 * 256 - 7, generator=g) * 2 - 1) * 0.5).to(dev)
     ts = WaveFlowTrainStep(m, learning_rate=2e-4)
-    return (lambda: [float(ts.step((mel, audio)))]), (lambda: {"net": state(ts)})
+    return (lambda: [float(ts.step((mel, audio)))]), (lambda: {"net": state(ts.opt)})
 
 
 def speedyspeech(dev):
@@ -80,7 +79,35 @@ def speedyspeech(dev):
     m.set_state_dict(oss.synth_params(40, cfg))
     batch = {k: v.to(dev) for k, v in sst.synth_batch(50, [9, 6, 8]).items()}
     ts = SpeedySpeechTrainStep(m, max_grad_norm=1.0, learning_rate=2e-5)
-    return (lambda: [float(v) for v in ts.step(batch).values()]), (lambda: {"net": state(ts)})
+    return (lambda: [float(v) for v in ts.step(batch).values()]), (lambda: {"net": state(ts.opt)})
+
+
+def transformer_tts(dev):
+    from oracle import transformer_tts_train as ot
+    from parakeet_b200.models import TransformerTTS
+    from parakeet_b200.training import TransformerTTSTrainStep
+    cfg = ot.TRAIN_SMALL
+    m = TransformerTTS(cfg["idim"], cfg["odim"], device=dev, **{k: v for k, v in cfg.items() if k not in ("idim", "odim")})
+    m.set_state_dict(ot.synth_params(51, cfg))
+    text, tl, sp, sl = ot.golden_batch(cfg, 52, lens=(9, 4, 6), frames=(40, 23, 31))
+    batch = dict(text=text.to(dev), text_lengths=tl.to(dev), speech=sp.to(dev), speech_lengths=sl.to(dev))
+    rates = {k: 0.1 for k in m.dropout_rates}
+    ts = TransformerTTSTrainStep(m, learning_rate=1e-4, guided_attn_loss_lambda=10.0, dropout=rates, seed=9)
+    return (lambda: [float(v) for v in ts.step(batch).values()]), (lambda: {"net": state(ts.opt)})
+
+
+def ge2e(dev):
+    """Three batch shapes A, B, A: the second A is captured while B's planes and graph are kept."""
+    from oracle import ge2e as og
+    from parakeet_b200.models import LSTMSpeakerEncoder
+    from parakeet_b200.training import GE2ETrainStep
+    cfg = (40, 3, 256, 256)
+    m = LSTMSpeakerEncoder(*cfg, device=dev)
+    m.set_state_dict(og.synth_params(13, *cfg))
+    xs = [og.synth_utterances(30 + i, 20, t, 40).to(dev) for i, t in enumerate((50, 31, 50))]
+    ts = GE2ETrainStep(m, num_speakers=4)
+    it = iter(xs)
+    return (lambda: [float(ts.step(next(it)))]), (lambda: {"net": state(ts.opt)})
 
 
 def pwg(dev):
@@ -114,7 +141,7 @@ def main():
     for mode, flag in (("graphs", "1"), ("eager", "0")):
         os.environ["PK_TRAIN_GRAPH"] = os.environ["PK_CUDA_GRAPHS"] = flag      # read when a step is constructed
         for name, make in (("FastSpeech2TrainStep", fastspeech2), ("WaveFlowTrainStep", waveflow), ("SpeedySpeechTrainStep", speedyspeech),
-                           ("PWGTrainStep", pwg)):
+                           ("TransformerTTSTrainStep", transformer_tts), ("GE2ETrainStep", ge2e), ("PWGTrainStep", pwg)):
             result.setdefault(name, {})[mode] = run(make, dev)
     os.makedirs(args.out_dir, exist_ok=True)
     path = os.path.join(args.out_dir, args.name)

@@ -51,16 +51,66 @@ def test_graph_runner_state_machine(monkeypatch):
 
 def test_training_steps_graph_switch(monkeypatch):
     """One switch for every training step: use_graphs when given, else PK_TRAIN_GRAPH; PK_CUDA_GRAPHS=0 wins over both."""
-    from parakeet_b200.training.flat import step_graphs
+    from parakeet_b200.training.flat import StepGraphs, step_graphs
     monkeypatch.delenv("PK_CUDA_GRAPHS", raising=False)
     monkeypatch.delenv("PK_TRAIN_GRAPH", raising=False)
-    assert step_graphs(4).enabled and not step_graphs(4, use_graphs=False).enabled and step_graphs(4).max_graphs == 4
+    for make in (step_graphs, StepGraphs):
+        assert make(4).enabled and not make(4, use_graphs=False).enabled and make(4).max_graphs == 4
     monkeypatch.setenv("PK_TRAIN_GRAPH", "0")
-    assert not step_graphs(4).enabled and step_graphs(4, use_graphs=True).enabled
+    for make in (step_graphs, StepGraphs):
+        assert not make(4).enabled and make(4, use_graphs=True).enabled
     assert G.GraphRunner().enabled                                                      # the inference graphs do not follow it
     monkeypatch.setenv("PK_CUDA_GRAPHS", "0")
     monkeypatch.setenv("PK_TRAIN_GRAPH", "1")
-    assert not step_graphs(4).enabled and not step_graphs(4, use_graphs=True).enabled
+    for make in (step_graphs, StepGraphs):
+        assert not make(4).enabled and not make(4, use_graphs=True).enabled
+
+
+def test_step_graphs_file_planes_and_graph_under_one_key(monkeypatch):
+    """training/flat.py StepGraphs: running a key makes its zero planes current, and evicting the planes of a key drops the graph
+    of the same key (its kernels hold the planes' addresses).  With a bound of 2 after A, A, B, B, C, A's planes and A's graph are
+    both gone; a replay makes its key the most recent.  GE2E used to file its planes under (B, T) and its graph under (B, T, n_mels),
+    so the eviction never found the graph."""
+    from parakeet_b200.training.flat import StepGraphs
+
+    class FakeGraph:
+        def replay(self):
+            pass
+
+    class Ctx:
+        def __enter__(self):
+            pass
+
+        def __exit__(self, *a):
+            return False
+
+    monkeypatch.setattr(torch.cuda, "synchronize", lambda: None)
+    monkeypatch.setattr(torch.cuda, "CUDAGraph", FakeGraph)
+    monkeypatch.setattr(torch.cuda, "graph", lambda g: Ctx())
+    sg = StepGraphs(2, use_graphs=True)
+    sg.enabled = True
+    planes = {}
+
+    def fn(x):                         # a step body: takes operand planes of the current key
+        planes.setdefault(sg.planes._cur, sg.planes.get("xt", (4, 64), "cpu"))
+        return x * 2
+
+    A, B, C = (20, 50, 40), (20, 31, 40), (20, 12, 40)        # GE2E's key: the specs' shape
+    x = torch.ones(3)
+    for k in (A, A, B, B, C):                                  # eager, capture; eager, capture; eager
+        sg.run(k, fn, [x])
+    assert A not in sg.planes._geoms and A not in sg._graphs and A not in sg._seen
+    assert B in sg._graphs and list(sg.planes._geoms) == [B, C]
+    assert sg.planes.get("xt", (4, 64), "cpu") is planes[C]
+    sg.run(C, fn, [x])                                         # capture C
+    sg.run(B, fn, [x])                                         # replay B: the most recent now
+    replays = sg.replays
+    sg.run(A, fn, [x])                                         # A again: C goes, with its graph; B stays captured
+    assert list(sg.planes._geoms) == [B, A] and C not in sg._graphs and B in sg._graphs
+    sg.run(B, fn, [x])
+    assert sg.replays == replays + 1 and sg.planes.get("xt", (4, 64), "cpu") is planes[B]
+    assert torch.equal(sg.run(C, fn, [x], graph=False), x * 2) and C not in sg._seen      # eager: planes only, no graph
+    assert list(sg.planes._geoms) == [B, C] and A not in sg._graphs
 
 
 def test_zero_planes_lru_is_tied_to_the_graphs():

@@ -2,13 +2,12 @@
 (scripts/make_golden_ref.py ge2e), the oracle LSTM against torch.nn.LSTM, the forward's grouping hazard, state-dict keys, the
 EER, the C ABI's argument checks, ptxas pins of the recurrence kernels and the persistent launch's scheduling argument."""
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
+
+import _ptxas
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden", "ref_executed_ge2e.npz")
@@ -190,29 +189,11 @@ def test_scheduling_argument(rows, hidden, max_ctas):
     assert served == {(m, s): 1 for m in range(tiles) for s in range(slices)}
 
 
-def _nvcc():
-    nv = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nv):
-        pytest.skip("nvcc not available")
-    return nv
-
-
-@pytest.fixture(scope="module")
-def ptxas_report(tmp_path_factory):
-    out = tmp_path_factory.mktemp("ptxas") / "lstm.o"
-    r = subprocess.run([_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "lstm.cu"), "-o", str(out)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return r.stderr
-
-
+@_ptxas.needs_nvcc
 @pytest.mark.parametrize("kernel", ["lstm_fwd_kernelILi256E", "lstm_bwd_kernelILi256E", "lstm_fwd_kernelILi64E", "lstm_bwd_kernelILi64E",
                                     "ge2e_loss_kernel"])
-def test_recurrence_kernels_do_not_spill(ptxas_report, kernel):
-    blocks = re.findall(r"Function properties for (\S+)\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads",
-                        ptxas_report)
-    hits = [b for b in blocks if kernel in b[0]]
-    assert hits, kernel
-    for _, _, st, ld in hits:
-        assert int(st) == 0 and int(ld) == 0
-    assert not re.search(r"C75(10|12|20)", ptxas_report)
+def test_recurrence_kernels_do_not_spill(kernel):
+    rep = _ptxas.report("lstm.cu")
+    e = _ptxas.entry(rep, kernel)
+    assert (e["spill_stores"], e["spill_loads"]) == (0, 0), e
+    assert not any(x["codes"] & _ptxas.SERIALIZED for x in rep["entries"]), rep["entries"]

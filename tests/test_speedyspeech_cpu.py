@@ -2,7 +2,6 @@
 padding="same" rule, what ptxas makes of the residual-block kernel, the C-ABI struct layout and the host errors."""
 import ctypes
 import os
-import re
 import shutil
 import subprocess
 
@@ -10,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+import _ptxas
 from conftest import rel_err
 from parakeet_b200 import _lib
 
@@ -77,41 +77,11 @@ def test_paddle_same_rule_known_answers(d):
 
 
 # ------------------------------------------------------------------------------------------------ ptxas on the kernel
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
-        if cand and os.path.isfile(cand) and os.access(cand, os.X_OK):
-            return cand
-    return None
-
-
-@pytest.fixture(scope="module")
-def ptxas_report(tmp_path_factory):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip("nvcc not available")
-    out = tmp_path_factory.mktemp("ptxas") / "speedyspeech.o"
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "speedyspeech.cu"), "-o", str(out)],
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return r.stderr
-
-
-def test_residual_block_kernel_no_spills_and_no_wgmma_serialization(ptxas_report):
-    remarks = [ln for ln in ptxas_report.splitlines() if re.search(r"C75(10|12|20)", ln) and KERNEL in ln]
-    assert not remarks, "\n".join(remarks)
-    lines = ptxas_report.splitlines()
-    start = [i for i, ln in enumerate(lines) if "Compiling entry function" in ln and KERNEL in ln]
-    assert start, f"ptxas reported no entry function {KERNEL}"
-    block = []
-    for ln in lines[start[0] + 1:]:
-        if "Compiling entry function" in ln:
-            break
-        block.append(ln)
-    spills = [re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", ln) for ln in block]
-    spills = [m for m in spills if m]
-    assert spills and all(m.group(1) == "0" and m.group(2) == "0" for m in spills), "\n".join(block)
-    assert any("0 bytes stack frame" in ln for ln in block), "\n".join(block)
+@_ptxas.needs_nvcc
+def test_residual_block_kernel_no_spills_and_no_wgmma_serialization():
+    e = _ptxas.entry(_ptxas.report("speedyspeech.cu"), KERNEL)
+    assert not e["codes"] & _ptxas.SERIALIZED, e
+    assert (e["stack"], e["spill_stores"], e["spill_loads"]) == (0, 0, 0), e
 
 
 # ------------------------------------------------------------------------------------------------ C-ABI

@@ -2,14 +2,12 @@
 (scripts/make_golden_ref.py tacotron2), state-dict keys (both LSTM key formats), the checks that run before any launch, the
 oracle's own consistency and stop rules, and what ptxas makes of the decoder kernel."""
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import _ptxas
 import oracle.tacotron2 as ot
 from parakeet_b200 import _lib
 from parakeet_b200.models import Tacotron2
@@ -168,27 +166,9 @@ def test_oracle_loss_terms():
     assert torch.isclose(out["loss"], out["mel_loss"] + out["post_mel_loss"] + out["guided_attn_loss"] + out["stop_loss"])
 
 
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
-        if cand and os.path.isfile(cand) and os.access(cand, os.X_OK):
-            return cand
-    return None
-
-
-def test_decoder_kernels_compile_for_sm90a_without_spills(tmp_path):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip("nvcc not available")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "tacotron2.cu"), "-o", str(tmp_path / "t.o")],
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lines = r.stderr.splitlines()
-    entries = [i for i, ln in enumerate(lines) if "Compiling entry function" in ln]
-    names = [re.search(r"'(\w+)'", lines[i]).group(1) for i in entries]
-    assert sum("taco2_decode_kernel" in n for n in names) == 2, names
-    for i, name in zip(entries, names):
-        block = lines[i + 1:i + 4]
-        spill = [ln for ln in block if "spill" in ln]
-        assert spill and re.search(r"\b0 bytes spill stores, 0 bytes spill loads", spill[0]), (name, block)
-        assert "0 bytes stack frame" in spill[0], (name, block)
+@_ptxas.needs_nvcc
+def test_decoder_kernels_compile_for_sm90a_without_spills():
+    entries = _ptxas.report("tacotron2.cu")["entries"]
+    assert sum("taco2_decode_kernel" in e["name"] for e in entries) == 2, [e["name"] for e in entries]
+    for e in entries:
+        assert (e["stack"], e["spill_stores"], e["spill_loads"]) == (0, 0, 0), e

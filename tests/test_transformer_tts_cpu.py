@@ -2,14 +2,12 @@
 (scripts/make_golden_ref.py transformer_tts), the state-dict keys, the checks that run before any launch, and what ptxas makes of
 the decoder kernel."""
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import _ptxas
 import oracle.transformer_tts as ot
 from parakeet_b200 import _lib
 from parakeet_b200.models import TransformerTTS
@@ -162,27 +160,9 @@ def test_prenet_masks_are_keyed_by_position():
     assert not torch.equal(m[0], m[1]) and 0.3 < m.mean().item() < 0.7
 
 
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
-        if cand and os.path.isfile(cand) and os.access(cand, os.X_OK):
-            return cand
-    return None
-
-
-def test_decoder_kernel_compiles_for_sm90a_without_spills(tmp_path):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip("nvcc not available")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "transformer_tts.cu"), "-o", str(tmp_path / "t.o")],
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lines = r.stderr.splitlines()
-    entries = [i for i, ln in enumerate(lines) if "Compiling entry function" in ln]
-    names = [re.search(r"'(\w+)'", lines[i]).group(1) for i in entries]
-    assert sum("tts_decode_kernel" in n for n in names) == 1, names
-    for i, name in zip(entries, names):
-        block = lines[i + 1:i + 4]
-        spill = [ln for ln in block if "spill" in ln]
-        assert spill and re.search(r"\b0 bytes spill stores, 0 bytes spill loads", spill[0]), (name, block)
-        assert "0 bytes stack frame" in spill[0], (name, block)
+@_ptxas.needs_nvcc
+def test_decoder_kernel_compiles_for_sm90a_without_spills():
+    rep = _ptxas.report("transformer_tts.cu")
+    _ptxas.entry(rep, "tts_decode_kernel")
+    for e in rep["entries"]:
+        assert (e["stack"], e["spill_stores"], e["spill_loads"]) == (0, 0, 0), e

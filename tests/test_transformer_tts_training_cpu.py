@@ -3,13 +3,12 @@
 entry points and what ptxas makes of its kernels."""
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import _ptxas
 from oracle import transformer_tts_train as ot
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -95,34 +94,13 @@ def test_step_entry_points_in_header_and_binding():
     assert len(_lib.PROTOTYPES["pk_masked_softmax"].argtypes) == 11
 
 
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
-        if cand and os.path.isfile(cand) and os.access(cand, os.X_OK):
-            return cand
-    return None
-
-
-def test_step_kernels_compile_for_sm90a_without_spills(tmp_path):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip("nvcc not available")
+@_ptxas.needs_nvcc
+def test_step_kernels_compile_for_sm90a_without_spills():
     kernels = {"fs2.cu": ("masked_softmax_kernel",), "train.cu": ("softmax_bwd_kernel",),
                "transformer_tts_train.cu": ("guided_loss_kernel", "tts_loss_partial_kernel", "tts_loss_final_kernel", "tts_loss_bwd_kernel")}
     for src, names in kernels.items():
-        r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                            os.path.join(ROOT, "parakeet_b200", "csrc", src), "-o", str(tmp_path / "t.o")],
-                           capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stderr[-4000:]
-        blocks, cur = {}, None
-        for ln in r.stderr.splitlines():
-            m = re.search(r"Compiling entry function '(\w+)'", ln)
-            if m:
-                cur = m.group(1)
-                blocks[cur] = []
-            elif cur:
-                blocks[cur].append(ln)
+        entries = _ptxas.report(src)["entries"]
         for k in names:
-            found = [v for name, v in blocks.items() if k in name]
+            found = [e for e in entries if k in e["name"]]          # softmax_bwd_kernel: with and without the guided loss
             assert found, f"ptxas reported no entry function {k} in {src}"
-            spills = [ln for ln in found[0] if "spill" in ln]
-            assert spills and all(re.search(r"\b0 bytes spill stores, 0 bytes spill loads", ln) for ln in spills), (k, spills)
+            assert all((e["spill_stores"], e["spill_loads"]) == (0, 0) for e in found), found

@@ -2,12 +2,11 @@
 graph) against finite differences and between fp32 and fp64, the zero-output_proj structure of the reference's initialisation,
 what ptxas makes of csrc/waveflow_train.cu, the C-ABI declarations, and the step's argument checks."""
 import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
+
+import _ptxas
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CFG = dict(n_flows=2, n_layers=2, n_group=8)
@@ -76,60 +75,34 @@ def test_oracle_zero_output_proj_gradients():
 
 
 # ------------------------------------------------------------------------------------------------ ptxas on the new kernels
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
-        if cand and os.path.isfile(cand) and os.access(cand, os.X_OK):
-            return cand
-    return None
+def _backward_layer(channels):
+    return _ptxas.entry(_ptxas.report("waveflow_train.cu"), f"waveflow_backward_layer_kernelILi{channels}E")
 
 
-@pytest.fixture(scope="module")
-def ptxas_report(tmp_path_factory):
-    nvcc = _nvcc()
-    if nvcc is None:
-        pytest.skip("nvcc not available")
-    out = tmp_path_factory.mktemp("ptxas") / "waveflow_train.o"
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        os.path.join(ROOT, "parakeet_b200", "csrc", "waveflow_train.cu"), "-o", str(out)],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return r.stderr
-
-
-def _spills(report, kernel):
-    lines = report.splitlines()
-    start = [i for i, ln in enumerate(lines) if "Compiling entry function" in ln and kernel in ln]
-    assert start, f"ptxas reported no entry function {kernel}"
-    for ln in lines[start[0] + 1:]:
-        assert "Compiling entry function" not in ln, f"no spill line for {kernel}"
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", ln)
-        if m:
-            return int(m.group(1)), int(m.group(2))
-
-
-def test_waveflow_train_glue_kernels_do_not_spill(ptxas_report):
-    entries = re.findall(r"Compiling entry function '(\w+)'", ptxas_report)
-    glue = [e for e in entries if "backward_layer" not in e]
+@_ptxas.needs_nvcc
+def test_waveflow_train_glue_kernels_do_not_spill():
+    glue = [e for e in _ptxas.report("waveflow_train.cu")["entries"] if "backward_layer" not in e["name"]]
     assert len(glue) >= 12
-    assert all(_spills(ptxas_report, e) == (0, 0) for e in glue), glue
+    assert all((e["spill_stores"], e["spill_loads"]) == (0, 0) for e in glue), glue
 
 
+@_ptxas.needs_nvcc
 @pytest.mark.parametrize("channels", [64, 128])
-def test_backward_layer_wgmma_not_serialized(ptxas_report, channels):
-    """ptxas remark C7510 / C7520: wgmma serialized (for lack of registers or around a call / branch)."""
-    kernel = f"waveflow_backward_layer_kernelILi{channels}E"
-    remarks = [ln for ln in ptxas_report.splitlines() if re.search(r"C75[12]\d", ln) and kernel in ln]
-    assert not remarks, "\n".join(remarks)
+def test_backward_layer_wgmma_not_serialized(channels):
+    """No C75xx remark at all: neither serialization (_ptxas.SERIALIZED) nor an injected warpgroup.arrive (C7519)."""
+    e = _backward_layer(channels)
+    assert not e["codes"], e
 
 
 # upper bounds: 0 bytes for both instantiations when this test was written (168 registers each, no stack frame)
 SPILL_BOUND = {64: (0, 0), 128: (0, 0)}
 
 
+@_ptxas.needs_nvcc
 @pytest.mark.parametrize("channels", [64, 128])
-def test_backward_layer_spill_bound(ptxas_report, channels):
-    stores, loads = _spills(ptxas_report, f"waveflow_backward_layer_kernelILi{channels}E")
-    assert stores <= SPILL_BOUND[channels][0] and loads <= SPILL_BOUND[channels][1], (stores, loads)
+def test_backward_layer_spill_bound(channels):
+    e = _backward_layer(channels)
+    assert e["spill_stores"] <= SPILL_BOUND[channels][0] and e["spill_loads"] <= SPILL_BOUND[channels][1], e
 
 
 # ------------------------------------------------------------------------------------------------ C-ABI and host checks
